@@ -1,8 +1,8 @@
 #!/usr/bin/env python
-"""bench.py — scans/sec of the B200 scan-matching hot path, with the live roofline of its residual kernel, a parity block
+"""bench.py — scans/sec of the H100 scan-matching hot path, with the live roofline of its residual kernel, a parity block
 against the CPU oracle on the very scans that were timed, and the CPU oracle timed beside it.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--workload NAME] [--impl ours|reference] [--batch B]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--workload NAME] [--impl ours|reference] [--batch B] [--dump-outputs DIR]
 
 One "step" = one batched Match of B synthetic scans per GPU against a static (replicated) map (SURVEY.md §8d/§8e).
 For N > 1 launch under torchrun (one rank per GPU): every rank matches its own B scans per step; the per-scan results
@@ -16,6 +16,10 @@ Timed legs (all inside this process, nothing under a profiler):
   roofline  same steps on a handle created with FLS_FLAG_PROFILE: CUDA events around every residual-kernel launch
   cpu_baseline / --impl reference: the CPU oracle (port of the reference algorithm, OpenMP; thread count chosen by a sweep)
   parity    GPU results of the scan pool vs the oracle's results for the same scans and guesses (N = 1, rank 0)
+
+--dump-outputs DIR writes what the `value` leg returned in its last timed step (rank 0): the B poses, converged flags,
+iterations and n_valid, and the indices of the scans in the seeded pool, as DIR/<name>.npy (float64).  The scene, the scans
+and the guesses are generated from fixed seeds, so two builds run with the same arguments can be compared output for output.
 """
 from __future__ import annotations
 
@@ -69,7 +73,7 @@ def load_peaks():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "fallback (H100 SXM data sheet: 3.35 TB/s HBM3, not a measurement)"
 
 
 # ---- host CPU: how many cores may this process really use ---------------------------------------------------------------
@@ -433,7 +437,11 @@ def main():
     ap.add_argument("--no-secondary", action="store_true", help="skip the short K2/K3/K4/K5 side measurements")
     ap.add_argument("--no-cpu", action="store_true", help="skip the cpu_baseline + parity leg (profiling runs)")
     ap.add_argument("--batch", type=int, default=8, help="scans per GPU per step (one fls_match_batch call; BASELINE config 4 uses batches of 8)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the results of the last timed step of the value leg as DIR/<name>.npy (float64)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     wl = WORKLOADS[args.workload]
     rank = int(os.environ.get("RANK", "0"))
     world_size = int(os.environ.get("WORLD_SIZE", "1"))
@@ -480,6 +488,12 @@ def main():
     # device buffer and all-gathered over NCCL asynchronously; consumed two steps later (never inside the step)
     gather = parallel.AsyncResultGather(B, device=dev, depth=3)
     gathered_steps = [0]
+    last_value_step = {}  # results of the last timed step of the value leg (--dump-outputs)
+
+    def keep_last(i, oks, Ts, st):
+        last_value_step.update(scan_index=np.array(ids(i), np.float64), pose=np.asarray(Ts, np.float64).reshape(-1, 4, 4),
+                               converged=np.asarray(oks, np.float64), iterations=np.array([x.iterations for x in st], np.float64),
+                               n_valid=np.array([x.n_valid for x in st], np.float64))
 
     def flush_l2():
         flush_buf.zero_()
@@ -549,6 +563,8 @@ def main():
             d2h += sum(x.d2h_bytes for x in st)
             for j, T in zip(ids(warmup + i), Ts):
                 errs.append(synth.pose_error(T, truths[j]))
+            if not host and i == steps - 1:
+                keep_last(warmup + i, oks, Ts, st)
         # the collectives still in flight belong to the K timed steps: drain them inside the timed region
         e0.record()
         gather.drain()
@@ -591,6 +607,8 @@ def main():
         def end(i, acc):
             h = i % 2
             oks, Ts = regs[h].match_batch_end()
+            if not host and i == warmup + steps - 1:
+                keep_last(i, oks, Ts, regs[h].last_batch_stats)
             gs[h].launch()
             if len(gs[h].pending) > 2:
                 gs[h]._collect(gs[h].pending.pop(0))
@@ -648,6 +666,10 @@ def main():
         ms_dev, launches, iters, _, _, errs, ranks_dev, drain_dev = timed(False, reg, args.steps, args.warmup)
         ms_e2e, _, _, h2d, d2h, _, ranks_e2e, _ = timed(True, reg, args.steps, args.warmup)
     reg.set_result_buffer_device(0, 0)
+    if args.dump_outputs and rank == 0:
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        for name, arr in last_value_step.items():
+            np.save(os.path.join(args.dump_outputs, f"{name}.npy"), arr)
 
     # roofline leg: same steps with CUDA events around every residual-kernel launch
     reg_p = Registration(make_cfg(wl, local_rank, len(mp), flags=_abi.FLS_FLAG_PROFILE))
@@ -667,14 +689,6 @@ def main():
     del reg_p
     peak, peak_src = load_peaks()
     achieved = (k_bytes / max(k_launch, 1)) / ((k_ms / max(k_launch, 1)) * 1e-3) / 1e9 if k_ms > 0 else 0.0
-    traffic = prof = None
-    tp = os.path.join(ROOT, "profiles", "traffic_k1.json")
-    if wl["method"] == _abi.FLS_P2PLANE_IVOX and os.path.exists(tp):
-        try:
-            prof = json.load(open(tp))
-            traffic = prof.get("dram_bytes_per_launch")
-        except Exception:
-            traffic = prof = None
 
     total_scans = args.steps * world_size * B
     value = total_scans / (ms_dev * 1e-3)
@@ -733,21 +747,11 @@ def main():
     if rank == 0:
         pos = float(np.median([e[0] for e in errs]))
         launch_us = 1e3 * k_ms / max(k_launch, 1)
-        roof = {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "traffic": traffic,
+        roof = {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
                 "peak_source": peak_src, "launches": int(k_launch), "avg_launch_us": launch_us, "algo_bytes_per_launch": k_bytes / max(k_launch, 1)}
         if wl["method"] == _abi.FLS_P2PLANE_IVOX:
             roof["kernel"] = ("p2plane_v9_kernel (whole GN loop fused: TMA-staged iVox 5-NN + plane fit + J/r + DMMA 6x6 reduction + solve; one "
                               "launch = every iteration of every scan of the batch)")
-            if prof:
-                # second roofline (VERDICT r1 item 4): what the kernel is really bound by.  Static inputs from the committed ncu
-                # capture of the shipped configuration (profiles/traffic_k1.json), times measured live above.
-                sm_clock = (clocks.get("sm_mhz") or 1965.0) * 1e6
-                if prof.get("warp_instructions_per_launch"):
-                    roof["issue_floor_us"] = 1e6 * prof["warp_instructions_per_launch"] / (148 * 4 * sm_clock)
-                    roof["issue_frac"] = roof["issue_floor_us"] / max(launch_us, 1e-9)
-                if traffic:
-                    roof["dram_frac"] = traffic / (launch_us * 1e-6) / 1e9 / peak
-                roof["traffic_source"] = prof.get("source")
         else:
             roof["kernel"] = ("ndt_gn_batch_kernel (one cooperative launch per batch: a sub-grid and a fused GN loop per scan — 7-probe NDT "
                               "residual + 6x6 reduction + solve)")

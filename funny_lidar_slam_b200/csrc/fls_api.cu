@@ -215,8 +215,8 @@ int Handle::enqueue_ivox_batch(int B, const float4* const* d_scans, const size_t
     off[0] = 0;
     int grid = 1;
     // K1 generations: the dataflow kernel (v9: TMA-staged runs, work ring, DMMA sums — fls_p2plane_v9.cu) serves batches; a single
-    // Match runs on the barrier kernel (v8, fls_p2plane.cu) whose one-chunk-per-warp round has the shorter hand-over (measured on
-    // B200, 108 k points: 139 vs 191 us per Match kernel; batch of 8: 683 vs 609 us).  FLS_K1=8 / 9 forces one of them.
+    // Match runs on the barrier kernel (v8, fls_p2plane.cu) whose one-chunk-per-warp round has the shorter hand-over (DESIGN.md
+    // §3.1 has the H100 numbers).  FLS_K1=8 / 9 forces one of them.
     const char* k1 = std::getenv("FLS_K1");
     const int k1v = k1 ? std::atoi(k1) : 0;
     const bool use_v9 = k1v == 9 || (k1v != 8 && B > 1);
@@ -1024,7 +1024,7 @@ const char* fls_strerror(int status) {
         case FLS_OK: return "ok";
         case FLS_ERR_INVALID_ARG: return "invalid argument";
         case FLS_ERR_CUDA: return "CUDA runtime error (see fls_last_error)";
-        case FLS_ERR_NO_DEVICE: return "no sm_100 CUDA device (this library has no CPU fallback)";
+        case FLS_ERR_NO_DEVICE: return "no sm_90 CUDA device (this library has no CPU fallback)";
         case FLS_ERR_UNSUPPORTED: return "method or mode not supported by this build";
         case FLS_ERR_NO_MAP: return "Match called before AddCloudToLocalMap";
         case FLS_ERR_CAPACITY: return "voxel capacity reached (LRU eviction is not emulated on the device)";

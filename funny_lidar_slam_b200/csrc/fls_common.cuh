@@ -1,4 +1,4 @@
-// fls_common.cuh — shared device/host helpers of the B200 (sm_100a) scan-matching library.
+// fls_common.cuh — shared device/host helpers of the H100 (sm_90a) scan-matching library.
 // Nothing in this tree includes or links anything under oracle/.
 #pragma once
 #include <cuda_runtime.h>

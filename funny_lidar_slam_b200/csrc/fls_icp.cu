@@ -205,7 +205,7 @@ int icp_grid_blocks(int n, int device) {
     }
     const int per_block = kIcpBlock / kIcpLanes;
     const int need = (n + per_block - 1) / per_block;
-    const int c = (device >= 0 && device < 64) ? cap[device] : 148;
+    const int c = (device >= 0 && device < 64) ? cap[device] : 132;
     const int g = need < c ? need : c;
     return g > 0 ? g : 1;
 }

@@ -230,7 +230,7 @@ int loam_grid_blocks(int n, int device) {
     }
     const int per_block = kLoamBlock / kLoamLanes;
     const int need = (n + per_block - 1) / per_block;
-    const int c = (device >= 0 && device < 64) ? cap[device] : 148;
+    const int c = (device >= 0 && device < 64) ? cap[device] : 132;
     const int g = need < c ? need : c;
     return g > 0 ? g : 1;
 }

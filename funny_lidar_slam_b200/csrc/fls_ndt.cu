@@ -421,7 +421,7 @@ int ndt_grid(int n, int device) {
         cap[device] = sms * (per_sm > 0 ? per_sm : 1);
     }
     const int need = (n + kNdtBlock - 1) / kNdtBlock;
-    const int c = (device >= 0 && device < 64) ? cap[device] : 148;
+    const int c = (device >= 0 && device < 64) ? cap[device] : 132;
     const int g = need < c ? need : c;
     return g > 0 ? g : 1;
 }
@@ -441,7 +441,7 @@ int ndt_max_grid(int device) {
         cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, ndt_gn_batch_kernel<kNdtBlock>, kNdtBlock, 0);
         cap[device] = sms * (per_sm > 0 ? per_sm : 1);
     }
-    return (device >= 0 && device < 64) ? cap[device] : 148;
+    return (device >= 0 && device < 64) ? cap[device] : 132;
 }
 void launch_ndt_batch(const NdtBatchItem* d_items, int n_scans, int grid, cudaStream_t st) {
     void* params[] = {&d_items, &n_scans};

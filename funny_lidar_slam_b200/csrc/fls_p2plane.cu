@@ -10,7 +10,7 @@
 // the CTA rows in a fixed order, solves the 6x6 system, updates the pose and applies the stop rule (:167-203), then publishes the
 // next pose.  No host round trip inside a Match.
 //
-// B200 mapping
+// Mapping onto the GPU
 //   * grid = the CTAs the scan's chunks need (one 24-warp CTA per SM, 768 threads, 80 registers) + the folding CTA, launched
 //     cooperatively only to guarantee co-residency; the scheduling unit is the WARP: warp w of CTA c works on 32-point chunk
 //     (c, w) of every scan of the visit group, a static round-robin (consecutive chunks stay in one CTA: Morton neighbours share
@@ -647,9 +647,8 @@ void prepare_queries(const float4* const* d_scan_ptrs, int n_total, const int* d
     sc.idx.reserve(m);
     sc.idx_sorted.reserve(m);
     const char* kb = std::getenv("FLS_SORT_KEY_BITS");
-    // measured on B200 (tools/match_timing.py, 108 k points): 24-bit keys 186 us / Match, 16-bit keys 165 us — one
-    // 12 us onesweep pass less, and the fused kernel is no slower (22.9 vs 23.8 us / iteration): an 8 m x 32 m x 32 m
-    // Morton window is all the locality the L1 broadcast needs
+    // 16-bit keys need one onesweep pass less than 24-bit keys, and an 8 m x 32 m x 32 m Morton window is all the locality the
+    // L1 broadcast needs (DESIGN.md §3.1 has the H100 comparison)
     int key_bits = kb ? std::atoi(kb) : 16;
     if (key_bits != 16 && key_bits != 20 && key_bits != 24) key_bits = 16;
     int scan_bits = 0;

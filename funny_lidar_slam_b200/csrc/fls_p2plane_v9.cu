@@ -4,9 +4,9 @@
 // What it computes is unchanged (include/registration/loam_point_to_plane_ivox.h:141-340, src/ivox_map/ivox_map.cpp:6-37
 // upstream; see fls_p2plane.cu for the per-point arithmetic and its rounding rules).  What changed is how the machine is
 // driven — ncu on the previous generation showed a latency-bound kernel (issue active 32 %, long scoreboard 40 % and CTA
-// barrier 26 % of the warp time, profiles/k1_r1f_summary.md), so this one removes both stalls:
+// barrier 26 % of the warp time), so this one removes both stalls:
 //
-//   * Roles.  A CTA (one per SM, all 148) has W compute warps, one SERVER warp and one FOLDER warp; nothing in the loop
+//   * Roles.  A CTA (one per SM: 132 on an H100 SXM) has W compute warps, one SERVER warp and one FOLDER warp; nothing in the loop
 //     is a CTA-wide barrier.  Compute warps walk the same sequence of (scan, iteration) items — iteration `it` of every
 //     live scan, round-robin — each at its own pace.
 //   * TMA-staged candidates, double-buffered per warp.  For its NEXT 32-point chunk a warp loads the source points,
@@ -777,7 +777,8 @@ __global__ void __launch_bounds__((W + 2) * 32, 1) p2plane_v9_kernel(P2PlaneLoop
         if (lane == 0) st_release_smem(&ctl->quit, 1u);
     } else {
         // =============================== folder warp: rows -> group rows -> totals -> gn_step -> next pose =================
-        // Two-level fold (one warp has 16 loads = one L2 round trip in flight; 148 rows in sequence were measured at ~30 us):
+        // Two-level fold (one warp has 16 loads = one L2 round trip in flight, so one warp folding every CTA row in sequence pays
+        // a round trip per 16 rows):
         //   * the folder warp of every kGroup-th CTA (a group leader) adds the CTA rows of its group in CTA order and publishes
         //     a group row;
         //   * the folder warp of CTA fold_cta(scan) adds the group rows in group order, runs gn_step and publishes the next pose.

@@ -15,7 +15,7 @@ namespace {
 // ascending-index tie-break IS the reference's "earlier candidate wins" rule.  Rejected candidates carry the
 // sentinel key {+inf, 0xffffffff}, which never displaces anything.
 // (measured: holding {distance bits, index} as one fp64 key and using fmin/fmax compiles to DSETP + 2 FSEL per
-//  min/max on sm_100a — slower than the separate float / index compare-exchange below.)
+//  min/max — slower than the separate float / index compare-exchange below.)
 struct Top5 {
     float d0, d1, d2, d3, d4;
     unsigned k0, k1, k2, k3, k4;

@@ -1,5 +1,5 @@
 /*
- * fls_b200.h — C ABI of the B200-native (sm_100a) scan-matching frontend.
+ * fls_b200.h — C ABI of the H100-native (sm_90a) scan-matching frontend.
  *
  * Drop-in boundary for funny_lidar_slam's registration plug-in interface.  Every entry point is what
  * a thin `RegistrationInterface` adapter (funny_lidar_slam_b200/shim/b200_registration.h, see
@@ -48,7 +48,7 @@ typedef enum {
     FLS_OK = 0,
     FLS_ERR_INVALID_ARG = -1,   /* null pointer, bad stride, sentinel ("NaN") parameter left unset */
     FLS_ERR_CUDA = -2,          /* a CUDA runtime call failed; fls_last_error() has the text */
-    FLS_ERR_NO_DEVICE = -3,     /* no sm_100 device visible — the product has NO CPU fallback */
+    FLS_ERR_NO_DEVICE = -3,     /* no sm_90 device visible — the product has NO CPU fallback */
     FLS_ERR_UNSUPPORTED = -4,   /* method / mode not implemented by this build */
     FLS_ERR_NO_MAP = -5,        /* Match before AddCloudToLocalMap (reference: CHECK(!grids_.empty())) */
     FLS_ERR_CAPACITY = -6,      /* voxel count would exceed the LRU capacity (eviction not emulated on device) */

@@ -4,6 +4,7 @@
 The reference cannot be built or imported here (SURVEY.md §8c) and ships no fixture for this path, so these
 goldens pin the ORACLE (regression anchor for the restatement), not the reference: parity stays "unpinned".
 Run from the repo root:  python tests/golden/make_golden.py
+(`--reference-tree DIR` instead rewrites reference_line_counts.json from a checkout of the reference.)
 """
 import os
 import sys
@@ -110,6 +111,25 @@ def round2():
     np.savez(os.path.join(OUT, "ivox_lru_cap5000.npz"), counts=np.array(counts, np.int64))
 
 
+def reference_line_counts(ref: str):
+    """Line counts of the reference's citable files (path relative to `ref`), which tests/test_citations.py checks the
+    `file:line` citations of this repository against."""
+    import json
+    counts = {}
+    for d, _, fs in os.walk(ref):
+        if "/.git" in d:
+            continue
+        for f in fs:
+            if f.endswith((".h", ".cpp", ".yaml", ".md", ".txt")):
+                with open(os.path.join(d, f), errors="ignore") as fh:
+                    counts[os.path.relpath(os.path.join(d, f), ref)] = sum(1 for _ in fh)
+    with open(os.path.join(OUT, "reference_line_counts.json"), "w") as fh:
+        json.dump(dict(sorted(counts.items())), fh, indent=0)
+
+
 if __name__ == "__main__":
-    main()
-    round2()
+    if len(sys.argv) == 3 and sys.argv[1] == "--reference-tree":
+        reference_line_counts(sys.argv[2])
+    else:
+        main()
+        round2()

@@ -1,13 +1,13 @@
 """Every `file:line` citation of the reference in the ABI header, the docs, the oracle and the CUDA sources must point at
-an existing file of the reference tree with at least that many lines.  Runs only where the read-only reference is mounted
-(the build container); skipped elsewhere (the GPU box has no /root/reference and nothing there needs it)."""
+an existing file of the reference tree with at least that many lines.  The reference tree is described by
+tests/golden/reference_line_counts.json (path relative to the reference root -> number of lines), regenerated with
+`python tests/golden/make_golden.py --reference-tree DIR`."""
+import json
 import os
 import re
 
-import pytest
-
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = "/root/reference"
+GOLDEN = os.path.join(ROOT, "tests", "golden", "reference_line_counts.json")
 PAT = re.compile(r"([A-Za-z0-9_/\.]+\.(?:h|cpp|yaml|md|txt)):(\d+)(?:-(\d+))?")
 
 
@@ -18,18 +18,12 @@ def _sources():
     return out
 
 
-@pytest.mark.skipif(not os.path.isdir(REF), reason="reference tree not mounted")
 def test_reference_citations_resolve():
+    with open(GOLDEN) as fh:
+        counts = json.load(fh)
     files = {}
-    for d, _, fs in os.walk(REF):
-        if "/.git" in d:
-            continue
-        for f in fs:
-            files.setdefault(f, []).append(os.path.join(d, f))
-
-    def n_lines(p):
-        with open(p, errors="ignore") as fh:
-            return sum(1 for _ in fh)
+    for rel in counts:
+        files.setdefault(os.path.basename(rel), []).append(rel)
 
     checked, bad = 0, []
     for src in _sources():
@@ -41,10 +35,10 @@ def test_reference_citations_resolve():
             checked += 1
             cands = files.get(base, [])
             if "/" in path:
-                cands = [c for c in cands if c.endswith(path)] or cands
+                cands = [c for c in cands if ("/" + c).endswith("/" + path.lstrip("./"))] or cands
             if not cands:
                 bad.append((os.path.relpath(src, ROOT), m.group(0), "no such file in the reference"))
-            elif max(n_lines(c) for c in cands) < last:
+            elif max(counts[c] for c in cands) < last:
                 bad.append((os.path.relpath(src, ROOT), m.group(0), "file is shorter than the cited line"))
     assert checked > 150
     assert not bad, bad
