@@ -157,9 +157,6 @@ struct GnState {
     int converged;  // value Match returns
     int failed;     // early-out (NDT effective_num < min)
     int pad[2];
-    // device-side phase timestamps (globaltimer ns) of the fused LOAM loop, first 16 iterations:
-    // [it][0] iteration start, [1] last CTA arrived, [2] partials reduced, [3] solved + released
-    unsigned long long dbg[16][4];
 };
 
 // upper-triangular index of a symmetric 6x6 (row <= col)

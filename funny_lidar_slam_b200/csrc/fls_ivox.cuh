@@ -23,7 +23,6 @@ struct IvoxView {
     const float4* __restrict__ lists;   // stencil lists (may be null)
     const HashSlot* __restrict__ ctab;  // centre table
     unsigned cmask;
-    unsigned prefetch;  // 0 none, 1 L2, 2 L1: request the whole candidate run right after the table probe
     unsigned fast_knn;  // 1: every stencil candidate is provably within max_range (range test and exact rounding not needed up front)
 };
 

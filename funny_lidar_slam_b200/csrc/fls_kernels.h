@@ -7,7 +7,7 @@
 
 namespace fls {
 
-static constexpr int kP2PlaneBlock = 768;  // default shape of the persistent LOAM-iVox kernel: one 24-warp CTA per SM (fls_p2plane.cu)
+static constexpr int kP2PlaneBlock = 768;  // shape of the persistent LOAM-iVox kernel: one 24-warp CTA per SM (fls_p2plane.cu)
 static constexpr int kNdtBlock = 512;  // few CTA rows for the folder: a dense scan fills the device with ~150-300 CTAs instead of > 1000
 static constexpr int kIcpBlock = 512;   // 64 queries x 8 lanes per CTA: few rows for the folder
 static constexpr int kLoamBlock = 256;
@@ -43,12 +43,10 @@ struct P2PlaneLoopArgs {
     int log_cap;
     const P2PlaneScan* scans;  // [n_scans]; every CTA serves every scan, CTA (s mod grid) folds and solves scan s
     int n_scans;
-    int visit_group;  // scans per visit (1..8): a warp works through its chunk of each of them between two CTA barriers
     unsigned* tickets;  // v9: chunk ticket counters [n_scans][ticket_stride], zeroed before the launch
     int ticket_stride;  // >= max_iterations + 2
     unsigned* abort_word;  // v9 watchdog: zeroed before the launch, non-zero when a wait loop gave up (protocol error)
 };
-int p2plane_block();                   // threads per CTA of the selected kernel shape
 int p2plane_max_grid(int device);      // co-resident CTAs
 int p2plane_chunks(int n);             // warp-sized (32-point) work chunks
 int p2plane_grid(int n, int device);    // CTAs that serve a scan of n points: its chunks / warps per CTA, + the folder, <= co-resident

@@ -40,12 +40,6 @@
 namespace fls {
 namespace {
 
-__device__ __forceinline__ unsigned long long globaltimer_ns() {
-    unsigned long long t;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-    return t;
-}
-
 // IVoxMap::GetClosestPoint through the stencil lists: one probe of the centre table, then a streaming scan of the
 // contiguous candidate run (already in the reference's visit order).  Indices refer to `lists`.
 __device__ __forceinline__ void knn5_stream(const IvoxView& m, float qx, float qy, float qz, Top5& nn, unsigned& n_cand) {
@@ -60,14 +54,10 @@ __device__ __forceinline__ void knn5_stream(const IvoxView& m, float qx, float q
     // A run is ~4 cache lines and the scan below touches them one after the other; when a line is not on chip yet (first
     // touch of a voxel in this Match) that would be one exposed HBM round trip per line.  Requesting the rest of the run
     // up front overlaps them (lanes that share a run issue the same addresses: one request).
-    if (m.prefetch) {
+    {
         const char* pl = reinterpret_cast<const char*>(L);
         const unsigned bytes = count * 16u;
-        if (m.prefetch == 1) {
-            for (unsigned off = 128u; off < bytes; off += 128u) asm volatile("prefetch.global.L2 [%0];" ::"l"(pl + off));
-        } else {
-            for (unsigned off = 128u; off < bytes; off += 128u) asm volatile("prefetch.global.L1 [%0];" ::"l"(pl + off));
-        }
+        for (unsigned off = 128u; off < bytes; off += 128u) asm volatile("prefetch.global.L2 [%0];" ::"l"(pl + off));
     }
     if (count > 64u) {  // position does not fit the 6-bit field
         knn5_exact(L, start, count, r2, qx, qy, qz, nn);
@@ -199,8 +189,7 @@ __global__ void __launch_bounds__(BLOCK, MINB) p2plane_gn_kernel(P2PlaneLoopArgs
     while (n_left > 0) {
         // ---- the group: the next (up to V) unfinished scans in round-robin order (uniform: s_iter is shared) -------------
         int gs[V], git[V], nv = 0;
-        const int vmax = a.visit_group < V ? a.visit_group : V;
-        for (int k = 0; k < a.n_scans && nv < vmax; ++k) {
+        for (int k = 0; k < a.n_scans && nv < V; ++k) {
             const int s = (next + k) % a.n_scans;
             const int it = s_iter[s];
             if (it == 255) continue;
@@ -246,7 +235,6 @@ __global__ void __launch_bounds__(BLOCK, MINB) p2plane_gn_kernel(P2PlaneLoopArgs
             const int s = gs[v];
             const P2PlaneScan* __restrict__ sc = a.scans + s;
             const int folder = s % G;
-            if (cta == folder && threadIdx.x == 0 && git[v] < 16) sc->state->dbg[git[v]][0] = globaltimer_ns();
             const int n = sc->n;
             const int n_chunks = (n + 31) >> 5;  // warp-sized chunks
             const float4* __restrict__ src = sc->src;
@@ -365,18 +353,13 @@ __global__ void __launch_bounds__(BLOCK, MINB) p2plane_gn_kernel(P2PlaneLoopArgs
             s_red[warp][lane] = sum;
             __syncthreads();
             if (warp == 0) {
-                if (lane == 0 && it < 16) state->dbg[it][1] = globaltimer_ns();
                 double t = 0;
 #pragma unroll
                 for (int w = 0; w < W; ++w) t += s_red[w][lane];
                 __syncwarp();
                 s_red[0][lane] = t;
                 __syncwarp();
-                if (lane == 0) {
-                    if (it < 16) state->dbg[it][2] = globaltimer_ns();
-                    gn_step_pre(state, pre, s_red[0], a.gp, sc->log, a.log_cap, sc->ll_pose, tag, sc->result);
-                    if (it < 16) state->dbg[it][3] = globaltimer_ns();
-                }
+                if (lane == 0) gn_step_pre(state, pre, s_red[0], a.gp, sc->log, a.log_cap, sc->ll_pose, tag, sc->result);
             }
             __syncthreads();  // s_red is reused by the next fold
         }
@@ -564,53 +547,25 @@ __global__ void ivox_insert_scatter_kernel(const unsigned char* __restrict__ cls
     else if (c == 2) out[n1 + (unsigned)(excl[i] >> 32)] = world[i];
 }
 
-// Shapes of the same kernel: BLOCK threads x kMinB CTAs per SM = the same 24 resident warps (<= 80 registers).  Small CTAs
-// mean small barrier groups (a visit ends with one __syncthreads: every warp waits for the slowest of its CTA) but more
-// rows to fold; with a batch the fold is hidden behind the other scans.  FLS_P2PLANE_BLOCK=96|192|384|768 overrides.
-template <int BLOCK>
-struct P2PlaneShape {
-    static constexpr int kMinB = BLOCK >= 768 ? 1 : 768 / BLOCK;
-    static const void* fn() { return (const void*)p2plane_gn_kernel<BLOCK, kMinB>; }
-    static size_t smem() {
-        constexpr int W = BLOCK / 32, V = kVisitGroup < W ? kVisitGroup : W;
-        return (size_t)W * 32 * kRecW * sizeof(double) + (size_t)V * W * 32 * sizeof(double);
-    }
-    static int max_grid(int sms) {
-        int per_sm = 0;
-        cudaFuncSetAttribute(fn(), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem());
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, p2plane_gn_kernel<BLOCK, kMinB>, BLOCK, smem());
-        return sms * (per_sm > 0 ? per_sm : 1);
-    }
-    static void launch(int grid, void** params, cudaStream_t st) {
-        FLS_CUDA(cudaLaunchCooperativeKernel(fn(), dim3(grid), dim3(BLOCK), params, smem(), st));
-    }
-};
+// One 768-thread CTA per SM: 24 resident warps (<= 80 registers).
+constexpr int kMinB = 1;
+const void* p2plane_fn() { return (const void*)p2plane_gn_kernel<kP2PlaneBlock, kMinB>; }
+size_t p2plane_smem() {
+    constexpr int W = kP2PlaneBlock / 32, V = kVisitGroup < W ? kVisitGroup : W;
+    return (size_t)W * 32 * kRecW * sizeof(double) + (size_t)V * W * 32 * sizeof(double);
+}
 
 }  // namespace
-
-int p2plane_block() {
-    static int block = 0;
-    if (!block) {
-        const char* e = std::getenv("FLS_P2PLANE_BLOCK");
-        const int v = e ? std::atoi(e) : 0;
-        block = (v == 96 || v == 192 || v == 384 || v == 768 || v == 1024) ? v : kP2PlaneBlock;
-    }
-    return block;
-}
 
 int p2plane_max_grid(int device) {
     static int cached[64] = {0};
     if (device >= 0 && device < 64 && cached[device]) return cached[device];
     int sms = 0;
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
-    int g;
-    switch (p2plane_block()) {
-        case 96: g = P2PlaneShape<96>::max_grid(sms); break;
-        case 192: g = P2PlaneShape<192>::max_grid(sms); break;
-        case 384: g = P2PlaneShape<384>::max_grid(sms); break;
-        case 1024: g = P2PlaneShape<1024>::max_grid(sms); break;
-        default: g = P2PlaneShape<768>::max_grid(sms); break;
-    }
+    int per_sm = 0;
+    cudaFuncSetAttribute(p2plane_fn(), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p2plane_smem());
+    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, p2plane_gn_kernel<kP2PlaneBlock, kMinB>, kP2PlaneBlock, p2plane_smem());
+    const int g = sms * (per_sm > 0 ? per_sm : 1);
     if (device >= 0 && device < 64) cached[device] = g;
     return g;
 }
@@ -618,7 +573,7 @@ int p2plane_max_grid(int device) {
 int p2plane_chunks(int n) { return (n + 31) / 32; }
 
 int p2plane_grid(int n, int device) {
-    const int W = p2plane_block() / 32;
+    const int W = kP2PlaneBlock / 32;
     const int need = (p2plane_chunks(n) + W - 1) / W;
     const int cap = p2plane_max_grid(device);
     const int g = need + 1 < cap ? need + 1 : cap;  // + the folding CTA (stays without chunks when there is room)
@@ -628,13 +583,7 @@ int p2plane_grid(int n, int device) {
 void launch_p2plane_loop(const P2PlaneLoopArgs& a, int grid, cudaStream_t st) {
     P2PlaneLoopArgs args = a;
     void* params[] = {&args};
-    switch (p2plane_block()) {
-        case 96: P2PlaneShape<96>::launch(grid, params, st); break;
-        case 192: P2PlaneShape<192>::launch(grid, params, st); break;
-        case 384: P2PlaneShape<384>::launch(grid, params, st); break;
-        case 1024: P2PlaneShape<1024>::launch(grid, params, st); break;
-        default: P2PlaneShape<768>::launch(grid, params, st); break;
-    }
+    FLS_CUDA(cudaLaunchCooperativeKernel(p2plane_fn(), dim3(grid), dim3(kP2PlaneBlock), params, p2plane_smem(), st));
 }
 
 // Per-batch preparation: state init + flag reset + locality keys (one kernel), then order every scan by the voxel each
@@ -646,16 +595,13 @@ void prepare_queries(const float4* const* d_scan_ptrs, int n_total, const int* d
     sc.k32b.reserve(m);
     sc.idx.reserve(m);
     sc.idx_sorted.reserve(m);
-    const char* kb = std::getenv("FLS_SORT_KEY_BITS");
     // 16-bit keys need one onesweep pass less than 24-bit keys, and an 8 m x 32 m x 32 m Morton window is all the locality the
     // L1 broadcast needs (DESIGN.md §3.1 has the H100 comparison)
-    int key_bits = kb ? std::atoi(kb) : 16;
-    if (key_bits != 16 && key_bits != 20 && key_bits != 24) key_bits = 16;
+    constexpr int key_bits = 16;
     int scan_bits = 0;
     while ((1 << scan_bits) < n_scans) ++scan_bits;
     p2plane_prep_kernel<<<(m + 255) / 256, 256, 0, st>>>(d_scan_ptrs, n_total, d_offsets, n_scans, d_poses, map.inv_res, (key_bits - 12) / 2, sc.k32a.p,
-                                                        sc.idx.p, d_flags, d_states, std::getenv("FLS_NO_PREFETCH") ? nullptr : map.ctab,
-                                                        map.cmask, map.lists);
+                                                        sc.idx.p, d_flags, d_states, map.ctab, map.cmask, map.lists);
     if (launches) *launches += 1;
     if (n_total <= 0) return;
     const int sort_bits = key_bits + scan_bits;

@@ -234,6 +234,10 @@ struct ChunkRegs {
 
 // ---- the kernel ----------------------------------------------------------------------------------------------------------
 constexpr int kRing = 256;  // entries of the CTA's work ring (power of two)
+// refill policy of the server warp: with several scans open it keeps kRefillQuarters / 4 x W chunks drawn and not done, and the
+// second-oldest open scan draws 1 / kSecondShareDiv of what the oldest does
+constexpr int kRefillQuarters = 12;
+constexpr int kSecondShareDiv = 4;
 
 template <int W, int CAP>
 __global__ void __launch_bounds__((W + 2) * 32, 1) p2plane_v9_kernel(P2PlaneLoopArgs a) {
@@ -260,10 +264,6 @@ __global__ void __launch_bounds__((W + 2) * 32, 1) p2plane_v9_kernel(P2PlaneLoop
         reinterpret_cast<unsigned long long*>(s_desc)[k] = reinterpret_cast<const unsigned long long*>(a.scans)[k];
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     fence_proxy_async_smem();
-#ifdef FLS_K1_TRACE
-    if (cta == 0 && threadIdx.x < 8) a.scans[0].state->dbg[8][threadIdx.x] = 0;
-    if (cta == 0 && threadIdx.x < 4) a.scans[0].state->dbg[10 + threadIdx.x][0] = 0;
-#endif
     __syncthreads();  // the only CTA-wide barrier of the kernel
 
     if (warp < W) {
@@ -280,15 +280,6 @@ __global__ void __launch_bounds__((W + 2) * 32, 1) p2plane_v9_kernel(P2PlaneLoop
         const int dr = lane >> 2, dc = lane & 3;
         const int dep0 = dep_index(dr, 2 * dc), dep1 = dep_index(dr, 2 * dc + 1);
         unsigned ph = 0;  // bit s: parity the next wait on stage s expects
-#ifdef FLS_K1_TRACE
-        unsigned long long* const trc = &s_desc[0].state->dbg[8][0];  // [0..3] ns waiting / prefetch / compute / -, [4] max compute ns, [5] chunks, [6] mixed chunks, [7] exact lanes
-        unsigned long long t_spin = 0, t_pre = 0, t_cmp = 0, t_max = 0, n_chunk = 0, n_mixed = 0;
-#define TRC_T0 const unsigned long long trc_t0 = globaltimer_ns9();
-#define TRC_ADD(x) x += globaltimer_ns9() - trc_t0;
-#else
-#define TRC_T0
-#define TRC_ADD(x)
-#endif
 
         // ---- prefetch stage: source points, transform, table probe, one bulk copy per distinct run ----------------------
         auto prefetch = [&](unsigned entry, int stg) {
@@ -381,9 +372,6 @@ __global__ void __launch_bounds__((W + 2) * 32, 1) p2plane_v9_kernel(P2PlaneLoop
             unsigned n_fb = 0;
             // every lane's run in the stage buffer with positions that fit the 6-bit key: the scan reads it with LDS
             const bool all_staged = __all_sync(0xffffffffu, cr.count == 0u || (cr.count <= 64u && cr.off != 0xffffffffu));
-#ifdef FLS_K1_TRACE
-            if (!all_staged) ++n_mixed;
-#endif
             if (i < n) {
                 bool use = false;
                 if (cr.count > 0u) {
@@ -409,9 +397,6 @@ __global__ void __launch_bounds__((W + 2) * 32, 1) p2plane_v9_kernel(P2PlaneLoop
                     }
                     if (exact) {  // positions that do not fit the key, or a tie the quantised keys cannot resolve: reference comparator
                         Top5 nn;
-#ifdef FLS_K1_TRACE
-                        atomicAdd(trc + 7, 1ull);
-#endif
                         knn5_exact_any(P, cr.count, r2, cr.qx, cr.qy, cr.qz, nn);
                         full = nn.full();
                         js[0] = nn.k0; js[1] = nn.k1; js[2] = nn.k2; js[3] = nn.k3; js[4] = nn.k4;
@@ -486,7 +471,6 @@ __global__ void __launch_bounds__((W + 2) * 32, 1) p2plane_v9_kernel(P2PlaneLoop
             if (!nxt_ready) {
                 bool avail = (int)(ld_acquire_smem(&ctl->ring_tail) - res) > 0;
                 if (!avail && !cur_pending) {  // nothing to compute meanwhile: wait for the server (or for the end)
-                    TRC_T0
                     unsigned ns = 32;
                     Watchdog wd;
                     for (;;) {
@@ -496,29 +480,19 @@ __global__ void __launch_bounds__((W + 2) * 32, 1) p2plane_v9_kernel(P2PlaneLoop
                         __nanosleep(ns);
                         if (ns < 256) ns <<= 1;
                     }
-                    TRC_ADD(t_spin)
                     if (!avail) break;  // quit: every scan is finished
                 }
                 if (avail) {
                     nxt = ctl->ring[res & (kRing - 1)];
                     nxt_stg = pstg;
                     pstg ^= 1;
-                    TRC_T0
                     prefetch(nxt, nxt_stg);
-                    TRC_ADD(t_pre)
                     nxt_ready = true;
                     have_res = false;
                 }
             }
             if (cur_pending) {
-                TRC_T0
                 compute(cur, cur_stg);
-#ifdef FLS_K1_TRACE
-                const unsigned long long dt = globaltimer_ns9() - trc_t0;
-                t_cmp += dt;
-                if (dt > t_max) t_max = dt;
-                ++n_chunk;
-#endif
                 cur_pending = false;
             }
             if (nxt_ready) {
@@ -528,12 +502,6 @@ __global__ void __launch_bounds__((W + 2) * 32, 1) p2plane_v9_kernel(P2PlaneLoop
                 nxt_ready = false;
             }
         }
-#ifdef FLS_K1_TRACE
-        if (lane == 0) {
-            atomicAdd(trc + 0, t_spin); atomicAdd(trc + 1, t_pre); atomicAdd(trc + 2, t_cmp);
-            atomicMax(trc + 4, t_max); atomicAdd(trc + 5, n_chunk); atomicAdd(trc + 6, n_mixed);
-        }
-#endif
     } else if (warp == W) {
         // =============================== server warp: the CTA's scheduler ===================================================
         // slot k serves scans k, k + 8, ... (one open item per slot).  Per slot: wait for the pose of (scan, it) -> open:
@@ -566,10 +534,6 @@ __global__ void __launch_bounds__((W + 2) * 32, 1) p2plane_v9_kernel(P2PlaneLoop
         }
         unsigned tail = 0;
         Watchdog wd;
-        // tuning knobs (P2PlaneLoopArgs::visit_group, unused by this generation otherwise): low byte = outstanding target with several
-        // scans open, in quarters of W (default 12 = 3 W); next byte = share divisor of the second-oldest scan (default 4)
-        const int tgt_q = (a.visit_group & 0xff) ? (a.visit_group & 0xff) : 12;
-        const int sec_div = ((a.visit_group >> 8) & 0xff) ? ((a.visit_group >> 8) & 0xff) : 4;
         while (live > 0) {
             bool progress = false;
             // ---- pose records: all waiting slots polled with independent loads ---------------------------------------------
@@ -615,7 +579,6 @@ __global__ void __launch_bounds__((W + 2) * 32, 1) p2plane_v9_kernel(P2PlaneLoop
                     exh[k] = false;
                     oseq[k] = n_opened++;
                     if (lane == 0) st_release_smem(&ctl->opened[k], (((unsigned)rit[k] << 8) | (unsigned)rs[k]) + 1u);
-                    if (cta == 0 && lane == 0 && rit[k] < 16) s_desc[rs[k]].state->dbg[rit[k]][0] = globaltimer_ns9();  // item opened on CTA 0
                 } else {
                     // the scan is finished: the slot moves on to its next live scan (pass order: iteration-major)
                     fin |= 1ull << rs[k];
@@ -651,7 +614,7 @@ __global__ void __launch_bounds__((W + 2) * 32, 1) p2plane_v9_kernel(P2PlaneLoop
                     n_open += (rph[k] == 1 && !exh[k]) ? 1 : 0;
                 }
                 // (with several scans in flight one more chunk per warp waits on the ring: the refill takes a server pass)
-                const int target = n_open > 1 ? (tgt_q * W) / 4 : 2 * W;
+                const int target = n_open > 1 ? (kRefillQuarters * W) / 4 : 2 * W;
                 if (n_open > 0 && (int)outstanding < target) {
                     const int want = target - (int)outstanding;
                     // Oldest item first: the scans of a batch start in phase, and drawing from all of them at the same rate keeps
@@ -670,7 +633,7 @@ __global__ void __launch_bounds__((W + 2) * 32, 1) p2plane_v9_kernel(P2PlaneLoop
                             }
                         }
                     }
-                    const int kb1 = want, kb2 = want / sec_div > 0 ? want / sec_div : 1;
+                    const int kb1 = want, kb2 = want / kSecondShareDiv > 0 ? want / kSecondShareDiv : 1;
                     int kb = 0;
                     unsigned base = 0;
                     int my_n = 0, my_s = 0;
@@ -712,10 +675,7 @@ __global__ void __launch_bounds__((W + 2) * 32, 1) p2plane_v9_kernel(P2PlaneLoop
                         const bool e = __shfl_sync(0xffffffffu, now_exh ? 1u : 0u, k) != 0u;
                         if (rph[k] == 1 && !exh[k] && (k == k1 || k == k2)) {
                             acq[k] += c;
-                            if (e) {
-                                exh[k] = true;
-                                if (cta == 0 && lane == 0 && rit[k] < 16) s_desc[rs[k]].state->dbg[rit[k]][1] = globaltimer_ns9();  // tickets exhausted (seen by CTA 0)
-                            }
+                            if (e) exh[k] = true;
                         }
                     }
                     __syncwarp();
@@ -750,10 +710,6 @@ __global__ void __launch_bounds__((W + 2) * 32, 1) p2plane_v9_kernel(P2PlaneLoop
                     dep[w * 32] = 0.0;
                 }
                 ll_store(sc->rows + (size_t)cta * 32 + lane, v, sc->tag_base | (unsigned)(rit[k] + 1));
-                if (cta == 0 && lane == 0 && rit[k] < 16) sc->state->dbg[rit[k]][2] = globaltimer_ns9();  // CTA 0's row went out
-#ifdef FLS_K1_TRACE
-                if (lane == 0 && rs[k] == 0 && rit[k] < 4) atomicMax(&sc->state->dbg[10 + rit[k]][0], globaltimer_ns9());  // last row out
-#endif
                 __syncwarp();
                 if (lane == 0) ctl->done[k] = 0;
                 // next item of the slot: its next live scan, wrapping into the next iteration
@@ -880,7 +836,6 @@ __global__ void __launch_bounds__((W + 2) * 32, 1) p2plane_v9_kernel(P2PlaneLoop
                     double acc = 0.0;
 #pragma unroll
                     for (int q = 0; q < 16; ++q) acc += v[q];
-                    if (lane == 0 && it < 16) state->dbg[it][3] = globaltimer_ns9();  // all rows in
                     s_tot[lane] = acc;
                     __threadfence();  // rows in -> pose out: keeps the chain of the per-point records causal across SMs
                     __syncwarp();
@@ -901,41 +856,17 @@ __global__ void __launch_bounds__((W + 2) * 32, 1) p2plane_v9_kernel(P2PlaneLoop
     }
 }
 
-template <int W, int CAP>
-struct V9Shape {
-    static const void* fn() { return (const void*)p2plane_v9_kernel<W, CAP>; }
-    static size_t smem() { return V9Smem<W, CAP>::bytes + sizeof(P2PlaneScan) * kMaxBatch; }
-    static void prepare() {
-        static bool done = false;
-        if (!done) {
-            FLS_CUDA(cudaFuncSetAttribute(fn(), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem()));
-            done = true;
-        }
-    }
-    static void launch(int grid, void** params, cudaStream_t st) {
-        prepare();
-        FLS_CUDA(cudaLaunchCooperativeKernel(fn(), dim3(grid), dim3((W + 2) * 32), params, smem(), st));
-    }
-};
+// 14 compute warps (+ server + folder: 512 threads) with a stage buffer of 352 candidates per warp and stage
+constexpr int kV9Warps = 14, kV9Cap = 352;
 
 }  // namespace
-
-int p2plane_v9_warps() {
-    static int w = 0;
-    if (!w) {
-        const char* e = std::getenv("FLS_K1_WARPS");
-        const int v = e ? std::atoi(e) : 0;
-        w = (v == 14 || v == 18) ? v : 14;  // W + 2 warps: 512 / 640 / 768 threads (register allocation is per 128)
-    }
-    return w;
-}
 
 // CTAs that serve a batch whose largest scan has n points: one per SM, fewer when there are not enough chunks to go round
 int p2plane_v9_grid(int n_max, int device) {
     static int sms[64] = {0};
     const int d = (device >= 0 && device < 64) ? device : 0;
     if (!sms[d]) cudaDeviceGetAttribute(&sms[d], cudaDevAttrMultiProcessorCount, device);
-    const int W = p2plane_v9_warps();
+    const int W = kV9Warps;
     const int need = ((n_max + 31) / 32 + W - 1) / W;
     int g = need < sms[d] ? need : sms[d];
     if (g > 192) g = 192;  // the second fold level holds 16 group rows of 12 CTAs
@@ -945,10 +876,14 @@ int p2plane_v9_grid(int n_max, int device) {
 void launch_p2plane_v9(const P2PlaneLoopArgs& a, int grid, cudaStream_t st) {
     P2PlaneLoopArgs args = a;
     void* params[] = {&args};
-    switch (p2plane_v9_warps()) {
-        case 18: V9Shape<18, 256>::launch(grid, params, st); break;
-        default: V9Shape<14, 352>::launch(grid, params, st); break;
+    const void* fn = (const void*)p2plane_v9_kernel<kV9Warps, kV9Cap>;
+    const size_t smem = V9Smem<kV9Warps, kV9Cap>::bytes + sizeof(P2PlaneScan) * kMaxBatch;
+    static bool prepared = false;
+    if (!prepared) {
+        FLS_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        prepared = true;
     }
+    FLS_CUDA(cudaLaunchCooperativeKernel(fn, dim3(grid), dim3((kV9Warps + 2) * 32), params, smem, st));
 }
 
 }  // namespace fls

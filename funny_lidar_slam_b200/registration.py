@@ -41,6 +41,31 @@ def _cloud(a):
     return a.ctypes.data_as(C.c_void_p), a.shape[0], a.shape[1] * 4, a
 
 
+def _batch_poses(Ts):
+    return np.ascontiguousarray(np.transpose(np.asarray(Ts, np.float64), (0, 2, 1))).copy()  # Eigen column-major per pose
+
+
+def _host_batch(scans, Ts):
+    """Host scans of a batch call: (keep-alive arrays, pointer array, count array, stride, column-major poses)."""
+    ptrs, ns, keep, stride = [], [], [], None
+    for c in scans:
+        p, n, s, a = _cloud(c)
+        if stride is not None and s != stride:
+            raise ValueError("all scans of one batch must share a layout")
+        stride = s
+        ptrs.append(p)
+        ns.append(n)
+        keep.append(a)
+    B = len(scans)
+    return keep, (C.c_void_p * B)(*ptrs), (C.c_size_t * B)(*ns), stride, _batch_poses(Ts)
+
+
+def _device_batch(d_ptrs, ns, Ts):
+    """Device-resident scans of a batch call: (pointer array, count array, column-major poses)."""
+    B = len(d_ptrs)
+    return (C.c_void_p * B)(*[int(p) for p in d_ptrs]), (C.c_size_t * B)(*[int(n) for n in ns]), _batch_poses(Ts)
+
+
 class Registration:
     def __init__(self, cfg: FlsConfig):
         self.cfg = cfg
@@ -92,54 +117,33 @@ class Registration:
         return float(out.value)
 
     # -- batched Match (throughput entry; LoamPointToPlaneIVOX in localization mode) -----------------------------
+    def _batch_results(self, conv, st, Tc):
+        self.last_batch_stats = list(st)
+        self.last_stats = st[0]
+        return np.array(conv[:], bool), np.transpose(Tc, (0, 2, 1)).copy()
+
     def match_batch(self, scans, Ts):
         """scans: list of (n,4)/(n,8) host clouds; Ts: (B,4,4) float64 initial poses.  Returns (converged[B], T[B,4,4]);
         self.last_batch_stats holds the per-scan fls_match_stats (call-level timings on element 0)."""
         B = len(scans)
-        ptrs, ns, keep, stride = [], [], [], None
-        for c in scans:
-            p, n, s, a = _cloud(c)
-            if stride is not None and s != stride:
-                raise ValueError("all scans of one batch must share a layout")
-            stride = s
-            ptrs.append(p)
-            ns.append(n)
-            keep.append(a)
-        Tc = np.ascontiguousarray(np.transpose(np.asarray(Ts, np.float64), (0, 2, 1))).copy()  # Eigen column-major per pose
+        keep, arr_p, arr_n, stride, Tc = _host_batch(scans, Ts)
         conv = (C.c_int * B)()
         st = (FlsMatchStats * B)()
-        arr_p = (C.c_void_p * B)(*ptrs)
-        arr_n = (C.c_size_t * B)(*ns)
         check(lib().fls_match_batch(self._h, B, arr_p, arr_n, stride, Tc.ctypes.data_as(C.c_void_p), conv, st), "fls_match_batch")
-        self.last_batch_stats = list(st)
-        self.last_stats = st[0]
-        return np.array(conv[:], bool), np.transpose(Tc, (0, 2, 1)).copy()
+        return self._batch_results(conv, st, Tc)
 
     def match_batch_begin(self, scans, Ts) -> None:
         """First half of match_batch: enqueue copies + matching + read-back on the handle's stream, do not wait (the scans should sit
         in pinned host memory).  With two handles the copy of one batch overlaps the kernels of the other."""
         B = len(scans)
-        ptrs, ns, keep, stride = [], [], [], None
-        for c in scans:
-            p, n, s, a = _cloud(c)
-            if stride is not None and s != stride:
-                raise ValueError("all scans of one batch must share a layout")
-            stride = s
-            ptrs.append(p)
-            ns.append(n)
-            keep.append(a)
-        Tc = np.ascontiguousarray(np.transpose(np.asarray(Ts, np.float64), (0, 2, 1))).copy()
-        arr_p = (C.c_void_p * B)(*ptrs)
-        arr_n = (C.c_size_t * B)(*ns)
+        keep, arr_p, arr_n, stride, Tc = _host_batch(scans, Ts)
         self._pending = (keep, arr_p, arr_n, Tc, B)
         check(lib().fls_match_batch_begin(self._h, B, arr_p, arr_n, stride, Tc.ctypes.data_as(C.c_void_p)), "fls_match_batch_begin")
 
     def match_batch_begin_device(self, d_ptrs, ns, Ts) -> None:
         """match_batch_begin with device-resident packed float4 scans."""
         B = len(d_ptrs)
-        Tc = np.ascontiguousarray(np.transpose(np.asarray(Ts, np.float64), (0, 2, 1))).copy()
-        arr_p = (C.c_void_p * B)(*[int(p) for p in d_ptrs])
-        arr_n = (C.c_size_t * B)(*[int(n) for n in ns])
+        arr_p, arr_n, Tc = _device_batch(d_ptrs, ns, Ts)
         self._pending = ((), arr_p, arr_n, Tc, B)
         check(lib().fls_match_batch_begin_device(self._h, B, arr_p, arr_n, Tc.ctypes.data_as(C.c_void_p)), "fls_match_batch_begin_device")
 
@@ -149,22 +153,16 @@ class Registration:
         st = (FlsMatchStats * B)()
         check(lib().fls_match_batch_end(self._h, Tc.ctypes.data_as(C.c_void_p), conv, st), "fls_match_batch_end")
         self._pending = None
-        self.last_batch_stats = list(st)
-        self.last_stats = st[0]
-        return np.array(conv[:], bool), np.transpose(Tc, (0, 2, 1)).copy()
+        return self._batch_results(conv, st, Tc)
 
     def match_batch_device(self, d_ptrs, ns, Ts):
         """Same with device-resident packed float4 scans: d_ptrs = list of device addresses, ns = point counts."""
         B = len(d_ptrs)
-        Tc = np.ascontiguousarray(np.transpose(np.asarray(Ts, np.float64), (0, 2, 1))).copy()
+        arr_p, arr_n, Tc = _device_batch(d_ptrs, ns, Ts)
         conv = (C.c_int * B)()
         st = (FlsMatchStats * B)()
-        arr_p = (C.c_void_p * B)(*[int(p) for p in d_ptrs])
-        arr_n = (C.c_size_t * B)(*[int(n) for n in ns])
         check(lib().fls_match_batch_device(self._h, B, arr_p, arr_n, Tc.ctypes.data_as(C.c_void_p), conv, st), "fls_match_batch_device")
-        self.last_batch_stats = list(st)
-        self.last_stats = st[0]
-        return np.array(conv[:], bool), np.transpose(Tc, (0, 2, 1)).copy()
+        return self._batch_results(conv, st, Tc)
 
     def set_result_buffer_device(self, d_ptr: int, capacity_scans: int) -> None:
         """Every later Match also writes {column-major pose, converged, iterations} (18 doubles per scan) to this device

@@ -117,7 +117,7 @@ typedef struct {
 } fls_config;
 
 #define FLS_FLAG_ITER_LOG 1u /* keep per-iteration H, g, dx, n_valid, sum_res for fls_get_iter_log */
-#define FLS_FLAG_PROFILE 2u  /* bracket every residual-kernel launch with CUDA events (fills kernel_ms / kernel_launches) */
+#define FLS_FLAG_PROFILE 2u  /* bracket the fused Gauss-Newton launch of a Match with CUDA events (fills kernel_ms / kernel_launches) */
 
 typedef struct {
     int32_t iterations;   /* GN iterations executed */
@@ -129,8 +129,8 @@ typedef struct {
     int32_t gpu_launches; /* kernels of this library launched by the call */
     int64_t h2d_bytes;    /* bytes copied host->device by the call */
     int64_t d2h_bytes;    /* bytes copied device->host by the call */
-    float kernel_ms;      /* FLS_FLAG_PROFILE: summed device time of the residual kernel over the executed iterations */
-    int32_t kernel_launches; /* FLS_FLAG_PROFILE: how many launches kernel_ms covers (= iterations) */
+    float kernel_ms;      /* FLS_FLAG_PROFILE: device time of the fused Gauss-Newton launch (all executed iterations) */
+    int32_t kernel_launches; /* FLS_FLAG_PROFILE: how many launches kernel_ms covers (1: one launch runs every iteration) */
     int64_t algo_bytes;   /* FLS_FLAG_PROFILE: algorithmic bytes those launches moved (DESIGN.md "roofline accounting") */
 } fls_match_stats;  /* valid only when the call returned FLS_OK */
 
