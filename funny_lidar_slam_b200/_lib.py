@@ -13,7 +13,7 @@ _lib = None
 
 EXPORTS = [
     "fls_abi_version", "fls_device_count", "fls_last_error", "fls_strerror", "fls_config_default", "fls_create", "fls_destroy",
-    "fls_add_cloud", "fls_match", "fls_match_device", "fls_fitness", "fls_get_iter_log", "fls_get_map_info", "fls_ivox_knn",
+    "fls_add_cloud", "fls_match", "fls_match_device", "fls_fitness", "fls_get_iter_log", "fls_get_iter_log_scan", "fls_get_map_info", "fls_ivox_knn",
     "fls_voxel_grid", "fls_extract_features", "fls_project", "fls_match_batch", "fls_match_batch_device",
     "fls_set_result_buffer_device", "fls_get_voxel_keys", "fls_get_map_points", "fls_ivox_add_points", "fls_preprocess", "fls_project_imu", "fls_match_batch_begin", "fls_match_batch_begin_device", "fls_match_batch_end", "fls_set_global_map", "fls_update_local_map",
     "fls_pcd_read", "fls_pcd_write",
@@ -62,6 +62,7 @@ def lib():
     L.fls_match_batch_end.argtypes = [vp, vp, C.POINTER(C.c_int), C.POINTER(FlsMatchStats)]
     L.fls_fitness.argtypes = [vp, f32, C.POINTER(f32)]
     L.fls_get_iter_log.argtypes = [vp, C.POINTER(FlsIterLog), C.c_int]
+    L.fls_get_iter_log_scan.argtypes = [vp, C.c_int, C.POINTER(FlsIterLog), C.c_int]
     L.fls_get_map_info.argtypes = [vp, C.POINTER(FlsMapInfo)]
     L.fls_get_voxel_keys.argtypes = [vp, vp, sz, C.POINTER(sz)]
     L.fls_get_map_points.argtypes = [vp, vp, sz, C.POINTER(sz)]

@@ -83,7 +83,7 @@ void Handle::init() {
     if (cfg.flags & FLS_FLAG_ITER_LOG) {
         log_cap = cfg.max_iterations > 0 ? cfg.max_iterations : 1;
         log.reserve((size_t)log_cap * kMaxBatch);
-        h_log.resize(log_cap);
+        h_log.resize((size_t)log_cap * kMaxBatch);
     }
 }
 
@@ -206,11 +206,15 @@ void Handle::send_batch_table(size_t bytes) {
 }
 
 void Handle::read_back(int B) {
+    // h_log is about to hold this call's logs: until unpack records their sizes, no scan has one (a Match that fails after
+    // its launch, e.g. through the v9 watchdog, leaves no log rather than a mix of two calls)
+    log_n.assign(1, 0);
     FLS_CUDA(cudaMemcpyAsync(h_state, state.p, sizeof(GnState) * (size_t)B, cudaMemcpyDeviceToHost, stream));
     d2h_bytes += (long long)(sizeof(GnState) * (size_t)B);
     if (log_cap) {
-        FLS_CUDA(cudaMemcpyAsync(h_log.data(), log.p, sizeof(fls_iter_log) * log_cap, cudaMemcpyDeviceToHost, stream));
-        d2h_bytes += (long long)(sizeof(fls_iter_log) * log_cap);
+        const size_t bytes = sizeof(fls_iter_log) * (size_t)log_cap * (size_t)B;
+        FLS_CUDA(cudaMemcpyAsync(h_log.data(), log.p, bytes, cudaMemcpyDeviceToHost, stream));
+        d2h_bytes += (long long)bytes;
     }
 }
 
@@ -244,7 +248,8 @@ void Handle::unpack(int B, const size_t* n, double* T, int* converged, fls_match
         }
     }
     std::memcpy(T_final, T, sizeof(T_final));
-    log_n = h_state[0].iter < log_cap ? h_state[0].iter : log_cap;
+    log_n.resize(B);
+    for (int s = 0; s < B; ++s) log_n[s] = h_state[s].iter < log_cap ? h_state[s].iter : log_cap;
 }
 
 // control block of a single-scan persistent GN loop (K2 / K3 / K5): CTA rows + pose record + stop rule
@@ -379,7 +384,7 @@ int Handle::enqueue_ivox_batch(int B, const float4* const* d_scans, const size_t
             launch_p2plane_loop(a, grid, stream);
         }
     });
-    // ---- read back: every scan's state (+ iteration log of scan 0) -----------------------------------------------------
+    // ---- read back: every scan's state (+ its iteration log) ----------------------------------------------------------
     read_back(B);
     *h_abort = 0;
     if (use_v9) FLS_CUDA(cudaMemcpyAsync(h_abort, a.abort_word, sizeof(unsigned), cudaMemcpyDeviceToHost, stream));
@@ -1151,13 +1156,16 @@ int fls_set_result_buffer_device(fls_handle* hh, double* d_results, size_t capac
     return FLS_OK;
 }
 
-int fls_get_iter_log(const fls_handle* hh, fls_iter_log* out, int capacity) {
+int fls_get_iter_log_scan(const fls_handle* hh, int scan, fls_iter_log* out, int capacity) {
     const Handle* h = reinterpret_cast<const Handle*>(hh);
-    if (!h || !out || capacity < 0) return FLS_ERR_INVALID_ARG;
-    const int n = h->log_n < capacity ? h->log_n : capacity;
-    for (int i = 0; i < n; ++i) out[i] = h->h_log[i];
+    if (!h || !out || capacity < 0 || scan < 0 || (size_t)scan >= h->log_n.size()) return FLS_ERR_INVALID_ARG;
+    const int n = h->log_n[scan] < capacity ? h->log_n[scan] : capacity;
+    const fls_iter_log* src = h->h_log.data() + (size_t)scan * h->log_cap;
+    for (int i = 0; i < n; ++i) out[i] = src[i];
     return n;
 }
+
+int fls_get_iter_log(const fls_handle* hh, fls_iter_log* out, int capacity) { return fls_get_iter_log_scan(hh, 0, out, capacity); }
 
 int fls_set_global_map(fls_handle* hh, const void* pts, size_t n, size_t stride) {
     Handle* h = reinterpret_cast<Handle*>(hh);

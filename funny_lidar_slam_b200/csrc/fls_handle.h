@@ -37,8 +37,9 @@ struct Handle {
     DevBuf<GnState> state;
     GnState* h_state = nullptr;  // pinned
     DevBuf<fls_iter_log> log;
-    std::vector<fls_iter_log> h_log;
-    int log_cap = 0, log_n = 0;
+    std::vector<fls_iter_log> h_log;  // FLS_FLAG_ITER_LOG: log_cap entries per scan of the last Match
+    int log_cap = 0;
+    std::vector<int> log_n = {0};     // entries of each scan's log (one element per scan of the last Match)
     double T_final[16] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1};
     cudaEvent_t prof_ev[2] = {nullptr, nullptr};  // FLS_FLAG_PROFILE: around the fused Gauss-Newton launch of a Match
     bool profile = false;
@@ -125,8 +126,8 @@ struct Handle {
         last_src = src;
         last_src_n = src_n;
     }
-    void read_back(int n_scans);  // enqueues the copy of the states and of scan 0's iteration log
-    // after end_call: T / converged / stats of every scan (call-level figures on stats[0]), T_final and log_n from scan 0
+    void read_back(int n_scans);  // enqueues the copy of the states and of every scan's iteration log
+    // after end_call: T / converged / stats and log_n of every scan (call-level figures on stats[0]), T_final from scan 0
     void unpack(int n_scans, const size_t* n_source, double* T, int* converged, fls_match_stats* st);
 
     int add_cloud_ivox(const void* pts, size_t n, size_t stride);

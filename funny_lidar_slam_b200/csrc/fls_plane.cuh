@@ -50,100 +50,112 @@ struct Top5 {
 };
 
 // ---- 5x3 least squares ---------------------------------------------------------------------------------------------
-// Householder reflection of column K (rows K..4) in the unnormalised form H = I - 2 v v^T / (v^T v), v = x - beta e_K:
-// the same reflector Eigen builds (loam_point_to_plane_ivox.h:283 -> colPivHouseholderQr), one sqrt + one division.
-template <int K>
-__device__ __forceinline__ void hh_step(double (&A)[5][3], double (&b)[5]) {
-    const double alpha = A[K][K];
-    double tail = 0;
-#pragma unroll
-    for (int i = K + 1; i < 5; ++i) tail += A[i][K] * A[i][K];
-    if (tail == 0.0) return;  // already upper-triangular in this column
-    double beta = sqrt(alpha * alpha + tail);
-    if (alpha >= 0) beta = -beta;
-    double v[5];
-    v[K] = alpha - beta;
-#pragma unroll
-    for (int i = K + 1; i < 5; ++i) v[i] = A[i][K];
-    const double f = 2.0 / (v[K] * v[K] + tail);
-    A[K][K] = beta;
-#pragma unroll
-    for (int j = K + 1; j < 3; ++j) {
-        double s = 0;
-#pragma unroll
-        for (int i = K; i < 5; ++i) s += v[i] * A[i][j];
-        s *= f;
-#pragma unroll
-        for (int i = K; i < 5; ++i) A[i][j] -= s * v[i];
-    }
-    double s = 0;
-#pragma unroll
-    for (int i = K; i < 5; ++i) s += v[i] * b[i];
-    s *= f;
-#pragma unroll
-    for (int i = K; i < 5; ++i) b[i] -= s * v[i];
-}
-
-template <int K, int J>
-__device__ __forceinline__ double colnorm2(const double (&A)[5][3]) {
-    double s = 0;
-#pragma unroll
-    for (int i = K; i < 5; ++i) s += A[i][J] * A[i][J];
-    return s;
-}
-template <int CA, int CB>
-__device__ __forceinline__ void swap_cols(double (&A)[5][3]) {
-#pragma unroll
-    for (int i = 0; i < 5; ++i) {
-        const double t = A[i][CA];
-        A[i][CA] = A[i][CB];
-        A[i][CB] = t;
-    }
-}
+// Column-pivoted Householder QR, operation for operation the one of the oracle (orc_math.h lstsq_colpiv_qr): the Eigen
+// reflector form (v = [1, x_tail / (alpha - beta)], tau = (beta - alpha) / beta), pivot norms recomputed per step, the rank
+// cut (eps sqrt(max column norm^2) / 5)^2.  Every product, sum, quotient and root is rounded on its own (no FMA contraction),
+// as the oracle's -ffp-contract=off build does.  A neighbourhood whose remaining column is rounding noise (repeated points, a
+// pole, an off-axis line) is decided by that noise against the cut; with the same arithmetic on both sides the GPU and the
+// oracle take the same rank decision bit for bit (DESIGN.md §5).
+__device__ __forceinline__ double rn_add(double a, double b) { return __dadd_rn(a, b); }
+__device__ __forceinline__ double rn_sub(double a, double b) { return __dadd_rn(a, -b); }
+__device__ __forceinline__ double rn_mul(double a, double b) { return __dmul_rn(a, b); }
+__device__ __forceinline__ double rn_div(double a, double b) { return __ddiv_rn(a, b); }
 
 // min || A c + 1 ||  — Eigen colPivHouseholderQr().solve(b) with b = -1 (loam_point_to_plane_ivox.h:275-283 upstream).
 // A is destroyed.
 __device__ __forceinline__ void plane_lstsq(double (&A)[5][3], double (&c)[3]) {
     double b[5] = {-1.0, -1.0, -1.0, -1.0, -1.0};
-    int p0 = 0, p1 = 1, p2 = 2;
+    int perm[3] = {0, 1, 2};
+    double maxcn = 0.0;
+#pragma unroll
+    for (int j = 0; j < 3; ++j) {
+        double s = 0.0;
+#pragma unroll
+        for (int i = 0; i < 5; ++i) s = rn_add(s, rn_mul(A[i][j], A[i][j]));
+        maxcn = fmax(maxcn, s);
+    }
+    const double h = rn_div(rn_mul(2.220446049250313e-16, __dsqrt_rn(maxcn)), 5.0);
+    const double thr = rn_mul(h, h);
     int rank = 3;
-    double n0 = colnorm2<0, 0>(A), n1 = colnorm2<0, 1>(A), n2 = colnorm2<0, 2>(A);
-    const double maxcn = fmax(n0, fmax(n1, n2));
-    const double thr = maxcn * (2.220446049250313e-16 / 5.0) * (2.220446049250313e-16 / 5.0);
-    {  // k = 0
-        int piv = 0;
-        double best = n0;
-        if (n1 > best) { best = n1; piv = 1; }
-        if (n2 > best) { best = n2; piv = 2; }
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+        int piv = k;
+        double best = -1.0;
+#pragma unroll
+        for (int j = k; j < 3; ++j) {
+            double s = 0.0;
+#pragma unroll
+            for (int i = k; i < 5; ++i) s = rn_add(s, rn_mul(A[i][j], A[i][j]));
+            if (s > best) {
+                best = s;
+                piv = j;
+            }
+        }
         if (best < thr || best == 0.0) {
-            rank = 0;
-        } else {
-            if (piv == 1) { swap_cols<0, 1>(A); int t = p0; p0 = p1; p1 = t; }
-            if (piv == 2) { swap_cols<0, 2>(A); int t = p0; p0 = p2; p2 = t; }
-            hh_step<0>(A, b);
+            rank = k;
+            break;
+        }
+        if (piv != k) {
+#pragma unroll
+            for (int i = 0; i < 5; ++i) {
+                const double t = A[i][k];
+                A[i][k] = A[i][piv];
+                A[i][piv] = t;
+            }
+            const int t = perm[k];
+            perm[k] = perm[piv];
+            perm[piv] = t;
+        }
+        const double alpha = A[k][k];
+        double tail = 0.0;
+#pragma unroll
+        for (int i = k + 1; i < 5; ++i) tail = rn_add(tail, rn_mul(A[i][k], A[i][k]));
+        double beta = alpha, tau = 0.0, v[5] = {0.0, 0.0, 0.0, 0.0, 0.0};
+        if (tail != 0.0) {
+            beta = __dsqrt_rn(rn_add(rn_mul(alpha, alpha), tail));
+            if (alpha >= 0) beta = -beta;
+            const double den = rn_sub(alpha, beta);
+#pragma unroll
+            for (int i = k + 1; i < 5; ++i) v[i] = rn_div(A[i][k], den);
+            tau = rn_div(rn_sub(beta, alpha), beta);
+        }
+        v[k] = 1.0;
+        A[k][k] = beta;
+#pragma unroll
+        for (int i = k + 1; i < 5; ++i) A[i][k] = 0.0;
+        if (tau != 0.0) {
+#pragma unroll
+            for (int j = k + 1; j < 3; ++j) {
+                double s = 0.0;
+#pragma unroll
+                for (int i = k; i < 5; ++i) s = rn_add(s, rn_mul(v[i], A[i][j]));
+                s = rn_mul(s, tau);
+#pragma unroll
+                for (int i = k; i < 5; ++i) A[i][j] = rn_sub(A[i][j], rn_mul(s, v[i]));
+            }
+            double s = 0.0;
+#pragma unroll
+            for (int i = k; i < 5; ++i) s = rn_add(s, rn_mul(v[i], b[i]));
+            s = rn_mul(s, tau);
+#pragma unroll
+            for (int i = k; i < 5; ++i) b[i] = rn_sub(b[i], rn_mul(s, v[i]));
         }
     }
-    if (rank == 3) {  // k = 1
-        n1 = colnorm2<1, 1>(A);
-        n2 = colnorm2<1, 2>(A);
-        if (fmax(n1, n2) < thr || fmax(n1, n2) == 0.0) {
-            rank = 1;
-        } else {
-            if (n2 > n1) { swap_cols<1, 2>(A); int t = p1; p1 = p2; p2 = t; }
-            hh_step<1>(A, b);
+    double y[3] = {0.0, 0.0, 0.0};
+#pragma unroll
+    for (int i = 2; i >= 0; --i) {
+        if (i < rank) {
+            double s = b[i];
+#pragma unroll
+            for (int j = i + 1; j < 3; ++j)
+                if (j < rank) s = rn_sub(s, rn_mul(A[i][j], y[j]));
+            y[i] = rn_div(s, A[i][i]);
         }
     }
-    if (rank == 3) {  // k = 2
-        n2 = colnorm2<2, 2>(A);
-        if (n2 < thr || n2 == 0.0) rank = 2;
-        else hh_step<2>(A, b);
-    }
-    const double y2 = (rank > 2) ? b[2] / A[2][2] : 0.0;
-    const double y1 = (rank > 1) ? (b[1] - A[1][2] * y2) / A[1][1] : 0.0;
-    const double y0 = (rank > 0) ? (b[0] - A[0][1] * y1 - A[0][2] * y2) / A[0][0] : 0.0;
-    c[0] = (p0 == 0) ? y0 : ((p1 == 0) ? y1 : y2);
-    c[1] = (p0 == 1) ? y0 : ((p1 == 1) ? y1 : y2);
-    c[2] = (p0 == 2) ? y0 : ((p1 == 2) ? y1 : y2);
+    c[0] = c[1] = c[2] = 0.0;
+#pragma unroll
+    for (int i = 0; i < 3; ++i)
+        if (i < rank) c[perm[i]] = y[i];
 }
 
 // neighbour fetch: read-only global path (kLdg) or a generic load (the point may sit in shared memory: K1 stages the

@@ -208,12 +208,13 @@ class Registration:
         check(lib().fls_get_voxel_keys(self._h, out.ctypes.data_as(C.c_void_p), cap, C.byref(n)), "fls_get_voxel_keys")
         return out[:min(cap, n.value)]
 
-    def iter_log(self):
+    def iter_log(self, scan: int = 0):
+        """Per-iteration H, g, dx, sum_residual, n_valid of scan `scan` of the last Match (needs FLS_FLAG_ITER_LOG)."""
         cap = max(1, self.cfg.max_iterations)
         buf = (FlsIterLog * cap)()
-        n = lib().fls_get_iter_log(self._h, buf, cap)
+        n = lib().fls_get_iter_log_scan(self._h, int(scan), buf, cap)
         if n < 0:
-            check(n, "fls_get_iter_log")
+            check(n, "fls_get_iter_log_scan")
         return [dict(H=np.array(b.H).reshape(6, 6), g=np.array(b.g), dx=np.array(b.dx), sum_residual=b.sum_residual, n_valid=b.n_valid)
                 for b in buf[:n]]
 

@@ -206,6 +206,9 @@ int fls_set_result_buffer_device(fls_handle* h, double* d_results, size_t capaci
 
 /* per-iteration log of the last fls_match (needs FLS_FLAG_ITER_LOG; batch: scan 0); returns the number of entries written */
 int fls_get_iter_log(const fls_handle* h, fls_iter_log* out, int capacity);
+/* the same for scan `scan` of the last Match call (the batch entries of FLS_P2PLANE_IVOX and FLS_NDT keep one log per scan);
+ * FLS_ERR_INVALID_ARG when `scan` is not below that call's n_scans; a Match that fails after its launch leaves no log */
+int fls_get_iter_log_scan(const fls_handle* h, int scan, fls_iter_log* out, int capacity);
 
 int fls_get_map_info(const fls_handle* h, fls_map_info* out);
 /* Keys (x, y, z voxel coordinates, int32 triples) of the voxels the map currently holds, in no particular order: FLS_NDT

@@ -147,7 +147,7 @@ void* orc_reg_create(const fls_config* c) {
         case FLS_P2PLANE_IVOX:
             r->p2p.reset(new LoamP2PlaneIvox(c->point_to_planar_thres, c->position_converge_thres, c->rotation_converge_thres,
                                              unsigned(c->max_iterations), c->localization_mode != 0, c->ivox_resolution, c->ivox_nearby,
-                                             size_t(c->ivox_capacity)));
+                                             size_t(c->ivox_capacity), c->ivox_max_range));
             break;
         case FLS_NDT:
             r->ndt.reset(new IncrementalNdt(c->ndt_voxel_size, c->ndt_outlier_thres, c->source_cloud_filter_size, c->rotation_converge_thres,

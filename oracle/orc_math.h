@@ -113,7 +113,9 @@ inline float fast_atan2f(float y, float x) {
 // ---- least squares: Householder QR with column pivoting -----------------------------------------
 // Restates Eigen::ColPivHouseholderQR<Matrix<double,M,N>>::solve as used at
 // loam_point_to_plane_ivox.h:283 (5x3 plane fit).  Solution of a full-rank LS problem is unique; on
-// exactly-zero remaining columns the corresponding unknowns are set to 0 (Eigen's nonzeroPivots rule).
+// exactly-zero remaining columns the corresponding unknowns are set to 0 (Eigen's nonzeroPivots rule).  The GPU's QR
+// (fls_plane.cuh plane_lstsq) performs the same operations in the same order, so rank decisions on rounding-level columns
+// agree bit for bit (DESIGN.md §5): change both or neither.
 template <int M, int N>
 inline void lstsq_colpiv_qr(const double* A_in /*MxN row-major*/, const double* b_in, double* x) {
     double A[M * N], b[M];

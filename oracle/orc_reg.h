@@ -71,9 +71,9 @@ inline float fitness_score(const ExactKnn& tree, const Cloud& src, const double*
 class LoamP2PlaneIvox {
 public:
     LoamP2PlaneIvox(double plane_thres, double pos_thres, double rot_thres, unsigned iters, bool localization,
-                    float ivox_res = 0.5f, int nearby = NEARBY18, size_t capacity = 1000000)
+                    float ivox_res = 0.5f, int nearby = NEARBY18, size_t capacity = 1000000, float max_range = 5.0f)
         : plane_thres_(plane_thres), pos_thres_(pos_thres), rot_thres_(rot_thres), iters_(iters), loc_(localization),
-          ivox_res_(ivox_res), nearby_(nearby), capacity_(capacity) {
+          ivox_res_(ivox_res), nearby_(nearby), capacity_(capacity), max_range_(max_range) {
         init_ivox();
     }
 
@@ -192,7 +192,7 @@ private:
             const P4& sp = src[i];
             const P4 q = transform_point_d(sp, T_);  // :265-266
             P4 nn[5];
-            const int found = ivox_->closest(q, 5, 5.0f, nn);  // :269
+            const int found = ivox_->closest(q, 5, max_range_, nn);  // :269 (the map's max_range_, ivox_map.h:58)
             // DELIBERATE DEVIATION (DESIGN.md §8): upstream's IVoxMap::GetClosestPoint returns false WITHOUT clearing `closest_pt`
             // when the stencil holds no candidate at all (ivox_map.cpp:21-23), so nearest_points_[i] keeps what index i found in an
             // earlier iteration — or in an earlier Match, where index i was a different point — and a plane is fitted to those
@@ -236,6 +236,7 @@ private:
     float ivox_res_;
     int nearby_;
     size_t capacity_;
+    float max_range_;
     double filter_size_ = 0.5;  // filter_size_map_min_ (:351)
     bool is_first_ = true;      // upstream: function-local static (:62)  [quirk 7]
     std::unique_ptr<IVox> ivox_;

@@ -27,7 +27,7 @@ def test_config4_batch8_64line_vs_oracle(world, surface_map):
     scans = [synth.make_scan(world, traj[3 + 5 * i], "hdl64", seed=100 + i)["points"] for i in range(8)]
     guesses = [synth.perturb_pose(traj[3 + 5 * i], seed=77 + i) for i in range(8)]  # 0.3 m / 3 deg, as the bench
     assert min(len(s) for s in scans) > 90000
-    cfg = default_config(FLS_P2PLANE_IVOX)
+    cfg = default_config(FLS_P2PLANE_IVOX, flags=FLS_FLAG_ITER_LOG)
     g, o = Registration(cfg), orc.Registration(cfg)
     g.AddCloudToLocalMap([surface_map])
     o.add_cloud(surface_map)
@@ -36,6 +36,12 @@ def test_config4_batch8_64line_vs_oracle(world, surface_map):
     for s in range(8):
         ok_o, To, st_o = o.match(scans[s], guesses[s])
         st_g = g.last_batch_stats[s]
+        # iteration 0 runs at the same pose on both sides: the normal equations of every scan agree to fp64 rounding
+        lg, lo = g.iter_log(s), o.iter_log()
+        assert len(lg) == st_g.iterations and lg[0]["n_valid"] == lo[0]["n_valid"], s
+        H0 = lo[0]["H"]
+        assert np.allclose(lg[0]["H"], H0, rtol=1e-9, atol=1e-9 * np.abs(H0).max()), s
+        assert np.allclose(lg[0]["g"], lo[0]["g"], rtol=1e-9, atol=1e-9 * np.abs(H0).max()), s
         assert bool(conv[s]) == ok_o, s
         assert st_g.iterations == st_o.iterations, (s, st_g.iterations, st_o.iterations)
         assert abs(st_g.n_valid - st_o.n_valid) <= max(2, st_o.n_valid // 2000), (s, st_g.n_valid, st_o.n_valid)

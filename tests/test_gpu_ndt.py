@@ -90,7 +90,7 @@ def test_streaming_mapping_mode(world, traj):
 def test_batch_equals_single_and_oracle(world, traj, scene64):
     """fls_match_batch for IncrementalNDT: one cooperative launch, a sub-grid and a Gauss-Newton loop per scan.  Every scan's
     result must equal its own single Match (same arithmetic, different CTA count -> fp64 rounding only) and the oracle."""
-    cfg = default_config(FLS_NDT)
+    cfg = default_config(FLS_NDT, flags=FLS_FLAG_ITER_LOG)
     g, o = _pair(cfg)
     g.AddCloudToLocalMap([scene64["map"]])
     o.add_cloud(scene64["map"])
@@ -101,10 +101,23 @@ def test_batch_equals_single_and_oracle(world, traj, scene64):
         guesses.append(synth.perturb_pose(traj[2 + k], seed=700 + k, dpos=0.05, drot_deg=0.5))
     oks, Ts = g.match_batch(scans, np.stack(guesses))
     sts = g.last_batch_stats
+    logs = [g.iter_log(k) for k in range(5)]
     for k in range(5):
         T1 = guesses[k].copy()
         ok1 = g.Match(_cluster(scans[k]), T1)
         ok_o, To, st_o = o.match(scans[k], guesses[k])
+        # iteration 0 of every scan of the batch against the oracle: same pose, same (point, voxel) pairs, the same terms
+        # summed in another order.  Two fp64 sums of n terms differ by at most 2 n eps sum|term| (recursive summation); each
+        # term is a few dozen flops (allow 64 n eps in all).  With every information matrix L positive semi-definite,
+        # Cauchy-Schwarz bounds sum|J_a^T L J_b| by sqrt(H_aa H_bb) and sum|J_a^T L e| by sqrt(H_aa sum e^T L e), and
+        # sum e^T L e is the logged sum_residual.
+        lo = o.iter_log()
+        assert len(logs[k]) == sts[k].iterations and logs[k][0]["n_valid"] == lo[0]["n_valid"], k
+        H0, n = lo[0]["H"], lo[0]["n_valid"]
+        dH = np.sqrt(np.abs(np.diag(H0)))
+        tol = 64 * n * np.finfo(np.float64).eps
+        assert np.all(np.abs(logs[k][0]["H"] - H0) <= tol * np.outer(dH, dH)), k
+        assert np.all(np.abs(logs[k][0]["g"] - lo[0]["g"]) <= tol * dH * np.sqrt(lo[0]["sum_residual"])), k
         assert bool(oks[k]) == ok1 == ok_o, k
         assert sts[k].iterations == g.last_stats.iterations == st_o.iterations, k
         assert sts[k].n_valid == g.last_stats.n_valid == st_o.n_valid, k

@@ -18,6 +18,17 @@ def _pair(cfg):
     return Registration(cfg), orc.Registration(cfg)
 
 
+def _assert_logs_equal(lb, l1, what):
+    """A scan's iteration log from a batch equals the log of its single Match: same neighbours and planes, only the fp64
+    summation order differs (1e-9 relative per iteration)."""
+    assert len(lb) == len(l1), what
+    for k, (a, b) in enumerate(zip(lb, l1)):
+        assert a["n_valid"] == b["n_valid"], (what, k)
+        sc = max(np.abs(b["H"]).max(), 1e-300)
+        assert np.allclose(a["H"], b["H"], rtol=1e-9, atol=1e-9 * sc), (what, k)
+        assert np.allclose(a["g"], b["g"], rtol=1e-9, atol=1e-9 * sc), (what, k)
+
+
 def test_ivox_knn_matches_oracle(scene16):
     from funny_lidar_slam_b200.registration import Registration
     from oracle import pyoracle as orc
@@ -167,7 +178,7 @@ def test_batch_equals_separate_matches(world, traj):
     from funny_lidar_slam_b200.registration import PointcloudCluster, Registration
     from oracle import pyoracle as orc
     mp = synth.make_map_from_scans(world, traj[0:12:2], "vlp16", leaf=0.3)
-    cfg = default_config(FLS_P2PLANE_IVOX)
+    cfg = default_config(FLS_P2PLANE_IVOX, flags=FLS_FLAG_ITER_LOG)
     g = Registration(cfg)
     g.AddCloudToLocalMap([mp])
     scans, guesses = [], []
@@ -181,13 +192,14 @@ def test_batch_equals_separate_matches(world, traj):
     for sc, gs in zip(scans, guesses):
         T = gs.copy()
         ok = g.Match(PointcloudCluster(planar_cloud=sc), T)
-        singles.append((ok, T, g.last_stats.iterations, g.last_stats.n_valid))
+        singles.append((ok, T, g.last_stats.iterations, g.last_stats.n_valid, g.iter_log()))
     conv, Tb = g.match_batch(scans, np.stack(guesses))
     its = [s.iterations for s in g.last_batch_stats]
     assert len(set(its)) > 1  # the scans really stop at different iterations
-    for s, (ok, T, it, nv) in enumerate(singles):
+    for s, (ok, T, it, nv, log1) in enumerate(singles):
         assert bool(conv[s]) == ok and g.last_batch_stats[s].iterations == it and g.last_batch_stats[s].n_valid == nv, s
         assert np.allclose(Tb[s], T, rtol=0, atol=1e-9), s
+        _assert_logs_equal(g.iter_log(s), log1, s)
     assert not conv[-1]
     # and against the oracle for one of them
     o = orc.Registration(cfg)
@@ -216,7 +228,7 @@ def test_batch_stress_many_small_and_empty_scans(world, traj):
     must terminate with each scan's own result — compared with separate Matches."""
     from funny_lidar_slam_b200.registration import PointcloudCluster, Registration
     mp = synth.make_map_from_scans(world, traj[0:12:2], "vlp16", leaf=0.3)
-    g = Registration(default_config(FLS_P2PLANE_IVOX))
+    g = Registration(default_config(FLS_P2PLANE_IVOX, flags=FLS_FLAG_ITER_LOG))
     g.AddCloudToLocalMap([mp])
     rng = np.random.default_rng(11)
     base = [synth.make_scan(world, traj[3 + k], "vlp16", seed=90 + k)["points"] for k in range(4)]
@@ -229,6 +241,7 @@ def test_batch_stress_many_small_and_empty_scans(world, traj):
         guesses.append(synth.perturb_pose(traj[3 + k], dpos=0.02 + 0.01 * (j % 5), drot_deg=0.3 + 0.2 * (j % 3), seed=200 + j))
     conv, Tb = g.match_batch(scans, np.stack(guesses))
     st_b = [(s.iterations, s.n_valid, s.converged) for s in g.last_batch_stats]
+    logs_b = [g.iter_log(j) for j in range(24)]
     assert not conv[0] and st_b[0][1] == 0          # the empty scan fails, nothing else is disturbed
     for j in range(24):
         T = guesses[j].copy()
@@ -236,6 +249,7 @@ def test_batch_stress_many_small_and_empty_scans(world, traj):
         st = g.last_stats
         assert bool(conv[j]) == ok and st_b[j][0] == st.iterations and st_b[j][1] == st.n_valid, j
         assert np.allclose(Tb[j], T, rtol=0, atol=1e-8), j
+        _assert_logs_equal(logs_b[j], g.iter_log(), j)
     assert conv.sum() >= 12
 
 

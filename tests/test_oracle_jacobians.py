@@ -2,7 +2,7 @@
 
   * ICP and NDT: the accumulated gradient of one point equals minus half the finite-difference gradient of the cost
     it linearises, under the RIGHT perturbation each plug-in applies (icp_optimized.h:135-136, incremental_ndt.h:311-313);
-  * LOAM-iVox: one PlanerMatch + SumCoefficient pass restated with numpy on a brute-force NEARBY18 candidate search;
+  * LOAM-iVox: one PlanerMatch + SumCoefficient pass restated with numpy on the brute-force k-NN of tests/ivox_ref.py;
   * LOAM-iVox mapping mode: the cached-5-NN insertion rule (loam_point_to_plane_ivox.h:79-128) restated with numpy."""
 import numpy as np
 import pytest
@@ -10,6 +10,7 @@ import pytest
 from funny_lidar_slam_b200 import FLS_ICP_P2P, FLS_NDT, FLS_P2PLANE_IVOX, default_config, synth
 from funny_lidar_slam_b200._abi import FLS_FLAG_ITER_LOG
 from oracle import pyoracle as orc
+from tests import ivox_ref
 
 
 def _hat(v):
@@ -114,27 +115,10 @@ def test_ndt_gradient_is_half_the_derivative_of_the_mahalanobis_cost():
     assert np.allclose(lg["H"], H, rtol=1e-9, atol=1e-9 * np.abs(H).max())
 
 
-def _nearby18():
-    offs = [(0, 0, 0), (-1, 0, 0), (1, 0, 0), (0, 1, 0), (0, -1, 0), (0, 0, -1), (0, 0, 1), (1, 1, 0), (-1, 1, 0), (1, -1, 0), (-1, -1, 0),
-            (1, 0, 1), (-1, 0, 1), (1, 0, -1), (-1, 0, -1), (0, 1, 1), (0, -1, 1), (0, 1, -1), (0, -1, -1)]
-    return np.array(offs)
-
-
-def _ivox_knn5(mp, mkeys, q, res=0.5, max_range=5.0):
-    """IVoxMap::GetClosestPoint by brute force: candidates = map points whose voxel is in the NEARBY18 stencil of the query's
-    voxel, visit order = stencil order then insertion order; the 5 nearest by (fp32 d2, visit order)."""
-    kq = np.round(q.astype(np.float32) * np.float32(1.0 / res)).astype(np.int64)
-    cand = []
-    for o in _nearby18():
-        cand.extend(np.where(np.all(mkeys == kq + o, axis=1))[0])
-    if not cand:
-        return np.zeros((0, 3))
-    c = mp[cand, :3]
-    d = c - q.astype(np.float32)
-    d2 = (d[:, 0] * d[:, 0] + d[:, 1] * d[:, 1]) + d[:, 2] * d[:, 2]  # fp32, the order of pointcloud_utility.h:13-17
-    keep = np.where(d2 < np.float32(max_range * max_range))[0]
-    order = keep[np.argsort(d2[keep], kind="stable")][:5]
-    return c[order].astype(np.float64)
+def _knn5_points(mp, q):
+    """The 5 nearest map points of every query (IVoxMap::GetClosestPoint at the default NEARBY18, 0.5 m, 5 m), fp64 rows."""
+    r = ivox_ref.knn5(mp, q, 0.5, 2, 5.0)
+    return [mp[r.idx[i, :r.found[i]], :3].astype(np.float64) for i in range(len(q))]
 
 
 def test_ivox_first_iteration_against_numpy(scene16):
@@ -146,13 +130,11 @@ def test_ivox_first_iteration_against_numpy(scene16):
     T = scene16["guess_small"]
     r.match(src, T)
     lg = r.iter_log()[0]
-    mkeys = np.round(mp[:, :3] * np.float32(2.0)).astype(np.int64)
     R, t = T[:3, :3], T[:3, 3]
     H, g, nv = np.zeros((6, 6)), np.zeros(6), 0
-    for sp in src:
+    qs = ivox_ref.transform(src, T)  # fp64 rows rounded to fp32, as transform_point_d
+    for sp, q, A in zip(src, qs, _knn5_points(mp, qs)):
         ps = sp[:3].astype(np.float64)
-        q = (R @ ps + t).astype(np.float32)
-        A = _ivox_knn5(mp, mkeys, q)
         if len(A) < 5:
             continue
         c = np.linalg.lstsq(A, -np.ones(5), rcond=None)[0]
@@ -186,13 +168,11 @@ def test_ivox_mapping_mode_insertion_rule_against_numpy(world, traj):
     ok, Tf, _ = r.match(scan, guess)
     assert ok
     added = r.map_points - n0
-    mkeys = np.round(first[:, :3] * np.float32(2.0)).astype(np.int64)
-    Rg, tg = guess[:3, :3], guess[:3, 3]   # the single PlanerMatch ran at the guess: its 5-NN are the cached ones
+    # the single PlanerMatch ran at the guess: its 5-NN are the cached ones
     Rf, tf = Tf[:3, :3], Tf[:3, 3]
     expect = 0
-    for sp in scan:
+    for sp, near in zip(scan, _knn5_points(first, ivox_ref.transform(scan, guess))):
         ps = sp[:3].astype(np.float64)
-        near = _ivox_knn5(first, mkeys, (Rg @ ps + tg).astype(np.float32))
         pw = (Rf @ ps + tf).astype(np.float32).astype(np.float64)
         if len(near) == 0:
             expect += 1
