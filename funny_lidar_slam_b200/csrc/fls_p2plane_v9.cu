@@ -232,6 +232,13 @@ struct ChunkRegs {
     unsigned off;         // record offset of the run inside the stage buffer; 0xffffffff: not staged (read from global)
 };
 
+// The folder's solve, out of line: inlined, its arrays share stack slots with the compute warps' `J` and keep it in local
+// memory.  `p` by value: a reference would take the kernel parameter's address and copy all of it to the stack.
+__device__ __noinline__ void gn_step_v9(GnState* s, const GnPre& q, const double* tot, const GnParams p, fls_iter_log* log, int log_cap,
+                                        uint4* ll_pose, unsigned ll_tag, double* result) {
+    gn_step_pre(s, q, tot, p, log, log_cap, ll_pose, ll_tag, result);
+}
+
 // ---- the kernel ----------------------------------------------------------------------------------------------------------
 constexpr int kRing = 256;  // entries of the CTA's work ring (power of two)
 // refill policy of the server warp: with several scans open it keeps kRefillQuarters / 4 x W chunks drawn and not done, and the
@@ -386,7 +393,9 @@ __global__ void __launch_bounds__((W + 2) * 32, 1) p2plane_v9_kernel(P2PlaneLoop
                             const unsigned Ls = stage_u32 + (unsigned)stg * kStageBytes + cr.off * 16u;
                             amb = knn_scan_hot<1>(Ls, cr.count, cr.qx, cr.qy, cr.qz, t);
                         } else {
-                            amb = knn_scan_any(P, cr.count, r2, cr.qx, cr.qy, cr.qz, fast, t);
+                            Top6q ta;  // the out-of-line scan's result goes through memory; `t` stays in registers
+                            amb = knn_scan_any(P, cr.count, r2, cr.qx, cr.qy, cr.qz, fast, ta);
+                            t = ta;
                         }
                         if (amb) {
                             exact = true;
@@ -841,7 +850,7 @@ __global__ void __launch_bounds__((W + 2) * 32, 1) p2plane_v9_kernel(P2PlaneLoop
                     __syncwarp();
                     int stop = 0;
                     if (lane == 0) {
-                        gn_step_pre(state, *s_pre, s_tot, a.gp, sc->log, a.log_cap, sc->ll_pose, tag, sc->result);
+                        gn_step_v9(state, *s_pre, s_tot, a.gp, sc->log, a.log_cap, sc->ll_pose, tag, sc->result);
                         stop = state->done;  // written by this thread just now
                     }
                     stop = __shfl_sync(0xffffffffu, stop, 0);

@@ -220,7 +220,11 @@ __device__ __forceinline__ bool plane_term(const float4* P, const unsigned (&js)
             c[2] = c2;
         } else {
             ++n_fallback;
-            plane_lstsq_qr<kLdg>(P, js[0], js[1], js[2], js[3], js[4], c);
+            double cq[3];  // the out-of-line solve's result goes through memory; `c` stays in registers on the fast path
+            plane_lstsq_qr<kLdg>(P, js[0], js[1], js[2], js[3], js[4], cq);
+            c[0] = cq[0];
+            c[1] = cq[1];
+            c[2] = cq[2];
         }
     }
     const double cn = sqrt(c[0] * c[0] + c[1] * c[1] + c[2] * c[2]);
