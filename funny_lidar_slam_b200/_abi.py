@@ -75,6 +75,12 @@ class FlsFeatureCfg(C.Structure):
     _fields_ = [("corner_threshold", C.c_float), ("planar_threshold", C.c_float), ("device", C.c_int32), ("reserved", C.c_int32)]
 
 
+class FlsLoamFrontendCfg(C.Structure):
+    _fields_ = [("device", C.c_int32), ("n_rows", C.c_int32), ("n_cols", C.c_int32), ("horizontal_resolution", C.c_float),
+                ("min_distance", C.c_float), ("max_distance", C.c_float), ("corner_threshold", C.c_float), ("planar_threshold", C.c_float),
+                ("corner_leaf", C.c_float), ("planar_leaf", C.c_float), ("reserved", C.c_uint32 * 4)]
+
+
 def default_config(method: int, **overrides) -> FlsConfig:
     """Python twin of fls_config_default(): the parameter sets the reference ships (SURVEY.md App. B):
     config/localization/config_turing.yaml:48-53 (P2PLANE_IVOX), config/mapping/config_nclt_ndt.yaml:42-51 (NDT),

@@ -9,6 +9,7 @@
 #include <new>
 #include <vector>
 
+#include "fls_frontend.h"
 #include "fls_gn.cuh"
 #include "fls_handle.h"
 
@@ -1033,6 +1034,30 @@ int fls_match_device(fls_handle* hh, const void* d_points, size_t n, double T[16
     FLS_CATCH
 }
 
+int fls_match_cluster_device(fls_handle* hh, const void* d_ordered, size_t n_ordered, const void* d_planar, size_t n_planar, const void* d_corner,
+                             size_t n_corner, double T[16], int* converged, fls_match_stats* st) {
+    Handle* h = reinterpret_cast<Handle*>(hh);
+    if (!h || !T) return FLS_ERR_INVALID_ARG;
+    // the clouds each plug-in reads, as in fls_match
+    const bool uses_planar = h->cfg.method >= FLS_P2PLANE_IVOX;
+    if (uses_planar) {
+        if (!d_planar && n_planar) return FLS_ERR_INVALID_ARG;
+        if (h->cfg.method == FLS_LOAM_FULL) {
+            if (!d_corner && n_corner) return FLS_ERR_INVALID_ARG;
+        } else {
+            n_corner = 0;
+        }
+    } else if (!d_ordered && n_ordered) {
+        return FLS_ERR_INVALID_ARG;
+    }
+    FLS_TRY
+    if (st) std::memset(st, 0, sizeof(*st));
+    h->begin_call();
+    return match_dispatch(h, static_cast<const float4*>(d_ordered), n_ordered, static_cast<const float4*>(d_planar), n_planar,
+                          static_cast<const float4*>(d_corner), n_corner, T, converged, st);
+    FLS_CATCH
+}
+
 // Uploads the host scans of a batch back to back into the handle's scan buffer; ptrs[s] receives scan s
 static int upload_scans(Handle* h, int B, const void* const* pts, const size_t* n, size_t stride, const float4** ptrs) {
     size_t total = 0, n_max = 0;
@@ -1343,6 +1368,26 @@ int fls_voxel_grid(int device, const void* pts, size_t n, size_t stride, float l
     }
     cudaStreamDestroy(st);
     return rc;
+    FLS_CATCH
+}
+
+int fls_preprocess_loam(const fls_loam_frontend_cfg* cfg, const void* raw, const int32_t* ring, const float* time, size_t n, size_t stride,
+                        const fls_imu_buffer* imu, float* corner, float* planar, float* d_corner, float* d_planar, size_t* n_corner, size_t* n_planar,
+                        fls_match_stats* stats) {
+    if (!cfg || !n_corner || !n_planar) return FLS_ERR_INVALID_ARG;
+    *n_corner = *n_planar = 0;
+    if ((!raw && n) || (!ring && n) || !stride_ok(stride) || n > 0x7fffffffull) return FLS_ERR_INVALID_ARG;
+    if (!corner && !planar && !d_corner && !d_planar) return FLS_ERR_INVALID_ARG;
+    if (cfg->n_rows <= 0 || cfg->n_cols <= 0 || (long long)cfg->n_rows * cfg->n_cols > 0x7fffffffll || !(cfg->horizontal_resolution > 0.f) ||
+        !(cfg->corner_leaf > 0.f) || !(cfg->planar_leaf > 0.f))
+        return FLS_ERR_INVALID_ARG;
+    // the reference CHECK_NE()s both feature thresholds against FloatNaN (feature_extractor.cpp:19-20)
+    if (!(cfg->corner_threshold < 3.0e38f) || !(cfg->planar_threshold < 3.0e38f)) return FLS_ERR_INVALID_ARG;
+    if (imu && imu->n_imu && !time && n) return FLS_ERR_INVALID_ARG;
+    int ndev = 0;
+    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0 || cfg->device < 0 || cfg->device >= ndev || cfg->device >= 64) return FLS_ERR_NO_DEVICE;
+    FLS_TRY
+    return fls::preprocess_loam_device(*cfg, raw, ring, time, n, stride, imu, corner, planar, d_corner, d_planar, n_corner, n_planar, stats);
     FLS_CATCH
 }
 

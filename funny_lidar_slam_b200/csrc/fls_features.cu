@@ -10,12 +10,13 @@
 // order: bitonic sort of (roughness, position) in shared memory by the whole CTA — the composite key makes the unstable
 // upstream std::sort deterministic exactly as the oracle pins it — then the two greedy passes by one thread on
 // shared-memory state (they are sequential by definition: every pick changes the validity of later candidates).
+#include <algorithm>
 #include <cstdlib>
 #include <cstring>
 #include <mutex>
 #include <vector>
 
-#include "fls_maps.h"
+#include "fls_frontend.h"
 
 namespace fls {
 namespace {
@@ -343,50 +344,93 @@ __global__ void ring_offsets_kernel(const int* __restrict__ row_start, const int
     }
 }
 
-// Per-device workspace: stream, events, device buffers and pinned staging survive across calls (the extractor runs
-// once per scan; allocating per call cost more than the kernels).  Calls on one device are serialised by the mutex.
+// Exclusive scan of the 2V segment counts [corner counts of rings 0..V-1][planar counts of rings 0..V-1] (one CTA): segment g's
+// records go to position off[g] of the compacted index list; totals = {n_corner, n_planar}.
+template <int BLOCK>
+__global__ void __launch_bounds__(BLOCK) feat_scan_kernel(const int* __restrict__ cnt, int n_rows, int* __restrict__ off, int* __restrict__ totals) {
+    __shared__ int s_warp[BLOCK / 32];
+    const int m = 2 * n_rows;
+    int carry = 0;
+    for (int base = 0; base < m; base += BLOCK) {
+        const int i = base + threadIdx.x;
+        int total;
+        const int ex = block_excl_scan<BLOCK>(i < m ? cnt[i] : 0, s_warp, total);
+        if (i < m) off[i] = carry + ex;
+        carry += total;
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        totals[0] = off[n_rows];
+        totals[1] = carry - off[n_rows];
+    }
+}
+
+// Emission in upstream's order (feature_extractor.cpp:147-157 corners, :184-216 planar points; rings in order): CTA column
+// g < V copies ring g's corner picks (corner_out[g*120 ..]), g >= V ring g-V's planar points (planar_out + planar_off[g-V]),
+// to position off[g] of the index list and / or of its class's cloud.  blockIdx.y splits long segments.
+__global__ void feat_emit_kernel(const int* __restrict__ corner_out, const int* __restrict__ planar_out, const int* __restrict__ planar_off,
+                                 const int* __restrict__ cnt, const int* __restrict__ off, int n_rows, const float4* __restrict__ ordered,
+                                 int* __restrict__ idx_out, float4* __restrict__ corner_cloud, float4* __restrict__ planar_cloud) {
+    const int g = blockIdx.x;
+    const bool corner = g < n_rows;
+    const int r = corner ? g : g - n_rows;
+    const int* src = corner ? corner_out + (size_t)r * 120 : planar_out + planar_off[r];
+    const int c = cnt[g], o = off[g];
+    float4* cloud = corner ? corner_cloud : planar_cloud;
+    const int co = corner ? o : o - off[n_rows];  // planar points start at n_corner in the index list, at 0 in their cloud
+    for (int k = blockIdx.y * blockDim.x + threadIdx.x; k < c; k += gridDim.y * blockDim.x) {
+        const int i = src[k];
+        if (idx_out) idx_out[o + k] = i;
+        if (cloud) cloud[co + k] = ordered[i];
+    }
+}
+
+// The kernels' dynamic shared-memory limits are per device and per function: raised, never lowered, under a lock of their own
+// (every caller of enqueue_features holds its workspace lock already; this one is taken last and alone).
+void ensure_feat_smem(int device, size_t smem_sort, size_t smem_ring) {
+    static std::mutex mu;
+    static size_t set[64][2];
+    std::lock_guard<std::mutex> lock(mu);
+    size_t* cur = set[device & 63];
+    if (smem_sort <= cur[0] && smem_ring <= cur[1]) return;
+    const int ss = (int)std::max(smem_sort, cur[0]), sr = (int)std::max(smem_ring, cur[1]);
+    FLS_CUDA(cudaFuncSetAttribute(feat_sort_kernel<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, ss));
+    FLS_CUDA(cudaFuncSetAttribute(feat_sort_kernel<1024>, cudaFuncAttributeMaxDynamicSharedMemorySize, ss));
+    FLS_CUDA(cudaFuncSetAttribute(feat_ring_kernel<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, sr));
+    FLS_CUDA(cudaFuncSetAttribute(feat_ring_kernel<1024>, cudaFuncAttributeMaxDynamicSharedMemorySize, sr));
+    cur[0] = (size_t)ss;
+    cur[1] = (size_t)sr;
+}
+
+template <int BLOCK>
+void launch_feat(const RingArgs& a, size_t smem_sort, size_t smem_ring, cudaStream_t st) {
+    feat_sort_kernel<BLOCK><<<dim3(6, a.n_rows), BLOCK, smem_sort, st>>>(a);
+    feat_ring_kernel<BLOCK><<<a.n_rows, BLOCK, smem_ring, st>>>(a);
+}
+
+// Per-device workspace of fls_extract_features: stream, events, device buffers and pinned staging survive across calls (the
+// extractor runs once per scan; allocating per call cost more than the kernels).  Calls on one device are serialised by the mutex.
 struct FeatWorkspace {
     std::mutex mu;
     bool ready = false;
     cudaStream_t st = nullptr;
     cudaEvent_t e0 = nullptr, e1 = nullptr, k0 = nullptr, k1 = nullptr;
-    DevBuf<float> d_depth, d_rough;
-    DevBuf<int> d_col, d_rows, d_out, d_poff;
-    DevBuf<unsigned char> d_meta;
-    DevBuf<unsigned long long> d_sorted;
-    int* h_out = nullptr;  // pinned: [corner n_rows*120][ccnt n_rows][pcnt n_rows][poff n_rows+1][planar cap]
+    DevBuf<float> d_depth;
+    DevBuf<int> d_col, d_rows, d_idx;
+    FeatStage s;
+    int* h_out = nullptr;  // pinned: [n_corner, n_planar][indices]
     size_t h_cap = 0;
-    int smem_sort = 0, smem_ring = 0;
 };
 FeatWorkspace& workspace(int device) {
     static FeatWorkspace ws[64];
     return ws[device & 63];
 }
 
-template <int BLOCK>
-void launch_feat(const RingArgs& a, size_t smem_sort, size_t smem_ring, FeatWorkspace& w) {
-    if ((int)smem_sort > w.smem_sort || (int)smem_ring > w.smem_ring) {
-        FLS_CUDA(cudaFuncSetAttribute(feat_sort_kernel<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_sort));
-        FLS_CUDA(cudaFuncSetAttribute(feat_sort_kernel<1024>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_sort));
-        FLS_CUDA(cudaFuncSetAttribute(feat_ring_kernel<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_ring));
-        FLS_CUDA(cudaFuncSetAttribute(feat_ring_kernel<1024>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_ring));
-        w.smem_sort = (int)smem_sort;
-        w.smem_ring = (int)smem_ring;
-    }
-    feat_sort_kernel<BLOCK><<<dim3(6, a.n_rows), BLOCK, smem_sort, w.st>>>(a);
-    feat_ring_kernel<BLOCK><<<a.n_rows, BLOCK, smem_ring, w.st>>>(a);
-}
-
 }  // namespace
 
-// Host driver.  Returns fls_status; fills corner_idx / planar_idx (host) in the reference's emission order.
-int extract_features_device(int device, const float* depth, const int* col, size_t n, const int* row_start, const int* row_end, int n_rows,
-                            float corner_thr, float planar_thr, int* corner_idx, size_t* n_corner, int* planar_idx, size_t* n_planar,
-                            fls_match_stats* stats) {
-    *n_corner = 0;
-    *n_planar = 0;
+int plan_features(const int* row_start, const int* row_end, int n_rows, size_t n, FeatPlan& p) {
+    std::memset(&p, 0, sizeof(p));
     if (n < 12 || n_rows <= 0) return FLS_OK;
-    if (device < 0 || device >= 64) return FLS_ERR_INVALID_ARG;
     int max_len = 0, max_ring = 0;
     long long planar_cap = 0;
     for (int r = 0; r < n_rows; ++r) {
@@ -400,10 +444,77 @@ int extract_features_device(int device, const float* depth, const int* col, size
     int lpad = 1;
     while (lpad < max_len) lpad <<= 1;
     const int lcap = max_len + 16;
-    const size_t smem_sort = (size_t)lpad * 8;
-    const size_t smem_ring = (size_t)lcap * 9 + (size_t)(max_ring > 0 ? max_ring : 1) + 16;
+    p.smem_sort = (size_t)lpad * 8;
+    p.smem_ring = (size_t)lcap * 9 + (size_t)(max_ring > 0 ? max_ring : 1) + 16;
     // block or ring too long for the shared-memory working set (DESIGN.md "limits")
-    if (smem_sort > 200 * 1024 || smem_ring > 200 * 1024) return FLS_ERR_UNSUPPORTED;
+    if (p.smem_sort > 200 * 1024 || p.smem_ring > 200 * 1024) return FLS_ERR_UNSUPPORTED;
+    p.active = true;
+    p.n = (int)n;
+    p.n_rows = n_rows;
+    p.max_len = max_len;
+    p.max_ring = max_ring;
+    p.lpad = lpad;
+    p.lcap = lcap;
+    p.planar_cap = (size_t)planar_cap;
+    return FLS_OK;
+}
+
+const int* enqueue_features(FeatStage& s, const FeatPlan& p, int device, const float* d_depth, const int* d_col, const int* d_rows, float corner_thr,
+                            float planar_thr, const float4* d_ordered, int* d_idx, float4* d_corner, float4* d_planar, cudaStream_t st) {
+    const int V = p.n_rows;
+    const size_t n = (size_t)p.n;
+    // d_out: [corner picks V*120][counts 2V][offsets 2V][planar_off V+1][totals 2][planar picks]
+    const size_t o_cnt = (size_t)V * 120, o_off = o_cnt + 2 * (size_t)V, o_poff = o_off + 2 * (size_t)V, o_tot = o_poff + V + 1, o_planar = o_tot + 2;
+    s.rough.reserve(n);
+    s.meta.reserve(n);
+    s.sorted.reserve(n);
+    s.out.reserve(o_planar + p.planar_cap + 8);
+    ensure_feat_smem(device, p.smem_sort, p.smem_ring);
+    int* out = s.out.p;
+    feat_point_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(d_depth, d_col, (int)n, s.rough.p, s.meta.p);
+    ring_offsets_kernel<<<1, 32, 0, st>>>(d_rows, d_rows + V, V, out + o_poff);
+    RingArgs a;
+    a.rough = s.rough.p;
+    a.meta = s.meta.p;
+    a.row_start = d_rows;
+    a.row_end = d_rows + V;
+    a.n_rows = V;
+    a.n = (int)n;
+    a.corner_thr = corner_thr;
+    a.planar_thr = planar_thr;
+    a.lpad = p.lpad;
+    a.lcap = p.lcap;
+    a.ring_cap = p.max_ring;
+    a.max_rounds = 96;
+    if (const char* e = std::getenv("FLS_FEAT_MAX_ROUNDS")) a.max_rounds = std::atoi(e) > 0 ? std::atoi(e) : 1;
+    a.sorted = s.sorted.p;
+    a.corner_out = out;
+    a.corner_cnt = out + o_cnt;
+    a.planar_cnt = out + o_cnt + V;
+    a.planar_off = out + o_poff;
+    a.planar_out = out + o_planar;
+    if (p.max_len > 512) launch_feat<1024>(a, p.smem_sort, p.smem_ring, st);
+    else launch_feat<256>(a, p.smem_sort, p.smem_ring, st);
+    feat_scan_kernel<1024><<<1, 1024, 0, st>>>(out + o_cnt, V, out + o_off, out + o_tot);
+    const size_t seg_cap = std::max<size_t>(120, 6 * ((size_t)p.max_len + 1));  // longest segment a ring can emit
+    const unsigned split = (unsigned)std::min<size_t>((seg_cap + 1023) / 1024, 64);
+    feat_emit_kernel<<<dim3(2 * V, split), 256, 0, st>>>(out, out + o_planar, out + o_poff, out + o_cnt, out + o_off, V, d_ordered, d_idx, d_corner,
+                                                         d_planar);
+    FLS_CUDA(cudaGetLastError());
+    return out + o_tot;
+}
+
+// Host driver of fls_extract_features.  Returns fls_status; fills corner_idx / planar_idx (host) in the reference's emission order.
+int extract_features_device(int device, const float* depth, const int* col, size_t n, const int* row_start, const int* row_end, int n_rows,
+                            float corner_thr, float planar_thr, int* corner_idx, size_t* n_corner, int* planar_idx, size_t* n_planar,
+                            fls_match_stats* stats) {
+    *n_corner = 0;
+    *n_planar = 0;
+    if (n < 12 || n_rows <= 0) return FLS_OK;
+    if (device < 0 || device >= 64) return FLS_ERR_INVALID_ARG;
+    FeatPlan p;
+    const int prc = plan_features(row_start, row_end, n_rows, n, p);
+    if (prc != FLS_OK) return prc;
     FeatWorkspace& w = workspace(device);
     std::lock_guard<std::mutex> lock(w.mu);
     int rc = FLS_OK;
@@ -418,21 +529,17 @@ int extract_features_device(int device, const float* depth, const int* col, size
             w.ready = true;
         }
         cudaStream_t st = w.st;
-        const size_t o_ccnt = (size_t)n_rows * 120, o_pcnt = o_ccnt + n_rows, o_poff = o_pcnt + n_rows, o_planar = o_poff + n_rows + 1;
-        const size_t out_len = o_planar + (size_t)planar_cap + 8;
+        const size_t idx_cap = (size_t)n_rows * 120 + p.planar_cap;
         w.d_depth.reserve(n);
-        w.d_rough.reserve(n);
         w.d_col.reserve(n);
-        w.d_meta.reserve(n);
-        w.d_sorted.reserve(n);
         w.d_rows.reserve((size_t)n_rows * 2);
-        w.d_out.reserve(out_len);
-        if (out_len > w.h_cap) {
+        w.d_idx.reserve(idx_cap);
+        if (idx_cap + 2 > w.h_cap) {
             if (w.h_out) cudaFreeHost(w.h_out);
             w.h_out = nullptr;
             w.h_cap = 0;
-            FLS_CUDA(cudaMallocHost(&w.h_out, out_len * 2 * sizeof(int)));
-            w.h_cap = out_len * 2;
+            FLS_CUDA(cudaMallocHost(&w.h_out, (idx_cap + 2) * 2 * sizeof(int)));
+            w.h_cap = (idx_cap + 2) * 2;
         }
         FLS_CUDA(cudaEventRecord(w.e0, st));
         FLS_CUDA(cudaMemcpyAsync(w.d_depth.p, depth, n * 4, cudaMemcpyHostToDevice, st));
@@ -440,44 +547,17 @@ int extract_features_device(int device, const float* depth, const int* col, size
         FLS_CUDA(cudaMemcpyAsync(w.d_rows.p, row_start, n_rows * 4, cudaMemcpyHostToDevice, st));
         FLS_CUDA(cudaMemcpyAsync(w.d_rows.p + n_rows, row_end, n_rows * 4, cudaMemcpyHostToDevice, st));
         FLS_CUDA(cudaEventRecord(w.k0, st));
-        feat_point_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(w.d_depth.p, w.d_col.p, (int)n, w.d_rough.p, w.d_meta.p);
-        ring_offsets_kernel<<<1, 32, 0, st>>>(w.d_rows.p, w.d_rows.p + n_rows, n_rows, w.d_out.p + o_poff);
-        RingArgs a;
-        a.rough = w.d_rough.p;
-        a.meta = w.d_meta.p;
-        a.row_start = w.d_rows.p;
-        a.row_end = w.d_rows.p + n_rows;
-        a.n_rows = n_rows;
-        a.n = (int)n;
-        a.corner_thr = corner_thr;
-        a.planar_thr = planar_thr;
-        a.lpad = lpad;
-        a.lcap = lcap;
-        a.ring_cap = max_ring;
-        a.max_rounds = 96;
-        if (const char* e = std::getenv("FLS_FEAT_MAX_ROUNDS")) a.max_rounds = std::atoi(e) > 0 ? std::atoi(e) : 1;
-        a.sorted = w.d_sorted.p;
-        a.corner_out = w.d_out.p;
-        a.corner_cnt = w.d_out.p + o_ccnt;
-        a.planar_cnt = w.d_out.p + o_pcnt;
-        a.planar_off = w.d_out.p + o_poff;
-        a.planar_out = w.d_out.p + o_planar;
-        if (max_len > 512) launch_feat<1024>(a, smem_sort, smem_ring, w);
-        else launch_feat<256>(a, smem_sort, smem_ring, w);
-        FLS_CUDA(cudaGetLastError());
+        const int* d_tot = enqueue_features(w.s, p, device, w.d_depth.p, w.d_col.p, w.d_rows.p, corner_thr, planar_thr, nullptr, w.d_idx.p, nullptr,
+                                            nullptr, st);
         FLS_CUDA(cudaEventRecord(w.k1, st));
-        FLS_CUDA(cudaMemcpyAsync(w.h_out, w.d_out.p, (o_planar + (size_t)planar_cap) * 4, cudaMemcpyDeviceToHost, st));
+        FLS_CUDA(cudaMemcpyAsync(w.h_out, d_tot, 2 * sizeof(int), cudaMemcpyDeviceToHost, st));
+        FLS_CUDA(cudaStreamSynchronize(st));  // the two counts size the read-back
+        const size_t nc = (size_t)w.h_out[0], np = (size_t)w.h_out[1];
+        if (nc + np) FLS_CUDA(cudaMemcpyAsync(w.h_out + 2, w.d_idx.p, (nc + np) * 4, cudaMemcpyDeviceToHost, st));
         FLS_CUDA(cudaEventRecord(w.e1, st));
         FLS_CUDA(cudaStreamSynchronize(st));
-        const int *h_corner = w.h_out, *h_ccnt = w.h_out + o_ccnt, *h_pcnt = w.h_out + o_pcnt, *h_poff = w.h_out + o_poff,
-                  *h_planar = w.h_out + o_planar;
-        size_t nc = 0, np = 0;
-        for (int r = 0; r < n_rows; ++r) {
-            std::memcpy(corner_idx + nc, h_corner + (size_t)r * 120, (size_t)h_ccnt[r] * 4);
-            nc += h_ccnt[r];
-            std::memcpy(planar_idx + np, h_planar + h_poff[r], (size_t)h_pcnt[r] * 4);
-            np += h_pcnt[r];
-        }
+        std::memcpy(corner_idx, w.h_out + 2, nc * 4);
+        std::memcpy(planar_idx, w.h_out + 2 + nc, np * 4);
         *n_corner = nc;
         *n_planar = np;
         if (stats) {
@@ -487,13 +567,13 @@ int extract_features_device(int device, const float* depth, const int* col, size
             std::memset(stats, 0, sizeof(*stats));
             stats->gpu_ms = ms;
             stats->kernel_ms = kms;
-            stats->kernel_launches = 4;
-            stats->gpu_launches = 4;
+            stats->kernel_launches = kFeatLaunches;
+            stats->gpu_launches = kFeatLaunches;
             stats->n_source = (long long)n;
             stats->h2d_bytes = (long long)(n * 8 + (size_t)n_rows * 8);
-            stats->d2h_bytes = (long long)((o_planar + (size_t)planar_cap) * 4);
+            stats->d2h_bytes = (long long)(2 + nc + np) * 4;
             // algorithmic bytes: depth + col in, roughness/meta/sort keys written and read once, indices out
-            stats->algo_bytes = (long long)(n * (4 + 4 + 2 * 4 + 2 * 1 + 2 * 8) + (nc + np) * 4);
+            stats->algo_bytes = feature_algo_bytes(n, nc, np);
         }
     } catch (const CudaError& e) {
         rc = e.status;

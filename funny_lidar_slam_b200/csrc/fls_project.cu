@@ -12,7 +12,7 @@
 #include <mutex>
 
 #include "fls_deskew.cuh"
-#include "fls_maps.h"
+#include "fls_frontend.h"
 
 namespace fls {
 namespace {
@@ -100,14 +100,7 @@ struct ProjWorkspace {
     std::mutex mu;
     bool ready = false;
     cudaStream_t st = nullptr;
-    DevBuf<float4> raw, ordered;
-    DevBuf<unsigned char> staging;
-    DevBuf<int> ring, col, rows;
-    DevBuf<unsigned> winner, flag, excl, total;
-    DevBuf<float> depth, time;
-    DevBuf<unsigned long long> imu_t;
-    DevBuf<double> imu_q;
-    DevBuf<unsigned char> cub_tmp;
+    ProjStage s;
 };
 ProjWorkspace& proj_workspace(int device) {
     static ProjWorkspace ws[64];
@@ -116,69 +109,86 @@ ProjWorkspace& proj_workspace(int device) {
 
 }  // namespace
 
-// Host driver: raw cloud (host, `stride` bytes per record) + ring per point -> projector arrays (host).  depth_out / col_out hold V*H
-// entries (the first *n_out are meaningful, as upstream), ordered_out V*H packed float4 records.
 int make_deskew_view(const fls_imu_buffer* imu, DevBuf<unsigned long long>& d_t, DevBuf<double>& d_q, cudaStream_t st, DeskewView& v);
 
+int enqueue_project(ProjStage& w, const void* raw, const int* ring, const float* time, const fls_imu_buffer* imu, size_t n, size_t stride, int V, int H,
+                    float h_res, float min_d, float max_d, cudaStream_t st, long long* h2d, int* launches) {
+    const size_t cells = (size_t)V * H;
+    DeskewView dv;
+    const bool use_imu = imu && imu->n_imu && time;
+    int rc = make_deskew_view(use_imu ? imu : nullptr, w.imu_t, w.imu_q, st, dv);
+    const bool ref_failed = rc == FLS_ERR_INVALID_ARG && use_imu && imu->imu_time_us && imu->imu_quat_xyzw;  // SetRefTime failed: no point is accepted
+    if (rc != FLS_OK && !ref_failed) return rc;
+    if (dv.m > 0) *h2d += (long long)(imu->n_imu * (sizeof(unsigned long long) + 4 * sizeof(double)));
+    if (ref_failed) n = 0;
+    w.raw.reserve(n + 1);
+    w.ring.reserve(n + 1);
+    w.time.reserve(n + 1);
+    if (n && use_imu) {
+        FLS_CUDA(cudaMemcpyAsync(w.time.p, time, n * sizeof(float), cudaMemcpyHostToDevice, st));
+        *h2d += (long long)(n * sizeof(float));
+    }
+    w.winner.reserve(cells);
+    w.flag.reserve(cells);
+    w.excl.reserve(cells);
+    w.total.reserve(1);
+    w.ordered.reserve(cells);
+    w.depth.reserve(cells);
+    w.col.reserve(cells);
+    w.rows.reserve((size_t)V * 2);
+    if (n) {
+        if (stride == FLS_LAYOUT_PACKED) {
+            FLS_CUDA(cudaMemcpyAsync(w.raw.p, raw, n * sizeof(float4), cudaMemcpyHostToDevice, st));
+        } else {
+            w.staging.reserve(n * stride);
+            FLS_CUDA(cudaMemcpyAsync(w.staging.p, raw, n * stride, cudaMemcpyHostToDevice, st));
+            launch_repack(w.staging.p, n, stride, w.raw.p, st);
+            ++*launches;
+        }
+        FLS_CUDA(cudaMemcpyAsync(w.ring.p, ring, n * sizeof(int), cudaMemcpyHostToDevice, st));
+        *h2d += (long long)(n * (stride + sizeof(int)));
+    }
+    const unsigned gc = (unsigned)((cells + 255) / 256);
+    proj_clear_kernel<<<gc, 256, 0, st>>>(w.winner.p, cells);
+    if (n) proj_claim_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(w.raw.p, w.ring.p, w.time.p, dv, (int)n, V, H, h_res, min_d, max_d, w.winner.p);
+    proj_flags_kernel<<<gc, 256, 0, st>>>(w.winner.p, cells, w.flag.p);
+    size_t tb = 0;
+    cub::DeviceScan::ExclusiveSum(nullptr, tb, w.flag.p, w.excl.p, (int)cells, st);
+    w.cub_tmp.reserve(tb + 256);
+    tb = w.cub_tmp.cap;
+    FLS_CUDA(cub::DeviceScan::ExclusiveSum(w.cub_tmp.p, tb, w.flag.p, w.excl.p, (int)cells, st));
+    // upstream leaves the tails of depth / col as they were (resize to V*H, col zero-filled): zero both
+    FLS_CUDA(cudaMemsetAsync(w.depth.p, 0, cells * sizeof(float), st));
+    FLS_CUDA(cudaMemsetAsync(w.col.p, 0, cells * sizeof(int), st));
+    proj_emit_kernel<<<gc, 256, 0, st>>>(w.raw.p, w.time.p, dv, w.winner.p, w.excl.p, V, H, w.ordered.p, w.depth.p, w.col.p, w.rows.p, w.rows.p + V, w.total.p);
+    FLS_CUDA(cudaGetLastError());
+    *launches += n ? 5 : 4;
+    return FLS_OK;
+}
+
+// Host driver: raw cloud (host, `stride` bytes per record) + ring per point -> projector arrays (host).  depth_out / col_out hold V*H
+// entries (the first *n_out are meaningful, as upstream), ordered_out V*H packed float4 records.
 int project_device(int device, const void* raw, const int* ring, const float* time, const fls_imu_buffer* imu, size_t n, size_t stride, int V, int H,
                    float h_res, float min_d, float max_d, float* ordered_out, float* depth_out, int* col_out, int* row_start, int* row_end, size_t* n_out) {
     *n_out = 0;
     if (V <= 0 || H <= 0 || !(h_res > 0.f) || device < 0 || device >= 64 || n > 0x7fffffffull) return FLS_ERR_INVALID_ARG;
     const size_t cells = (size_t)V * H;
     if (cells > 0x7fffffffull) return FLS_ERR_INVALID_ARG;
-    ProjWorkspace& w = proj_workspace(device);
-    std::lock_guard<std::mutex> lock(w.mu);
+    ProjWorkspace& ws = proj_workspace(device);
+    std::lock_guard<std::mutex> lock(ws.mu);
     int rc = FLS_OK;
     try {
         FLS_CUDA(cudaSetDevice(device));
-        if (!w.ready) {
-            FLS_CUDA(cudaStreamCreateWithFlags(&w.st, cudaStreamNonBlocking));
-            w.ready = true;
+        if (!ws.ready) {
+            FLS_CUDA(cudaStreamCreateWithFlags(&ws.st, cudaStreamNonBlocking));
+            ws.ready = true;
         }
-        cudaStream_t st = w.st;
-        DeskewView dv;
-        const bool use_imu = imu && imu->n_imu && time;
-        rc = make_deskew_view(use_imu ? imu : nullptr, w.imu_t, w.imu_q, st, dv);
-        const bool ref_failed = rc == FLS_ERR_INVALID_ARG && use_imu && imu->imu_time_us && imu->imu_quat_xyzw;  // SetRefTime failed: no point is accepted
-        if (rc != FLS_OK && !ref_failed) return rc;
-        rc = FLS_OK;
-        if (ref_failed) n = 0;
-        w.raw.reserve(n + 1);
-        w.ring.reserve(n + 1);
-        w.time.reserve(n + 1);
-        if (n && use_imu) FLS_CUDA(cudaMemcpyAsync(w.time.p, time, n * sizeof(float), cudaMemcpyHostToDevice, st));
-        w.winner.reserve(cells);
-        w.flag.reserve(cells);
-        w.excl.reserve(cells);
-        w.total.reserve(1);
-        w.ordered.reserve(cells);
-        w.depth.reserve(cells);
-        w.col.reserve(cells);
-        w.rows.reserve((size_t)V * 2);
-        if (n) {
-            if (stride == FLS_LAYOUT_PACKED) {
-                FLS_CUDA(cudaMemcpyAsync(w.raw.p, raw, n * sizeof(float4), cudaMemcpyHostToDevice, st));
-            } else {
-                w.staging.reserve(n * stride);
-                FLS_CUDA(cudaMemcpyAsync(w.staging.p, raw, n * stride, cudaMemcpyHostToDevice, st));
-                launch_repack(w.staging.p, n, stride, w.raw.p, st);
-            }
-            FLS_CUDA(cudaMemcpyAsync(w.ring.p, ring, n * sizeof(int), cudaMemcpyHostToDevice, st));
-        }
-        const unsigned gc = (unsigned)((cells + 255) / 256);
-        proj_clear_kernel<<<gc, 256, 0, st>>>(w.winner.p, cells);
-        if (n) proj_claim_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(w.raw.p, w.ring.p, w.time.p, dv, (int)n, V, H, h_res, min_d, max_d, w.winner.p);
-        proj_flags_kernel<<<gc, 256, 0, st>>>(w.winner.p, cells, w.flag.p);
-        size_t tb = 0;
-        cub::DeviceScan::ExclusiveSum(nullptr, tb, w.flag.p, w.excl.p, (int)cells, st);
-        w.cub_tmp.reserve(tb + 256);
-        tb = w.cub_tmp.cap;
-        FLS_CUDA(cub::DeviceScan::ExclusiveSum(w.cub_tmp.p, tb, w.flag.p, w.excl.p, (int)cells, st));
-        // upstream leaves the tails of depth / col as they were (resize to V*H, col zero-filled): zero both
-        FLS_CUDA(cudaMemsetAsync(w.depth.p, 0, cells * sizeof(float), st));
-        FLS_CUDA(cudaMemsetAsync(w.col.p, 0, cells * sizeof(int), st));
-        proj_emit_kernel<<<gc, 256, 0, st>>>(w.raw.p, w.time.p, dv, w.winner.p, w.excl.p, V, H, w.ordered.p, w.depth.p, w.col.p, w.rows.p, w.rows.p + V, w.total.p);
-        FLS_CUDA(cudaGetLastError());
+        cudaStream_t st = ws.st;
+        ProjStage& w = ws.s;
+        long long h2d = 0;
+        int launches = 0;
+        rc = enqueue_project(w, raw, ring, time, imu, n, stride, V, H, h_res, min_d, max_d, st, &h2d, &launches);
+        if (rc != FLS_OK) return rc;
         unsigned total = 0;
         FLS_CUDA(cudaMemcpyAsync(&total, w.total.p, sizeof(total), cudaMemcpyDeviceToHost, st));
         FLS_CUDA(cudaMemcpyAsync(depth_out, w.depth.p, cells * sizeof(float), cudaMemcpyDeviceToHost, st));

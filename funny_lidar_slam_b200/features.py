@@ -10,7 +10,7 @@ import ctypes as C
 
 import numpy as np
 
-from ._abi import FlsFeatureCfg, FlsMatchStats
+from ._abi import FlsFeatureCfg, FlsLoamFrontendCfg, FlsMatchStats
 from ._lib import check, lib
 from .registration import PointcloudCluster
 
@@ -148,3 +148,61 @@ def project_imu(projector: "PointcloudProjector", raw, ring, time, imu):
                                C.c_float(projector.max_d), vp(ordered), vp(depth), vp(col), vp(rs), vp(re), C.byref(n_out))
     check(rc, "fls_project_imu")
     return dict(ordered=ordered[:n_out.value].copy(), depth=depth, col=col, row_start=rs, row_end=re, n=n_out.value)
+
+
+class LoamFrontEnd:
+    """PreProcessing::Run, the LoamFull branch (src/slam/preprocessing.cpp:226-237 upstream), in one device call
+    (fls_preprocess_loam): projection with de-skew, feature extraction and the corner / planar voxel filters.
+    `Process(cluster)` reads cluster.extra["raw_cloud"] ((n,4) xyzi or (n,8) pcl records, firing order), ["ring"], ["time"]
+    (seconds relative to the scan's reference time; only read with an IMU buffer) and, optionally, ["imu"], and fills cluster.corner_cloud / planar_cloud,
+    as upstream's branch fills the PointcloudCluster."""
+
+    def __init__(self, lidar_horizontal_scan: int, lidar_vertical_scan: int, lidar_horizontal_resolution: float, min_distance: float,
+                 max_distance: float, corner_thr: float, planar_thr: float, corner_leaf: float, planar_leaf: float, device: int = 0):
+        self.cfg = FlsLoamFrontendCfg(int(device), int(lidar_vertical_scan), int(lidar_horizontal_scan), float(lidar_horizontal_resolution),
+                                      float(min_distance), float(max_distance), float(corner_thr), float(planar_thr), float(corner_leaf),
+                                      float(planar_leaf))
+        self.last_stats = FlsMatchStats()
+        self.last_counts = (0, 0)
+
+    def run(self, raw, ring, time, imu=None, device_out=None, host_out: bool = True):
+        """Returns (corner, planar) as (n,4) float32.  device_out=(d_corner, d_planar): device addresses on the configured device
+        (capacities 120*V and V*H records) that receive the same clouds; with host_out=False only those are written and (None, None)
+        is returned.  self.last_counts holds (n_corner, n_planar), self.last_stats the call's fls_match_stats."""
+        raw = np.ascontiguousarray(raw, np.float32)
+        if raw.ndim != 2 or raw.shape[1] not in (4, 8):
+            raise ValueError("raw cloud must be (n,4) packed xyzi or (n,8) pcl records")
+        ring = np.ascontiguousarray(ring, np.int32)
+        time = np.ascontiguousarray(time, np.float32) if time is not None else None  # needed only to de-skew
+        if len(ring) != len(raw) or (time is not None and len(time) != len(raw)):
+            raise ValueError("ring and time need one entry per raw point")
+        V, H = self.cfg.n_rows, self.cfg.n_cols
+        corner = np.zeros((120 * V, 4), np.float32) if host_out else None
+        planar = np.zeros((V * H, 4), np.float32) if host_out else None
+        d_c, d_p = (int(device_out[0]), int(device_out[1])) if device_out is not None else (0, 0)
+        nc, npl = C.c_size_t(0), C.c_size_t(0)
+        st = FlsMatchStats()
+        b, keep = _imu_struct(imu)
+        vp = lambda a: a.ctypes.data_as(C.c_void_p) if a is not None else None
+        rc = lib().fls_preprocess_loam(C.byref(self.cfg), vp(raw), vp(ring), vp(time), len(raw), raw.shape[1] * 4, C.byref(b) if b is not None else None,
+                                       vp(corner), vp(planar), C.c_void_p(d_c) if d_c else None, C.c_void_p(d_p) if d_p else None, C.byref(nc),
+                                       C.byref(npl), C.byref(st))
+        check(rc, "fls_preprocess_loam")
+        self.last_stats = st
+        self.last_counts = (nc.value, npl.value)
+        if not host_out:
+            return None, None
+        return corner[:nc.value].copy(), planar[:npl.value].copy()
+
+    def Process(self, cluster: PointcloudCluster) -> None:
+        e = cluster.extra
+        cluster.corner_cloud, cluster.planar_cloud = self.run(e["raw_cloud"], e["ring"], e.get("time"), e.get("imu"))
+
+
+def preprocess_loam(raw, ring, time, imu, lidar_horizontal_scan, lidar_vertical_scan, lidar_horizontal_resolution, min_distance, max_distance,
+                    corner_thr, planar_thr, corner_leaf, planar_leaf, device: int = 0, device_out=None):
+    """PreProcessing::Run's LoamFull branch on the device (fls_preprocess_loam): returns (corner_cloud, planar_cloud) as (n,4) float32;
+    with device_out=(d_corner, d_planar) the same clouds are also written to those device buffers."""
+    fe = LoamFrontEnd(lidar_horizontal_scan, lidar_vertical_scan, lidar_horizontal_resolution, min_distance, max_distance, corner_thr, planar_thr,
+                      corner_leaf, planar_leaf, device)
+    return fe.run(raw, ring, time, imu, device_out)

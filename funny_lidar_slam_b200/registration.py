@@ -179,6 +179,19 @@ class Registration:
         self.last_stats = st
         return bool(conv.value)
 
+    def match_cluster_device(self, d_ordered: int, n_ordered: int, d_planar: int, n_planar: int, d_corner: int, n_corner: int, T: np.ndarray) -> bool:
+        """Match with the cluster's clouds already in device memory (packed float4 device addresses, 0 for an unused cloud); the
+        plug-in reads the same clouds as Match.  The device-resident Match of LoamFull (planar + corner)."""
+        Tc = np.ascontiguousarray(np.asarray(T, np.float64).T).copy()
+        conv = C.c_int(0)
+        st = FlsMatchStats()
+        vp = lambda a: C.c_void_p(int(a)) if a else None
+        check(lib().fls_match_cluster_device(self._h, vp(d_ordered), int(n_ordered), vp(d_planar), int(n_planar), vp(d_corner), int(n_corner),
+                                             Tc.ctypes.data_as(C.c_void_p), C.byref(conv), C.byref(st)), "fls_match_cluster_device")
+        T[...] = Tc.T
+        self.last_stats = st
+        return bool(conv.value)
+
     # -- localization-mode map path (Localization::LoadLocalMap upstream) ---------------------------------
     def set_global_map(self, cloud: np.ndarray) -> None:
         p, n, s, keep = _cloud(cloud)

@@ -18,6 +18,8 @@
  *   fls_preprocess             <- PreProcessing::Run range gate + LidarDistortionCorrector::ProcessPoint + jump span + VoxelGrid
  *                                 (src/slam/preprocessing.cpp:181-225, src/lidar/lidar_distortion_corrector.cpp:37-64)
  *   fls_voxel_grid             <- VoxelGridCloud (include/common/pointcloud_utility.h:216-224,263-271)
+ *   fls_preprocess_loam        <- PreProcessing::Run, LoamFull branch: Project + ExtractFeatures + corner / planar VoxelGrid
+ *                                 (src/slam/preprocessing.cpp:226-237)
  *
  * Conventions
  *   * Points are read from caller memory as {float x, y, z, <pad>, intensity ...} records `stride_bytes`
@@ -175,6 +177,14 @@ int fls_match(fls_handle* h, const void* ordered, size_t n_ordered, const void* 
  * meaningful only when the call returns FLS_OK. */
 int fls_match_device(fls_handle* h, const void* d_points, size_t n, double T_colmajor[16], int* converged, fls_match_stats* stats);
 
+/* fls_match with the three PointcloudCluster clouds already in device memory on the handle's device (packed float4 {x,y,z,i}); the
+ * plug-in reads the same clouds as in fls_match (unused ones may be NULL/0).  This is the device-resident Match of FLS_LOAM_FULL, which
+ * reads two clouds (fls_match_device takes one and returns FLS_ERR_UNSUPPORTED for it), e.g. straight from fls_preprocess_loam's
+ * device outputs.  The LOAM plug-ins keep the planar pointer for a later fls_fitness, as in fls_match_device: the buffer must stay
+ * valid and unchanged until the next Match on the handle, or fls_fitness must not be called. */
+int fls_match_cluster_device(fls_handle* h, const void* d_ordered, size_t n_ordered, const void* d_planar, size_t n_planar, const void* d_corner,
+                             size_t n_corner, double T_colmajor[16], int* converged, fls_match_stats* stats);
+
 /* GetFitnessScore(max_range): FLT_MAX when unsupported / no inliers, as upstream. */
 int fls_fitness(fls_handle* h, float max_range, float* score);
 
@@ -292,6 +302,28 @@ int fls_preprocess(int device, const float* raw_xyzit, size_t n, const fls_imu_b
 int fls_project_imu(int device, const void* raw, const int32_t* ring, const float* time, size_t n, size_t stride_bytes, const fls_imu_buffer* imu,
                     int32_t n_rows, int32_t n_cols, float horizontal_resolution, float min_distance, float max_distance, float* ordered,
                     float* depth, int32_t* col, int32_t* row_start, int32_t* row_end, size_t* n_ordered);
+
+/* PreProcessing::Run, the LoamFull branch (src/slam/preprocessing.cpp:226-237), in one device call: fls_project_imu (range gate,
+ * projection, de-skew) -> fls_extract_features -> corner_cloud_ = VoxelGrid(corner_leaf), planar_cloud_ = VoxelGrid(planar_leaf).
+ * The outputs are bit-identical to that chain of per-stage calls with the features gathered from ordered_cloud_ in between; no point
+ * data returns to the host between the stages.  Inputs are those of fls_project_imu (`time` may be NULL without de-skew; imu == NULL
+ * or n_imu == 0: no de-skew; a reference time outside the IMU buffer gives empty clouds).  Outputs, packed x, y, z, intensity:
+ * `corner` / `planar` on the host and `d_corner` / `d_planar` in device memory on cfg->device; any of the four may be NULL, not all.
+ * Capacities: corner >= 120 * n_rows records, planar >= n_rows * n_cols records.  A ring or block too long for the feature kernels'
+ * shared memory returns FLS_ERR_UNSUPPORTED with both counts 0 and no output written.  stats: gpu_ms, gpu_launches, h2d_bytes,
+ * d2h_bytes, n_source = n, algo_bytes (sum of the three stages). */
+typedef struct {
+    int32_t device;
+    int32_t n_rows, n_cols;       /* LidarModel vertical_scan_num_ / horizon_scan_num_ */
+    float horizontal_resolution;  /* radians per column */
+    float min_distance, max_distance;
+    float corner_threshold, planar_threshold; /* frontend/feature/corner_thres, planar_thres */
+    float corner_leaf, planar_leaf;           /* frontend/feature/corner_voxel_filter_size, planar_voxel_filter_size */
+    uint32_t reserved[4];
+} fls_loam_frontend_cfg;
+int fls_preprocess_loam(const fls_loam_frontend_cfg* cfg, const void* raw, const int32_t* ring, const float* time, size_t n, size_t stride_bytes,
+                        const fls_imu_buffer* imu, float* corner, float* planar, float* d_corner, float* d_planar, size_t* n_corner,
+                        size_t* n_planar, fls_match_stats* stats);
 
 const char* fls_strerror(int status);
 const char* fls_last_error(void); /* thread-local text of the last CUDA failure */
