@@ -141,3 +141,32 @@ def default_config(method: int, **overrides) -> FlsConfig:
             raise AttributeError(f"fls_config has no field {k!r}")
         setattr(c, k, v)
     return c
+
+
+# fls_lidar_type — LidarModel::LidarSensorType (include/lidar/lidar_model.h:25 upstream), same order
+FLS_LIDAR_VELODYNE, FLS_LIDAR_OUSTER, FLS_LIDAR_LIVOX_AVIA, FLS_LIDAR_ROBOSENSE, FLS_LIDAR_LEISHEN, FLS_LIDAR_LIVOX_MID_360, FLS_LIDAR_NONE = range(7)
+LIDAR_TYPE_BY_NAME = {"velodyne": FLS_LIDAR_VELODYNE, "ouster": FLS_LIDAR_OUSTER, "livox_avia": FLS_LIDAR_LIVOX_AVIA, "robosense": FLS_LIDAR_ROBOSENSE,
+                      "leishen": FLS_LIDAR_LEISHEN, "livox_mid_360": FLS_LIDAR_LIVOX_MID_360, "none": FLS_LIDAR_NONE}
+# sensor_msgs/PointField datatypes
+FLS_PF_INT8, FLS_PF_UINT8, FLS_PF_INT16, FLS_PF_UINT16, FLS_PF_INT32, FLS_PF_UINT32, FLS_PF_FLOAT32, FLS_PF_FLOAT64 = range(1, 9)
+
+
+class FlsPointField(C.Structure):
+    _fields_ = [("name", C.c_char_p), ("offset", C.c_uint32), ("datatype", C.c_uint32), ("count", C.c_uint32), ("reserved", C.c_uint32)]
+
+
+class FlsPointCloud2(C.Structure):
+    """sensor_msgs/PointCloud2 (fls_pointcloud2)."""
+    _fields_ = [("data", C.c_void_p), ("data_on_device", C.c_int32), ("height", C.c_uint32), ("width", C.c_uint32), ("point_step", C.c_uint32),
+                ("row_step", C.c_uint32), ("is_dense", C.c_int32), ("is_bigendian", C.c_int32), ("n_fields", C.c_uint32),
+                ("fields", C.POINTER(FlsPointField)), ("stamp_us", C.c_uint64), ("reserved", C.c_uint32 * 4)]
+
+
+class FlsConvertCfg(C.Structure):
+    _fields_ = [("device", C.c_int32), ("lidar_type", C.c_int32), ("n_rows", C.c_int32), ("lower_angle", C.c_float), ("v_res", C.c_float),
+                ("time_scale", C.c_double), ("reserved", C.c_uint32 * 4)]
+
+
+class FlsConvertResult(C.Structure):
+    _fields_ = [("stamp_us", C.c_uint64), ("start_us", C.c_uint64), ("end_us", C.c_uint64), ("min_time", C.c_float), ("max_time", C.c_float),
+                ("valid", C.c_int32), ("recomputed", C.c_int32), ("reserved", C.c_uint32 * 2)]

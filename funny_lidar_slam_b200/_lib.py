@@ -5,7 +5,8 @@ from __future__ import annotations
 import ctypes as C
 import os
 
-from ._abi import FlsConfig, FlsFeatureCfg, FlsIterLog, FlsLoamFrontendCfg, FlsMapInfo, FlsMatchStats
+from ._abi import (FlsConfig, FlsConvertCfg, FlsConvertResult, FlsFeatureCfg, FlsIterLog, FlsLoamFrontendCfg, FlsMapInfo, FlsMatchStats,
+                   FlsPointCloud2)
 
 _PKG = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_PKG, "libfls_b200.so")
@@ -16,7 +17,8 @@ EXPORTS = [
     "fls_add_cloud", "fls_match", "fls_match_device", "fls_fitness", "fls_get_iter_log", "fls_get_iter_log_scan", "fls_get_map_info", "fls_ivox_knn",
     "fls_voxel_grid", "fls_extract_features", "fls_project", "fls_match_batch", "fls_match_batch_device",
     "fls_set_result_buffer_device", "fls_get_voxel_keys", "fls_get_map_points", "fls_ivox_add_points", "fls_preprocess", "fls_project_imu", "fls_match_batch_begin", "fls_match_batch_begin_device", "fls_match_batch_end", "fls_set_global_map", "fls_update_local_map",
-    "fls_pcd_read", "fls_pcd_write", "fls_preprocess_loam", "fls_match_cluster_device",
+    "fls_pcd_read", "fls_pcd_write", "fls_preprocess_loam", "fls_match_cluster_device", "fls_convert_cloud", "fls_preprocess_loam_device",
+    "fls_preprocess_device",
 ]
 
 
@@ -53,6 +55,11 @@ def lib():
     L.fls_match_cluster_device.argtypes = [vp, vp, sz, vp, sz, vp, sz, vp, C.POINTER(C.c_int), C.POINTER(FlsMatchStats)]
     L.fls_preprocess_loam.argtypes = [C.POINTER(FlsLoamFrontendCfg), vp, vp, vp, sz, sz, vp, vp, vp, vp, vp, C.POINTER(sz), C.POINTER(sz),
                                       C.POINTER(FlsMatchStats)]
+    L.fls_preprocess_loam_device.argtypes = [C.POINTER(FlsLoamFrontendCfg), vp, vp, vp, sz, vp, vp, vp, vp, vp, C.POINTER(sz), C.POINTER(sz),
+                                             C.POINTER(FlsMatchStats)]
+    L.fls_preprocess_device.argtypes = [C.c_int, vp, vp, sz, vp, f32, f32, i32, f32, vp, vp, C.POINTER(sz), vp, vp, C.POINTER(sz)]
+    L.fls_convert_cloud.argtypes = [C.POINTER(FlsConvertCfg), C.POINTER(FlsPointCloud2), vp, vp, vp, vp, vp, vp, C.POINTER(sz),
+                                    C.POINTER(FlsConvertResult), C.POINTER(FlsMatchStats)]
     L.fls_match_batch.argtypes = [vp, C.c_int, C.POINTER(vp), C.POINTER(sz), sz, vp, C.POINTER(C.c_int), C.POINTER(FlsMatchStats)]
     L.fls_match_batch_device.argtypes = [vp, C.c_int, C.POINTER(vp), C.POINTER(sz), vp, C.POINTER(C.c_int), C.POINTER(FlsMatchStats)]
     L.fls_set_result_buffer_device.argtypes = [vp, vp, sz]

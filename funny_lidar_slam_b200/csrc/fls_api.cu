@@ -1387,7 +1387,70 @@ int fls_preprocess_loam(const fls_loam_frontend_cfg* cfg, const void* raw, const
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0 || cfg->device < 0 || cfg->device >= ndev || cfg->device >= 64) return FLS_ERR_NO_DEVICE;
     FLS_TRY
-    return fls::preprocess_loam_device(*cfg, raw, ring, time, n, stride, imu, corner, planar, d_corner, d_planar, n_corner, n_planar, stats);
+    return fls::preprocess_loam_device(*cfg, raw, ring, time, n, stride, imu, corner, planar, d_corner, d_planar, n_corner, n_planar, stats, false);
+    FLS_CATCH
+}
+
+int fls_preprocess_loam_device(const fls_loam_frontend_cfg* cfg, const float* d_xyzi, const int32_t* d_ring, const float* d_time, size_t n,
+                               const fls_imu_buffer* imu, float* corner, float* planar, float* d_corner, float* d_planar, size_t* n_corner,
+                               size_t* n_planar, fls_match_stats* stats) {
+    if (!cfg || !n_corner || !n_planar) return FLS_ERR_INVALID_ARG;
+    *n_corner = *n_planar = 0;
+    if ((!d_xyzi && n) || (!d_ring && n) || n > 0x7fffffffull) return FLS_ERR_INVALID_ARG;
+    if (!corner && !planar && !d_corner && !d_planar) return FLS_ERR_INVALID_ARG;
+    if (cfg->n_rows <= 0 || cfg->n_cols <= 0 || (long long)cfg->n_rows * cfg->n_cols > 0x7fffffffll || !(cfg->horizontal_resolution > 0.f) ||
+        !(cfg->corner_leaf > 0.f) || !(cfg->planar_leaf > 0.f))
+        return FLS_ERR_INVALID_ARG;
+    if (!(cfg->corner_threshold < 3.0e38f) || !(cfg->planar_threshold < 3.0e38f)) return FLS_ERR_INVALID_ARG;
+    if (imu && imu->n_imu && !d_time && n) return FLS_ERR_INVALID_ARG;
+    int ndev = 0;
+    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0 || cfg->device < 0 || cfg->device >= ndev || cfg->device >= 64) return FLS_ERR_NO_DEVICE;
+    FLS_TRY
+    return fls::preprocess_loam_device(*cfg, d_xyzi, d_ring, d_time, n, FLS_LAYOUT_PACKED, imu, corner, planar, d_corner, d_planar, n_corner, n_planar,
+                                       stats, true);
+    FLS_CATCH
+}
+
+int fls_preprocess_device(int device, const float* d_xyzi, const float* d_time, size_t n, const fls_imu_buffer* imu, float min_distance,
+                          float max_distance, int32_t jump_span, float planar_leaf, float* ordered, float* d_ordered, size_t* n_ordered, float* planar,
+                          float* d_planar, size_t* n_planar) {
+    if (!n_ordered || !n_planar) return FLS_ERR_INVALID_ARG;
+    *n_ordered = *n_planar = 0;
+    if ((!d_xyzi && n) || (!ordered && !d_ordered && !planar && !d_planar) || jump_span < 1 || !(planar_leaf > 0.f)) return FLS_ERR_INVALID_ARG;
+    if (imu && imu->n_imu && !d_time && n) return FLS_ERR_INVALID_ARG;
+    int ndev = 0;
+    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0 || device < 0 || device >= ndev) return FLS_ERR_NO_DEVICE;
+    FLS_TRY
+    return fls::preprocess_device_input(device, d_xyzi, d_time, n, imu, min_distance, max_distance, jump_span, planar_leaf, ordered, d_ordered, n_ordered,
+                                        planar, d_planar, n_planar);
+    FLS_CATCH
+}
+
+int fls_convert_cloud(const fls_convert_cfg* cfg, const fls_pointcloud2* msg, float* xyzi, int32_t* ring, float* time, float* d_xyzi, int32_t* d_ring,
+                      float* d_time, size_t* n, fls_convert_result* result, fls_match_stats* stats) {
+    if (!cfg || !msg || !n || !result) return FLS_ERR_INVALID_ARG;
+    *n = 0;
+    const size_t cap = (size_t)msg->width * msg->height;
+    if (cfg->lidar_type < FLS_LIDAR_VELODYNE || cfg->lidar_type > FLS_LIDAR_NONE || cfg->n_rows <= 0 || !std::isfinite(cfg->time_scale))
+        return FLS_ERR_INVALID_ARG;
+    // LidarModel's FLT_MAX sentinels of lower_angle_ / v_res_ (include/lidar/lidar_model.h:90-91) must be set for None
+    if (cfg->lidar_type == FLS_LIDAR_NONE && (!(cfg->v_res > 0.f) || !(cfg->v_res < 3.0e38f) || !(std::fabs(cfg->lower_angle) < 3.0e38f)))
+        return FLS_ERR_INVALID_ARG;
+    if (cap > 0x7fffffffull || (cap && !msg->data) || (msg->n_fields && !msg->fields)) return FLS_ERR_INVALID_ARG;
+    if ((size_t)msg->row_step < (size_t)msg->width * msg->point_step) return FLS_ERR_INVALID_ARG;
+    for (uint32_t j = 0; j < msg->n_fields; ++j) {
+        const fls_point_field& f = msg->fields[j];
+        static const unsigned kSize[9] = {0, 1, 1, 2, 2, 4, 4, 4, 8};
+        if (!f.name) return FLS_ERR_INVALID_ARG;
+        if (f.datatype >= 1 && f.datatype <= 8 && (uint64_t)f.offset + (uint64_t)kSize[f.datatype] * (f.count ? f.count : 1) > msg->point_step)
+            return FLS_ERR_INVALID_ARG;
+    }
+    if (msg->is_bigendian) return FLS_ERR_UNSUPPORTED;
+    if (!xyzi && !ring && !time && !d_xyzi && !d_ring && !d_time) return FLS_ERR_INVALID_ARG;
+    int ndev = 0;
+    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0 || cfg->device < 0 || cfg->device >= ndev || cfg->device >= 64) return FLS_ERR_NO_DEVICE;
+    FLS_TRY
+    return fls::convert_cloud_device(*cfg, *msg, xyzi, ring, time, d_xyzi, d_ring, d_time, n, result, stats);
     FLS_CATCH
 }
 

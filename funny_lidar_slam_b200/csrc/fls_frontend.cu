@@ -33,7 +33,7 @@ LoamWorkspace& loam_workspace(int device) {
 
 int preprocess_loam_device(const fls_loam_frontend_cfg& c, const void* raw, const int* ring, const float* time, size_t n, size_t stride,
                            const fls_imu_buffer* imu, float* corner, float* planar, float* d_corner, float* d_planar, size_t* n_corner,
-                           size_t* n_planar, fls_match_stats* stats) {
+                           size_t* n_planar, fls_match_stats* stats, bool src_on_device) {
     *n_corner = *n_planar = 0;
     const int V = c.n_rows, H = c.n_cols;
     LoamWorkspace& w = loam_workspace(c.device);
@@ -59,7 +59,7 @@ int preprocess_loam_device(const fls_loam_frontend_cfg& c, const void* raw, cons
         int launches = 0;
         FLS_CUDA(cudaEventRecord(w.e0, st));
         // ---- projector (+ de-skew) ----
-        rc = enqueue_project(w.proj, raw, ring, time, imu, n, stride, V, H, c.horizontal_resolution, c.min_distance, c.max_distance, st, &h2d, &launches);
+        rc = enqueue_project(w.proj, raw, ring, time, imu, n, stride, V, H, c.horizontal_resolution, c.min_distance, c.max_distance, st, &h2d, &launches, src_on_device);
         if (rc != FLS_OK) return rc;
         // sync 1: n_ordered and the row bounds size the feature kernels (shared memory, planar capacity)
         FLS_CUDA(cudaMemcpyAsync(w.h_small, w.proj.total.p, sizeof(int), cudaMemcpyDeviceToHost, st));

@@ -2,12 +2,15 @@
 // PreProcessing::Run's branch for PointToPlane_IVOX / PointToPlane_KdTree / IcpOptimized / IncrementalNDT
 // (src/slam/preprocessing.cpp:181-225 upstream): range gate -> IMU de-skew of every point (fls_deskew.cuh) -> ordered_cloud_
 // (every kept point) and planar_cloud_ (every lidar_point_jump_span-th RAW index among the kept ones, then pcl::VoxelGrid).
+// fls_preprocess reads host records {x, y, z, intensity, time}; fls_preprocess_device reads float4 xyzi + float time already in device
+// memory (fls_convert_cloud's outputs).  Both run run_preprocess below: the same kernels on the same values.
 #include <cub/cub.cuh>
 
 #include <cmath>
 #include <mutex>
 
 #include "fls_deskew.cuh"
+#include "fls_frontend.h"
 #include "fls_maps.h"
 
 namespace fls {
@@ -42,17 +45,18 @@ __device__ __forceinline__ float depth_ref_pp(float x, float y, float z) {
     return __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(x, x), __fmul_rn(y, y)), __fmul_rn(z, z)));
 }
 
-// one thread per raw point: gate + de-skew; flags: bit 0 kept (ordered cloud), bit 1 kept and i % jump == 0 (planar candidates)
-__global__ void pp_point_kernel(const float* __restrict__ raw /*x,y,z,i,t*/, int n, DeskewView dv, float min_d, float max_d, int jump,
-                                float4* __restrict__ corrected, unsigned* __restrict__ f_ord, unsigned* __restrict__ f_pl) {
+// one thread per raw point: gate + de-skew; flags: bit 0 kept (ordered cloud), bit 1 kept and i % jump == 0 (planar candidates).
+// Point i is xyzi[xs*i .. xs*i+3] with its time at t[ts*i] (host records: xs = ts = 5; device arrays: xs = 4, ts = 1).
+__global__ void pp_point_kernel(const float* __restrict__ xyzi, int xs, const float* __restrict__ t, int ts, int n, DeskewView dv, float min_d,
+                                float max_d, int jump, float4* __restrict__ corrected, unsigned* __restrict__ f_ord, unsigned* __restrict__ f_pl) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    const float* p = raw + 5 * (size_t)i;
+    const float* p = xyzi + (size_t)xs * i;
     float x = p[0], y = p[1], z = p[2];
     bool keep = true;
     const float depth = depth_ref_pp(x, y, z);
     if (depth < min_d || depth > max_d) keep = false;  // preprocessing.cpp:199-203
-    if (keep && dv.m > 0) keep = deskew_point(dv, x, y, z, p[4], x, y, z);  // :205-211
+    if (keep && dv.m > 0) keep = deskew_point(dv, x, y, z, t[(size_t)ts * i], x, y, z);  // :205-211
     corrected[i] = make_float4(x, y, z, p[3]);
     f_ord[i] = keep ? 1u : 0u;
     f_pl[i] = (keep && (i % jump) == 0) ? 1u : 0u;  // :219-222
@@ -101,8 +105,13 @@ int make_deskew_view(const fls_imu_buffer* imu, DevBuf<unsigned long long>& d_t,
     return FLS_OK;
 }
 
-int preprocess_device(int device, const float* raw_xyzit, size_t n, const fls_imu_buffer* imu, float min_d, float max_d, int jump_span, float leaf,
-                      float* ordered_out, size_t* n_ordered, float* planar_out, size_t* n_planar) {
+namespace {
+
+// The points are host records {x, y, z, intensity, time} (src_on_device false: uploaded first) or device arrays (float4 xyzi, float time).
+// ordered_cloud_ goes to ordered_out (host) and / or d_ordered, planar_cloud_ to planar_out and / or d_planar (NULL: not written).
+int run_preprocess(int device, const float* xyzi, const float* time, bool src_on_device, size_t n, const fls_imu_buffer* imu, float min_d, float max_d,
+                   int jump_span, float leaf, float* ordered_out, float* d_ordered, size_t* n_ordered, float* planar_out, float* d_planar,
+                   size_t* n_planar) {
     *n_ordered = *n_planar = 0;
     if (device < 0 || device >= 64 || n > 0x7fffffffull || jump_span < 1 || !(leaf > 0.f)) return FLS_ERR_INVALID_ARG;
     if (n == 0) return FLS_OK;
@@ -119,18 +128,25 @@ int preprocess_device(int device, const float* raw_xyzit, size_t n, const fls_im
         DeskewView dv;
         rc = make_deskew_view(imu, w.imu_t, w.imu_q, st, dv);
         if (rc != FLS_OK) return rc == FLS_ERR_INVALID_ARG && imu && imu->n_imu ? FLS_OK : rc;  // SetRefTime failed: upstream drops the scan (:178-183) -> empty clouds
-        w.raw.reserve(n * 5);
         w.corrected.reserve(n);
-        w.ordered.reserve(n);
+        float4* ord = d_ordered ? reinterpret_cast<float4*>(d_ordered) : w.ordered.reserve(n);
         w.planar.reserve(n);
-        w.filtered.reserve(n);
+        float4* filtered = d_planar ? reinterpret_cast<float4*>(d_planar) : w.filtered.reserve(n);
         w.f_ord.reserve(n);
         w.f_pl.reserve(n);
         w.e_ord.reserve(n);
         w.e_pl.reserve(n);
-        FLS_CUDA(cudaMemcpyAsync(w.raw.p, raw_xyzit, n * 5 * sizeof(float), cudaMemcpyHostToDevice, st));
+        const float *px = xyzi, *pt = time;
+        int xs = 4, ts = 1;
+        if (!src_on_device) {
+            w.raw.reserve(n * 5);
+            FLS_CUDA(cudaMemcpyAsync(w.raw.p, xyzi, n * 5 * sizeof(float), cudaMemcpyHostToDevice, st));
+            px = w.raw.p;
+            pt = w.raw.p + 4;
+            xs = ts = 5;
+        }
         const unsigned g = (unsigned)((n + 255) / 256);
-        pp_point_kernel<<<g, 256, 0, st>>>(w.raw.p, (int)n, dv, min_d, max_d, jump_span, w.corrected.p, w.f_ord.p, w.f_pl.p);
+        pp_point_kernel<<<g, 256, 0, st>>>(px, xs, pt, ts, (int)n, dv, min_d, max_d, jump_span, w.corrected.p, w.f_ord.p, w.f_pl.p);
         size_t tb = 0;
         cub::DeviceScan::ExclusiveSum(nullptr, tb, w.f_ord.p, w.e_ord.p, (int)n, st);
         w.cub_tmp.reserve(tb + 256);
@@ -138,7 +154,7 @@ int preprocess_device(int device, const float* raw_xyzit, size_t n, const fls_im
         FLS_CUDA(cub::DeviceScan::ExclusiveSum(w.cub_tmp.p, tb, w.f_ord.p, w.e_ord.p, (int)n, st));
         tb = w.cub_tmp.cap;
         FLS_CUDA(cub::DeviceScan::ExclusiveSum(w.cub_tmp.p, tb, w.f_pl.p, w.e_pl.p, (int)n, st));
-        pp_scatter_kernel<<<g, 256, 0, st>>>(w.corrected.p, (int)n, w.f_ord.p, w.e_ord.p, w.ordered.p);
+        pp_scatter_kernel<<<g, 256, 0, st>>>(w.corrected.p, (int)n, w.f_ord.p, w.e_ord.p, ord);
         pp_scatter_kernel<<<g, 256, 0, st>>>(w.corrected.p, (int)n, w.f_pl.p, w.e_pl.p, w.planar.p);
         unsigned last[4] = {0, 0, 0, 0};
         FLS_CUDA(cudaMemcpyAsync(&last[0], w.e_ord.p + (n - 1), sizeof(unsigned), cudaMemcpyDeviceToHost, st));
@@ -148,9 +164,9 @@ int preprocess_device(int device, const float* raw_xyzit, size_t n, const fls_im
         FLS_CUDA(cudaStreamSynchronize(st));
         const size_t no = (size_t)last[0] + last[1], npl = (size_t)last[2] + last[3];
         int l = 0;
-        const size_t nf = npl ? voxel_grid_device(w.planar.p, npl, leaf, w.filtered.p, w.scratch, st, &l) : 0;  // :224-225
-        if (no) FLS_CUDA(cudaMemcpyAsync(ordered_out, w.ordered.p, no * sizeof(float4), cudaMemcpyDeviceToHost, st));
-        if (nf) FLS_CUDA(cudaMemcpyAsync(planar_out, w.filtered.p, nf * sizeof(float4), cudaMemcpyDeviceToHost, st));
+        const size_t nf = npl ? voxel_grid_device(w.planar.p, npl, leaf, filtered, w.scratch, st, &l) : 0;  // :224-225
+        if (no && ordered_out) FLS_CUDA(cudaMemcpyAsync(ordered_out, ord, no * sizeof(float4), cudaMemcpyDeviceToHost, st));
+        if (nf && planar_out) FLS_CUDA(cudaMemcpyAsync(planar_out, filtered, nf * sizeof(float4), cudaMemcpyDeviceToHost, st));
         FLS_CUDA(cudaStreamSynchronize(st));
         *n_ordered = no;
         *n_planar = nf;
@@ -158,6 +174,21 @@ int preprocess_device(int device, const float* raw_xyzit, size_t n, const fls_im
         rc = e.status;
     }
     return rc;
+}
+
+}  // namespace
+
+int preprocess_device(int device, const float* raw_xyzit, size_t n, const fls_imu_buffer* imu, float min_d, float max_d, int jump_span, float leaf,
+                      float* ordered_out, size_t* n_ordered, float* planar_out, size_t* n_planar) {
+    return run_preprocess(device, raw_xyzit, nullptr, false, n, imu, min_d, max_d, jump_span, leaf, ordered_out, nullptr, n_ordered, planar_out, nullptr,
+                          n_planar);
+}
+
+int preprocess_device_input(int device, const float* d_xyzi, const float* d_time, size_t n, const fls_imu_buffer* imu, float min_d, float max_d,
+                            int jump_span, float leaf, float* ordered_out, float* d_ordered, size_t* n_ordered, float* planar_out, float* d_planar,
+                            size_t* n_planar) {
+    return run_preprocess(device, d_xyzi, d_time, true, n, imu, min_d, max_d, jump_span, leaf, ordered_out, d_ordered, n_ordered, planar_out, d_planar,
+                          n_planar);
 }
 
 }  // namespace fls

@@ -11,32 +11,12 @@
 
 #include <mutex>
 
+#include "fls_atan.cuh"
 #include "fls_deskew.cuh"
 #include "fls_frontend.h"
 
 namespace fls {
 namespace {
-
-__device__ __forceinline__ float fast_atan2_ref(float y, float x) {
-    const float p1 = 0.9997878412794807f, p3 = -0.3258083974640975f, p5 = 0.1555786518463281f, p7 = -0.04432655554792128f;
-    const float ax = fabsf(x), ay = fabsf(y);
-    const float eps = 1.1920928955078125e-07f;
-    float a;
-    if (ax >= ay) {
-        const float c = __fdiv_rn(ay, __fadd_rn(ax, eps));
-        const float c2 = __fmul_rn(c, c);
-        a = __fmul_rn(__fadd_rn(__fmul_rn(__fadd_rn(__fmul_rn(__fadd_rn(__fmul_rn(p7, c2), p5), c2), p3), c2), p1), c);
-    } else {
-        const float c = __fdiv_rn(ax, __fadd_rn(ay, eps));
-        const float c2 = __fmul_rn(c, c);
-        a = __fsub_rn(1.57079632679489661923f,
-                      __fmul_rn(__fadd_rn(__fmul_rn(__fadd_rn(__fmul_rn(__fadd_rn(__fmul_rn(p7, c2), p5), c2), p3), c2), p1), c));
-    }
-    if (x < 0.f) a = __fsub_rn(3.14159265358979323846f, a);
-    if (y < 0.f) a = __fsub_rn(6.28318530717958647692f, a);
-    if (a > 3.14159265358979323846f) a = __fsub_rn(a, 6.28318530717958647692f);
-    return a;
-}
 
 __device__ __forceinline__ float depth_ref(float x, float y, float z) {
     return __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(x, x), __fmul_rn(y, y)), __fmul_rn(z, z)));
@@ -112,7 +92,7 @@ ProjWorkspace& proj_workspace(int device) {
 int make_deskew_view(const fls_imu_buffer* imu, DevBuf<unsigned long long>& d_t, DevBuf<double>& d_q, cudaStream_t st, DeskewView& v);
 
 int enqueue_project(ProjStage& w, const void* raw, const int* ring, const float* time, const fls_imu_buffer* imu, size_t n, size_t stride, int V, int H,
-                    float h_res, float min_d, float max_d, cudaStream_t st, long long* h2d, int* launches) {
+                    float h_res, float min_d, float max_d, cudaStream_t st, long long* h2d, int* launches, bool src_on_device) {
     const size_t cells = (size_t)V * H;
     DeskewView dv;
     const bool use_imu = imu && imu->n_imu && time;
@@ -124,7 +104,11 @@ int enqueue_project(ProjStage& w, const void* raw, const int* ring, const float*
     w.raw.reserve(n + 1);
     w.ring.reserve(n + 1);
     w.time.reserve(n + 1);
-    if (n && use_imu) {
+    // the records the kernels read: the caller's device arrays, or the stage buffers the host records are uploaded to
+    const float4* d_raw = src_on_device ? reinterpret_cast<const float4*>(raw) : w.raw.p;
+    const int* d_ring = src_on_device ? ring : w.ring.p;
+    const float* d_time = src_on_device && use_imu ? time : w.time.p;
+    if (n && use_imu && !src_on_device) {
         FLS_CUDA(cudaMemcpyAsync(w.time.p, time, n * sizeof(float), cudaMemcpyHostToDevice, st));
         *h2d += (long long)(n * sizeof(float));
     }
@@ -136,7 +120,7 @@ int enqueue_project(ProjStage& w, const void* raw, const int* ring, const float*
     w.depth.reserve(cells);
     w.col.reserve(cells);
     w.rows.reserve((size_t)V * 2);
-    if (n) {
+    if (n && !src_on_device) {
         if (stride == FLS_LAYOUT_PACKED) {
             FLS_CUDA(cudaMemcpyAsync(w.raw.p, raw, n * sizeof(float4), cudaMemcpyHostToDevice, st));
         } else {
@@ -150,7 +134,7 @@ int enqueue_project(ProjStage& w, const void* raw, const int* ring, const float*
     }
     const unsigned gc = (unsigned)((cells + 255) / 256);
     proj_clear_kernel<<<gc, 256, 0, st>>>(w.winner.p, cells);
-    if (n) proj_claim_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(w.raw.p, w.ring.p, w.time.p, dv, (int)n, V, H, h_res, min_d, max_d, w.winner.p);
+    if (n) proj_claim_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(d_raw, d_ring, d_time, dv, (int)n, V, H, h_res, min_d, max_d, w.winner.p);
     proj_flags_kernel<<<gc, 256, 0, st>>>(w.winner.p, cells, w.flag.p);
     size_t tb = 0;
     cub::DeviceScan::ExclusiveSum(nullptr, tb, w.flag.p, w.excl.p, (int)cells, st);
@@ -160,7 +144,7 @@ int enqueue_project(ProjStage& w, const void* raw, const int* ring, const float*
     // upstream leaves the tails of depth / col as they were (resize to V*H, col zero-filled): zero both
     FLS_CUDA(cudaMemsetAsync(w.depth.p, 0, cells * sizeof(float), st));
     FLS_CUDA(cudaMemsetAsync(w.col.p, 0, cells * sizeof(int), st));
-    proj_emit_kernel<<<gc, 256, 0, st>>>(w.raw.p, w.time.p, dv, w.winner.p, w.excl.p, V, H, w.ordered.p, w.depth.p, w.col.p, w.rows.p, w.rows.p + V, w.total.p);
+    proj_emit_kernel<<<gc, 256, 0, st>>>(d_raw, d_time, dv, w.winner.p, w.excl.p, V, H, w.ordered.p, w.depth.p, w.col.p, w.rows.p, w.rows.p + V, w.total.p);
     FLS_CUDA(cudaGetLastError());
     *launches += n ? 5 : 4;
     return FLS_OK;
@@ -187,7 +171,7 @@ int project_device(int device, const void* raw, const int* ring, const float* ti
         ProjStage& w = ws.s;
         long long h2d = 0;
         int launches = 0;
-        rc = enqueue_project(w, raw, ring, time, imu, n, stride, V, H, h_res, min_d, max_d, st, &h2d, &launches);
+        rc = enqueue_project(w, raw, ring, time, imu, n, stride, V, H, h_res, min_d, max_d, st, &h2d, &launches, false);
         if (rc != FLS_OK) return rc;
         unsigned total = 0;
         FLS_CUDA(cudaMemcpyAsync(&total, w.total.p, sizeof(total), cudaMemcpyDeviceToHost, st));

@@ -10,7 +10,8 @@ import ctypes as C
 
 import numpy as np
 
-from ._abi import FlsFeatureCfg, FlsLoamFrontendCfg, FlsMatchStats
+from ._abi import (FLS_PF_FLOAT32, FLS_PF_FLOAT64, FLS_PF_INT8, FLS_PF_INT16, FLS_PF_INT32, FLS_PF_UINT8, FLS_PF_UINT16, FLS_PF_UINT32, FlsConvertCfg,
+                   FlsConvertResult, FlsFeatureCfg, FlsLoamFrontendCfg, FlsMatchStats, FlsPointCloud2, FlsPointField)
 from ._lib import check, lib
 from .registration import PointcloudCluster
 
@@ -194,6 +195,27 @@ class LoamFrontEnd:
             return None, None
         return corner[:nc.value].copy(), planar[:npl.value].copy()
 
+    def run_device(self, d_xyzi: int, d_ring: int, d_time: int, n: int, imu=None, device_out=None, host_out: bool = True):
+        """run() on a cloud already in device memory on the configured device (fls_preprocess_loam_device): d_xyzi (n packed float4),
+        d_ring (n int32) and d_time (n float, 0 without de-skew) are device addresses, e.g. convert_message's device outputs."""
+        V, H = self.cfg.n_rows, self.cfg.n_cols
+        corner = np.zeros((120 * V, 4), np.float32) if host_out else None
+        planar = np.zeros((V * H, 4), np.float32) if host_out else None
+        d_c, d_p = (int(device_out[0]), int(device_out[1])) if device_out is not None else (0, 0)
+        nc, npl = C.c_size_t(0), C.c_size_t(0)
+        st = FlsMatchStats()
+        b, keep = _imu_struct(imu)
+        vp = lambda a: a.ctypes.data_as(C.c_void_p) if a is not None else None
+        dp = lambda a: C.c_void_p(int(a)) if a else None
+        rc = lib().fls_preprocess_loam_device(C.byref(self.cfg), dp(d_xyzi), dp(d_ring), dp(d_time), int(n), C.byref(b) if b is not None else None,
+                                              vp(corner), vp(planar), dp(d_c), dp(d_p), C.byref(nc), C.byref(npl), C.byref(st))
+        check(rc, "fls_preprocess_loam_device")
+        self.last_stats = st
+        self.last_counts = (nc.value, npl.value)
+        if not host_out:
+            return None, None
+        return corner[:nc.value].copy(), planar[:npl.value].copy()
+
     def Process(self, cluster: PointcloudCluster) -> None:
         e = cluster.extra
         cluster.corner_cloud, cluster.planar_cloud = self.run(e["raw_cloud"], e["ring"], e.get("time"), e.get("imu"))
@@ -206,3 +228,114 @@ def preprocess_loam(raw, ring, time, imu, lidar_horizontal_scan, lidar_vertical_
     fe = LoamFrontEnd(lidar_horizontal_scan, lidar_vertical_scan, lidar_horizontal_resolution, min_distance, max_distance, corner_thr, planar_thr,
                       corner_leaf, planar_leaf, device)
     return fe.run(raw, ring, time, imu, device_out)
+
+
+def preprocess_device(d_xyzi: int, d_time: int, n: int, imu, min_distance, max_distance, jump_span, planar_leaf, device: int = 0, device_out=None,
+                      host_out: bool = True):
+    """preprocess() on a cloud already in device memory (fls_preprocess_device): d_xyzi (n packed float4) and d_time (n float, 0 without
+    de-skew) are device addresses.  Returns (ordered_cloud, planar_cloud) as (n,4) float32 (None, None with host_out=False);
+    device_out=(d_ordered, d_planar), each with room for n records (0: not written), receives the same clouds; the ordered cloud may go
+    nowhere (host_out=False, d_ordered 0).  The counts are in
+    the returned clouds or, without host outputs, in preprocess_device.last_counts."""
+    cap = max(int(n), 1)
+    ordered = np.zeros((cap, 4), np.float32) if host_out else None
+    planar = np.zeros((cap, 4), np.float32) if host_out else None
+    d_o, d_p = (int(device_out[0]), int(device_out[1])) if device_out is not None else (0, 0)
+    no, npl = C.c_size_t(0), C.c_size_t(0)
+    b, keep = _imu_struct(imu)
+    vp = lambda a: a.ctypes.data_as(C.c_void_p) if a is not None else None
+    dp = lambda a: C.c_void_p(int(a)) if a else None
+    rc = lib().fls_preprocess_device(int(device), dp(d_xyzi), dp(d_time), int(n), C.byref(b) if b is not None else None, float(min_distance),
+                                     float(max_distance), int(jump_span), float(planar_leaf), vp(ordered), dp(d_o), C.byref(no), vp(planar), dp(d_p),
+                                     C.byref(npl))
+    check(rc, "fls_preprocess_device")
+    preprocess_device.last_counts = (no.value, npl.value)
+    if not host_out:
+        return None, None
+    return ordered[:no.value].copy(), planar[:npl.value].copy()
+
+
+preprocess_device.last_counts = (0, 0)
+
+# numpy scalar type -> sensor_msgs/PointField datatype
+_PF_BY_DTYPE = {np.dtype(np.int8): FLS_PF_INT8, np.dtype(np.uint8): FLS_PF_UINT8, np.dtype(np.int16): FLS_PF_INT16, np.dtype(np.uint16): FLS_PF_UINT16,
+                np.dtype(np.int32): FLS_PF_INT32, np.dtype(np.uint32): FLS_PF_UINT32, np.dtype(np.float32): FLS_PF_FLOAT32,
+                np.dtype(np.float64): FLS_PF_FLOAT64}
+
+
+class PointCloud2:
+    """sensor_msgs/PointCloud2 as the library reads it: `data` (bytes / uint8 array of height * row_step bytes, or a device address with
+    data_on_device=True), the layout, and the PointField table as (name, offset, datatype, count) tuples.  stamp_us is
+    header.stamp.toNSec() / 1000."""
+
+    def __init__(self, data, fields, width, height=1, point_step=None, row_step=None, is_dense=True, is_bigendian=False, stamp_us=0,
+                 data_on_device=False):
+        self.fields = [(str(n), int(o), int(d), int(c)) for n, o, d, c in fields]
+        self.width, self.height = int(width), int(height)
+        self.point_step = int(point_step)
+        self.row_step = int(row_step) if row_step is not None else self.width * self.point_step
+        self.is_dense, self.is_bigendian = bool(is_dense), bool(is_bigendian)
+        self.stamp_us = int(stamp_us)
+        self.data_on_device = bool(data_on_device)
+        self.data = int(data) if data_on_device else np.frombuffer(bytes(data), np.uint8) if not isinstance(data, np.ndarray) else \
+            np.ascontiguousarray(data).view(np.uint8).reshape(-1)
+
+    @classmethod
+    def from_records(cls, rec: np.ndarray, **kw):
+        """A message from a numpy structured array (1-D: one row; 2-D: organized), one PointField per named scalar field of its dtype
+        (offsets and itemsize as the dtype has them, e.g. np.dtype({'names': ..., 'formats': ..., 'offsets': ..., 'itemsize': ...}))."""
+        rec = np.ascontiguousarray(rec)
+        h, w = (1, rec.shape[0]) if rec.ndim == 1 else rec.shape
+        fields = [(n, rec.dtype.fields[n][1], _PF_BY_DTYPE[rec.dtype.fields[n][0]], 1) for n in rec.dtype.names]
+        return cls(rec.view(np.uint8).reshape(-1), fields, w, h, rec.dtype.itemsize, **kw)
+
+    def struct(self):
+        """(fls_pointcloud2, keep-alive)"""
+        names = [C.c_char_p(n.encode()) for n, _, _, _ in self.fields]
+        tab = (FlsPointField * max(len(self.fields), 1))()
+        for k, (n, o, d, c) in enumerate(self.fields):
+            tab[k] = FlsPointField(names[k].value, o, d, c, 0)
+        m = FlsPointCloud2()
+        m.data = self.data if self.data_on_device else (self.data.ctypes.data if self.data.size else None)
+        m.data_on_device = int(self.data_on_device)
+        m.height, m.width, m.point_step, m.row_step = self.height, self.width, self.point_step, self.row_step
+        m.is_dense, m.is_bigendian = int(self.is_dense), int(self.is_bigendian)
+        m.n_fields = len(self.fields)
+        m.fields = C.cast(tab, C.POINTER(FlsPointField))
+        m.stamp_us = self.stamp_us
+        return m, (names, tab, self.data)
+
+
+def convert_cfg(lidar_type: int, n_rows: int, time_scale: float, lower_angle: float = 0.0, v_res: float = 0.0, device: int = 0) -> FlsConvertCfg:
+    c = FlsConvertCfg()
+    c.device, c.lidar_type, c.n_rows = int(device), int(lidar_type), int(n_rows)
+    c.lower_angle, c.v_res, c.time_scale = float(lower_angle), float(v_res), float(time_scale)
+    return c
+
+
+def convert_message(msg: PointCloud2, lidar_type: int, n_rows: int, time_scale: float, lower_angle: float = 0.0, v_res: float = 0.0,
+                    device: int = 0, device_out=None, host_out: bool = True):
+    """PreProcessing::ConvertMessageToCloud on the device (fls_convert_cloud, src/slam/preprocessing.cpp:262-571 upstream).  Returns a dict:
+    xyzi (n,4) float32, ring (n,) int32, time (n,) float32 (None with host_out=False), n, and the scan's time window: stamp_us,
+    start_us, end_us, min_time, max_time, valid, recomputed, stats.  device_out=(d_xyzi, d_ring, d_time): device addresses with room for
+    width * height records that receive the same arrays (0: not written)."""
+    cap = msg.width * msg.height
+    cfg = convert_cfg(lidar_type, n_rows, time_scale, lower_angle, v_res, device)
+    xyzi = np.zeros((max(cap, 1), 4), np.float32) if host_out else None
+    ring = np.zeros(max(cap, 1), np.int32) if host_out else None
+    time = np.zeros(max(cap, 1), np.float32) if host_out else None
+    d = [int(a) for a in device_out] if device_out is not None else [0, 0, 0]
+    m, keep = msg.struct()
+    n = C.c_size_t(0)
+    res = FlsConvertResult()
+    st = FlsMatchStats()
+    vp = lambda a: a.ctypes.data_as(C.c_void_p) if a is not None else None
+    dp = lambda a: C.c_void_p(a) if a else None
+    rc = lib().fls_convert_cloud(C.byref(cfg), C.byref(m), vp(xyzi), vp(ring), vp(time), dp(d[0]), dp(d[1]), dp(d[2]), C.byref(n), C.byref(res),
+                                 C.byref(st))
+    check(rc, "fls_convert_cloud")
+    k = n.value
+    out = dict(n=k, stamp_us=res.stamp_us, start_us=res.start_us, end_us=res.end_us, min_time=res.min_time, max_time=res.max_time,
+               valid=bool(res.valid), recomputed=bool(res.recomputed), stats=st)
+    out.update(xyzi=xyzi[:k].copy(), ring=ring[:k].copy(), time=time[:k].copy()) if host_out else out.update(xyzi=None, ring=None, time=None)
+    return out

@@ -20,6 +20,10 @@
  *   fls_voxel_grid             <- VoxelGridCloud (include/common/pointcloud_utility.h:216-224,263-271)
  *   fls_preprocess_loam        <- PreProcessing::Run, LoamFull branch: Project + ExtractFeatures + corner / planar VoxelGrid
  *                                 (src/slam/preprocessing.cpp:226-237)
+ *   fls_convert_cloud          <- PreProcessing::ConvertMessageToCloud + ComputePointOffsetTime + GetLidarPointMinMaxOffsetTime
+ *                                 (src/slam/preprocessing.cpp:262-571) and the scan's time window (:86-104)
+ *   fls_preprocess_device /    <- fls_preprocess / fls_preprocess_loam reading a cloud already in device memory
+ *   fls_preprocess_loam_device
  *
  * Conventions
  *   * Points are read from caller memory as {float x, y, z, <pad>, intensity ...} records `stride_bytes`
@@ -324,6 +328,95 @@ typedef struct {
 int fls_preprocess_loam(const fls_loam_frontend_cfg* cfg, const void* raw, const int32_t* ring, const float* time, size_t n, size_t stride_bytes,
                         const fls_imu_buffer* imu, float* corner, float* planar, float* d_corner, float* d_planar, size_t* n_corner,
                         size_t* n_planar, fls_match_stats* stats);
+
+/* ---- PreProcessing::ConvertMessageToCloud on the device (src/slam/preprocessing.cpp:262-571) ---- */
+
+/* LidarModel::LidarSensorType (include/lidar/lidar_model.h:25), same order */
+typedef enum {
+    FLS_LIDAR_VELODYNE = 0,
+    FLS_LIDAR_OUSTER = 1,
+    FLS_LIDAR_LIVOX_AVIA = 2,
+    FLS_LIDAR_ROBOSENSE = 3,
+    FLS_LIDAR_LEISHEN = 4,
+    FLS_LIDAR_LIVOX_MID_360 = 5,
+    FLS_LIDAR_NONE = 6
+} fls_lidar_type;
+
+/* sensor_msgs/PointField datatypes */
+#define FLS_PF_INT8 1u
+#define FLS_PF_UINT8 2u
+#define FLS_PF_INT16 3u
+#define FLS_PF_UINT16 4u
+#define FLS_PF_INT32 5u
+#define FLS_PF_UINT32 6u
+#define FLS_PF_FLOAT32 7u
+#define FLS_PF_FLOAT64 8u
+
+typedef struct {
+    const char* name; /* NUL-terminated */
+    uint32_t offset;
+    uint32_t datatype; /* FLS_PF_* */
+    uint32_t count;
+    uint32_t reserved;
+} fls_point_field;
+
+/* sensor_msgs/PointCloud2.  `data` holds height * row_step bytes: host memory, or a device pointer on cfg->device when
+ * data_on_device is 1.  stamp_us is header.stamp.toNSec() / 1000, the stamp pcl_conversions gives the PCL cloud. */
+typedef struct {
+    const void* data;
+    int32_t data_on_device;
+    uint32_t height, width, point_step, row_step;
+    int32_t is_dense, is_bigendian;
+    uint32_t n_fields;
+    const fls_point_field* fields;
+    uint64_t stamp_us;
+    uint32_t reserved[4];
+} fls_pointcloud2;
+
+typedef struct {
+    int32_t device;
+    int32_t lidar_type;       /* fls_lidar_type */
+    int32_t n_rows;           /* LidarModel vertical_scan_num_ */
+    float lower_angle, v_res; /* LidarModel lower_angle_ / v_res_, read for FLS_LIDAR_NONE only */
+    double time_scale;        /* lidar_point_time_scale_ (include/slam/config_parameters.h:69) */
+    uint32_t reserved[4];
+} fls_convert_cfg;
+
+/* What PreProcessing::Run derives from the converted cloud before the IMU gate (preprocessing.cpp:86-104). */
+typedef struct {
+    uint64_t stamp_us;          /* header.stamp of the converted cloud (RoboSense: uint64(first kept timestamp * 1e6), :376) */
+    uint64_t start_us, end_us;  /* cloud_start_timestamp / cloud_end_timestamp after the one-sided widening of :100-104 */
+    float min_time, max_time;   /* GetLidarPointMinMaxOffsetTime (:554-571) */
+    int32_t valid;              /* 0 when no point is kept: the other fields are 0 and stamp_us is the message's */
+    int32_t recomputed;         /* ComputePointOffsetTime (:513-552) replaced the offsets (the last point's time was <= 0) */
+    uint32_t reserved[2];
+} fls_convert_result;
+
+/* ConvertMessageToCloud: pcl::fromROSMsg into the sensor's point type (a struct field reads the first message field with its name,
+ * datatype and a count of 0 or 1, else 0), the sensor's filter (NaN removal when not dense, the Livox Avia line / tag filter, the
+ * ring of FLS_LIDAR_NONE from elevation), ring and time, and ComputePointOffsetTime(cloud, 10.0) when the last kept point's time is
+ * <= 0.  Outputs, *n records: packed float4 {x, y, z, intensity}, int32 ring, float time, on the host (xyzi / ring / time) and / or in
+ * device memory on cfg->device (d_*); any of the six may be NULL.  Capacities: width * height records.  The host copies cover the whole
+ * capacity (the call waits once, at its end).  An empty message or one with no kept point returns FLS_OK with *n = 0 and
+ * result->valid = 0.  FLS_ERR_INVALID_ARG when a field does not fit in point_step or row_step < width * point_step;
+ * FLS_ERR_UNSUPPORTED for a big-endian message.  stats: gpu_ms, gpu_launches, h2d_bytes, d2h_bytes, n_source, algo_bytes. */
+int fls_convert_cloud(const fls_convert_cfg* cfg, const fls_pointcloud2* msg, float* xyzi, int32_t* ring, float* time, float* d_xyzi,
+                      int32_t* d_ring, float* d_time, size_t* n, fls_convert_result* result, fls_match_stats* stats);
+
+/* fls_preprocess_loam on a cloud already in device memory on cfg->device (e.g. fls_convert_cloud's device outputs): packed float4
+ * d_xyzi, int32 d_ring and float d_time (may be NULL without de-skew).  Nothing is uploaded but the IMU buffer; the stages and the
+ * outputs are those of fls_preprocess_loam on the same records. */
+int fls_preprocess_loam_device(const fls_loam_frontend_cfg* cfg, const float* d_xyzi, const int32_t* d_ring, const float* d_time, size_t n,
+                               const fls_imu_buffer* imu, float* corner, float* planar, float* d_corner, float* d_planar, size_t* n_corner,
+                               size_t* n_planar, fls_match_stats* stats);
+
+/* fls_preprocess on a cloud already in device memory on `device`: packed float4 d_xyzi and float d_time (relative time [s]; may be
+ * NULL without de-skew).  ordered_cloud_ goes to `ordered` (host) and / or `d_ordered` (device), planar_cloud_ to `planar` and / or
+ * `d_planar`; each needs room for n records and any of the four may be NULL, not all (the counts are returned either way).  Outputs equal fls_preprocess's on the same
+ * records; the planar device output is what fls_match_device takes. */
+int fls_preprocess_device(int device, const float* d_xyzi, const float* d_time, size_t n, const fls_imu_buffer* imu, float min_distance,
+                          float max_distance, int32_t jump_span, float planar_leaf, float* ordered, float* d_ordered, size_t* n_ordered, float* planar,
+                          float* d_planar, size_t* n_planar);
 
 const char* fls_strerror(int status);
 const char* fls_last_error(void); /* thread-local text of the last CUDA failure */
