@@ -320,12 +320,14 @@ int Handle::enqueue_ivox_batch(int B, const float4* const* d_scans, const size_t
     // one LL row per CTA + one LL pose record per scan (+ the group rows of v9)
     const unsigned tag_base = next_ll_epoch((size_t)B * grid * 32 + (size_t)B * kLlPoseLen + (size_t)B * 16 * 32);
     // ---- per-batch tables, staged in one pinned block and sent with one copy -------------------------------------------
-    const size_t o_pose = 0, o_off = o_pose + sizeof(PoseArg) * kMaxBatch, o_desc = o_off + sizeof(int) * (kMaxBatch + 4),
-                 o_ptr = o_desc + sizeof(P2PlaneScan) * kMaxBatch;
+    const size_t o_pose = 0, o_off = o_pose + sizeof(PoseArg) * kMaxBatch, o_toff = o_off + sizeof(int) * (kMaxBatch + 4),
+                 o_desc = o_toff + sizeof(int) * (kMaxBatch + 4), o_ptr = o_desc + sizeof(P2PlaneScan) * kMaxBatch;
     const size_t tbl_bytes = o_ptr + sizeof(void*) * kMaxBatch;
     unsigned char* const tbl = batch_table(tbl_bytes);
     PoseArg* hp = reinterpret_cast<PoseArg*>(tbl + o_pose);
     int* ho = reinterpret_cast<int*>(tbl + o_off);
+    int* ht = reinterpret_cast<int*>(tbl + o_toff);
+    ht[0] = 0;
     P2PlaneScan* hd = reinterpret_cast<P2PlaneScan*>(tbl + o_desc);
     const float4** hq = reinterpret_cast<const float4**>(tbl + o_ptr);
     uint4* pose_base = ll_rows.p + (size_t)B * grid * 32;
@@ -336,6 +338,7 @@ int Handle::enqueue_ivox_batch(int B, const float4* const* d_scans, const size_t
             hp[s].t[r] = Ts[12 + r];
         }
         ho[s] = off[s];
+        ht[s + 1] = ht[s] + order_tiles((int)n[s]);
         hq[s] = d_scans[s];
         P2PlaneScan& d = hd[s];
         d.src = src_f.p + off[s];
@@ -355,12 +358,19 @@ int Handle::enqueue_ivox_batch(int B, const float4* const* d_scans, const size_t
     send_batch_table(tbl_bytes);
     const PoseArg* d_poses = reinterpret_cast<const PoseArg*>(d_batch.p + o_pose);
     const int* d_off = reinterpret_cast<const int*>(d_batch.p + o_off);
+    const int* d_toff = reinterpret_cast<const int*>(d_batch.p + o_toff);
     const P2PlaneScan* d_desc = reinterpret_cast<const P2PlaneScan*>(d_batch.p + o_desc);
     const float4* const* d_ptrs = reinterpret_cast<const float4* const*>(d_batch.p + o_ptr);
-    // one prep kernel (state init, flag reset, locality keys) + ONE radix sort + gather for the whole batch: the queries of
-    // every scan end up in Morton order of the voxel they fall into at the initial pose (locality only: the sums are
-    // order-free up to fp64 rounding, and the persistent per-point records live in the same order for the whole Match)
-    prepare_queries(d_ptrs, n_total, d_off, B, d_poses, state.p, ivox_view(), flags.p, src_f.p, scratch, stream, &launches);
+    // chunk tickets of v9's dynamic work distribution: one counter per (scan, iteration) + the watchdog's abort word, zeroed by
+    // the prep kernel
+    const int ticket_stride = cfg.max_iterations + 2;
+    const int n_tickets = use_v9 ? B * ticket_stride + 4 : 0;
+    if (use_v9) tickets.reserve((size_t)n_tickets);
+    // ONE prep kernel for the whole batch (state init, flag and ticket reset): every tile of a scan ends up in Morton order of the
+    // voxel its points fall into at the initial pose (locality only: the sums are order-free up to fp64 rounding, and the
+    // persistent per-point records live in the same order for the whole Match)
+    prepare_queries(d_ptrs, d_off, d_toff, ht[B], B, d_poses, state.p, ivox_view(), flags.p, src_f.p, use_v9 ? tickets.p : nullptr, n_tickets,
+                    stream, &launches);
     P2PlaneLoopArgs a;
     a.map = ivox_view();
     a.plane_thres = cfg.point_to_planar_thres;
@@ -374,10 +384,8 @@ int Handle::enqueue_ivox_batch(int B, const float4* const* d_scans, const size_t
     // roofline accounting (SURVEY.md §8d, K1 — the REFERENCE algorithm's traffic): 16 B source point + n_stencil x 16 B
     // slot probes + 32 B persistent record per point-iteration, 16 B per map record resident in the stencil voxels.
     gn_launch(16 + 16LL * a.map.n_stencil + 32, 16, d_scans[0], n[0], [&] {
-        if (use_v9) {  // chunk tickets of the dynamic work distribution: one counter per (scan, iteration)
-            a.ticket_stride = cfg.max_iterations + 2;
-            tickets.reserve((size_t)B * a.ticket_stride + 4);
-            FLS_CUDA(cudaMemsetAsync(tickets.p, 0, sizeof(unsigned) * ((size_t)B * a.ticket_stride + 4), stream));
+        if (use_v9) {
+            a.ticket_stride = ticket_stride;
             a.tickets = tickets.p;
             a.abort_word = tickets.p + (size_t)B * a.ticket_stride;
             launch_p2plane_v9(a, grid, stream);

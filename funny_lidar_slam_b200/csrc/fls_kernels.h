@@ -54,9 +54,14 @@ void launch_p2plane_loop(const P2PlaneLoopArgs& a, int grid, cudaStream_t st);
 // generation 9 of the same loop (fls_p2plane_v9.cu): barrier-free dataflow, TMA-staged candidate runs, DMMA sums
 int p2plane_v9_grid(int n_max, int device);
 void launch_p2plane_v9(const P2PlaneLoopArgs& a, int grid, cudaStream_t st);
-// d_scan_ptrs[n_scans]: device pointers of the scans; d_offsets[n_scans + 1]: their positions in the batch; d_poses / d_states[n_scans]
-void prepare_queries(const float4* const* d_scan_ptrs, int n_total, const int* d_offsets, int n_scans, const PoseArg* d_poses, GnState* d_states,
-                     const IvoxView& map, unsigned char* d_flags, float4* d_sorted, BuildScratch& sc, cudaStream_t st, int* launches);
+// queries of a batch are put in locality order in tiles of this many consecutive points; a tile never spans two scans
+static constexpr int kOrderTile = 8192;
+inline int order_tiles(int n) { return (n + kOrderTile - 1) / kOrderTile; }
+// d_scan_ptrs[n_scans]: device pointers of the scans; d_offsets[n_scans + 1]: their positions in the batch; d_tile_off[n_scans + 1]:
+// prefix sums of order_tiles(n) over the scans; d_poses / d_states[n_scans]; d_zero[n_zero]: words zeroed on the way (v9 tickets)
+void prepare_queries(const float4* const* d_scan_ptrs, const int* d_offsets, const int* d_tile_off, int n_tiles, int n_scans,
+                     const PoseArg* d_poses, GnState* d_states, const IvoxView& map, unsigned char* d_flags, float4* d_sorted,
+                     unsigned* d_zero, int n_zero, cudaStream_t st, int* launches);
 // LOAM-iVox Match-internal AddCloudToLocalMap: classify + compact the points that enter the map (d_world, d_out: n records)
 size_t select_ivox_inserts(const IvoxView& map, const float4* d_src, int n, const double* R_prev, const double* t_prev, const double* R_fin,
                            const double* t_fin, double filter, float4* d_world, float4* d_out, BuildScratch& sc, cudaStream_t st, int* launches);

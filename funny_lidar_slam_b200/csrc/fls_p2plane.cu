@@ -1,7 +1,7 @@
 // fls_p2plane.cu — K1 (+ fused K6), generation 8: the whole LoamPointToPlaneIVOX Gauss-Newton loop as ONE persistent kernel with a
 // CTA barrier per visit.  It serves the single Match (fls_match / fls_match_device); batches run on generation 9
 // (fls_p2plane_v9.cu), which shares the per-point arithmetic (fls_knn.cuh, fls_plane.cuh).  This file also holds the per-batch query
-// preparation (prep kernel + radix sort + gather), the Match-internal insertion rule of mapping mode and the k-NN test entry.
+// preparation (one kernel: state init + tile-local locality sort), the Match-internal insertion rule of mapping mode and the k-NN test entry.
 //
 // Per source point and iteration it fuses what LoamPointToPlaneIVOX::PlanerMatch / ::SumCoefficient do
 // (include/registration/loam_point_to_plane_ivox.h:256-340 upstream): transform with the current pose, bounded
@@ -381,85 +381,95 @@ __device__ __forceinline__ unsigned spread_bits3(unsigned v) {  // up to 10 bits
 }
 
 // Per-batch preparation in ONE launch: for every scan initialise its GN state from the caller's pose, clear the per-point
-// valid flags [quirk 1: reset once per Match], and compute the locality key of every query.
-// Key = scan index on top of the 3-D Morton code of the low 4 bits per axis of the query's voxel at the initial pose (an
-// 8 m cube) and `hbits` more bits each of x and y; wrap-around beyond that only costs locality, never correctness.
-// morton bits = 12 + 2*hbits (16: two 8-bit radix passes); the scan bits keep every scan contiguous after the sort.
-__global__ void p2plane_prep_kernel(const float4* const* __restrict__ scan_ptrs, int n_total, const int* __restrict__ offsets, int n_scans,
-                                    const PoseArg* __restrict__ poses, float inv_res, int hbits, unsigned* __restrict__ keys,
-                                    unsigned* __restrict__ idx, unsigned char* __restrict__ flags, GnState* __restrict__ states,
-                                    const HashSlot* __restrict__ ctab, unsigned cmask, const float4* __restrict__ lists) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (blockIdx.x == 0 && (int)threadIdx.x < n_scans) {
-        GnState* s = states + threadIdx.x;
-        const PoseArg& pose = poses[threadIdx.x];
-        for (int k = 0; k < 9; ++k) s->R[k] = s->R0[k] = s->Rprev[k] = pose.R[k];
-        for (int k = 0; k < 3; ++k) s->t[k] = s->t0[k] = s->tprev[k] = pose.t[k];
-        s->last_rot = s->last_pos = 0.0;
-        s->sum_res = 0;
-        s->cand_total = s->hits_total = 0;
-        s->n_valid = 0;
-        s->iter = 0;
-        s->done = 0;
-        s->converged = 0;
-        s->failed = 0;
+// valid flags [quirk 1: reset once per Match] and `zero` (the v9 chunk tickets), and write every scan in locality order.
+// Each block owns a tile of kOrderTile consecutive points of one scan and sorts it in shared memory by the key of the voxel each
+// point falls into at its initial pose: the 3-D Morton code of the low 4 bits per axis (an 8 m cube) and 2 more bits each of
+// x and y (wrap-around beyond that only costs locality, never correctness).  Lanes of a warp then share centre voxels; a
+// voxel whose points fall into two tiles is visited from two chunks.  The order is a fixed function of the input (block radix
+// sort, ties in the sort's fixed order), so the per-point records and the single-scan kernel's sums stay reproducible.
+constexpr int kOrdThreads = 512, kOrdItems = kOrderTile / kOrdThreads;
+
+__global__ void __launch_bounds__(kOrdThreads) p2plane_prep_kernel(const float4* const* __restrict__ scan_ptrs, const int* __restrict__ offsets,
+                                                                   const int* __restrict__ tile_off, int n_scans, const PoseArg* __restrict__ poses,
+                                                                   float inv_res, unsigned* __restrict__ zero, int n_zero,
+                                                                   unsigned char* __restrict__ flags, GnState* __restrict__ states,
+                                                                   float4* __restrict__ dst, const HashSlot* __restrict__ ctab, unsigned cmask,
+                                                                   const float4* __restrict__ lists) {
+    using Sort = cub::BlockRadixSort<unsigned, kOrdThreads, kOrdItems, unsigned>;
+    __shared__ typename Sort::TempStorage s_sort;
+    if (blockIdx.x == 0) {
+        if ((int)threadIdx.x < n_scans) {
+            GnState* s = states + threadIdx.x;
+            const PoseArg& pose = poses[threadIdx.x];
+            for (int k = 0; k < 9; ++k) s->R[k] = s->R0[k] = s->Rprev[k] = pose.R[k];
+            for (int k = 0; k < 3; ++k) s->t[k] = s->t0[k] = s->tprev[k] = pose.t[k];
+            s->last_rot = s->last_pos = 0.0;
+            s->sum_res = 0;
+            s->cand_total = s->hits_total = 0;
+            s->n_valid = 0;
+            s->iter = 0;
+            s->done = 0;
+            s->converged = 0;
+            s->failed = 0;
+        }
+        for (int k = threadIdx.x; k < n_zero; k += blockDim.x) zero[k] = 0;
     }
-    if (i >= n_total) return;
-    flags[i] = 0;
-    int sid = 0;  // scan of point i: offsets is ascending, n_scans <= kMaxBatch
+    const int tile = (int)blockIdx.x;
+    if (tile >= __ldg(tile_off + n_scans)) return;  // the one block of an empty batch
+    int sid = 0;  // scan of this tile (block-uniform)
     {
         int lo = 0, hi = n_scans;
         while (hi - lo > 1) {
             const int mid = (lo + hi) >> 1;
-            if (__ldg(offsets + mid) <= i) lo = mid;
+            if (__ldg(tile_off + mid) <= tile) lo = mid;
             else hi = mid;
         }
         sid = lo;
     }
-    const float4 sp = scan_ptrs[sid][i - __ldg(offsets + sid)];
+    const int first = __ldg(offsets + sid) + (tile - __ldg(tile_off + sid)) * kOrderTile;  // batch position of the tile
+    const int n_here = min(kOrderTile, __ldg(offsets + sid + 1) - first);
+    const float4* __restrict__ src = scan_ptrs[sid] + (first - __ldg(offsets + sid));
     const PoseArg& pose = poses[sid];
-    const float qx = xform_row_d(__ldg(&pose.R[0]), __ldg(&pose.R[1]), __ldg(&pose.R[2]), __ldg(&pose.t[0]), sp.x, sp.y, sp.z);
-    const float qy = xform_row_d(__ldg(&pose.R[3]), __ldg(&pose.R[4]), __ldg(&pose.R[5]), __ldg(&pose.t[1]), sp.x, sp.y, sp.z);
-    const float qz = xform_row_d(__ldg(&pose.R[6]), __ldg(&pose.R[7]), __ldg(&pose.R[8]), __ldg(&pose.t[2]), sp.x, sp.y, sp.z);
-    const unsigned kx = (unsigned)ivox_coord(qx, inv_res), ky = (unsigned)ivox_coord(qy, inv_res), kz = (unsigned)ivox_coord(qz, inv_res);
-    const unsigned lo = spread_bits3(kx & 15u) | (spread_bits3(ky & 15u) << 1) | (spread_bits3(kz & 15u) << 2);  // 12 bits
-    const unsigned hm = (1u << hbits) - 1u;
-    const unsigned hx = (kx >> 4) & hm, hy = (ky >> 4) & hm;
-    unsigned hi = 0;
-    for (int b = 0; b < hbits; ++b) hi |= (((hx >> b) & 1u) << (2 * b)) | (((hy >> b) & 1u) << (2 * b + 1));
-    keys[i] = lo | (hi << 12) | ((unsigned)sid << (12 + 2 * hbits));
-    idx[i] = (unsigned)i;
-    // Warm L2 for the first iteration: the candidate run of the voxel this point starts in is requested now and arrives
-    // while the radix sort runs (the GN kernel is latency-bound on exactly these lines when they come from HBM).  One
-    // lane per distinct voxel of the warp issues the prefetches.
-    if (ctab) {
-        const unsigned long long key = pack_key((int)kx, (int)ky, (int)kz);
-        const unsigned peers = __match_any_sync(__activemask(), key);
-        if ((int)(__ffs(peers) - 1) == (int)(threadIdx.x & 31)) {
-            unsigned start, count;
-            if (table_find(ctab, cmask, key, start, count)) {
-                const char* p = reinterpret_cast<const char*>(lists + start);
-                const unsigned bytes = count * 16u;
-                for (unsigned off = 0; off < bytes; off += 128u) asm volatile("prefetch.global.L2 [%0];" ::"l"(p + off));
-                asm volatile("prefetch.global.L2 [%0];" ::"l"(p + bytes - 1));
+    unsigned key[kOrdItems], pos[kOrdItems];
+#pragma unroll
+    for (int k = 0; k < kOrdItems; ++k) {  // striped: item k of thread t is point k * kOrdThreads + t of the tile (coalesced)
+        const int q = k * kOrdThreads + (int)threadIdx.x;
+        pos[k] = (unsigned)q;
+        key[k] = 1u << 16;  // past the tile's end: a 17th key bit sorts it behind every real point, never written
+        if (q < n_here) {
+            flags[first + q] = 0;
+            const float4 sp = src[q];
+            const float qx = xform_row_d(__ldg(&pose.R[0]), __ldg(&pose.R[1]), __ldg(&pose.R[2]), __ldg(&pose.t[0]), sp.x, sp.y, sp.z);
+            const float qy = xform_row_d(__ldg(&pose.R[3]), __ldg(&pose.R[4]), __ldg(&pose.R[5]), __ldg(&pose.t[1]), sp.x, sp.y, sp.z);
+            const float qz = xform_row_d(__ldg(&pose.R[6]), __ldg(&pose.R[7]), __ldg(&pose.R[8]), __ldg(&pose.t[2]), sp.x, sp.y, sp.z);
+            const unsigned kx = (unsigned)ivox_coord(qx, inv_res), ky = (unsigned)ivox_coord(qy, inv_res), kz = (unsigned)ivox_coord(qz, inv_res);
+            const unsigned lo = spread_bits3(kx & 15u) | (spread_bits3(ky & 15u) << 1) | (spread_bits3(kz & 15u) << 2);  // 12 bits
+            const unsigned hx = (kx >> 4) & 3u, hy = (ky >> 4) & 3u;
+            key[k] = lo | (((hx & 1u) | ((hy & 1u) << 1) | ((hx & 2u) << 1) | ((hy & 2u) << 2)) << 12);
+            // Warm L2 for the first iteration: the candidate run of the voxel this point starts in is requested now and arrives
+            // while the tile is sorted (the GN kernel is latency-bound on exactly these lines when they come from HBM).  One
+            // lane per distinct voxel of the warp issues the prefetches.
+            if (ctab) {
+                const unsigned long long vkey = pack_key((int)kx, (int)ky, (int)kz);
+                const unsigned peers = __match_any_sync(__activemask(), vkey);
+                if ((int)(__ffs(peers) - 1) == (int)(threadIdx.x & 31)) {
+                    unsigned start, count;
+                    if (table_find(ctab, cmask, vkey, start, count)) {
+                        const char* p = reinterpret_cast<const char*>(lists + start);
+                        const unsigned bytes = count * 16u;
+                        for (unsigned off = 0; off < bytes; off += 128u) asm volatile("prefetch.global.L2 [%0];" ::"l"(p + off));
+                        asm volatile("prefetch.global.L2 [%0];" ::"l"(p + bytes - 1));
+                    }
+                }
             }
         }
     }
-}
-
-// dst[i] = point idx[i] of the batch, where the batch is the concatenation of the scans behind `scan_ptrs`
-__global__ void gather4_kernel(const float4* const* __restrict__ scan_ptrs, const int* __restrict__ offsets, int n_scans,
-                               const unsigned* __restrict__ idx, int n, float4* __restrict__ dst) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    const int g = (int)idx[i];
-    int lo = 0, hi = n_scans;
-    while (hi - lo > 1) {
-        const int mid = (lo + hi) >> 1;
-        if (__ldg(offsets + mid) <= g) lo = mid;
-        else hi = mid;
+    Sort(s_sort).SortBlockedToStriped(key, pos, 0, 17);
+#pragma unroll
+    for (int k = 0; k < kOrdItems; ++k) {  // sorted position k * kOrdThreads + t: coalesced stores
+        const int r = k * kOrdThreads + (int)threadIdx.x;
+        if (r < n_here) dst[first + r] = src[pos[k]];
     }
-    dst[i] = scan_ptrs[lo][g - __ldg(offsets + lo)];
 }
 
 __global__ void ivox_knn_test_kernel(IvoxView map, const float4* __restrict__ q, int n, float4* __restrict__ out, int* __restrict__ found) {
@@ -586,32 +596,14 @@ void launch_p2plane_loop(const P2PlaneLoopArgs& a, int grid, cudaStream_t st) {
     FLS_CUDA(cudaLaunchCooperativeKernel(p2plane_fn(), dim3(grid), dim3(kP2PlaneBlock), params, p2plane_smem(), st));
 }
 
-// Per-batch preparation: state init + flag reset + locality keys (one kernel), then order every scan by the voxel each
-// point falls into at its initial pose (ONE CUB radix sort of {scan | key, index} over the whole batch, gather).
-void prepare_queries(const float4* const* d_scan_ptrs, int n_total, const int* d_offsets, int n_scans, const PoseArg* d_poses, GnState* d_states,
-                     const IvoxView& map, unsigned char* d_flags, float4* d_sorted, BuildScratch& sc, cudaStream_t st, int* launches) {
-    const int m = n_total > 0 ? n_total : 1;
-    sc.k32a.reserve(m);
-    sc.k32b.reserve(m);
-    sc.idx.reserve(m);
-    sc.idx_sorted.reserve(m);
-    // 16-bit keys need one onesweep pass less than 24-bit keys, and an 8 m x 32 m x 32 m Morton window is all the locality the
-    // L1 broadcast needs (DESIGN.md §3.1 has the H100 comparison)
-    constexpr int key_bits = 16;
-    int scan_bits = 0;
-    while ((1 << scan_bits) < n_scans) ++scan_bits;
-    p2plane_prep_kernel<<<(m + 255) / 256, 256, 0, st>>>(d_scan_ptrs, n_total, d_offsets, n_scans, d_poses, map.inv_res, (key_bits - 12) / 2, sc.k32a.p,
-                                                        sc.idx.p, d_flags, d_states, map.ctab, map.cmask, map.lists);
+// Per-batch preparation: state init, flag and ticket reset and the locality order of every scan, in one launch of one block per
+// tile (one block for an empty batch).
+void prepare_queries(const float4* const* d_scan_ptrs, const int* d_offsets, const int* d_tile_off, int n_tiles, int n_scans,
+                     const PoseArg* d_poses, GnState* d_states, const IvoxView& map, unsigned char* d_flags, float4* d_sorted,
+                     unsigned* d_zero, int n_zero, cudaStream_t st, int* launches) {
+    p2plane_prep_kernel<<<n_tiles > 0 ? n_tiles : 1, kOrdThreads, 0, st>>>(d_scan_ptrs, d_offsets, d_tile_off, n_scans, d_poses, map.inv_res, d_zero,
+                                                                          n_zero, d_flags, d_states, d_sorted, map.ctab, map.cmask, map.lists);
     if (launches) *launches += 1;
-    if (n_total <= 0) return;
-    const int sort_bits = key_bits + scan_bits;
-    size_t t1 = 0;
-    cub::DeviceRadixSort::SortPairs(nullptr, t1, sc.k32a.p, sc.k32b.p, sc.idx.p, sc.idx_sorted.p, n_total, 0, sort_bits, st);
-    sc.cub_tmp.reserve(t1 + 256);
-    size_t tb = sc.cub_tmp.cap;
-    FLS_CUDA(cub::DeviceRadixSort::SortPairs(sc.cub_tmp.p, tb, sc.k32a.p, sc.k32b.p, sc.idx.p, sc.idx_sorted.p, n_total, 0, sort_bits, st));
-    gather4_kernel<<<(n_total + 255) / 256, 256, 0, st>>>(d_scan_ptrs, d_offsets, n_scans, sc.idx_sorted.p, n_total, d_sorted);
-    if (launches) *launches += 2 + (sort_bits + 7) / 8 + 1;
 }
 
 // Returns the number of points selected for insertion (class 1 then class 2, input order) in d_out; synchronises the stream.
