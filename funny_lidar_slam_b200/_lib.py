@@ -18,7 +18,8 @@ EXPORTS = [
     "fls_voxel_grid", "fls_extract_features", "fls_project", "fls_match_batch", "fls_match_batch_device",
     "fls_set_result_buffer_device", "fls_get_voxel_keys", "fls_get_map_points", "fls_ivox_add_points", "fls_preprocess", "fls_project_imu", "fls_match_batch_begin", "fls_match_batch_begin_device", "fls_match_batch_end", "fls_set_global_map", "fls_update_local_map",
     "fls_pcd_read", "fls_pcd_write", "fls_preprocess_loam", "fls_match_cluster_device", "fls_convert_cloud", "fls_preprocess_loam_device",
-    "fls_preprocess_device",
+    "fls_preprocess_device", "fls_keyframes_create", "fls_keyframes_destroy", "fls_keyframes_add", "fls_keyframes_add_device",
+    "fls_keyframes_count", "fls_keyframes_assemble",
 ]
 
 
@@ -81,6 +82,13 @@ def lib():
     L.fls_voxel_grid.argtypes = [C.c_int, vp, sz, sz, f32, vp, C.POINTER(sz)]
     L.fls_extract_features.argtypes = [C.POINTER(FlsFeatureCfg), vp, vp, sz, vp, vp, i32, vp, C.POINTER(sz), vp, C.POINTER(sz),
                                        C.POINTER(FlsMatchStats)]
+    L.fls_keyframes_create.argtypes = [C.c_int, sz, C.POINTER(vp)]
+    L.fls_keyframes_destroy.argtypes = [vp]
+    L.fls_keyframes_destroy.restype = None
+    L.fls_keyframes_add.argtypes = [vp, C.c_int64, vp, sz, sz]
+    L.fls_keyframes_add_device.argtypes = [vp, C.c_int64, vp, sz]
+    L.fls_keyframes_count.argtypes = [vp, C.POINTER(sz), C.POINTER(sz)]
+    L.fls_keyframes_assemble.argtypes = [vp, vp, sz, vp, f32, f32, vp, sz, vp, vp, sz, C.POINTER(sz), C.POINTER(FlsMatchStats)]
     for name in EXPORTS:
         getattr(L, name)  # AttributeError if the ABI drifted
     if L.fls_abi_version() != 1:

@@ -30,8 +30,10 @@ struct BuildScratch {
     ~BuildScratch();
 };
 
-// K7: VoxelGridCloud on the device.  d_out must hold n records; returns the output count.
-size_t voxel_grid_device(const float4* d_pts, size_t n, float leaf, float4* d_out, BuildScratch& sc, cudaStream_t st, int* launches);
+// K7: VoxelGridCloud on the device.  d_out must hold n records; returns the output count.  `waits` (optional) counts the
+// stream synchronisations the call made.
+size_t voxel_grid_device(const float4* d_pts, size_t n, float leaf, float4* d_out, BuildScratch& sc, cudaStream_t st, int* launches,
+                         int* waits = nullptr);
 
 // Point grid: voxel-contiguous float4 points + open-addressing table of {key, start, count} (see fls_ivox.cuh).
 // key_mode 0: round(p/res)  — IVoxMap::Pos2Grid (iVox map of the LOAM plug-in)

@@ -2,37 +2,15 @@
 // (include/common/pointcloud_utility.h:216-224,263-271 upstream; PCL 1.10 semantics, SURVEY.md §8c):
 //   bounding box -> cell = floor(x*inv_leaf) - min_b (fp32) -> linear id -> sort by id -> one fp32 centroid
 //   (xyz AND intensity) per occupied cell, cells in ascending id; dx*dy*dz > INT_MAX returns the input unchanged.
-// The radix sort is stable, so every centroid is summed in input order — the order the oracle pins.
+// The radix sort is stable, so every centroid is summed in input order — the order the oracle pins.  The key and centroid
+// arithmetic lives in fls_voxel.cuh, shared with the keyframe store's segmented pass (fls_keyframes.cu).
 #include <cub/cub.cuh>
 
 #include "fls_maps.h"
+#include "fls_voxel.cuh"
 
 namespace fls {
 namespace {
-
-struct MinMax6 {
-    float mn[3], mx[3];
-};
-
-// order-preserving float <-> uint encoding so the bounding box can be reduced with integer atomicMin / atomicMax
-__device__ __forceinline__ unsigned f2ord(float f) {
-    const unsigned u = __float_as_uint(f);
-    return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-}
-__host__ __device__ __forceinline__ float ord2f(unsigned o) {
-    const unsigned u = (o & 0x80000000u) ? (o & 0x7fffffffu) : ~o;
-#ifdef __CUDA_ARCH__
-    return __uint_as_float(u);
-#else
-    float f;
-    memcpy(&f, &u, 4);
-    return f;
-#endif
-}
-
-struct MinMaxOrd {
-    unsigned mn[3], mx[3];
-};
 
 __global__ void minmax_kernel(const float4* __restrict__ pts, size_t n, MinMaxOrd* __restrict__ out) {
     __shared__ float s[6][256];
@@ -64,15 +42,10 @@ __global__ void minmax_init_kernel(MinMaxOrd* o) {
     }
 }
 
-__global__ void vg_keys_kernel(const float4* __restrict__ pts, size_t n, float inv, int mb0, int mb1, int mb2, int mul1, int mul2,
-                               unsigned* __restrict__ keys, unsigned* __restrict__ idx) {
+__global__ void vg_keys_kernel(const float4* __restrict__ pts, size_t n, float inv, VgParams g, unsigned* __restrict__ keys, unsigned* __restrict__ idx) {
     const size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
     if (i >= n) return;
-    const float4 p = pts[i];
-    const int i0 = (int)(floorf(__fmul_rn(p.x, inv)) - (float)mb0);
-    const int i1 = (int)(floorf(__fmul_rn(p.y, inv)) - (float)mb1);
-    const int i2 = (int)(floorf(__fmul_rn(p.z, inv)) - (float)mb2);
-    keys[i] = (unsigned)(i0 + i1 * mul1 + i2 * mul2);
+    keys[i] = vg_cell_id(pts[i], inv, g);
     idx[i] = (unsigned)i;
 }
 
@@ -82,16 +55,9 @@ __global__ void vg_centroid_kernel(const float4* __restrict__ pts, const unsigne
     const int r = blockIdx.x * blockDim.x + threadIdx.x;
     if (r >= runs) return;
     const unsigned s = starts[r], c = counts[r];
-    float sx = 0.f, sy = 0.f, sz = 0.f, si = 0.f;
-    for (unsigned k = 0; k < c; ++k) {
-        const float4 p = __ldg(pts + idx_sorted[s + k]);
-        sx = __fadd_rn(sx, p.x);
-        sy = __fadd_rn(sy, p.y);
-        sz = __fadd_rn(sz, p.z);
-        si = __fadd_rn(si, p.w);
-    }
-    const float n = (float)c;
-    out[r] = make_float4(__fdiv_rn(sx, n), __fdiv_rn(sy, n), __fdiv_rn(sz, n), __fdiv_rn(si, n));
+    VgCentroid acc;
+    for (unsigned k = 0; k < c; ++k) acc.add(__ldg(pts + idx_sorted[s + k]));
+    out[r] = acc.mean(c);
 }
 
 inline unsigned grid_for(size_t n, int block) { return (unsigned)((n + block - 1) / block); }
@@ -100,37 +66,25 @@ inline unsigned grid_for(size_t n, int block) { return (unsigned)((n + block - 1
 
 // Returns the number of output points; d_out must hold n records.  Synchronises the stream twice
 // (bounding box, run count) — both values size the following launches.
-size_t voxel_grid_device(const float4* d_pts, size_t n, float leaf, float4* d_out, BuildScratch& sc, cudaStream_t st, int* launches) {
+size_t voxel_grid_device(const float4* d_pts, size_t n, float leaf, float4* d_out, BuildScratch& sc, cudaStream_t st, int* launches, int* waits) {
     if (n == 0) return 0;
     const float inv = 1.0f / leaf;
     sc.minmax.reserve(16);
     MinMaxOrd* d_mm = reinterpret_cast<MinMaxOrd*>(sc.minmax.p);
     sc.num_runs.reserve(2);
     minmax_init_kernel<<<1, 1, 0, st>>>(d_mm);
-    const unsigned g = grid_for(n, 256) < 592 ? grid_for(n, 256) : 592;
-    minmax_kernel<<<g, 256, 0, st>>>(d_pts, n, d_mm);
+    const unsigned nb = grid_for(n, 256) < 592 ? grid_for(n, 256) : 592;
+    minmax_kernel<<<nb, 256, 0, st>>>(d_pts, n, d_mm);
     MinMaxOrd ho;
     FLS_CUDA(cudaMemcpyAsync(&ho, d_mm, sizeof(ho), cudaMemcpyDeviceToHost, st));
     FLS_CUDA(cudaStreamSynchronize(st));
-    MinMax6 h;
-    for (int a = 0; a < 3; ++a) {
-        h.mn[a] = ord2f(ho.mn[a]);
-        h.mx[a] = ord2f(ho.mx[a]);
-    }
     if (launches) *launches += 2;
-    const long long dx = (long long)((h.mx[0] - h.mn[0]) * inv) + 1, dy = (long long)((h.mx[1] - h.mn[1]) * inv) + 1,
-                    dz = (long long)((h.mx[2] - h.mn[2]) * inv) + 1;
-    if (dx * dy * dz > 2147483647LL) {  // PCL: "Leaf size is too small" -> output = input
+    if (waits) *waits += 1;
+    const VgParams g = vg_params(ho, inv);
+    if (g.overflow) {  // PCL: "Leaf size is too small" -> output = input
         FLS_CUDA(cudaMemcpyAsync(d_out, d_pts, n * sizeof(float4), cudaMemcpyDeviceToDevice, st));
         return n;
     }
-    int minb[3], divb[3];
-    for (int a = 0; a < 3; ++a) {
-        minb[a] = (int)floorf(h.mn[a] * inv);
-        const int maxb = (int)floorf(h.mx[a] * inv);
-        divb[a] = maxb - minb[a] + 1;
-    }
-    const int mul1 = divb[0], mul2 = divb[0] * divb[1];
     sc.idx.reserve(n);
     sc.idx_sorted.reserve(n);
     sc.counts.reserve(n);
@@ -138,10 +92,10 @@ size_t voxel_grid_device(const float4* d_pts, size_t n, float leaf, float4* d_ou
     sc.k32a.reserve(n);
     sc.k32b.reserve(n);
     sc.uniq32.reserve(n);
-    vg_keys_kernel<<<grid_for(n, 256), 256, 0, st>>>(d_pts, n, inv, minb[0], minb[1], minb[2], mul1, mul2, sc.k32a.p, sc.idx.p);
+    vg_keys_kernel<<<grid_for(n, 256), 256, 0, st>>>(d_pts, n, inv, g, sc.k32a.p, sc.idx.p);
     int end_bit = 1;
     {
-        const long long maxid = (long long)divb[0] * divb[1] * divb[2];
+        const long long maxid = (long long)g.divb[0] * g.divb[1] * g.divb[2];
         while ((1LL << end_bit) < maxid && end_bit < 32) ++end_bit;
     }
     size_t t1 = 0, t2 = 0, t3 = 0;
@@ -157,6 +111,7 @@ size_t voxel_grid_device(const float4* d_pts, size_t n, float leaf, float4* d_ou
     FLS_CUDA(cub::DeviceRunLengthEncode::Encode(sc.cub_tmp.p, tb, sc.k32b.p, sc.uniq32.p, sc.counts.p, sc.num_runs.p, (int)n, st));
     FLS_CUDA(cudaMemcpyAsync(sc.h_num_runs, sc.num_runs.p, sizeof(int), cudaMemcpyDeviceToHost, st));
     FLS_CUDA(cudaStreamSynchronize(st));
+    if (waits) *waits += 1;
     const int runs = *sc.h_num_runs;
     tb = sc.cub_tmp.cap;
     FLS_CUDA(cub::DeviceScan::ExclusiveSum(sc.cub_tmp.p, tb, sc.counts.p, sc.starts.p, runs, st));

@@ -24,6 +24,9 @@
  *                                 (src/slam/preprocessing.cpp:262-571) and the scan's time window (:86-104)
  *   fls_preprocess_device /    <- fls_preprocess / fls_preprocess_loam reading a cloud already in device memory
  *   fls_preprocess_loam_device
+ *   fls_keyframes_*            <- the keyframe-map loops of System::SaveMap (src/slam/system.cpp:299-341),
+ *                                 System::VisualizeGlobalMap (src/slam/system.cpp:847-896) and
+ *                                 LoopClosure::GetSubMap (src/slam/loop_closure.cpp:179-231)
  *
  * Conventions
  *   * Points are read from caller memory as {float x, y, z, <pad>, intensity ...} records `stride_bytes`
@@ -417,6 +420,48 @@ int fls_preprocess_loam_device(const fls_loam_frontend_cfg* cfg, const float* d_
 int fls_preprocess_device(int device, const float* d_xyzi, const float* d_time, size_t n, const fls_imu_buffer* imu, float min_distance,
                           float max_distance, int32_t jump_span, float planar_leaf, float* ordered, float* d_ordered, size_t* n_ordered, float* planar,
                           float* d_planar, size_t* n_planar);
+
+/* ---- Keyframe maps on the device: System::SaveMap, System::VisualizeGlobalMap, LoopClosure::GetSubMap ---- */
+
+/* A device-resident store of keyframe clouds (the ordered_cloud_ every KeyFrame keeps, include/common/keyframe.h:31-74), separate from
+ * any fls_handle: upstream reads keyframes from the loop-closure thread, the visualization thread and the save-map service, none of
+ * which owns a matcher.  The store owns one CUDA stream and a mutex; calls from several host threads are serialized.  Clouds are held
+ * as packed float4 {x, y, z, intensity} in one arena of `capacity_points` records, fixed at creation.  Poses are not stored: every
+ * assemble call takes the current poses of its selection (upstream re-optimises them after each loop closure, system.cpp:711-717). */
+typedef struct fls_keyframes fls_keyframes;
+
+/* capacity_points in [1, 2^32 - 1]; FLS_ERR_NO_DEVICE when `device` is not a visible CUDA device. */
+int fls_keyframes_create(int device, size_t capacity_points, fls_keyframes** out);
+void fls_keyframes_destroy(fls_keyframes* s);
+/* Append keyframe `id`'s ordered cloud, as System keeps keyframes_ indexed by id (include/slam/system.h:187): ids are dense and
+ * appended in order, so `id` must equal the current count (else FLS_ERR_INVALID_ARG).  FLS_ERR_CAPACITY when the arena cannot take n
+ * more records (the store does not grow).  An empty cloud is a valid keyframe.  _add reads host records `stride_bytes` apart
+ * (FLS_LAYOUT_*); _add_device copies n packed float4 records from device memory on the store's device, e.g. the ordered or planar
+ * output of fls_preprocess_loam_device, so the cloud never passes through the host.  Both return once the copy is complete. */
+int fls_keyframes_add(fls_keyframes* s, int64_t id, const void* pts, size_t n, size_t stride_bytes);
+int fls_keyframes_add_device(fls_keyframes* s, int64_t id, const void* d_pts, size_t n);
+/* number of keyframes and of arena records in use (either pointer may be NULL) */
+int fls_keyframes_count(fls_keyframes* s, size_t* n_keyframes, size_t* n_points);
+/* map = [base] ++ concat_k TransformPointCloud(VoxelGridCloud(cloud[ids[k]], leaf), T[k]);  if final_leaf > 0: map = VoxelGridCloud(map,
+ * final_leaf).  This is the loop of System::SaveMap (src/slam/system.cpp:310-316, leaf = final_leaf = 0.3), of one round of
+ * System::VisualizeGlobalMap (src/slam/system.cpp:884-892, base = the running global_map, leaf = final_leaf = the visualization
+ * resolution) and of LoopClosure::GetSubMap (src/slam/loop_closure.cpp:217-230, leaf 0.2, no final pass).
+ *   ids / T_colmajor: n_ids keyframe ids (below the count; repeats allowed) and their poses, 16 doubles each (Eigen Mat4d memory).
+ *       The transform is TransformPointCloud's (include/common/pointcloud_utility.h:141-158): R and t cast to float first.
+ *   Each keyframe is filtered on its own; one whose extent overflows at `leaf` (PCL's dx*dy*dz > INT_MAX) keeps its points unchanged
+ *       and in input order, as PCL does.  The output is in selection order and, within a keyframe, in ascending cell order.
+ *   d_base / n_base: optional device records (packed float4, on the store's device) placed before the keyframes; they must not overlap
+ *       d_out.  Two caller buffers used in turn carry a running global map from one round to the next.
+ *   final_leaf: <= 0 for no final pass.
+ *   out (host) and / or d_out (device, on the store's device) receive the map; `capacity` is the room of each given buffer in records.
+ *       *n_out always receives the size of the map; when it exceeds `capacity` the call returns FLS_ERR_CAPACITY and writes nothing
+ *       (with both buffers NULL and capacity 0 this is a size query).
+ * Device inputs (d_base) must be complete when the call is made.  The number of host waits and kernel launches does not depend on
+ * n_ids.  stats (optional): gpu_ms, gpu_launches, h2d_bytes, d2h_bytes, n_source = records entering the per-keyframe pass, n_valid =
+ * records after it, iterations = the host waits (stream synchronisations) of the call.  FLS_ERR_CAPACITY also when the selection
+ * holds more than 2^31 - 1 records. */
+int fls_keyframes_assemble(fls_keyframes* s, const int64_t* ids, size_t n_ids, const double* T_colmajor, float leaf, float final_leaf,
+                           const void* d_base, size_t n_base, float* out, float* d_out, size_t capacity, size_t* n_out, fls_match_stats* stats);
 
 const char* fls_strerror(int status);
 const char* fls_last_error(void); /* thread-local text of the last CUDA failure */
