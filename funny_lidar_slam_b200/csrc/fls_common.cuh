@@ -6,6 +6,9 @@
 #include <stdint.h>
 
 #include <cstdio>
+#include <cstring>
+#include <mutex>
+#include <new>
 #include <string>
 
 #include "../../include/fls_b200.h"
@@ -25,6 +28,35 @@ struct CudaError { int status; };
             throw ::fls::CudaError{FLS_ERR_CUDA};                                                                   \
         }                                                                                                           \
     } while (0)
+
+// The error boundary of every extern "C" entry whose body can throw: a CUDA or host allocation failure becomes its status.
+#define FLS_TRY try {
+#define FLS_CATCH                                              \
+    }                                                          \
+    catch (const fls::CudaError& e) { return e.status; }       \
+    catch (const std::bad_alloc&) {                            \
+        fls::set_last_error("host allocation failed");         \
+        return FLS_ERR_CUDA;                                   \
+    }
+
+// per-device tables (workspaces, kernel attributes) have this many slots
+constexpr int kMaxDevices = 64;
+
+// FLS_OK when `device` is a visible CUDA device with a slot in the per-device tables, FLS_ERR_NO_DEVICE otherwise
+int check_device(int device);
+
+// caller record layouts: packed float4, or x y z at 0 / 4 / 8 and the intensity at 16 of a larger record
+inline bool stride_ok(size_t stride) { return stride == 16 || (stride >= 20 && stride % 4 == 0); }
+
+// clears *st (when given) and fills the call-level figures: device time from e0 to e1 (both complete), launches and copies
+inline void fill_call_stats(fls_match_stats* st, cudaEvent_t e0, cudaEvent_t e1, int launches, long long h2d, long long d2h) {
+    if (!st) return;
+    std::memset(st, 0, sizeof(*st));
+    FLS_CUDA(cudaEventElapsedTime(&st->gpu_ms, e0, e1));
+    st->gpu_launches = launches;
+    st->h2d_bytes = h2d;
+    st->d2h_bytes = d2h;
+}
 
 // ---- device buffer (grow-only) ------------------------------------------------------------------------
 template <typename T>
@@ -52,6 +84,58 @@ struct DevBuf {
     }
     size_t bytes() const { return cap * sizeof(T); }
 };
+
+// ---- pinned host buffer (grow-only): staging whose copies do not make the enqueue wait ------------------
+template <typename T>
+struct PinnedBuf {
+    T* p = nullptr;
+    size_t cap = 0;
+    PinnedBuf() = default;
+    PinnedBuf(const PinnedBuf&) = delete;
+    PinnedBuf& operator=(const PinnedBuf&) = delete;
+    ~PinnedBuf() { release(); }
+    void release() {
+        if (p) cudaFreeHost(p);
+        p = nullptr;
+        cap = 0;
+    }
+    // ensure capacity for n elements; contents are NOT preserved on growth
+    T* reserve(size_t n) {
+        if (n > cap) {
+            release();
+            size_t want = n + n / 4 + 64;
+            FLS_CUDA(cudaMallocHost(&p, want * sizeof(T)));
+            cap = want;
+        }
+        return p;
+    }
+};
+
+// ---- per-device workspaces of the handle-free entries ---------------------------------------------------
+// W derives from Workspace and adds its stage buffers.  There is one W per device and entry type, so a call takes only its own
+// entry's lock; buffers, stream and events survive across calls (allocating per call costs more than the kernels).
+struct Workspace {
+    std::mutex mu;
+    bool ready = false;
+    cudaStream_t st = nullptr;  // created on first use
+    cudaEvent_t e0 = nullptr, e1 = nullptr;
+};
+
+// Runs body(W&) on `device` (checked by check_device) under the workspace's lock.
+template <class W, class F>
+int with_workspace(int device, F&& body) {
+    static W ws[kMaxDevices];
+    W& w = ws[device];
+    std::lock_guard<std::mutex> lock(w.mu);
+    FLS_CUDA(cudaSetDevice(device));
+    if (!w.ready) {
+        FLS_CUDA(cudaStreamCreateWithFlags(&w.st, cudaStreamNonBlocking));
+        FLS_CUDA(cudaEventCreate(&w.e0));
+        FLS_CUDA(cudaEventCreate(&w.e1));
+        w.ready = true;
+    }
+    return body(w);
+}
 
 // ---- voxel keys / hash table ---------------------------------------------------------------------------
 // Hash slot = one 16-byte record so a probe is a single LDG.128:

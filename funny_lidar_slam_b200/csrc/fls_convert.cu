@@ -22,7 +22,6 @@
 #include <climits>
 #include <cmath>
 #include <cstring>
-#include <mutex>
 
 #include "fls_atan.cuh"
 #include "fls_frontend.h"
@@ -318,11 +317,7 @@ __global__ void __launch_bounds__(kWinThreads) conv_window_kernel(ConvParams p, 
     *res = r;
 }
 
-struct ConvWorkspace {
-    std::mutex mu;
-    bool ready = false;
-    cudaStream_t st = nullptr;
-    cudaEvent_t e0 = nullptr, e1 = nullptr;
+struct ConvWorkspace : Workspace {
     DevBuf<unsigned char> staging, cub_tmp, map, state;
     DevBuf<unsigned> flag, pos;
     DevBuf<int> small;  // [count][first_kept][go][first per ring: 256]
@@ -331,13 +326,9 @@ struct ConvWorkspace {
     DevBuf<float> time, yaw;
     DevBuf<unsigned short> key, key_sorted;
     DevBuf<fls_convert_result> res;
-    fls_convert_result* h_res = nullptr;  // pinned
-    int* h_count = nullptr;               // pinned
+    PinnedBuf<fls_convert_result> h_res;
+    PinnedBuf<int> h_count;
 };
-ConvWorkspace& conv_workspace(int device) {
-    static ConvWorkspace ws[64];
-    return ws[device & 63];
-}
 
 }  // namespace
 
@@ -377,20 +368,10 @@ int convert_cloud_device(const fls_convert_cfg& c, const fls_pointcloud2& m, flo
     if (stats) std::memset(stats, 0, sizeof(*stats));
     if (n == 0) return FLS_OK;  // upstream reads points.back() of the empty cloud here (DESIGN.md §8)
 
-    ConvWorkspace& w = conv_workspace(c.device);
-    std::lock_guard<std::mutex> lock(w.mu);
-    int rc = FLS_OK;
-    try {
-        FLS_CUDA(cudaSetDevice(c.device));
-        if (!w.ready) {
-            FLS_CUDA(cudaStreamCreateWithFlags(&w.st, cudaStreamNonBlocking));
-            FLS_CUDA(cudaEventCreate(&w.e0));
-            FLS_CUDA(cudaEventCreate(&w.e1));
-            FLS_CUDA(cudaMallocHost(&w.h_res, sizeof(fls_convert_result)));
-            FLS_CUDA(cudaMallocHost(&w.h_count, sizeof(int)));
-            w.ready = true;
-        }
+    return with_workspace<ConvWorkspace>(c.device, [&](ConvWorkspace& w) -> int {
         cudaStream_t st = w.st;
+        fls_convert_result* const h_res = w.h_res.reserve(1);
+        int* const h_count = w.h_count.reserve(1);
         long long h2d = 0, d2h = 0;
         int launches = 0;
         FLS_CUDA(cudaEventRecord(w.e0, st));
@@ -461,30 +442,22 @@ int convert_cloud_device(const fls_convert_cfg& c, const fls_pointcloud2& m, flo
         if (xyzi) FLS_CUDA(cudaMemcpyAsync(xyzi, ox, n * sizeof(float4), cudaMemcpyDeviceToHost, st));
         if (ring) FLS_CUDA(cudaMemcpyAsync(ring, orr, n * sizeof(int), cudaMemcpyDeviceToHost, st));
         if (time) FLS_CUDA(cudaMemcpyAsync(time, ot, n * sizeof(float), cudaMemcpyDeviceToHost, st));
-        FLS_CUDA(cudaMemcpyAsync(w.h_count, d_count, sizeof(int), cudaMemcpyDeviceToHost, st));
-        FLS_CUDA(cudaMemcpyAsync(w.h_res, w.res.p, sizeof(fls_convert_result), cudaMemcpyDeviceToHost, st));
+        FLS_CUDA(cudaMemcpyAsync(h_count, d_count, sizeof(int), cudaMemcpyDeviceToHost, st));
+        FLS_CUDA(cudaMemcpyAsync(h_res, w.res.p, sizeof(fls_convert_result), cudaMemcpyDeviceToHost, st));
         d2h += (long long)(n * ((xyzi ? 16 : 0) + (ring ? 4 : 0) + (time ? 4 : 0)) + sizeof(int) + sizeof(fls_convert_result));
         FLS_CUDA(cudaEventRecord(w.e1, st));
         FLS_CUDA(cudaStreamSynchronize(st));  // the only wait
-        const size_t cnt = (size_t)*w.h_count;
+        const size_t cnt = (size_t)*h_count;
         *n_out = cnt;
-        *res = *w.h_res;
+        *res = *h_res;
         if (stats) {
-            float ms = 0;
-            FLS_CUDA(cudaEventElapsedTime(&ms, w.e0, w.e1));
-            std::memset(stats, 0, sizeof(*stats));
-            stats->gpu_ms = ms;
-            stats->gpu_launches = launches;
-            stats->h2d_bytes = h2d;
-            stats->d2h_bytes = d2h;
+            fill_call_stats(stats, w.e0, w.e1, launches, h2d, d2h);
             stats->n_source = (long long)n;
             // the message read once, the outputs written once; the offsets read xyzi + ring and rewrite the times
             stats->algo_bytes = (long long)(n * m.point_step + cnt * 24 + (res->recomputed ? cnt * 24 : 0));
         }
-    } catch (const CudaError& e) {
-        rc = e.status;
-    }
-    return rc;
+        return FLS_OK;
+    });
 }
 
 }  // namespace fls

@@ -389,9 +389,9 @@ __global__ void feat_emit_kernel(const int* __restrict__ corner_out, const int* 
 // (every caller of enqueue_features holds its workspace lock already; this one is taken last and alone).
 void ensure_feat_smem(int device, size_t smem_sort, size_t smem_ring) {
     static std::mutex mu;
-    static size_t set[64][2];
+    static size_t set[kMaxDevices][2];
     std::lock_guard<std::mutex> lock(mu);
-    size_t* cur = set[device & 63];
+    size_t* cur = set[device];
     if (smem_sort <= cur[0] && smem_ring <= cur[1]) return;
     const int ss = (int)std::max(smem_sort, cur[0]), sr = (int)std::max(smem_ring, cur[1]);
     FLS_CUDA(cudaFuncSetAttribute(feat_sort_kernel<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, ss));
@@ -408,23 +408,13 @@ void launch_feat(const RingArgs& a, size_t smem_sort, size_t smem_ring, cudaStre
     feat_ring_kernel<BLOCK><<<a.n_rows, BLOCK, smem_ring, st>>>(a);
 }
 
-// Per-device workspace of fls_extract_features: stream, events, device buffers and pinned staging survive across calls (the
-// extractor runs once per scan; allocating per call cost more than the kernels).  Calls on one device are serialised by the mutex.
-struct FeatWorkspace {
-    std::mutex mu;
-    bool ready = false;
-    cudaStream_t st = nullptr;
-    cudaEvent_t e0 = nullptr, e1 = nullptr, k0 = nullptr, k1 = nullptr;
+struct FeatWorkspace : Workspace {
+    cudaEvent_t k0 = nullptr, k1 = nullptr;  // around the kernels (created on first use)
     DevBuf<float> d_depth;
     DevBuf<int> d_col, d_rows, d_idx;
     FeatStage s;
-    int* h_out = nullptr;  // pinned: [n_corner, n_planar][indices]
-    size_t h_cap = 0;
+    PinnedBuf<int> h_out;  // [n_corner, n_planar][indices]
 };
-FeatWorkspace& workspace(int device) {
-    static FeatWorkspace ws[64];
-    return ws[device & 63];
-}
 
 }  // namespace
 
@@ -511,22 +501,13 @@ int extract_features_device(int device, const float* depth, const int* col, size
     *n_corner = 0;
     *n_planar = 0;
     if (n < 12 || n_rows <= 0) return FLS_OK;
-    if (device < 0 || device >= 64) return FLS_ERR_INVALID_ARG;
     FeatPlan p;
     const int prc = plan_features(row_start, row_end, n_rows, n, p);
     if (prc != FLS_OK) return prc;
-    FeatWorkspace& w = workspace(device);
-    std::lock_guard<std::mutex> lock(w.mu);
-    int rc = FLS_OK;
-    try {
-        FLS_CUDA(cudaSetDevice(device));
-        if (!w.ready) {
-            FLS_CUDA(cudaStreamCreateWithFlags(&w.st, cudaStreamNonBlocking));
-            FLS_CUDA(cudaEventCreate(&w.e0));
-            FLS_CUDA(cudaEventCreate(&w.e1));
+    return with_workspace<FeatWorkspace>(device, [&](FeatWorkspace& w) -> int {
+        if (!w.k1) {
             FLS_CUDA(cudaEventCreate(&w.k0));
             FLS_CUDA(cudaEventCreate(&w.k1));
-            w.ready = true;
         }
         cudaStream_t st = w.st;
         const size_t idx_cap = (size_t)n_rows * 120 + p.planar_cap;
@@ -534,13 +515,7 @@ int extract_features_device(int device, const float* depth, const int* col, size
         w.d_col.reserve(n);
         w.d_rows.reserve((size_t)n_rows * 2);
         w.d_idx.reserve(idx_cap);
-        if (idx_cap + 2 > w.h_cap) {
-            if (w.h_out) cudaFreeHost(w.h_out);
-            w.h_out = nullptr;
-            w.h_cap = 0;
-            FLS_CUDA(cudaMallocHost(&w.h_out, (idx_cap + 2) * 2 * sizeof(int)));
-            w.h_cap = (idx_cap + 2) * 2;
-        }
+        int* const h_out = w.h_out.reserve(idx_cap + 2);
         FLS_CUDA(cudaEventRecord(w.e0, st));
         FLS_CUDA(cudaMemcpyAsync(w.d_depth.p, depth, n * 4, cudaMemcpyHostToDevice, st));
         FLS_CUDA(cudaMemcpyAsync(w.d_col.p, col, n * 4, cudaMemcpyHostToDevice, st));
@@ -550,35 +525,26 @@ int extract_features_device(int device, const float* depth, const int* col, size
         const int* d_tot = enqueue_features(w.s, p, device, w.d_depth.p, w.d_col.p, w.d_rows.p, corner_thr, planar_thr, nullptr, w.d_idx.p, nullptr,
                                             nullptr, st);
         FLS_CUDA(cudaEventRecord(w.k1, st));
-        FLS_CUDA(cudaMemcpyAsync(w.h_out, d_tot, 2 * sizeof(int), cudaMemcpyDeviceToHost, st));
+        FLS_CUDA(cudaMemcpyAsync(h_out, d_tot, 2 * sizeof(int), cudaMemcpyDeviceToHost, st));
         FLS_CUDA(cudaStreamSynchronize(st));  // the two counts size the read-back
-        const size_t nc = (size_t)w.h_out[0], np = (size_t)w.h_out[1];
-        if (nc + np) FLS_CUDA(cudaMemcpyAsync(w.h_out + 2, w.d_idx.p, (nc + np) * 4, cudaMemcpyDeviceToHost, st));
+        const size_t nc = (size_t)h_out[0], np = (size_t)h_out[1];
+        if (nc + np) FLS_CUDA(cudaMemcpyAsync(h_out + 2, w.d_idx.p, (nc + np) * 4, cudaMemcpyDeviceToHost, st));
         FLS_CUDA(cudaEventRecord(w.e1, st));
         FLS_CUDA(cudaStreamSynchronize(st));
-        std::memcpy(corner_idx, w.h_out + 2, nc * 4);
-        std::memcpy(planar_idx, w.h_out + 2 + nc, np * 4);
+        std::memcpy(corner_idx, h_out + 2, nc * 4);
+        std::memcpy(planar_idx, h_out + 2 + nc, np * 4);
         *n_corner = nc;
         *n_planar = np;
         if (stats) {
-            float ms = 0, kms = 0;
-            FLS_CUDA(cudaEventElapsedTime(&ms, w.e0, w.e1));
-            FLS_CUDA(cudaEventElapsedTime(&kms, w.k0, w.k1));
-            std::memset(stats, 0, sizeof(*stats));
-            stats->gpu_ms = ms;
-            stats->kernel_ms = kms;
+            fill_call_stats(stats, w.e0, w.e1, kFeatLaunches, (long long)(n * 8 + (size_t)n_rows * 8), (long long)(2 + nc + np) * 4);
+            FLS_CUDA(cudaEventElapsedTime(&stats->kernel_ms, w.k0, w.k1));
             stats->kernel_launches = kFeatLaunches;
-            stats->gpu_launches = kFeatLaunches;
             stats->n_source = (long long)n;
-            stats->h2d_bytes = (long long)(n * 8 + (size_t)n_rows * 8);
-            stats->d2h_bytes = (long long)(2 + nc + np) * 4;
             // algorithmic bytes: depth + col in, roughness/meta/sort keys written and read once, indices out
             stats->algo_bytes = feature_algo_bytes(n, nc, np);
         }
-    } catch (const CudaError& e) {
-        rc = e.status;
-    }
-    return rc;
+        return FLS_OK;
+    });
 }
 
 }  // namespace fls

@@ -2,32 +2,20 @@
 // PointcloudProjector::Project with the per-point de-skew -> FeatureExtractor::ExtractFeatures -> corner_voxel_filter_ and
 // planer_voxel_filter_.  The stages are the ones behind fls_project_imu, fls_extract_features and fls_voxel_grid (fls_frontend.h);
 // point data stays on the device between them.  The host reads back only the sizes that shape a later launch (DESIGN.md §3.8).
-#include <cstring>
-#include <mutex>
-
 #include "fls_frontend.h"
 
 namespace fls {
 namespace {
 
-// One workspace per device, with stage buffers of its own: the call takes this lock only (never the projector's or the
-// extractor's), so it cannot deadlock against them.
-struct LoamWorkspace {
-    std::mutex mu;
-    bool ready = false;
-    cudaStream_t st = nullptr;
-    cudaEvent_t e0 = nullptr, e1 = nullptr;
+// Stage buffers of its own: the call takes its workspace's lock only (never the projector's or the extractor's), so it cannot
+// deadlock against them.
+struct LoamWorkspace : Workspace {
     ProjStage proj;
     FeatStage feat;
     BuildScratch vg;
     DevBuf<float4> corner, planar, corner_f, planar_f;  // gathered features, filtered clouds (when the caller gives no device output)
-    int* h_small = nullptr;                              // pinned: [n_ordered][row_start V][row_end V] or [n_corner, n_planar]
-    size_t h_cap = 0;
+    PinnedBuf<int> h_small;                              // [n_ordered][row_start V][row_end V] or [n_corner, n_planar]
 };
-LoamWorkspace& loam_workspace(int device) {
-    static LoamWorkspace ws[64];
-    return ws[device & 63];
-}
 
 }  // namespace
 
@@ -36,39 +24,23 @@ int preprocess_loam_device(const fls_loam_frontend_cfg& c, const void* raw, cons
                            size_t* n_planar, fls_match_stats* stats, bool src_on_device) {
     *n_corner = *n_planar = 0;
     const int V = c.n_rows, H = c.n_cols;
-    LoamWorkspace& w = loam_workspace(c.device);
-    std::lock_guard<std::mutex> lock(w.mu);
-    int rc = FLS_OK;
-    try {
-        FLS_CUDA(cudaSetDevice(c.device));
-        if (!w.ready) {
-            FLS_CUDA(cudaStreamCreateWithFlags(&w.st, cudaStreamNonBlocking));
-            FLS_CUDA(cudaEventCreate(&w.e0));
-            FLS_CUDA(cudaEventCreate(&w.e1));
-            w.ready = true;
-        }
+    return with_workspace<LoamWorkspace>(c.device, [&](LoamWorkspace& w) -> int {
         cudaStream_t st = w.st;
-        if ((size_t)2 * V + 1 > w.h_cap) {
-            if (w.h_small) cudaFreeHost(w.h_small);
-            w.h_small = nullptr;
-            w.h_cap = 0;
-            FLS_CUDA(cudaMallocHost(&w.h_small, ((size_t)2 * V + 1) * sizeof(int)));
-            w.h_cap = (size_t)2 * V + 1;
-        }
+        int* const h_small = w.h_small.reserve((size_t)2 * V + 1);
         long long h2d = 0, d2h = 0;
         int launches = 0;
         FLS_CUDA(cudaEventRecord(w.e0, st));
         // ---- projector (+ de-skew) ----
-        rc = enqueue_project(w.proj, raw, ring, time, imu, n, stride, V, H, c.horizontal_resolution, c.min_distance, c.max_distance, st, &h2d, &launches, src_on_device);
+        int rc = enqueue_project(w.proj, raw, ring, time, imu, n, stride, V, H, c.horizontal_resolution, c.min_distance, c.max_distance, st, &h2d, &launches, src_on_device);
         if (rc != FLS_OK) return rc;
         // sync 1: n_ordered and the row bounds size the feature kernels (shared memory, planar capacity)
-        FLS_CUDA(cudaMemcpyAsync(w.h_small, w.proj.total.p, sizeof(int), cudaMemcpyDeviceToHost, st));
-        FLS_CUDA(cudaMemcpyAsync(w.h_small + 1, w.proj.rows.p, (size_t)2 * V * sizeof(int), cudaMemcpyDeviceToHost, st));
+        FLS_CUDA(cudaMemcpyAsync(h_small, w.proj.total.p, sizeof(int), cudaMemcpyDeviceToHost, st));
+        FLS_CUDA(cudaMemcpyAsync(h_small + 1, w.proj.rows.p, (size_t)2 * V * sizeof(int), cudaMemcpyDeviceToHost, st));
         FLS_CUDA(cudaStreamSynchronize(st));
         d2h += (long long)((2 * (size_t)V + 1) * sizeof(int));
-        const size_t n_ord = (size_t)(unsigned)w.h_small[0];
+        const size_t n_ord = (size_t)(unsigned)h_small[0];
         FeatPlan p;
-        rc = plan_features(w.h_small + 1, w.h_small + 1 + V, V, n_ord, p);
+        rc = plan_features(h_small + 1, h_small + 1 + V, V, n_ord, p);
         if (rc != FLS_OK) return rc;  // a ring or block beyond the shared-memory working set: FLS_ERR_UNSUPPORTED, nothing written
         // ---- features, gathered into two contiguous clouds ----
         size_t nc = 0, np = 0;
@@ -79,11 +51,11 @@ int preprocess_loam_device(const fls_loam_frontend_cfg& c, const void* raw, cons
                                                 w.proj.ordered.p, nullptr, w.corner.p, w.planar.p, st);
             launches += kFeatLaunches;
             // sync 2: the feature counts size the voxel filters
-            FLS_CUDA(cudaMemcpyAsync(w.h_small, d_tot, 2 * sizeof(int), cudaMemcpyDeviceToHost, st));
+            FLS_CUDA(cudaMemcpyAsync(h_small, d_tot, 2 * sizeof(int), cudaMemcpyDeviceToHost, st));
             FLS_CUDA(cudaStreamSynchronize(st));
             d2h += 2 * sizeof(int);
-            nc = (size_t)w.h_small[0];
-            np = (size_t)w.h_small[1];
+            nc = (size_t)h_small[0];
+            np = (size_t)h_small[1];
         }
         // ---- voxel filters (syncs 3-6: bounding box and run count of each), straight into the caller's device buffers ----
         float4* oc = d_corner ? reinterpret_cast<float4*>(d_corner) : w.corner_f.reserve(nc + 1);
@@ -98,22 +70,14 @@ int preprocess_loam_device(const fls_loam_frontend_cfg& c, const void* raw, cons
         *n_corner = mc;
         *n_planar = mp;
         if (stats) {
-            float ms = 0;
-            FLS_CUDA(cudaEventElapsedTime(&ms, w.e0, w.e1));
-            std::memset(stats, 0, sizeof(*stats));
-            stats->gpu_ms = ms;
-            stats->gpu_launches = launches;
-            stats->h2d_bytes = h2d;
-            stats->d2h_bytes = d2h;
+            fill_call_stats(stats, w.e0, w.e1, launches, h2d, d2h);
             stats->n_source = (long long)n;
             const bool with_time = imu && imu->n_imu && time;
             stats->algo_bytes = project_algo_bytes(n, with_time, n_ord) + (p.active ? feature_algo_bytes(n_ord, nc, np) : 0) +
                                 voxel_algo_bytes(nc, mc) + voxel_algo_bytes(np, mp);
         }
-    } catch (const CudaError& e) {
-        rc = e.status;
-    }
-    return rc;
+        return FLS_OK;
+    });
 }
 
 }  // namespace fls

@@ -18,7 +18,6 @@ struct Handle {
     // per-call accounting (fls_match_stats)
     int launches = 0;
     long long h2d_bytes = 0, d2h_bytes = 0;
-    float last_gpu_ms = 0.f;
 
     // scan-side buffers
     DevBuf<unsigned char> raw;  // strided caller records before repacking
@@ -31,8 +30,7 @@ struct Handle {
     DevBuf<unsigned> tickets;   // chunk ticket counters of the LOAM-iVox kernel (dynamic work distribution)
     DevBuf<uint4> ll_rows;      // LL hand-over records of the persistent LOAM-iVox kernel: [grid][32] rows + pose record
     unsigned match_epoch = 0;   // tag prefix of those records
-    unsigned char* h_batch = nullptr;  // pinned staging of the per-batch tables (poses, offsets, scan descriptors, CTA map, pointers)
-    size_t h_batch_cap = 0;
+    PinnedBuf<unsigned char> h_batch;  // staging of the per-batch tables (poses, offsets, scan descriptors, CTA map, pointers)
     DevBuf<unsigned char> d_batch;
     DevBuf<GnState> state;
     GnState* h_state = nullptr;  // pinned

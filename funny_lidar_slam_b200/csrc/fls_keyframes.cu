@@ -126,8 +126,7 @@ struct KeyframeStore {
     std::vector<unsigned> count;            // per keyframe id: records
     // per-call scratch
     DevBuf<unsigned char> table, raw;
-    unsigned char* h_table = nullptr;  // pinned staging of the per-call table
-    size_t h_table_cap = 0;
+    PinnedBuf<unsigned char> h_table;  // staging of the per-call table
     DevBuf<float4> cat, fin;
     BuildScratch sc;  // segmented pass (keys, keys_sorted, uniq, idx, idx_sorted, counts, starts, cub_tmp, num_runs)
     BuildScratch vg;  // final voxel_grid_device pass
@@ -146,25 +145,14 @@ struct KeyframeStore {
     }
     ~KeyframeStore() { release(); }
     void release() {
-        if (h_table) cudaFreeHost(h_table);
+        h_table.release();
         if (arena) cudaFree(arena);
         if (ev0) cudaEventDestroy(ev0);
         if (ev1) cudaEventDestroy(ev1);
         if (stream) cudaStreamDestroy(stream);
-        h_table = nullptr;
         arena = nullptr;
         ev0 = ev1 = nullptr;
         stream = nullptr;
-    }
-    unsigned char* host_table(size_t bytes) {
-        if (bytes > h_table_cap) {
-            if (h_table) cudaFreeHost(h_table);
-            h_table = nullptr;
-            h_table_cap = 0;
-            FLS_CUDA(cudaMallocHost(&h_table, bytes + bytes / 4 + 256));
-            h_table_cap = bytes + bytes / 4 + 256;
-        }
-        return h_table;
     }
 
     int add(long long id, const void* pts, size_t n, size_t stride, bool on_device) {
@@ -176,13 +164,10 @@ struct KeyframeStore {
             float4* dst = arena + used;
             if (on_device) {
                 FLS_CUDA(cudaMemcpyAsync(dst, pts, n * sizeof(float4), cudaMemcpyDeviceToDevice, stream));
-            } else if (stride == 16) {
-                FLS_CUDA(cudaMemcpyAsync(dst, pts, n * sizeof(float4), cudaMemcpyHostToDevice, stream));
             } else {
-                raw.reserve(n * stride);
-                FLS_CUDA(cudaMemcpyAsync(raw.p, pts, n * stride, cudaMemcpyHostToDevice, stream));
-                launch_repack(raw.p, n, stride, dst, stream);
-                FLS_CUDA(cudaGetLastError());
+                long long h2d = 0;  // the store reports no figures for an add
+                int launches = 0;
+                upload_records(pts, n, stride, dst, raw, stream, &h2d, &launches);
             }
             FLS_CUDA(cudaStreamSynchronize(stream));
         }
@@ -219,7 +204,7 @@ struct KeyframeStore {
             // one upload: [segments | empty bounding boxes | tiles]
             const size_t off_mm = align16(K * sizeof(KfSeg)), off_tiles = align16(off_mm + K * sizeof(MinMaxOrd));
             const size_t bytes = off_tiles + n_tiles * sizeof(KfTile);
-            unsigned char* h = host_table(bytes);
+            unsigned char* h = h_table.reserve(bytes);
             KfSeg* hs = reinterpret_cast<KfSeg*>(h);
             MinMaxOrd* hm = reinterpret_cast<MinMaxOrd*>(h + off_mm);
             KfTile* ht = reinterpret_cast<KfTile*>(h + off_tiles);
@@ -318,12 +303,8 @@ struct KeyframeStore {
         ++waits;
         *n_out = m;
         if (stats) {
-            std::memset(stats, 0, sizeof(*stats));
-            FLS_CUDA(cudaEventElapsedTime(&stats->gpu_ms, ev0, ev1));
-            stats->gpu_launches = launches;
+            fill_call_stats(stats, ev0, ev1, launches, h2d, d2h);
             stats->iterations = waits;
-            stats->h2d_bytes = h2d;
-            stats->d2h_bytes = d2h;
             stats->n_source = (int64_t)N;
             stats->n_valid = (int64_t)runs;
         }
@@ -333,29 +314,17 @@ struct KeyframeStore {
 
 }  // namespace fls
 
-#define FLS_KF_TRY try {
-#define FLS_KF_CATCH                                           \
-    }                                                          \
-    catch (const fls::CudaError& e) { return e.status; }       \
-    catch (const std::bad_alloc&) {                            \
-        fls::set_last_error("host allocation failed");         \
-        return FLS_ERR_CUDA;                                   \
-    }
-
-static bool kf_stride_ok(size_t stride) { return stride == 16 || (stride >= 20 && stride % 4 == 0); }
-
 extern "C" {
 
 int fls_keyframes_create(int device, size_t capacity_points, fls_keyframes** out) {
     if (!out) return FLS_ERR_INVALID_ARG;
     *out = nullptr;
     if (capacity_points == 0 || capacity_points > 0xffffffffull) return FLS_ERR_INVALID_ARG;
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0 || device < 0 || device >= ndev) return FLS_ERR_NO_DEVICE;
-    FLS_KF_TRY
+    if (fls::check_device(device) != FLS_OK) return FLS_ERR_NO_DEVICE;
+    FLS_TRY
     *out = reinterpret_cast<fls_keyframes*>(new fls::KeyframeStore(device, capacity_points));
     return FLS_OK;
-    FLS_KF_CATCH
+    FLS_CATCH
 }
 
 void fls_keyframes_destroy(fls_keyframes* s) {
@@ -366,26 +335,28 @@ void fls_keyframes_destroy(fls_keyframes* s) {
 }
 
 int fls_keyframes_add(fls_keyframes* s, int64_t id, const void* pts, size_t n, size_t stride_bytes) {
-    if (!s || (!pts && n) || !kf_stride_ok(stride_bytes)) return FLS_ERR_INVALID_ARG;
-    FLS_KF_TRY
+    if (!s || (!pts && n) || !fls::stride_ok(stride_bytes)) return FLS_ERR_INVALID_ARG;
+    FLS_TRY
     return reinterpret_cast<fls::KeyframeStore*>(s)->add(id, pts, n, stride_bytes, false);
-    FLS_KF_CATCH
+    FLS_CATCH
 }
 
 int fls_keyframes_add_device(fls_keyframes* s, int64_t id, const void* d_pts, size_t n) {
     if (!s || (!d_pts && n)) return FLS_ERR_INVALID_ARG;
-    FLS_KF_TRY
+    FLS_TRY
     return reinterpret_cast<fls::KeyframeStore*>(s)->add(id, d_pts, n, FLS_LAYOUT_PACKED, true);
-    FLS_KF_CATCH
+    FLS_CATCH
 }
 
 int fls_keyframes_count(fls_keyframes* s, size_t* n_keyframes, size_t* n_points) {
     fls::KeyframeStore* k = reinterpret_cast<fls::KeyframeStore*>(s);
     if (!k) return FLS_ERR_INVALID_ARG;
+    FLS_TRY
     std::lock_guard<std::mutex> lk(k->mu);
     if (n_keyframes) *n_keyframes = k->count.size();
     if (n_points) *n_points = k->used;
     return FLS_OK;
+    FLS_CATCH
 }
 
 int fls_keyframes_assemble(fls_keyframes* s, const int64_t* ids, size_t n_ids, const double* T_colmajor, float leaf, float final_leaf,
@@ -398,10 +369,10 @@ int fls_keyframes_assemble(fls_keyframes* s, const int64_t* ids, size_t n_ids, c
         const uintptr_t b0 = (uintptr_t)d_base, b1 = b0 + n_base * 16, o0 = (uintptr_t)d_out, o1 = o0 + capacity * 16;
         if (b0 < o1 && o0 < b1) return FLS_ERR_INVALID_ARG;
     }
-    FLS_KF_TRY
+    FLS_TRY
     return reinterpret_cast<fls::KeyframeStore*>(s)->assemble(ids, n_ids, T_colmajor, leaf, final_leaf, reinterpret_cast<const float4*>(d_base),
                                                               n_base, out, reinterpret_cast<float4*>(d_out), capacity, n_out, stats);
-    FLS_KF_CATCH
+    FLS_CATCH
 }
 
 }  // extern "C"

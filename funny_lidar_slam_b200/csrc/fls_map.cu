@@ -297,9 +297,24 @@ void launch_transform_d(const float4* d_in, size_t n, const double* T, float4* d
     transform_d_kernel<<<grid_for(n, 256), 256, 0, st>>>(d_in, n, T[0], T[4], T[8], T[1], T[5], T[9], T[2], T[6], T[10], T[12], T[13], T[14], d_out);
 }
 
-void launch_repack(const unsigned char* d_raw, size_t n, size_t stride, float4* d_out, cudaStream_t st) {
+static void launch_repack(const unsigned char* d_raw, size_t n, size_t stride, float4* d_out, cudaStream_t st) {
     if (n == 0) return;
     repack_kernel<<<grid_for(n, 256), 256, 0, st>>>(d_raw, n, stride, d_out);
+}
+
+void upload_records(const void* pts, size_t n, size_t stride, float4* dst, DevBuf<unsigned char>& staging, cudaStream_t st, long long* h2d,
+                    int* launches) {
+    if (n == 0) return;
+    if (stride == FLS_LAYOUT_PACKED) {
+        FLS_CUDA(cudaMemcpyAsync(dst, pts, n * 16, cudaMemcpyHostToDevice, st));
+    } else {
+        staging.reserve(n * stride);  // stream order: the previous repack out of `staging` has run before this copy lands
+        FLS_CUDA(cudaMemcpyAsync(staging.p, pts, n * stride, cudaMemcpyHostToDevice, st));
+        launch_repack(staging.p, n, stride, dst, st);
+        FLS_CUDA(cudaGetLastError());
+        ++*launches;
+    }
+    *h2d += (long long)(n * stride);
 }
 
 void launch_transform_f(const float4* d_in, size_t n, const double* T, float4* d_out, cudaStream_t st) {

@@ -176,7 +176,10 @@ int project_device(int device, const void* raw, const int* ring, const float* ti
 // PreProcessing::Run, non-feature branch (preprocessing.cpp:181-225): raw x,y,z,intensity,time records -> ordered + planar clouds (host)
 int preprocess_device(int device, const float* raw_xyzit, size_t n, const fls_imu_buffer* imu, float min_d, float max_d, int jump_span, float leaf,
                       float* ordered_out, size_t* n_ordered, float* planar_out, size_t* n_planar);
-void launch_repack(const unsigned char* d_raw, size_t n, size_t stride, float4* d_out, cudaStream_t st);
+// Copies n host records of `stride` bytes (stride_ok) to packed float4 at dst on st: one copy when they are packed already, else a
+// copy to `staging` and one repack kernel.  Adds the bytes copied to *h2d and the kernel to *launches.
+void upload_records(const void* pts, size_t n, size_t stride, float4* dst, DevBuf<unsigned char>& staging, cudaStream_t st, long long* h2d,
+                    int* launches);
 // TransformPointCloud(cloud, Mat4d) with R, t cast to float first (pointcloud_utility.h:141-158 upstream); T column-major
 void launch_transform_f(const float4* d_in, size_t n, const double* T_colmajor, float4* d_out, cudaStream_t st);
 void launch_transform_d(const float4* d_in, size_t n, const double* T_colmajor, float4* d_out, cudaStream_t st);

@@ -7,7 +7,6 @@
 #include <cub/cub.cuh>
 
 #include <cmath>
-#include <mutex>
 
 #include "fls_deskew.cuh"
 #include "fls_frontend.h"
@@ -67,10 +66,7 @@ __global__ void pp_scatter_kernel(const float4* __restrict__ corrected, int n, c
     if (i < n && f[i]) out[excl[i]] = corrected[i];
 }
 
-struct PpWorkspace {
-    std::mutex mu;
-    bool ready = false;
-    cudaStream_t st = nullptr;
+struct PpWorkspace : Workspace {
     DevBuf<float> raw;
     DevBuf<float4> corrected, ordered, planar, filtered;
     DevBuf<unsigned> f_ord, f_pl, e_ord, e_pl;
@@ -79,10 +75,6 @@ struct PpWorkspace {
     DevBuf<unsigned char> cub_tmp;
     BuildScratch scratch;
 };
-PpWorkspace& pp_workspace(int device) {
-    static PpWorkspace ws[64];
-    return ws[device & 63];
-}
 
 }  // namespace
 
@@ -113,20 +105,12 @@ int run_preprocess(int device, const float* xyzi, const float* time, bool src_on
                    int jump_span, float leaf, float* ordered_out, float* d_ordered, size_t* n_ordered, float* planar_out, float* d_planar,
                    size_t* n_planar) {
     *n_ordered = *n_planar = 0;
-    if (device < 0 || device >= 64 || n > 0x7fffffffull || jump_span < 1 || !(leaf > 0.f)) return FLS_ERR_INVALID_ARG;
+    if (n > 0x7fffffffull || jump_span < 1 || !(leaf > 0.f)) return FLS_ERR_INVALID_ARG;
     if (n == 0) return FLS_OK;
-    PpWorkspace& w = pp_workspace(device);
-    std::lock_guard<std::mutex> lock(w.mu);
-    int rc = FLS_OK;
-    try {
-        FLS_CUDA(cudaSetDevice(device));
-        if (!w.ready) {
-            FLS_CUDA(cudaStreamCreateWithFlags(&w.st, cudaStreamNonBlocking));
-            w.ready = true;
-        }
+    return with_workspace<PpWorkspace>(device, [&](PpWorkspace& w) -> int {
         cudaStream_t st = w.st;
         DeskewView dv;
-        rc = make_deskew_view(imu, w.imu_t, w.imu_q, st, dv);
+        const int rc = make_deskew_view(imu, w.imu_t, w.imu_q, st, dv);
         if (rc != FLS_OK) return rc == FLS_ERR_INVALID_ARG && imu && imu->n_imu ? FLS_OK : rc;  // SetRefTime failed: upstream drops the scan (:178-183) -> empty clouds
         w.corrected.reserve(n);
         float4* ord = d_ordered ? reinterpret_cast<float4*>(d_ordered) : w.ordered.reserve(n);
@@ -170,10 +154,8 @@ int run_preprocess(int device, const float* xyzi, const float* time, bool src_on
         FLS_CUDA(cudaStreamSynchronize(st));
         *n_ordered = no;
         *n_planar = nf;
-    } catch (const CudaError& e) {
-        rc = e.status;
-    }
-    return rc;
+        return FLS_OK;
+    });
 }
 
 }  // namespace

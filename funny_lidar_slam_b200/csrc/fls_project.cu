@@ -9,8 +9,6 @@
 // (fls_project_imu; fls_deskew.cuh); without one the points pass through unchanged.
 #include <cub/cub.cuh>
 
-#include <mutex>
-
 #include "fls_atan.cuh"
 #include "fls_deskew.cuh"
 #include "fls_frontend.h"
@@ -76,16 +74,9 @@ __global__ void proj_emit_kernel(const float4* __restrict__ raw, const float* __
     }
 }
 
-struct ProjWorkspace {
-    std::mutex mu;
-    bool ready = false;
-    cudaStream_t st = nullptr;
+struct ProjWorkspace : Workspace {
     ProjStage s;
 };
-ProjWorkspace& proj_workspace(int device) {
-    static ProjWorkspace ws[64];
-    return ws[device & 63];
-}
 
 }  // namespace
 
@@ -121,16 +112,9 @@ int enqueue_project(ProjStage& w, const void* raw, const int* ring, const float*
     w.col.reserve(cells);
     w.rows.reserve((size_t)V * 2);
     if (n && !src_on_device) {
-        if (stride == FLS_LAYOUT_PACKED) {
-            FLS_CUDA(cudaMemcpyAsync(w.raw.p, raw, n * sizeof(float4), cudaMemcpyHostToDevice, st));
-        } else {
-            w.staging.reserve(n * stride);
-            FLS_CUDA(cudaMemcpyAsync(w.staging.p, raw, n * stride, cudaMemcpyHostToDevice, st));
-            launch_repack(w.staging.p, n, stride, w.raw.p, st);
-            ++*launches;
-        }
+        upload_records(raw, n, stride, w.raw.p, w.staging, st, h2d, launches);
         FLS_CUDA(cudaMemcpyAsync(w.ring.p, ring, n * sizeof(int), cudaMemcpyHostToDevice, st));
-        *h2d += (long long)(n * (stride + sizeof(int)));
+        *h2d += (long long)(n * sizeof(int));
     }
     const unsigned gc = (unsigned)((cells + 255) / 256);
     proj_clear_kernel<<<gc, 256, 0, st>>>(w.winner.p, cells);
@@ -155,23 +139,15 @@ int enqueue_project(ProjStage& w, const void* raw, const int* ring, const float*
 int project_device(int device, const void* raw, const int* ring, const float* time, const fls_imu_buffer* imu, size_t n, size_t stride, int V, int H,
                    float h_res, float min_d, float max_d, float* ordered_out, float* depth_out, int* col_out, int* row_start, int* row_end, size_t* n_out) {
     *n_out = 0;
-    if (V <= 0 || H <= 0 || !(h_res > 0.f) || device < 0 || device >= 64 || n > 0x7fffffffull) return FLS_ERR_INVALID_ARG;
+    if (V <= 0 || H <= 0 || !(h_res > 0.f) || n > 0x7fffffffull) return FLS_ERR_INVALID_ARG;
     const size_t cells = (size_t)V * H;
     if (cells > 0x7fffffffull) return FLS_ERR_INVALID_ARG;
-    ProjWorkspace& ws = proj_workspace(device);
-    std::lock_guard<std::mutex> lock(ws.mu);
-    int rc = FLS_OK;
-    try {
-        FLS_CUDA(cudaSetDevice(device));
-        if (!ws.ready) {
-            FLS_CUDA(cudaStreamCreateWithFlags(&ws.st, cudaStreamNonBlocking));
-            ws.ready = true;
-        }
+    return with_workspace<ProjWorkspace>(device, [&](ProjWorkspace& ws) -> int {
         cudaStream_t st = ws.st;
         ProjStage& w = ws.s;
         long long h2d = 0;
         int launches = 0;
-        rc = enqueue_project(w, raw, ring, time, imu, n, stride, V, H, h_res, min_d, max_d, st, &h2d, &launches, false);
+        const int rc = enqueue_project(w, raw, ring, time, imu, n, stride, V, H, h_res, min_d, max_d, st, &h2d, &launches, false);
         if (rc != FLS_OK) return rc;
         unsigned total = 0;
         FLS_CUDA(cudaMemcpyAsync(&total, w.total.p, sizeof(total), cudaMemcpyDeviceToHost, st));
@@ -182,10 +158,8 @@ int project_device(int device, const void* raw, const int* ring, const float* ti
         FLS_CUDA(cudaStreamSynchronize(st));
         if (total) FLS_CUDA(cudaMemcpy(ordered_out, w.ordered.p, (size_t)total * sizeof(float4), cudaMemcpyDeviceToHost));
         *n_out = total;
-    } catch (const CudaError& e) {
-        rc = e.status;
-    }
-    return rc;
+        return FLS_OK;
+    });
 }
 
 }  // namespace fls
