@@ -71,6 +71,11 @@ class FlsMapInfo(C.Structure):
                 ("incremental_inserts", C.c_int64), ("full_builds", C.c_int64)]
 
 
+class FlsNdtVoxel(C.Structure):
+    _fields_ = [("key", C.c_int32 * 3), ("estimated", C.c_int32), ("num_points", C.c_int32), ("carry_count", C.c_int32),
+                ("mu", C.c_double * 3), ("info", C.c_double * 6)]
+
+
 class FlsFeatureCfg(C.Structure):
     _fields_ = [("corner_threshold", C.c_float), ("planar_threshold", C.c_float), ("device", C.c_int32), ("reserved", C.c_int32)]
 

@@ -1260,6 +1260,24 @@ int fls_get_voxel_keys(fls_handle* hh, int32_t* keys_xyz, size_t capacity, size_
     FLS_CATCH
 }
 
+int fls_get_ndt_voxels(fls_handle* hh, fls_ndt_voxel* out, size_t capacity, size_t* n) {
+    Handle* h = reinterpret_cast<Handle*>(hh);
+    if (!h || !n || (capacity && !out)) return FLS_ERR_INVALID_ARG;
+    if (h->cfg.method != FLS_NDT) return FLS_ERR_UNSUPPORTED;
+    FLS_TRY
+    FLS_CUDA(cudaSetDevice(h->cfg.device));
+    std::vector<fls_ndt_voxel> v;
+    h->ndt.dump_voxels(v, h->stream);
+    std::sort(v.begin(), v.end(), [](const fls_ndt_voxel& a, const fls_ndt_voxel& b) {
+        return std::lexicographical_compare(a.key, a.key + 3, b.key, b.key + 3);
+    });
+    const size_t m = v.size() < capacity ? v.size() : capacity;
+    if (m) std::memcpy(out, v.data(), m * sizeof(fls_ndt_voxel));
+    *n = v.size();
+    return FLS_OK;
+    FLS_CATCH
+}
+
 int fls_get_map_points(fls_handle* hh, float* xyzi, size_t capacity, size_t* n) {
     Handle* h = reinterpret_cast<Handle*>(hh);
     if (!h || !n || (capacity && !xyzi)) return FLS_ERR_INVALID_ARG;

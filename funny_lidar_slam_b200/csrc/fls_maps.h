@@ -147,6 +147,8 @@ struct NdtMap {
     int evict_lru(int runs, int n_new, int n_touched, cudaStream_t st, int* n_victims, int* n_recreated);
     // packed voxel keys of the live voxels (tests); returns how many
     size_t dump_keys(unsigned long long* h_out, size_t cap, cudaStream_t st);
+    // every live voxel with its mean, information and counters, in device order (tests)
+    void dump_voxels(std::vector<fls_ndt_voxel>& out, cudaStream_t st);
     // VoxelGridCloud(cloud, leaf) then insert/update voxels; `first_scan` = flag_first_scan_ upstream
     int add_cloud(const float4* d_cloud, size_t n, float leaf, bool first_scan, cudaStream_t st);
     NdtView view() const {

@@ -295,6 +295,26 @@ __global__ void ndt_dump_keys_kernel(const NdtCold* __restrict__ cold, int hi_wa
     if (vi >= hi_water || !cold[vi].alive) return;
     out[atomicAdd(cursor, 1)] = cold[vi].key;
 }
+__device__ __forceinline__ int unpack21(unsigned long long k, int shift) {
+    const int c = (int)((k >> shift) & 0x1fffffu);
+    return (c & 0x100000) ? c - 0x200000 : c;  // 21-bit two's complement
+}
+__global__ void ndt_dump_voxels_kernel(const NdtCold* __restrict__ cold, const NdtHot* __restrict__ hot, int hi_water, fls_ndt_voxel* __restrict__ out,
+                                       int* cursor) {
+    const int vi = blockIdx.x * blockDim.x + threadIdx.x;
+    if (vi >= hi_water || !cold[vi].alive) return;
+    const NdtCold& c = cold[vi];
+    fls_ndt_voxel v;
+    v.key[0] = unpack21(c.key, 42);
+    v.key[1] = unpack21(c.key, 21);
+    v.key[2] = unpack21(c.key, 0);
+    v.estimated = c.estimated;
+    v.num_points = c.num_points;
+    v.carry_count = c.carry_count;
+    for (int k = 0; k < 3; ++k) v.mu[k] = c.estimated ? hot[vi].mu[k] : 0.0;  // the hot record is written by the first estimate
+    for (int k = 0; k < 6; ++k) v.info[k] = c.estimated ? hot[vi].info[k] : 0.0;
+    out[atomicAdd(cursor, 1)] = v;
+}
 
 // ---- K2: NDT residual kernel -----------------------------------------------------------------------------------
 // One persistent launch runs every Gauss-Newton iteration of a Match (gn_handover, fls_gn.cuh): grid-stride over the
@@ -620,6 +640,20 @@ size_t NdtMap::dump_keys(unsigned long long* h_out, size_t cap, cudaStream_t st)
     const size_t m = (size_t)n < cap ? (size_t)n : cap;
     FLS_CUDA(cudaMemcpy(h_out, lru_keys.p, sizeof(unsigned long long) * m, cudaMemcpyDeviceToHost));
     return m;
+}
+
+void NdtMap::dump_voxels(std::vector<fls_ndt_voxel>& out, cudaStream_t st) {
+    out.clear();
+    if (n_vox == 0 || hi_water == 0) return;
+    DevBuf<fls_ndt_voxel> d;
+    d.reserve(n_vox + 1);
+    FLS_CUDA(cudaMemsetAsync(counter.p + 7, 0, sizeof(int), st));
+    ndt_dump_voxels_kernel<<<grid_for(hi_water, 256), 256, 0, st>>>(cold.p, hot.p, hi_water, d.p, counter.p + 7);
+    int n = 0;
+    FLS_CUDA(cudaMemcpyAsync(&n, counter.p + 7, sizeof(int), cudaMemcpyDeviceToHost, st));
+    FLS_CUDA(cudaStreamSynchronize(st));
+    out.resize((size_t)n);
+    if (n) FLS_CUDA(cudaMemcpy(out.data(), d.p, sizeof(fls_ndt_voxel) * (size_t)n, cudaMemcpyDeviceToHost));
 }
 
 }  // namespace fls

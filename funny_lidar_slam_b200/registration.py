@@ -221,6 +221,17 @@ class Registration:
         check(lib().fls_get_voxel_keys(self._h, out.ctypes.data_as(C.c_void_p), cap, C.byref(n)), "fls_get_voxel_keys")
         return out[:min(cap, n.value)]
 
+    def ndt_voxels(self) -> dict:
+        """Every live voxel of the NDT map sorted by key: key (n,3) int32, mu (n,3), info (n,6) as stored (xx, xy, xz, yy, yz, zz),
+        estimated, num_points, carry_count (n,) int32."""
+        cap = max(int(self.map_info().n_voxels), 1)
+        buf = (_abi.FlsNdtVoxel * cap)()
+        n = C.c_size_t(0)
+        check(lib().fls_get_ndt_voxels(self._h, buf, cap, C.byref(n)), "fls_get_ndt_voxels")
+        a = np.frombuffer(buf, dtype=np.dtype([("key", "<i4", 3), ("estimated", "<i4"), ("num_points", "<i4"), ("carry_count", "<i4"),
+                                               ("mu", "<f8", 3), ("info", "<f8", 6)]))[:min(cap, n.value)]
+        return {f: a[f].copy() for f in a.dtype.names}
+
     def iter_log(self, scan: int = 0):
         """Per-iteration H, g, dx, sum_residual, n_valid of scan `scan` of the last Match (needs FLS_FLAG_ITER_LOG)."""
         cap = max(1, self.cfg.max_iterations)

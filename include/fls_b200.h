@@ -232,6 +232,21 @@ int fls_get_map_info(const fls_handle* h, fls_map_info* out);
  * (IncrementalNDT::grids_, incremental_ndt.h:393) and FLS_P2PLANE_IVOX (IVoxMap::grids_map_, ivox_map.h:70).  Introspection for the
  * LRU parity tests; writes at most `capacity` triples and returns the voxel count in *n. */
 int fls_get_voxel_keys(fls_handle* h, int32_t* keys_xyz, size_t capacity, size_t* n);
+/* One live voxel of the FLS_NDT map (IncrementalNDT::VoxelData, incremental_ndt.h:65-85 upstream).  mu and info are what Match
+ * reads: the mean and the symmetrised information matrix (xx, xy, xz, yy, yz, zz); both are zero while estimated == 0, as in a
+ * fresh VoxelData.  num_points is num_points_; carry_count the points buffered for a later estimate (points_.size(); 0 once the
+ * voxel is frozen past max_points_in_voxel, whose later points upstream keeps but never reads). */
+typedef struct {
+    int32_t key[3];
+    int32_t estimated;
+    int32_t num_points;
+    int32_t carry_count;
+    double mu[3];
+    double info[6];
+} fls_ndt_voxel;
+/* Every live voxel of the FLS_NDT map, sorted by key (x, then y, then z).  Read-only introspection for the map parity tests; writes at
+ * most `capacity` records and returns the voxel count in *n.  FLS_ERR_UNSUPPORTED for other plug-ins. */
+int fls_get_ndt_voxels(fls_handle* h, fls_ndt_voxel* out, size_t capacity, size_t* n);
 /* The points the FLS_P2PLANE_IVOX map holds (packed x, y, z, intensity), in insertion order; at most `capacity` points are written, the
  * count is returned in *n.  Introspection for the map parity tests. */
 int fls_get_map_points(fls_handle* h, float* xyzi, size_t capacity, size_t* n);

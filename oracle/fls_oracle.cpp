@@ -298,17 +298,20 @@ size_t orc_reg_map_copy(void* h, int which, float* out, size_t cap) {
     std::memcpy(out, m->data(), n * sizeof(P4));
     return m->size();
 }
-// NDT voxel dump: returns count; arrays sized by orc_reg_map_voxels
-size_t orc_reg_ndt_dump(void* h, int* keys, double* mu, double* info, int* est) {
+// NDT voxel dump in LRU order (front first): returns count; arrays sized by orc_reg_map_voxels.  num_points and pending (the
+// points_ buffer awaiting an estimate) may be NULL.
+size_t orc_reg_ndt_dump(void* h, int* keys, double* mu, double* info, int* est, int* num_points, int* pending) {
     auto* r = static_cast<Reg*>(h);
     if (!r->ndt) return 0;
-    std::vector<int> k, e;
+    std::vector<int> k, e, np, pd;
     std::vector<double> m, i;
-    r->ndt->dump(k, m, i, e);
+    r->ndt->dump(k, m, i, e, np, pd);
     std::memcpy(keys, k.data(), k.size() * sizeof(int));
     std::memcpy(mu, m.data(), m.size() * sizeof(double));
     std::memcpy(info, i.data(), i.size() * sizeof(double));
     std::memcpy(est, e.data(), e.size() * sizeof(int));
+    if (num_points) std::memcpy(num_points, np.data(), np.size() * sizeof(int));
+    if (pending) std::memcpy(pending, pd.data(), pd.size() * sizeof(int));
     return e.size();
 }
 

@@ -410,8 +410,9 @@ public:
     }
 
     size_t num_voxels() const { return grids_.size(); }
-    // export estimated voxels for tests: key(3 int), mu(3), info(9), estimated flag
-    void dump(std::vector<int>& keys, std::vector<double>& mu, std::vector<double>& info, std::vector<int>& est) const {
+    // export the voxels for tests, LRU order: key(3 int), mu(3), info(9), estimated flag, num_points_, points_.size()
+    void dump(std::vector<int>& keys, std::vector<double>& mu, std::vector<double>& info, std::vector<int>& est, std::vector<int>& num_points,
+              std::vector<int>& pending) const {
         for (const auto& kv : data_) {
             int k[3];
             unpack(kv.first, k);
@@ -419,6 +420,8 @@ public:
             mu.insert(mu.end(), kv.second.mu, kv.second.mu + 3);
             info.insert(info.end(), kv.second.info, kv.second.info + 9);
             est.push_back(kv.second.estimated ? 1 : 0);
+            num_points.push_back(kv.second.num_points);
+            pending.push_back(int(kv.second.pts.size() / 3));
         }
     }
 

@@ -70,7 +70,7 @@ def lib():
         L.orc_reg_map_points.restype = sz
         L.orc_reg_map_points.argtypes = [vp]
         L.orc_reg_ndt_dump.restype = sz
-        L.orc_reg_ndt_dump.argtypes = [vp, vp, vp, vp, vp]
+        L.orc_reg_ndt_dump.argtypes = [vp, vp, vp, vp, vp, vp, vp]
         L.orc_project.restype = sz
         L.orc_project.argtypes = [vp, vp, sz, i32, i32, f32, f32, f32, vp, vp, vp, vp, vp]
         L.orc_preprocess.restype = sz
@@ -296,8 +296,17 @@ class Registration:
         mu = np.zeros((n, 3))
         info = np.zeros((n, 9))
         est = np.zeros(n, np.int32)
-        m = lib().orc_reg_ndt_dump(self._h, _p(keys), _p(mu), _p(info), _p(est))
+        m = lib().orc_reg_ndt_dump(self._h, _p(keys), _p(mu), _p(info), _p(est), None, None)
         return keys[:m], mu[:m], info[:m].reshape(-1, 3, 3), est[:m]
+
+    def ndt_voxels(self):
+        """Every NDT voxel in LRU order (front first): key (n,3), mu (n,3), info (n,3,3), estimated, num_points and pending (the
+        points_ buffer, incremental_ndt.h:78 upstream) per voxel."""
+        n = self.map_voxels
+        keys, mu, info = np.zeros((n, 3), np.int32), np.zeros((n, 3)), np.zeros((n, 9))
+        est, num, pend = np.zeros(n, np.int32), np.zeros(n, np.int32), np.zeros(n, np.int32)
+        m = lib().orc_reg_ndt_dump(self._h, _p(keys), _p(mu), _p(info), _p(est), _p(num), _p(pend))
+        return dict(key=keys[:m], mu=mu[:m], info=info[:m].reshape(-1, 3, 3), estimated=est[:m], num_points=num[:m], pending=pend[:m])
 
     def __del__(self):
         if getattr(self, "_h", None):

@@ -117,6 +117,7 @@ def test_round2_entries_argument_checks():
     assert L.fls_update_local_map(None, None, None, None) == _abi.FLS_ERR_INVALID_ARG
     assert L.fls_get_voxel_keys(None, None, 0, None) == _abi.FLS_ERR_INVALID_ARG
     assert L.fls_get_map_points(None, None, 0, None) == _abi.FLS_ERR_INVALID_ARG
+    assert L.fls_get_ndt_voxels(None, None, 0, None) == _abi.FLS_ERR_INVALID_ARG
     assert L.fls_pcd_read(None, None, 0, None) == _abi.FLS_ERR_INVALID_ARG
     assert L.fls_pcd_write(None, None, 0) == _abi.FLS_ERR_INVALID_ARG
 
@@ -134,12 +135,13 @@ def test_header_is_plain_c_and_struct_layouts_match_ctypes(tmp_path):
         '#include <stdio.h>\n#include <stddef.h>\n#include "fls_b200.h"\n'
         "int main(void) {\n"
         '  printf("%zu %zu %zu %zu %zu ", sizeof(fls_config), sizeof(fls_match_stats), sizeof(fls_iter_log), sizeof(fls_map_info), sizeof(fls_feature_cfg));\n'
-        '  printf("%zu %zu %zu %zu\\n", offsetof(fls_config, point_to_planar_thres), offsetof(fls_config, ndt_voxel_size), offsetof(fls_config, point_search_thres), offsetof(fls_match_stats, algo_bytes));\n'
+        '  printf("%zu %zu %zu %zu ", offsetof(fls_config, point_to_planar_thres), offsetof(fls_config, ndt_voxel_size), offsetof(fls_config, point_search_thres), offsetof(fls_match_stats, algo_bytes));\n'
+        '  printf("%zu %zu %zu\\n", sizeof(fls_ndt_voxel), offsetof(fls_ndt_voxel, carry_count), offsetof(fls_ndt_voxel, mu));\n'
         "  return 0;\n}\n")
     exe = tmp_path / "abi"
     subprocess.check_call([gcc, "-std=c99", "-Wall", "-Wextra", "-Werror", "-pedantic", "-I", os.path.join(ROOT, "include"), str(src), "-o", str(exe)])
     got = [int(x) for x in subprocess.check_output([str(exe)]).split()]
     want = [C.sizeof(_abi.FlsConfig), C.sizeof(_abi.FlsMatchStats), C.sizeof(_abi.FlsIterLog), C.sizeof(_abi.FlsMapInfo), C.sizeof(_abi.FlsFeatureCfg),
             _abi.FlsConfig.point_to_planar_thres.offset, _abi.FlsConfig.ndt_voxel_size.offset, _abi.FlsConfig.point_search_thres.offset,
-            _abi.FlsMatchStats.algo_bytes.offset]
+            _abi.FlsMatchStats.algo_bytes.offset, C.sizeof(_abi.FlsNdtVoxel), _abi.FlsNdtVoxel.carry_count.offset, _abi.FlsNdtVoxel.mu.offset]
     assert got == want, (got, want)
