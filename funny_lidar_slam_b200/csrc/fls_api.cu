@@ -233,25 +233,10 @@ void Handle::unpack(int B, const size_t* n, double* T, int* converged, fls_match
     for (int s = 0; s < B; ++s) log_n[s] = h_state[s].iter < log_cap ? h_state[s].iter : log_cap;
 }
 
-// control block of a single-scan persistent GN loop (K2 / K3 / K5): CTA rows + pose record + stop rule
-static GnLoopCtl make_ctl(Handle& h, int method, int grid, int min_effective) {
-    GnLoopCtl c;
-    c.tag_base = h.next_ll_epoch((size_t)grid * 32 + kLlPoseLen);
-    c.state = h.state.p;
-    c.ll_rows = h.ll_rows.p;
-    c.ll_pose = h.ll_rows.p + (size_t)grid * 32;
-    c.gp = h.gn_params(method, min_effective);
-    c.log = h.scan_log(0);
-    c.log_cap = h.log_cap;
-    c.result = h.scan_result(0);
-    return c;
-}
-
-// single-scan Match: wait, then unpack
-static void finish_match(Handle& h, double* T, int* converged, fls_match_stats* st, size_t n_source) {
-    h.read_back(1);
-    h.end_call(st);
-    h.unpack(1, &n_source, T, converged, st);
+int Handle::inserted(int rc, fls_match_stats* st) {
+    FLS_CUDA(cudaStreamSynchronize(stream));
+    if (st) st->gpu_launches = launches;
+    return rc;
 }
 
 // ---- LoamPointToPlaneIVOX ------------------------------------------------------------------------------------
@@ -415,9 +400,7 @@ int Handle::match_p2plane_ivox(const float4* d_src, size_t n, double* T, int* co
         const int rc2 = ivox.append_and_build(stage.p, n_add, cfg.ivox_capacity, stream);
         launches += ivox.launches;
         ivox.launches = 0;
-        FLS_CUDA(cudaStreamSynchronize(stream));
-        if (st) st->gpu_launches = launches;
-        if (rc2 != FLS_OK) return rc2;
+        return inserted(rc2, st);
     }
     return FLS_OK;
 }
@@ -442,11 +425,8 @@ int Handle::match_ndt(const float4* d_in, size_t n_in, double* T, int* converged
     const size_t n = voxel_grid_device(d_in, n_in, cfg.source_cloud_filter_size, src_f.p, scratch, stream, &launches);  // :232
     const int ni = (int)n;
     const int grid = ndt_grid(ni, cfg.device);
-    GnLoopCtl ctl = make_ctl(*this, FLS_NDT, grid, cfg.ndt_min_effective_pts);
     double T_in[16];
     std::memcpy(T_in, T, sizeof(T_in));
-    launch_gn_init(state.p, T, stream);
-    launches++;
     NdtArgs a;
     a.src = src_f.p;
     a.n = ni;
@@ -455,17 +435,14 @@ int Handle::match_ndt(const float4* d_in, size_t n_in, double* T, int* converged
     a.state = state.p;
     // roofline accounting (SURVEY.md §8d, K2): 16 B source point + 7 x 16 B slot probes per point-iteration,
     // 80 B voxel record per estimated voxel hit; the 6x6 sums are fused (no per-point output).
-    gn_launch(16 + 16LL * 7, 80, src_f.p, n, [&] { launch_ndt_loop(a, ctl, grid, stream); });
-    finish_match(*this, T, converged, st, n);
+    match_single(FLS_NDT, cfg.ndt_min_effective_pts, grid, 16 + 16LL * 7, 80, src_f.p, n, n, T, converged, st,
+                 [&](const GnLoopCtl& ctl) { launch_ndt_loop(a, ctl, grid, stream); });
     if (!h_state->failed && !cfg.localization_mode) {
         // :326-330 — the scan enters the map transformed by the INPUT guess T, not the optimised pose  [quirk 6]
         stage2.reserve(n);
         launch_transform_f(src_f.p, n, T_in, stage2.p, stream);
         launches++;
-        const int rc2 = add_cloud_ndt(stage2.p, n);
-        FLS_CUDA(cudaStreamSynchronize(stream));
-        if (st) st->gpu_launches = launches;
-        if (rc2 != FLS_OK) return rc2;
+        return inserted(add_cloud_ndt(stage2.p, n), st);
     }
     return FLS_OK;
 }
@@ -588,9 +565,6 @@ int Handle::match_icp(const float4* d_in, size_t n_in, double* T, int* converged
     const size_t n = voxel_grid_device(d_in, n_in, cfg.source_cloud_filter_size, src_f.p, scratch, stream, &launches);  // :57
     const int ni = (int)n;
     const int grid = icp_grid_blocks(ni, cfg.device);
-    GnLoopCtl ctl = make_ctl(*this, FLS_ICP_P2P, grid, 0);
-    launch_gn_init(state.p, T, stream);
-    launches++;
     IcpArgs a;
     a.src = src_f.p;
     a.n = ni;
@@ -598,18 +572,15 @@ int Handle::match_icp(const float4* d_in, size_t n_in, double* T, int* converged
     a.max_corr = cfg.icp_max_correspond_distance;
     a.state = state.p;
     // roofline accounting (SURVEY.md §8d, K3): 16 B source point + 27 x 16 B slot probes, 16 B per scanned map record
-    gn_launch(16 + 16LL * 27, 16, src_f.p, n, [&] { launch_icp_loop(a, ctl, grid, stream); });
-    finish_match(*this, T, converged, st, n);
+    match_single(FLS_ICP_P2P, 0, grid, 16 + 16LL * 27, 16, src_f.p, n, n, T, converged, st,
+                 [&](const GnLoopCtl& ctl) { launch_icp_loop(a, ctl, grid, stream); });
     if (h_state->converged && !cfg.localization_mode) {
         // IsNeedAddCloud (:218-236): key-frame gating on translation / RPY deltas against a persistent last_T
         if (need_add_cloud(T)) {
             stage.reserve(n);
             launch_transform_f(src_f.p, n, T, stage.p, stream);  // :156 TransformPointCloud(source, final) in float
             launches++;
-            const int rc2 = add_cloud_icp(stage.p, n);
-            FLS_CUDA(cudaStreamSynchronize(stream));
-            if (st) st->gpu_launches = launches;
-            if (rc2 != FLS_OK) return rc2;
+            return inserted(add_cloud_icp(stage.p, n), st);
         }
     }
     return FLS_OK;
@@ -689,9 +660,6 @@ int Handle::match_kd(const float4* d_planar, size_t n_planar, const float4* d_co
     const size_t n = n_planar + n_corner;
     const int ni = (int)n;
     const int grid = loam_grid_blocks(ni, cfg.device);
-    GnLoopCtl ctl = make_ctl(*this, cfg.method, grid, 50);
-    launch_gn_init(state.p, T, stream);
-    launches++;
     rec_d.reserve(n * 8 + 8);
     flags.reserve(n + 1);
     LoamArgs a;
@@ -709,11 +677,10 @@ int Handle::match_kd(const float4* d_planar, size_t n_planar, const float4* d_co
     a.rec = rec_d.p;
     a.flags = flags.p;
     // roofline accounting (K5): 16 B source point + 27 x 16 B slot probes + 56 B persistent record, 16 B per scanned map record
-    gn_launch(16 + 16LL * 27 + 56, 16, d_planar, n_planar, [&] {
+    match_single(cfg.method, 50, grid, 16 + 16LL * 27 + 56, 16, d_planar, n_planar, n, T, converged, st, [&](const GnLoopCtl& ctl) {
         launch_loam_loop(a, ctl, grid, stream);
         launches++;  // the flag reset in front of the loop
     });
-    finish_match(*this, T, converged, st, n);
     // key-frame insertion: loam_point_to_plane_kdtree.h:146-150 (gate evaluated before the mode test), loam_full_kdtree.h:178-186
     if (h_state->converged && need_add_cloud(T) && (full || !cfg.localization_mode)) {
         int rc2;
@@ -730,9 +697,7 @@ int Handle::match_kd(const float4* d_planar, size_t n_planar, const float4* d_co
             launches++;
             rc2 = add_cloud_kd(stage.p, n_planar, nullptr, 0);
         }
-        FLS_CUDA(cudaStreamSynchronize(stream));
-        if (st) st->gpu_launches = launches;
-        if (rc2 != FLS_OK) return rc2;
+        return inserted(rc2, st);
     }
     return FLS_OK;
 }
@@ -988,80 +953,50 @@ int fls_add_cloud(fls_handle* hh, int n_clouds, const void* const* pts, const si
     FLS_CATCH
 }
 
-static int match_dispatch(Handle* h, const float4* d_ordered, size_t n_ordered, const float4* d_planar, size_t n_planar, const float4* d_corner,
-                          size_t n_corner, double* T, int* converged, fls_match_stats* st) {
-    switch (h->cfg.method) {
-        case FLS_P2PLANE_IVOX: return h->match_p2plane_ivox(d_planar, n_planar, T, converged, st);
-        case FLS_NDT: return h->match_ndt(d_ordered, n_ordered, T, converged, st);
-        case FLS_ICP_P2P: return h->match_icp(d_ordered, n_ordered, T, converged, st);
-        case FLS_P2PLANE_KNN:
-        case FLS_LOAM_FULL: return h->match_kd(d_planar, n_planar, d_corner, n_corner, T, converged, st);
-        default: return FLS_ERR_UNSUPPORTED;
+// A single-scan Match on the clouds the plug-in reads: the ordered scan (NDT, ICP), the planar features (LOAM-iVox, kd-tree
+// point-to-plane) or the planar and corner features (LoamFull).  FLS_ERR_INVALID_ARG when one of them is NULL but not empty.
+// The clouds are host records of `host_stride` bytes, uploaded here, or (host_stride 0) packed float4 already on the device.
+static int match_clouds(Handle* h, const void* ordered, size_t n_ordered, const void* planar, size_t n_planar, const void* corner, size_t n_corner,
+                        size_t host_stride, double* T, int* converged, fls_match_stats* st) {
+    if (!h || !T) return FLS_ERR_INVALID_ARG;
+    const int method = h->cfg.method;
+    const bool features = method >= FLS_P2PLANE_IVOX, full = method == FLS_LOAM_FULL;
+    if (features ? !planar && n_planar : !ordered && n_ordered) return FLS_ERR_INVALID_ARG;
+    if (full && !corner && n_corner) return FLS_ERR_INVALID_ARG;
+    FLS_TRY
+    if (st) std::memset(st, 0, sizeof(*st));
+    h->begin_call();
+    auto dev = [&](const void* p, size_t n, fls::DevBuf<float4>& buf) {
+        return host_stride ? h->upload(p, n, host_stride, buf) : static_cast<const float4*>(p);
+    };
+    if (!features) {
+        const float4* d = dev(ordered, n_ordered, h->src);
+        return method == FLS_NDT ? h->match_ndt(d, n_ordered, T, converged, st) : h->match_icp(d, n_ordered, T, converged, st);
     }
+    const float4* d_pla = dev(planar, n_planar, h->src);
+    if (method == FLS_P2PLANE_IVOX) return h->match_p2plane_ivox(d_pla, n_planar, T, converged, st);
+    const float4* d_cor = full ? dev(corner, n_corner, h->src2) : nullptr;
+    return h->match_kd(d_pla, n_planar, d_cor, full ? n_corner : 0, T, converged, st);
+    FLS_CATCH
 }
 
 int fls_match(fls_handle* hh, const void* ordered, size_t n_ordered, const void* planar, size_t n_planar, const void* corner, size_t n_corner,
               size_t stride, double T[16], int* converged, fls_match_stats* st) {
-    Handle* h = reinterpret_cast<Handle*>(hh);
-    if (!h || !T || !stride_ok(stride)) return FLS_ERR_INVALID_ARG;
-    FLS_TRY
-    if (st) std::memset(st, 0, sizeof(*st));
-    h->begin_call();
-    const float4* d_ord = nullptr;
-    const float4* d_pla = nullptr;
-    const float4* d_cor = nullptr;
-    const bool uses_planar = h->cfg.method >= FLS_P2PLANE_IVOX;
-    if (uses_planar) {
-        if (!planar && n_planar) return FLS_ERR_INVALID_ARG;
-        d_pla = h->upload(planar, n_planar, stride, h->src);
-        if (h->cfg.method == FLS_LOAM_FULL) {
-            if (!corner && n_corner) return FLS_ERR_INVALID_ARG;
-            d_cor = h->upload(corner, n_corner, stride, h->src2);
-        } else {
-            n_corner = 0;
-        }
-    } else {
-        if (!ordered && n_ordered) return FLS_ERR_INVALID_ARG;
-        d_ord = h->upload(ordered, n_ordered, stride, h->src);
-    }
-    return match_dispatch(h, d_ord, n_ordered, d_pla, n_planar, d_cor, n_corner, T, converged, st);
-    FLS_CATCH
+    if (!stride_ok(stride)) return FLS_ERR_INVALID_ARG;
+    return match_clouds(reinterpret_cast<Handle*>(hh), ordered, n_ordered, planar, n_planar, corner, n_corner, stride, T, converged, st);
 }
 
 int fls_match_device(fls_handle* hh, const void* d_points, size_t n, double T[16], int* converged, fls_match_stats* st) {
     Handle* h = reinterpret_cast<Handle*>(hh);
-    if (!h || !T || (!d_points && n)) return FLS_ERR_INVALID_ARG;
-    FLS_TRY
-    if (st) std::memset(st, 0, sizeof(*st));
-    h->begin_call();
-    const float4* d = static_cast<const float4*>(d_points);
-    if (h->cfg.method == FLS_LOAM_FULL) return FLS_ERR_UNSUPPORTED;  // two feature clouds: use fls_match
-    return match_dispatch(h, d, n, d, n, nullptr, 0, T, converged, st);
-    FLS_CATCH
+    // LoamFull reads two feature clouds: fls_match_cluster_device
+    if (h && T && h->cfg.method == FLS_LOAM_FULL) return !d_points && n ? FLS_ERR_INVALID_ARG : FLS_ERR_UNSUPPORTED;
+    // the one cloud is the ordered scan or the planar features, whichever the plug-in reads
+    return match_clouds(h, d_points, n, d_points, n, nullptr, 0, 0, T, converged, st);
 }
 
 int fls_match_cluster_device(fls_handle* hh, const void* d_ordered, size_t n_ordered, const void* d_planar, size_t n_planar, const void* d_corner,
                              size_t n_corner, double T[16], int* converged, fls_match_stats* st) {
-    Handle* h = reinterpret_cast<Handle*>(hh);
-    if (!h || !T) return FLS_ERR_INVALID_ARG;
-    // the clouds each plug-in reads, as in fls_match
-    const bool uses_planar = h->cfg.method >= FLS_P2PLANE_IVOX;
-    if (uses_planar) {
-        if (!d_planar && n_planar) return FLS_ERR_INVALID_ARG;
-        if (h->cfg.method == FLS_LOAM_FULL) {
-            if (!d_corner && n_corner) return FLS_ERR_INVALID_ARG;
-        } else {
-            n_corner = 0;
-        }
-    } else if (!d_ordered && n_ordered) {
-        return FLS_ERR_INVALID_ARG;
-    }
-    FLS_TRY
-    if (st) std::memset(st, 0, sizeof(*st));
-    h->begin_call();
-    return match_dispatch(h, static_cast<const float4*>(d_ordered), n_ordered, static_cast<const float4*>(d_planar), n_planar,
-                          static_cast<const float4*>(d_corner), n_corner, T, converged, st);
-    FLS_CATCH
+    return match_clouds(reinterpret_cast<Handle*>(hh), d_ordered, n_ordered, d_planar, n_planar, d_corner, n_corner, 0, T, converged, st);
 }
 
 // Uploads the host scans of a batch back to back into the handle's scan buffer; ptrs[s] receives scan s

@@ -45,6 +45,30 @@ constexpr int kMaxDevices = 64;
 // FLS_OK when `device` is a visible CUDA device with a slot in the per-device tables, FLS_ERR_NO_DEVICE otherwise
 int check_device(int device);
 
+// ---- kernel attributes per device (fls_gn.cu), cached per (function, device) under one lock ------------------------------
+// The caller has made `device` current.  A persistent (cooperatively launched) kernel is launched only after its sizing call
+// on the same device — coresident_ctas, or raise_smem_limit for a kernel sized by SMs — since that call is what raises the
+// kernel's dynamic shared-memory limit there.
+
+// Raises fn's dynamic shared-memory limit on `device` to `bytes`; never lowers it.
+void raise_smem_limit(const void* fn, size_t bytes, int device);
+// CTAs of fn that can be resident at once on `device` (SMs x blocks per SM at this block and dynamic shared memory; a function
+// is always sized with the same block and smem).  Raises fn's shared-memory limit first; no resident block is an error.
+int coresident_ctas(const void* fn, int block, size_t smem, int device);
+int device_sms(int device);
+// grid of a persistent launch: what the work needs, at least one CTA and at most what can be co-resident
+inline int clamp_grid(int need, int coresident) { return need < 1 ? 1 : need < coresident ? need : coresident; }
+
+// Cooperative launch of fn; the arguments are taken by value with fn's own parameter types, so params[] points at exactly what
+// the kernel reads.
+template <class T>
+struct same_type { using type = T; };
+template <class... P>
+void launch_cooperative(void (*fn)(P...), int grid, int block, size_t smem, cudaStream_t st, typename same_type<P>::type... args) {
+    void* params[] = {&args...};
+    FLS_CUDA(cudaLaunchCooperativeKernel((const void*)fn, dim3(grid), dim3(block), params, smem, st));
+}
+
 // caller record layouts: packed float4, or x y z at 0 / 4 / 8 and the intensity at 16 of a larger record
 inline bool stride_ok(size_t stride) { return stride == 16 || (stride >= 20 && stride % 4 == 0); }
 

@@ -13,7 +13,6 @@
 #include <algorithm>
 #include <cstdlib>
 #include <cstring>
-#include <mutex>
 #include <vector>
 
 #include "fls_frontend.h"
@@ -385,21 +384,13 @@ __global__ void feat_emit_kernel(const int* __restrict__ corner_out, const int* 
     }
 }
 
-// The kernels' dynamic shared-memory limits are per device and per function: raised, never lowered, under a lock of their own
-// (every caller of enqueue_features holds its workspace lock already; this one is taken last and alone).
+// The kernels' dynamic shared-memory limits are per device and per function (every caller of enqueue_features holds its
+// workspace lock already; raise_smem_limit's lock is taken last and alone).
 void ensure_feat_smem(int device, size_t smem_sort, size_t smem_ring) {
-    static std::mutex mu;
-    static size_t set[kMaxDevices][2];
-    std::lock_guard<std::mutex> lock(mu);
-    size_t* cur = set[device];
-    if (smem_sort <= cur[0] && smem_ring <= cur[1]) return;
-    const int ss = (int)std::max(smem_sort, cur[0]), sr = (int)std::max(smem_ring, cur[1]);
-    FLS_CUDA(cudaFuncSetAttribute(feat_sort_kernel<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, ss));
-    FLS_CUDA(cudaFuncSetAttribute(feat_sort_kernel<1024>, cudaFuncAttributeMaxDynamicSharedMemorySize, ss));
-    FLS_CUDA(cudaFuncSetAttribute(feat_ring_kernel<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, sr));
-    FLS_CUDA(cudaFuncSetAttribute(feat_ring_kernel<1024>, cudaFuncAttributeMaxDynamicSharedMemorySize, sr));
-    cur[0] = (size_t)ss;
-    cur[1] = (size_t)sr;
+    raise_smem_limit((const void*)feat_sort_kernel<256>, smem_sort, device);
+    raise_smem_limit((const void*)feat_sort_kernel<1024>, smem_sort, device);
+    raise_smem_limit((const void*)feat_ring_kernel<256>, smem_ring, device);
+    raise_smem_limit((const void*)feat_ring_kernel<1024>, smem_ring, device);
 }
 
 template <int BLOCK>

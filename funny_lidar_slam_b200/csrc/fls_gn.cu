@@ -1,6 +1,10 @@
 // fls_gn.cu — state initialisation of a Gauss-Newton loop (NDT / ICP / kd-tree LOAM; the LOAM-iVox path initialises its
-// states in its batch prep kernel).  The solve / update / stop rule itself (K6) is device code shared by every persistent
-// kernel: gn_step / gn_handover in fls_gn.cuh.
+// states in its batch prep kernel), and the per-device kernel attributes that size and prepare every persistent launch.
+// The solve / update / stop rule itself (K6) is device code shared by every persistent kernel: gn_step / gn_handover in
+// fls_gn.cuh.
+#include <map>
+#include <utility>
+
 #include "fls_gn.cuh"
 
 namespace fls {
@@ -31,6 +35,56 @@ __global__ void gn_init_kernel(GnState* s, double t00, double t10, double t20, d
 void launch_gn_init(GnState* d_state, const double* T, cudaStream_t st) {
     // T is column-major: T[c*4 + r]
     gn_init_kernel<<<1, 32, 0, st>>>(d_state, T[0], T[1], T[2], T[4], T[5], T[6], T[8], T[9], T[10], T[12], T[13], T[14]);
+}
+
+// ---- kernel attributes per device ----------------------------------------------------------------------------------------
+// Handles on different threads size their kernels concurrently: one lock over every entry.
+namespace {
+struct KernelSlot {
+    size_t smem_limit = 0;  // dynamic shared-memory limit raised so far (0: the default)
+    int ctas = 0;           // co-resident CTAs (0: not queried yet)
+};
+std::mutex g_attr_mu;
+std::map<std::pair<const void*, int>, KernelSlot> g_slots;  // (function, device)
+int g_sms[kMaxDevices];
+
+void raise_locked(KernelSlot& k, const void* fn, size_t bytes) {
+    if (bytes <= k.smem_limit) return;
+    FLS_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+    k.smem_limit = bytes;
+}
+
+int sms_locked(int device) {
+    if (!g_sms[device]) FLS_CUDA(cudaDeviceGetAttribute(&g_sms[device], cudaDevAttrMultiProcessorCount, device));
+    return g_sms[device];
+}
+}  // namespace
+
+void raise_smem_limit(const void* fn, size_t bytes, int device) {
+    std::lock_guard<std::mutex> lock(g_attr_mu);
+    raise_locked(g_slots[{fn, device}], fn, bytes);
+}
+
+int coresident_ctas(const void* fn, int block, size_t smem, int device) {
+    std::lock_guard<std::mutex> lock(g_attr_mu);
+    KernelSlot& k = g_slots[{fn, device}];
+    if (!k.ctas) {
+        raise_locked(k, fn, smem);
+        int per_sm = 0;
+        FLS_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, block, smem));
+        if (per_sm < 1) {
+            set_last_error("cudaOccupancyMaxActiveBlocksPerMultiprocessor: no block of " + std::to_string(block) + " threads and " +
+                           std::to_string(smem) + " B of shared memory fits on an SM of device " + std::to_string(device));
+            throw CudaError{FLS_ERR_CUDA};
+        }
+        k.ctas = sms_locked(device) * per_sm;
+    }
+    return k.ctas;
+}
+
+int device_sms(int device) {
+    std::lock_guard<std::mutex> lock(g_attr_mu);
+    return sms_locked(device);
 }
 
 }  // namespace fls

@@ -127,6 +127,29 @@ struct Handle {
     void read_back(int n_scans);  // enqueues the copy of the states and of every scan's iteration log
     // after end_call: T / converged / stats and log_n of every scan (call-level figures on stats[0]), T_final from scan 0
     void unpack(int n_scans, const size_t* n_source, double* T, int* converged, fls_match_stats* st);
+    // A single-scan Match on a persistent kernel of `grid` CTAs (NDT, ICP, kd-tree LOAM): control block, state from T, the
+    // gn_launch of launch(ctl), then the wait and T / converged / stats of a scan of n_source points
+    template <class F>
+    void match_single(int method, int min_effective, int grid, long long point_iter_bytes, long long cand_bytes, const float4* src, size_t src_n,
+                      size_t n_source, double* T, int* converged, fls_match_stats* st, F&& launch) {
+        GnLoopCtl ctl;
+        ctl.tag_base = next_ll_epoch((size_t)grid * 32 + kLlPoseLen);
+        ctl.state = state.p;
+        ctl.ll_rows = ll_rows.p;
+        ctl.ll_pose = ll_rows.p + (size_t)grid * 32;
+        ctl.gp = gn_params(method, min_effective);
+        ctl.log = scan_log(0);
+        ctl.log_cap = log_cap;
+        ctl.result = scan_result(0);
+        launch_gn_init(state.p, T, stream);
+        launches++;
+        gn_launch(point_iter_bytes, cand_bytes, src, src_n, [&] { launch(ctl); });
+        read_back(1);
+        end_call(st);
+        unpack(1, &n_source, T, converged, st);
+    }
+    // end of a Match that added its scan to the map with status rc: waits for the insertion and counts its launches too
+    int inserted(int rc, fls_match_stats* st);
 
     int add_cloud_ivox(const void* pts, size_t n, size_t stride);
     int match_p2plane_ivox(const float4* d_src, size_t n, double* T, int* converged, fls_match_stats* st);

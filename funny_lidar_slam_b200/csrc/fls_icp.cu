@@ -196,24 +196,11 @@ __global__ void fitness_kernel(IvoxView g, const float4* __restrict__ src, int n
 }  // namespace
 
 int icp_grid_blocks(int n, int device) {
-    static int cap[64] = {0};
-    if (device >= 0 && device < 64 && !cap[device]) {
-        int sms = 0, per_sm = 0;
-        cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, icp_gn_kernel<kIcpBlock>, kIcpBlock, 0);
-        cap[device] = sms * (per_sm > 0 ? per_sm : 1);
-    }
     const int per_block = kIcpBlock / kIcpLanes;
-    const int need = (n + per_block - 1) / per_block;
-    const int c = (device >= 0 && device < 64) ? cap[device] : 132;
-    const int g = need < c ? need : c;
-    return g > 0 ? g : 1;
+    return clamp_grid((n + per_block - 1) / per_block, coresident_ctas((const void*)icp_gn_kernel<kIcpBlock>, kIcpBlock, 0, device));
 }
 void launch_icp_loop(const IcpArgs& a, const GnLoopCtl& ctl, int grid, cudaStream_t st) {
-    IcpArgs a_ = a;
-    GnLoopCtl c_ = ctl;
-    void* params[] = {&a_, &c_};
-    FLS_CUDA(cudaLaunchCooperativeKernel((const void*)icp_gn_kernel<kIcpBlock>, dim3(grid), dim3(kIcpBlock), params, 0, st));
+    launch_cooperative(icp_gn_kernel<kIcpBlock>, grid, kIcpBlock, 0, st, a, ctl);
 }
 
 void launch_fitness(const IvoxView& g, const float4* d_src, int n, const double* T, float max_range, double* d_out2, cudaStream_t st) {

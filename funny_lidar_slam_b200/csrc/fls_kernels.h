@@ -47,12 +47,12 @@ struct P2PlaneLoopArgs {
     int ticket_stride;  // >= max_iterations + 2
     unsigned* abort_word;  // v9 watchdog: zeroed before the launch, non-zero when a wait loop gave up (protocol error)
 };
-int p2plane_max_grid(int device);      // co-resident CTAs
+// Each persistent kernel below is sized by its *_grid call on the device it then runs on (see coresident_ctas, fls_common.cuh).
 int p2plane_chunks(int n);             // warp-sized (32-point) work chunks
 int p2plane_grid(int n, int device);    // CTAs that serve a scan of n points: its chunks / warps per CTA, + the folder, <= co-resident
 void launch_p2plane_loop(const P2PlaneLoopArgs& a, int grid, cudaStream_t st);
 // generation 9 of the same loop (fls_p2plane_v9.cu): barrier-free dataflow, TMA-staged candidate runs, DMMA sums
-int p2plane_v9_grid(int n_max, int device);
+int p2plane_v9_grid(int n_max, int device);  // also raises the kernel's shared-memory limit on `device`
 void launch_p2plane_v9(const P2PlaneLoopArgs& a, int grid, cudaStream_t st);
 // queries of a batch are put in locality order in tiles of this many consecutive points; a tile never spans two scans
 static constexpr int kOrderTile = 8192;
@@ -74,7 +74,7 @@ struct NdtArgs {
     double outlier_thres;
     GnState* state;
 };
-int ndt_grid(int n, int device);  // co-resident grid of the persistent kernel
+int ndt_grid(int n, int device);
 void launch_ndt_loop(const NdtArgs& a, const GnLoopCtl& ctl, int grid, cudaStream_t st);
 // batch of scans in one launch: scan s is served by CTAs [cta0, cta0 + ncta) of the grid (its own persistent loop)
 struct __align__(16) NdtBatchItem {

@@ -221,27 +221,14 @@ __global__ void loam_clear_flags_kernel(unsigned char* flags, int n) {
 }  // namespace
 
 int loam_grid_blocks(int n, int device) {
-    static int cap[64] = {0};
-    if (device >= 0 && device < 64 && !cap[device]) {
-        int sms = 0, per_sm = 0;
-        cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, loam_gn_kernel<kLoamBlock>, kLoamBlock, 0);
-        cap[device] = sms * (per_sm > 0 ? per_sm : 1);
-    }
     const int per_block = kLoamBlock / kLoamLanes;
-    const int need = (n + per_block - 1) / per_block;
-    const int c = (device >= 0 && device < 64) ? cap[device] : 132;
-    const int g = need < c ? need : c;
-    return g > 0 ? g : 1;
+    return clamp_grid((n + per_block - 1) / per_block, coresident_ctas((const void*)loam_gn_kernel<kLoamBlock>, kLoamBlock, 0, device));
 }
 
 void launch_loam_loop(const LoamArgs& a, const GnLoopCtl& ctl, int grid, cudaStream_t st) {
-    LoamArgs a_ = a;
-    GnLoopCtl c_ = ctl;
     const int n = a.n_corner + a.n_planar;
     if (n > 0) loam_clear_flags_kernel<<<(n + 255) / 256, 256, 0, st>>>(a.flags, n);
-    void* params[] = {&a_, &c_};
-    FLS_CUDA(cudaLaunchCooperativeKernel((const void*)loam_gn_kernel<kLoamBlock>, dim3(grid), dim3(kLoamBlock), params, 0, st));
+    launch_cooperative(loam_gn_kernel<kLoamBlock>, grid, kLoamBlock, 0, st, a, ctl);
 }
 
 }  // namespace fls

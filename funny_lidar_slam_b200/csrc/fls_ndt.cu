@@ -433,39 +433,15 @@ __global__ void __launch_bounds__(BLOCK) ndt_gn_batch_kernel(const NdtBatchItem*
 }  // namespace
 
 int ndt_grid(int n, int device) {
-    static int cap[64] = {0};
-    if (device >= 0 && device < 64 && !cap[device]) {
-        int sms = 0, per_sm = 0;
-        cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, ndt_gn_kernel<kNdtBlock>, kNdtBlock, 0);
-        cap[device] = sms * (per_sm > 0 ? per_sm : 1);
-    }
-    const int need = (n + kNdtBlock - 1) / kNdtBlock;
-    const int c = (device >= 0 && device < 64) ? cap[device] : 132;
-    const int g = need < c ? need : c;
-    return g > 0 ? g : 1;
+    return clamp_grid((n + kNdtBlock - 1) / kNdtBlock, coresident_ctas((const void*)ndt_gn_kernel<kNdtBlock>, kNdtBlock, 0, device));
 }
 void launch_ndt_loop(const NdtArgs& a, const GnLoopCtl& ctl, int grid, cudaStream_t st) {
-    NdtArgs a_ = a;
-    GnLoopCtl c_ = ctl;
-    void* params[] = {&a_, &c_};
-    FLS_CUDA(cudaLaunchCooperativeKernel((const void*)ndt_gn_kernel<kNdtBlock>, dim3(grid), dim3(kNdtBlock), params, 0, st));
+    launch_cooperative(ndt_gn_kernel<kNdtBlock>, grid, kNdtBlock, 0, st, a, ctl);
 }
 
-int ndt_max_grid(int device) {
-    ndt_grid(1, device);  // fills the cache
-    static int cap[64] = {0};
-    if (device >= 0 && device < 64 && !cap[device]) {
-        int sms = 0, per_sm = 0;
-        cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, ndt_gn_batch_kernel<kNdtBlock>, kNdtBlock, 0);
-        cap[device] = sms * (per_sm > 0 ? per_sm : 1);
-    }
-    return (device >= 0 && device < 64) ? cap[device] : 132;
-}
+int ndt_max_grid(int device) { return coresident_ctas((const void*)ndt_gn_batch_kernel<kNdtBlock>, kNdtBlock, 0, device); }
 void launch_ndt_batch(const NdtBatchItem* d_items, int n_scans, int grid, cudaStream_t st) {
-    void* params[] = {&d_items, &n_scans};
-    FLS_CUDA(cudaLaunchCooperativeKernel((const void*)ndt_gn_batch_kernel<kNdtBlock>, dim3(grid), dim3(kNdtBlock), params, 0, st));
+    launch_cooperative(ndt_gn_batch_kernel<kNdtBlock>, grid, kNdtBlock, 0, st, d_items, n_scans);
 }
 
 void NdtMap::configure(double voxel_size, int min_points, int max_points, long long cap) {

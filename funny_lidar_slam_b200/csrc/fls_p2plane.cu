@@ -559,7 +559,6 @@ __global__ void ivox_insert_scatter_kernel(const unsigned char* __restrict__ cls
 
 // One 768-thread CTA per SM: 24 resident warps (<= 80 registers).
 constexpr int kMinB = 1;
-const void* p2plane_fn() { return (const void*)p2plane_gn_kernel<kP2PlaneBlock, kMinB>; }
 size_t p2plane_smem() {
     constexpr int W = kP2PlaneBlock / 32, V = kVisitGroup < W ? kVisitGroup : W;
     return (size_t)W * 32 * kRecW * sizeof(double) + (size_t)V * W * 32 * sizeof(double);
@@ -567,33 +566,17 @@ size_t p2plane_smem() {
 
 }  // namespace
 
-int p2plane_max_grid(int device) {
-    static int cached[64] = {0};
-    if (device >= 0 && device < 64 && cached[device]) return cached[device];
-    int sms = 0;
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
-    int per_sm = 0;
-    cudaFuncSetAttribute(p2plane_fn(), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p2plane_smem());
-    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, p2plane_gn_kernel<kP2PlaneBlock, kMinB>, kP2PlaneBlock, p2plane_smem());
-    const int g = sms * (per_sm > 0 ? per_sm : 1);
-    if (device >= 0 && device < 64) cached[device] = g;
-    return g;
-}
-
 int p2plane_chunks(int n) { return (n + 31) / 32; }
 
 int p2plane_grid(int n, int device) {
     const int W = kP2PlaneBlock / 32;
     const int need = (p2plane_chunks(n) + W - 1) / W;
-    const int cap = p2plane_max_grid(device);
-    const int g = need + 1 < cap ? need + 1 : cap;  // + the folding CTA (stays without chunks when there is room)
-    return g > 0 ? g : 1;
+    // + the folding CTA (stays without chunks when there is room)
+    return clamp_grid(need + 1, coresident_ctas((const void*)p2plane_gn_kernel<kP2PlaneBlock, kMinB>, kP2PlaneBlock, p2plane_smem(), device));
 }
 
 void launch_p2plane_loop(const P2PlaneLoopArgs& a, int grid, cudaStream_t st) {
-    P2PlaneLoopArgs args = a;
-    void* params[] = {&args};
-    FLS_CUDA(cudaLaunchCooperativeKernel(p2plane_fn(), dim3(grid), dim3(kP2PlaneBlock), params, p2plane_smem(), st));
+    launch_cooperative(p2plane_gn_kernel<kP2PlaneBlock, kMinB>, grid, kP2PlaneBlock, p2plane_smem(), st, a);
 }
 
 // Per-batch preparation: state init, flag and ticket reset and the locality order of every scan, in one launch of one block per

@@ -867,32 +867,21 @@ __global__ void __launch_bounds__((W + 2) * 32, 1) p2plane_v9_kernel(P2PlaneLoop
 
 // 14 compute warps (+ server + folder: 512 threads) with a stage buffer of 352 candidates per warp and stage
 constexpr int kV9Warps = 14, kV9Cap = 352;
+constexpr size_t kV9Smem = V9Smem<kV9Warps, kV9Cap>::bytes + sizeof(P2PlaneScan) * kMaxBatch;
 
 }  // namespace
 
 // CTAs that serve a batch whose largest scan has n points: one per SM, fewer when there are not enough chunks to go round
 int p2plane_v9_grid(int n_max, int device) {
-    static int sms[64] = {0};
-    const int d = (device >= 0 && device < 64) ? device : 0;
-    if (!sms[d]) cudaDeviceGetAttribute(&sms[d], cudaDevAttrMultiProcessorCount, device);
+    raise_smem_limit((const void*)p2plane_v9_kernel<kV9Warps, kV9Cap>, kV9Smem, device);
     const int W = kV9Warps;
     const int need = ((n_max + 31) / 32 + W - 1) / W;
-    int g = need < sms[d] ? need : sms[d];
-    if (g > 192) g = 192;  // the second fold level holds 16 group rows of 12 CTAs
-    return g > 0 ? g : 1;
+    const int sms = device_sms(device);
+    return clamp_grid(need, sms < 192 ? sms : 192);  // the second fold level holds 16 group rows of 12 CTAs
 }
 
 void launch_p2plane_v9(const P2PlaneLoopArgs& a, int grid, cudaStream_t st) {
-    P2PlaneLoopArgs args = a;
-    void* params[] = {&args};
-    const void* fn = (const void*)p2plane_v9_kernel<kV9Warps, kV9Cap>;
-    const size_t smem = V9Smem<kV9Warps, kV9Cap>::bytes + sizeof(P2PlaneScan) * kMaxBatch;
-    static bool prepared = false;
-    if (!prepared) {
-        FLS_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        prepared = true;
-    }
-    FLS_CUDA(cudaLaunchCooperativeKernel(fn, dim3(grid), dim3((kV9Warps + 2) * 32), params, smem, st));
+    launch_cooperative(p2plane_v9_kernel<kV9Warps, kV9Cap>, grid, (kV9Warps + 2) * 32, kV9Smem, st, a);
 }
 
 }  // namespace fls
