@@ -354,8 +354,18 @@ int Handle::enqueue_ivox_batch(int B, const float4* const* d_scans, const size_t
             a.tickets = tickets.p;
             a.abort_word = tickets.p + (size_t)B * a.ticket_stride;
             launch_p2plane_v9(a, grid, stream);
-        } else {
-            launch_p2plane_loop(a, grid, stream);
+        } else {  // the single scan: the same buffers as scan 0's descriptor above
+            const P2PlaneArgs one{a.map, a.plane_thres, src_f.p, (int)n[0], rec0.p, rec1.p, flags.p};
+            GnLoopCtl ctl;
+            ctl.state = state.p;
+            ctl.ll_rows = ll_rows.p;
+            ctl.ll_pose = pose_base;
+            ctl.tag_base = tag_base;
+            ctl.gp = a.gp;
+            ctl.log = scan_log(0);
+            ctl.log_cap = log_cap;
+            ctl.result = scan_result(0);
+            launch_p2plane_loop(one, ctl, grid, stream);
         }
     });
     // ---- read back: every scan's state (+ its iteration log) ----------------------------------------------------------

@@ -1,7 +1,7 @@
 // fls_gn.cu — state initialisation of a Gauss-Newton loop (NDT / ICP / kd-tree LOAM; the LOAM-iVox path initialises its
 // states in its batch prep kernel), and the per-device kernel attributes that size and prepare every persistent launch.
-// The solve / update / stop rule itself (K6) is device code shared by every persistent kernel: gn_step / gn_handover in
-// fls_gn.cuh.
+// The solve / update / stop rule itself (K6) is device code in fls_gn.cuh: gn_step_pre, which every persistent kernel runs, and
+// the single-level fold around it (gn_handover / gn_handover_rows), which every one but the LOAM-iVox batch kernel uses.
 #include <map>
 #include <utility>
 

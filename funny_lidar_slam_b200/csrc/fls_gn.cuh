@@ -199,23 +199,11 @@ __device__ inline void gn_step_pre(GnState* s, const GnPre& q, const double* tot
     }
 }
 
-// Tail of one iteration of a persistent GN loop (all threads of all CTAs call it with their per-thread sums):
-// block reduction -> CTA row published as LL records (no fence, no atomic) -> CTA 0 sweeps the rows until every tag matches,
-// folds them in a fixed order, runs gn_step and publishes the next pose + stop word as LL records -> everybody polls that
-// record.  Needs co-resident CTAs (cooperative launch).  On return s_pose[0..11] (shared memory, row-major R then t) holds
-// the pose of the next iteration; returns true when the loop is finished.
+// Tail of one iteration of a persistent GN loop, in two halves; gn_handover below runs both.
+// gn_warp_rows: the shuffle reduction of every thread's sums into its warp's row of s_red.
 template <int BLOCK>
-__device__ __forceinline__ bool gn_handover(double (&acc)[kNumAcc], const GnLoopCtl& c, int it, double* s_pose, int cta = -1, int ncta = -1) {
-    // (cta, ncta): position of this CTA in the sub-grid that serves the scan (batch launches); default: the whole grid
-    if (cta < 0) {
-        cta = (int)blockIdx.x;
-        ncta = (int)gridDim.x;
-    }
-    constexpr int W = BLOCK / 32;
-    __shared__ double s_red[W][kAccStride];
-    __shared__ int s_stop;
+__device__ __forceinline__ void gn_warp_rows(const double (&acc)[kNumAcc], double (&s_red)[BLOCK / 32][kAccStride]) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const unsigned tag = c.tag_base | (unsigned)(it + 1);
 #pragma unroll
     for (int k = 0; k < kNumAcc; ++k) {
         double v = acc[k];
@@ -224,6 +212,24 @@ __device__ __forceinline__ bool gn_handover(double (&acc)[kNumAcc], const GnLoop
         if (lane == 0) s_red[warp][k] = v;
     }
     if (lane == 0) s_red[warp][kNumAcc] = 0.0;
+}
+
+// gn_handover_rows: every thread calls it once its warp's row of s_red (shared memory, like s_stop) is written; `tag` is the
+// LL tag of the iteration.  The CTA row (the warp rows summed in warp order) is published as LL records (no fence, no atomic)
+// -> CTA 0 sweeps the rows until every tag matches, folds them in a fixed order, runs gn_step and publishes the next pose +
+// stop word as LL records -> everybody polls that record.  Needs co-resident CTAs (cooperative launch).  On return
+// s_pose[0..11] (shared memory, row-major R then t) holds the pose of the next iteration and s_red is free; returns true when
+// the loop is finished.
+template <int BLOCK>
+__device__ __forceinline__ bool gn_handover_rows(double (&s_red)[BLOCK / 32][kAccStride], int& s_stop, const GnLoopCtl& c, unsigned tag,
+                                                 double* s_pose, int cta = -1, int ncta = -1) {
+    // (cta, ncta): position of this CTA in the sub-grid that serves the scan (batch launches); default: the whole grid
+    if (cta < 0) {
+        cta = (int)blockIdx.x;
+        ncta = (int)gridDim.x;
+    }
+    constexpr int W = BLOCK / 32;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     __syncthreads();
     if (warp == 0) {
         double v = 0;
@@ -293,6 +299,16 @@ __device__ __forceinline__ bool gn_handover(double (&acc)[kNumAcc], const GnLoop
     }
     __syncthreads();
     return s_stop != 0;
+}
+
+// The whole tail of iteration `it` from every thread's sums `acc`.
+template <int BLOCK>
+__device__ __forceinline__ bool gn_handover(double (&acc)[kNumAcc], const GnLoopCtl& c, int it, double* s_pose, int cta = -1, int ncta = -1) {
+    __shared__ double s_red[BLOCK / 32][kAccStride];
+    __shared__ int s_stop;
+    const unsigned tag = c.tag_base | (unsigned)(it + 1);
+    gn_warp_rows<BLOCK>(acc, s_red);
+    return gn_handover_rows<BLOCK>(s_red, s_stop, c, tag, s_pose, cta, ncta);
 }
 #endif
 

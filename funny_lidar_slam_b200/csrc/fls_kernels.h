@@ -19,7 +19,7 @@ struct PoseArg {
     double t[3];
 };
 
-// One scan of a batch (device-resident descriptor read by the persistent LoamPointToPlaneIVOX kernel)
+// One scan of a batch (device-resident descriptor read by the LoamPointToPlaneIVOX batch kernel, v9)
 struct P2PlaneScan {
     const float4* src;  // body-frame scan in Morton order of the query voxel, packed float4
     int n;
@@ -29,29 +29,39 @@ struct P2PlaneScan {
     float4* rec1;  //                              J4, J5, |d|, 1
     unsigned char* flags;
     uint4* rows;     // [grid][32] LL records {lo, tag, hi, tag}: one per CTA and sum
-    uint4* ll_pose;  // [kLlPoseLen] LL records: next pose + stop word, published by the folding CTA
+    uint4* ll_pose;  // [kLlPoseLen] LL records: next pose + stop word, published by the scan's folder
     fls_iter_log* log;
     double* result;  // optional packed result (kResultLen doubles), written by the folder when the scan stops
-    uint4* grows;    // v9: [16][32] LL records: group rows of the two-level fold
+    uint4* grows;    // [16][32] LL records: group rows of the two-level fold
 };
 
-// whole-loop arguments of the persistent LoamPointToPlaneIVOX kernel (K1 + fused K6); one launch = a batch of scans
+// whole-loop arguments of the LoamPointToPlaneIVOX batch kernel (v9, K1 + fused K6); one launch = a batch of scans
 struct P2PlaneLoopArgs {
     IvoxView map;
     double plane_thres;
     GnParams gp;
     int log_cap;
-    const P2PlaneScan* scans;  // [n_scans]; every CTA serves every scan, CTA (s mod grid) folds and solves scan s
+    const P2PlaneScan* scans;  // [n_scans]; CTAs draw chunks of any scan, the folder warp of CTA (12 s + 1) mod grid solves scan s
     int n_scans;
-    unsigned* tickets;  // v9: chunk ticket counters [n_scans][ticket_stride], zeroed before the launch
+    unsigned* tickets;  // chunk ticket counters [n_scans][ticket_stride], zeroed before the launch
     int ticket_stride;  // >= max_iterations + 2
-    unsigned* abort_word;  // v9 watchdog: zeroed before the launch, non-zero when a wait loop gave up (protocol error)
+    unsigned* abort_word;  // watchdog: zeroed before the launch, non-zero when a wait loop gave up (protocol error)
 };
 // Each persistent kernel below is sized by its *_grid call on the device it then runs on (see coresident_ctas, fls_common.cuh).
+// generation 8 (fls_p2plane.cu): the single-scan Match
+struct P2PlaneArgs {
+    IvoxView map;
+    double plane_thres;
+    const float4* src;  // body-frame scan in Morton order of the query voxel (prepare_queries), packed float4
+    int n;
+    float4* rec0;  // persistent per-point record: J0..J3
+    float4* rec1;  //                              J4, J5, |d|, 1
+    unsigned char* flags;
+};
 int p2plane_chunks(int n);             // warp-sized (32-point) work chunks
 int p2plane_grid(int n, int device);    // CTAs that serve a scan of n points: its chunks / warps per CTA, + the folder, <= co-resident
-void launch_p2plane_loop(const P2PlaneLoopArgs& a, int grid, cudaStream_t st);
-// generation 9 of the same loop (fls_p2plane_v9.cu): barrier-free dataflow, TMA-staged candidate runs, DMMA sums
+void launch_p2plane_loop(const P2PlaneArgs& a, const GnLoopCtl& ctl, int grid, cudaStream_t st);
+// generation 9 (fls_p2plane_v9.cu), batches: barrier-free dataflow, TMA-staged candidate runs, DMMA sums
 int p2plane_v9_grid(int n_max, int device);  // also raises the kernel's shared-memory limit on `device`
 void launch_p2plane_v9(const P2PlaneLoopArgs& a, int grid, cudaStream_t st);
 // queries of a batch are put in locality order in tiles of this many consecutive points; a tile never spans two scans

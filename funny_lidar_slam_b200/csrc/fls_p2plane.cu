@@ -1,23 +1,22 @@
-// fls_p2plane.cu — K1 (+ fused K6), generation 8: the whole LoamPointToPlaneIVOX Gauss-Newton loop as ONE persistent kernel with a
-// CTA barrier per visit.  It serves the single Match (fls_match / fls_match_device); batches run on generation 9
+// fls_p2plane.cu — K1 (+ fused K6), generation 8: the whole LoamPointToPlaneIVOX Gauss-Newton loop of ONE scan as one persistent
+// kernel with a CTA barrier per iteration.  It serves the single Match (fls_match / fls_match_device); batches run on generation 9
 // (fls_p2plane_v9.cu), which shares the per-point arithmetic (fls_knn.cuh, fls_plane.cuh).  This file also holds the per-batch query
 // preparation (one kernel: state init + tile-local locality sort), the Match-internal insertion rule of mapping mode and the k-NN test entry.
 //
 // Per source point and iteration it fuses what LoamPointToPlaneIVOX::PlanerMatch / ::SumCoefficient do
 // (include/registration/loam_point_to_plane_ivox.h:256-340 upstream): transform with the current pose, bounded
 // 5-NN in the iVox map, least-squares plane through the 5 neighbours (normal equations, column-pivoted Householder QR as the
-// fallback, fp64), validity / near-point gates, J (6) and |d|, and the 21+6+2 Gauss-Newton sums; the scan's folding CTA reduces
+// fallback, fp64), validity / near-point gates, J (6) and |d|, and the 21+6+2 Gauss-Newton sums; the folding CTA reduces
 // the CTA rows in a fixed order, solves the 6x6 system, updates the pose and applies the stop rule (:167-203), then publishes the
 // next pose.  No host round trip inside a Match.
 //
 // Mapping onto the GPU
 //   * grid = the CTAs the scan's chunks need (one 24-warp CTA per SM, 768 threads, 80 registers) + the folding CTA, launched
 //     cooperatively only to guarantee co-residency; the scheduling unit is the WARP: warp w of CTA c works on 32-point chunk
-//     (c, w) of every scan of the visit group, a static round-robin (consecutive chunks stay in one CTA: Morton neighbours share
-//     candidate runs in L1);
-//   * a visit = one Gauss-Newton iteration of up to 8 scans: poses in (LL records), chunks, one __syncthreads, CTA rows out (LL
-//     records, no fence, no atomic); only the scan's folding CTA waits for the other rows — 24 warps x 8 loads in flight sweep
-//     them until every tag matches, sums in a fixed order (bitwise reproducible for a given grid), gn_step, next pose out;
+//     (c, w), a static round-robin (consecutive chunks stay in one CTA: Morton neighbours share candidate runs in L1);
+//   * an iteration = chunks, then the shared hand-over (gn_handover_rows, fls_gn.cuh): one __syncthreads, CTA row out (LL
+//     records, no fence, no atomic); only CTA 0 waits for the other rows — 24 warps x 8 loads in flight sweep them until every
+//     tag matches, sums in a fixed order (bitwise reproducible for a given grid), gn_step, next pose out, every CTA polls it;
 //   * queries are processed in Morton order of their voxel (sorted once per Match), so the lanes of a warp share
 //     centre voxels: the table probe and the candidate stream are the same addresses -> L1 broadcast, no divergence;
 //   * k-NN = 1 probe of the centre table + a streaming scan of that centre's contiguous stencil list (fls_ivox.cuh),
@@ -134,19 +133,14 @@ __device__ __forceinline__ bool p2plane_point(const IvoxView& map, const float4 
 // columns of the per-point staging record
 constexpr int kRecAd = 6, kRecValid = 7, kRecCand = 8, kRecHits = 9, kRecOne = 10, kRecW = 12;
 
-constexpr int kVisitGroup = 8;  // most scans whose chunks a warp works through between two CTA barriers
-
 template <int BLOCK, int MINB>
-__global__ void __launch_bounds__(BLOCK, MINB) p2plane_gn_kernel(P2PlaneLoopArgs a) {
+__global__ void __launch_bounds__(BLOCK, MINB) p2plane_gn_kernel(P2PlaneArgs a, GnLoopCtl ctl) {
     constexpr int W = BLOCK / 32;
-    constexpr int V = kVisitGroup < W ? kVisitGroup : W;
     extern __shared__ __align__(16) unsigned char s_dyn[];
     double (*s_rec)[32][kRecW] = reinterpret_cast<double (*)[32][kRecW]>(s_dyn);  // [W][32][kRecW] per-lane staging records
-    double (*s_part)[W][32] = reinterpret_cast<double (*)[W][32]>(s_dyn + sizeof(double) * W * 32 * kRecW);  // [V][W][32] per scan of the group: every warp's 32 sums
-    __shared__ double s_pose[V][12];
-    __shared__ double s_red[W][32];      // fold scratch of the folding CTA
-    __shared__ int s_stop[V];
-    __shared__ unsigned char s_iter[kMaxBatch];  // iterations this CTA has completed of every scan (255 = scan finished)
+    __shared__ double s_red[W][kAccStride];  // every warp's 32 sums
+    __shared__ int s_stop;
+    __shared__ double s_pose[12];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int G = (int)gridDim.x, cta = (int)blockIdx.x;
     const int n_warps = G * W;
@@ -172,201 +166,56 @@ __global__ void __launch_bounds__(BLOCK, MINB) p2plane_gn_kernel(P2PlaneLoopArgs
     } else {
         sgn = 0.0;
     }
-    if (threadIdx.x < kMaxBatch) s_iter[threadIdx.x] = 0;
+    // iteration 0 starts from the state the prep kernel wrote; gn_handover_rows leaves every later pose in s_pose
+    if (threadIdx.x < 12) s_pose[threadIdx.x] = threadIdx.x < 9 ? __ldcg(&ctl.state->R[threadIdx.x]) : __ldcg(&ctl.state->t[threadIdx.x - 9]);
     __syncthreads();
-
-    // One launch serves a batch of independent scans and EVERY CTA works on EVERY scan: the grid sweeps the scans round-
-    // robin, one Gauss-Newton iteration of each scan per visit, up to V scans per visit.  Inside a visit a warp works
-    // through its chunk of every scan of the group back to back — the CTA barrier that ends the visit then waits for the
-    // slowest SUM of V chunks instead of V times for the slowest chunk.  A visit ends with this CTA's rows of partial sums
-    // going out as LL records; only a scan's folding CTA waits for the other rows, solves and publishes the next pose —
-    // everybody else moves straight on, and by the time the sweep returns to a scan its pose has long been published.  The
-    // hand-over latency of one scan is hidden behind the work on the others; finished scans drop out of the sweep, so the
-    // remaining ones come round faster (no static partition of the SMs, no idle CTAs).
-    // With a single scan the sweep degenerates to: work, publish, wait for the pose.
-    int n_left = a.n_scans;
-    int next = 0;  // where the sweep continues
-    while (n_left > 0) {
-        // ---- the group: the next (up to V) unfinished scans in round-robin order (uniform: s_iter is shared) -------------
-        int gs[V], git[V], nv = 0;
-        for (int k = 0; k < a.n_scans && nv < V; ++k) {
-            const int s = (next + k) % a.n_scans;
-            const int it = s_iter[s];
-            if (it == 255) continue;
-            gs[nv] = s;
-            git[nv] = it;
-            ++nv;
-        }
-        next = (gs[nv - 1] + 1) % a.n_scans;
-        // ---- poses of this visit: the prep kernel's state for iteration 0, afterwards the LL record published by the
-        // scan's folder at the end of iteration it-1 (12 values + the stop word); 16 threads per scan of the group
-        {
-            const int v = threadIdx.x >> 4, k = threadIdx.x & 15;
-            if (v < nv && k < 13) {
-                const P2PlaneScan* __restrict__ sc = a.scans + gs[v];
-                if (git[v] == 0) {
-                    if (k < 9) s_pose[v][k] = __ldcg(&sc->state->R[k]);
-                    else if (k < 12) s_pose[v][k] = __ldcg(&sc->state->t[k - 9]);
-                    else s_stop[v] = 0;
+    const int n_chunks = (a.n + 31) >> 5;  // warp-sized chunks
+    // CTA 0 folds, so it takes the last block of chunks: it is the CTA that stays idle when the scan has fewer chunks than
+    // the grid has warps (p2plane_grid adds one CTA for that purpose)
+    const int slot = (cta - 1 + G) % G;
+    for (int it = 0;; ++it) {  // ends on the stop word, which gn_step raises at max_iterations at the latest
+        double acc = 0.0;  // lane k's running sum over every chunk of this warp
+        // warp-granular work loop, static round-robin over 32-point chunks: no barrier, no atomics inside
+        // (consecutive chunks stay in one CTA: Morton neighbours share candidate lists in L1 — spreading them over SMs
+        //  for balance was measured 35 % slower)
+        for (int chunk = slot * W + warp; chunk < n_chunks; chunk += n_warps) {
+            const int i = (chunk << 5) + lane;
+            double J[6] = {0, 0, 0, 0, 0, 0}, ad = 0.0, vflag = 0.0;
+            unsigned n_cand = 0, n_fb = 0;
+            if (i < a.n) {
+                const float4 sp = a.src[i];
+                bool use = p2plane_point(a.map, sp, s_pose, a.plane_thres, J, ad, n_cand, n_fb);
+                if (use) {
+                    a.rec0[i] = make_float4((float)J[0], (float)J[1], (float)J[2], (float)J[3]);
+                    a.rec1[i] = make_float4((float)J[4], (float)J[5], (float)ad, 1.0f);
+                    a.flags[i] = 1;
+                } else if (a.flags[i]) {  // stale contribution [quirk 1]
+                    const float4 r0 = a.rec0[i], r1 = a.rec1[i];
+                    J[0] = r0.x; J[1] = r0.y; J[2] = r0.z; J[3] = r0.w; J[4] = r1.x; J[5] = r1.y;
+                    ad = r1.z;
+                    use = true;
                 } else {
-                    const unsigned ptag = sc->tag_base | (unsigned)git[v];
-                    const uint4* ll = sc->ll_pose;
-                    double val;
-                    while (!ll_load(ll + k, ptag, val)) __nanosleep(100);
-                    if (k < 12) s_pose[v][k] = val;
-                    else s_stop[v] = val != 0.0;
+#pragma unroll
+                    for (int k = 0; k < 6; ++k) J[k] = 0.0;
+                    ad = 0.0;
                 }
+                vflag = use ? 1.0 : 0.0;
             }
-        }
-        __syncthreads();
-        bool live[V];
+            double* rec = s_rec[warp][lane];
 #pragma unroll
-        for (int v = 0; v < V; ++v) {
-            live[v] = v < nv && !s_stop[v];
-            if (v < nv && s_stop[v]) {  // uniform: the scan finished with iteration it-1
-                if (threadIdx.x == 0) s_iter[gs[v]] = 255;
-                --n_left;
-            }
-        }
-        // ---- work: this warp's chunks of every live scan of the group, no barrier in between ---------------------------
-#pragma unroll 1
-        for (int v = 0; v < nv; ++v) {
-            if (!live[v]) continue;
-            const int s = gs[v];
-            const P2PlaneScan* __restrict__ sc = a.scans + s;
-            const int folder = s % G;
-            const int n = sc->n;
-            const int n_chunks = (n + 31) >> 5;  // warp-sized chunks
-            const float4* __restrict__ src = sc->src;
-            float4* __restrict__ rec0 = sc->rec0;
-            float4* __restrict__ rec1 = sc->rec1;
-            unsigned char* __restrict__ flags = sc->flags;
-            // the folder takes the last block of chunks: it is the CTA that stays idle when the scan has fewer chunks than
-            // the grid has warps (p2plane_grid adds one CTA for that purpose)
-            const int slot = (cta - folder - 1 + G) % G;
-            const double* pose = s_pose[v];
-
-            double acc = 0.0;  // lane k's running sum over every chunk of this warp
-            // warp-granular work loop, static round-robin over 32-point chunks: no barrier, no atomics inside
-            // (consecutive chunks stay in one CTA: Morton neighbours share candidate lists in L1 — spreading them over SMs
-            //  for balance was measured 35 % slower; letting the CTA's warps pull the V x W chunk lists of a visit from a
-            //  shared counter was measured too: 709 vs 704 us per 8-scan launch, no gain)
-            for (int chunk = slot * W + warp; chunk < n_chunks; chunk += n_warps) {
-                const int i = (chunk << 5) + lane;
-                double J[6] = {0, 0, 0, 0, 0, 0}, ad = 0.0, vflag = 0.0;
-                unsigned n_cand = 0, n_fb = 0;
-                if (i < n) {
-                    const float4 sp = src[i];
-                    bool use = p2plane_point(a.map, sp, pose, a.plane_thres, J, ad, n_cand, n_fb);
-                    if (use) {
-                        rec0[i] = make_float4((float)J[0], (float)J[1], (float)J[2], (float)J[3]);
-                        rec1[i] = make_float4((float)J[4], (float)J[5], (float)ad, 1.0f);
-                        flags[i] = 1;
-                    } else if (flags[i]) {  // stale contribution [quirk 1]
-                        const float4 r0 = rec0[i], r1 = rec1[i];
-                        J[0] = r0.x; J[1] = r0.y; J[2] = r0.z; J[3] = r0.w; J[4] = r1.x; J[5] = r1.y;
-                        ad = r1.z;
-                        use = true;
-                    } else {
-#pragma unroll
-                        for (int k = 0; k < 6; ++k) J[k] = 0.0;
-                        ad = 0.0;
-                    }
-                    vflag = use ? 1.0 : 0.0;
-                }
-                double* rec = s_rec[warp][lane];
-#pragma unroll
-                for (int k = 0; k < 6; ++k) rec[k] = J[k];
-                rec[kRecAd] = ad;
-                rec[kRecValid] = vflag;
-                rec[kRecCand] = (double)n_cand;
-                rec[kRecHits] = (double)n_fb;  // points that took the QR path (diagnostic; reported as hits_total)
-                rec[kRecOne] = 1.0;
-                __syncwarp();
+            for (int k = 0; k < 6; ++k) rec[k] = J[k];
+            rec[kRecAd] = ad;
+            rec[kRecValid] = vflag;
+            rec[kRecCand] = (double)n_cand;
+            rec[kRecHits] = (double)n_fb;  // points that took the QR path (diagnostic; reported as hits_total)
+            rec[kRecOne] = 1.0;
+            __syncwarp();
 #pragma unroll 8
-                for (int p = 0; p < 32; ++p) acc += s_rec[warp][p][ca] * s_rec[warp][p][cb];
-                __syncwarp();
-            }
-            s_part[v][warp][lane] = acc * sgn;
+            for (int p = 0; p < 32; ++p) acc += s_rec[warp][p][ca] * s_rec[warp][p][cb];
+            __syncwarp();
         }
-        __syncthreads();
-        // ---- CTA rows: warp v publishes the row of the group's v-th scan — LL records, no fence, no atomic ---------------
-        if (warp < nv && live[warp]) {
-            const P2PlaneScan* __restrict__ sc = a.scans + gs[warp];
-            double val = 0;
-#pragma unroll
-            for (int w = 0; w < W; ++w) val += s_part[warp][w][lane];
-            ll_store(sc->rows + (size_t)cta * 32 + lane, val, sc->tag_base | (unsigned)(git[warp] + 1));
-        }
-        // ---- folds: for the scans of the group this CTA is the folder of -------------------------------------------------
-#pragma unroll 1
-        for (int v = 0; v < nv; ++v) {
-            if (!live[v] || cta != gs[v] % G) continue;  // uniform per CTA
-            const P2PlaneScan* __restrict__ sc = a.scans + gs[v];
-            GnState* const state = sc->state;
-            const int it = git[v];
-            const unsigned tag = sc->tag_base | (unsigned)(it + 1);
-            uint4* const rows = sc->rows;
-            // warp w owns rows w, w+W, ...; every sweep re-reads all of them (independent loads, one L2 round trip) until
-            // each carries this iteration's tag, then the sums are taken in a fixed order — bitwise reproducible, and the
-            // fold is finished one sweep after the slowest CTA's row lands
-            GnPre pre;
-            if (threadIdx.x == 0) gn_load(state, pre);  // off the critical path: the state is stable until gn_step below
-            const int nrows = G;
-            double sum;
-            for (;;) {
-                bool ok = true;
-                double a0 = 0, a1 = 0, a2 = 0, a3 = 0;
-                int r = warp;
-                for (; r + 7 * W < nrows; r += 8 * W) {  // 8 independent 16-byte loads in flight per lane
-                    double v0, v1, v2, v3, v4, v5, v6, v7;
-                    const bool k0 = ll_load(rows + (size_t)r * 32 + lane, tag, v0);
-                    const bool k1 = ll_load(rows + (size_t)(r + W) * 32 + lane, tag, v1);
-                    const bool k2 = ll_load(rows + (size_t)(r + 2 * W) * 32 + lane, tag, v2);
-                    const bool k3 = ll_load(rows + (size_t)(r + 3 * W) * 32 + lane, tag, v3);
-                    const bool k4 = ll_load(rows + (size_t)(r + 4 * W) * 32 + lane, tag, v4);
-                    const bool k5 = ll_load(rows + (size_t)(r + 5 * W) * 32 + lane, tag, v5);
-                    const bool k6 = ll_load(rows + (size_t)(r + 6 * W) * 32 + lane, tag, v6);
-                    const bool k7 = ll_load(rows + (size_t)(r + 7 * W) * 32 + lane, tag, v7);
-                    ok = ok && k0 && k1 && k2 && k3 && k4 && k5 && k6 && k7;
-                    a0 += v0; a1 += v1; a2 += v2; a3 += v3;
-                    a0 += v4; a1 += v5; a2 += v6; a3 += v7;
-                }
-                for (; r + 3 * W < nrows; r += 4 * W) {
-                    double v0, v1, v2, v3;
-                    const bool k0 = ll_load(rows + (size_t)r * 32 + lane, tag, v0);
-                    const bool k1 = ll_load(rows + (size_t)(r + W) * 32 + lane, tag, v1);
-                    const bool k2 = ll_load(rows + (size_t)(r + 2 * W) * 32 + lane, tag, v2);
-                    const bool k3 = ll_load(rows + (size_t)(r + 3 * W) * 32 + lane, tag, v3);
-                    ok = ok && k0 && k1 && k2 && k3;
-                    a0 += v0; a1 += v1; a2 += v2; a3 += v3;
-                }
-                for (; r < nrows; r += W) {
-                    double v0;
-                    ok = ok && ll_load(rows + (size_t)r * 32 + lane, tag, v0);
-                    a0 += v0;
-                }
-                sum = (a0 + a1) + (a2 + a3);
-                if (__all_sync(0xffffffffu, ok)) break;
-                __nanosleep(100);
-            }
-            s_red[warp][lane] = sum;
-            __syncthreads();
-            if (warp == 0) {
-                double t = 0;
-#pragma unroll
-                for (int w = 0; w < W; ++w) t += s_red[w][lane];
-                __syncwarp();
-                s_red[0][lane] = t;
-                __syncwarp();
-                if (lane == 0) gn_step_pre(state, pre, s_red[0], a.gp, sc->log, a.log_cap, sc->ll_pose, tag, sc->result);
-            }
-            __syncthreads();  // s_red is reused by the next fold
-        }
-        if (threadIdx.x == 0)
-            for (int v = 0; v < nv; ++v)
-                if (live[v]) s_iter[gs[v]] = (unsigned char)(git[v] + 1);
-        __syncthreads();  // s_part / s_pose / s_stop / s_iter are reused by the next visit
+        s_red[warp][lane] = acc * sgn;
+        if (gn_handover_rows<BLOCK>(s_red, s_stop, ctl, ctl.tag_base | (unsigned)(it + 1), s_pose)) break;
     }
 }
 
@@ -386,7 +235,8 @@ __device__ __forceinline__ unsigned spread_bits3(unsigned v) {  // up to 10 bits
 // point falls into at its initial pose: the 3-D Morton code of the low 4 bits per axis (an 8 m cube) and 2 more bits each of
 // x and y (wrap-around beyond that only costs locality, never correctness).  Lanes of a warp then share centre voxels; a
 // voxel whose points fall into two tiles is visited from two chunks.  The order is a fixed function of the input (block radix
-// sort, ties in the sort's fixed order), so the per-point records and the single-scan kernel's sums stay reproducible.
+// sort, ties in the sort's fixed order), so the per-point records and the single-scan kernel's sums stay reproducible.  A single
+// Match is the batch of one; its kernel starts from the state written here.
 constexpr int kOrdThreads = 512, kOrdItems = kOrderTile / kOrdThreads;
 
 __global__ void __launch_bounds__(kOrdThreads) p2plane_prep_kernel(const float4* const* __restrict__ scan_ptrs, const int* __restrict__ offsets,
@@ -559,10 +409,7 @@ __global__ void ivox_insert_scatter_kernel(const unsigned char* __restrict__ cls
 
 // One 768-thread CTA per SM: 24 resident warps (<= 80 registers).
 constexpr int kMinB = 1;
-size_t p2plane_smem() {
-    constexpr int W = kP2PlaneBlock / 32, V = kVisitGroup < W ? kVisitGroup : W;
-    return (size_t)W * 32 * kRecW * sizeof(double) + (size_t)V * W * 32 * sizeof(double);
-}
+size_t p2plane_smem() { return (size_t)(kP2PlaneBlock / 32) * 32 * kRecW * sizeof(double); }
 
 }  // namespace
 
@@ -575,8 +422,8 @@ int p2plane_grid(int n, int device) {
     return clamp_grid(need + 1, coresident_ctas((const void*)p2plane_gn_kernel<kP2PlaneBlock, kMinB>, kP2PlaneBlock, p2plane_smem(), device));
 }
 
-void launch_p2plane_loop(const P2PlaneLoopArgs& a, int grid, cudaStream_t st) {
-    launch_cooperative(p2plane_gn_kernel<kP2PlaneBlock, kMinB>, grid, kP2PlaneBlock, p2plane_smem(), st, a);
+void launch_p2plane_loop(const P2PlaneArgs& a, const GnLoopCtl& ctl, int grid, cudaStream_t st) {
+    launch_cooperative(p2plane_gn_kernel<kP2PlaneBlock, kMinB>, grid, kP2PlaneBlock, p2plane_smem(), st, a, ctl);
 }
 
 // Per-batch preparation: state init, flag and ticket reset and the locality order of every scan, in one launch of one block per
