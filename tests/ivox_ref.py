@@ -229,6 +229,75 @@ def normal_error_bound(cond, rho, share):
 
 
 @dataclass
+class PlaneTerm:
+    """One point's PlanerMatch term (J, |d|), its gate margins and the bounds dJ, dad on how far fp64 may move J and |d|."""
+    valid: bool
+    J: np.ndarray          # (6,) 0 unless valid
+    ad: float
+    plane_margin: float    # thres - max_j |A_j c + 1| / |c|   (> 0: the plane gate passes; nan: |c| = 0)
+    near_margin: float     # (|p| - 81 d^2) / |p|             (>= 0: the near-point gate passes; nan: not reached)
+    normal_err: float      # bound on the relative error of the fp64 normal (normal_error_bound)
+    rank: int
+    scale: float           # largest coordinate magnitude of the neighbourhood
+    dJ: np.ndarray         # (6,)
+    dad: float
+
+
+def plane_term(A, q, ps, R, plane_thres, qr_rule=False):
+    """The plane term shared by every LOAM plug-in (loam_point_to_plane_ivox.h:275-321 == loam_point_to_plane_kdtree.h:226-269 ==
+    loam_full_kdtree.h:295-342 upstream) for the five fp32 neighbours A (nearest first), the transformed fp32 query q, the body-frame
+    point ps and the rotation R, with the plane solved in 50-digit arithmetic.  qr_rule: take the plane from colpiv_qr (the only
+    reference for neighbourhoods whose rank is decided by rounding)."""
+    A = np.asarray(A, np.float64)
+    q = np.asarray(q, F32)
+    if qr_rule:
+        cq, rank = colpiv_qr(A)
+        c, cond = [mpmath.mpf(float(x)) for x in cq], 0.0
+    else:
+        c, rank, cond = _plane_mp(A)
+    t = PlaneTerm(False, np.zeros(6), 0.0, np.nan, np.nan, 0.0, rank, float(np.abs(A).max()), np.zeros(6), 0.0)
+    with mpmath.workdps(50):
+        cn = mpmath.sqrt(c[0] ** 2 + c[1] ** 2 + c[2] ** 2)
+        if cn == 0:
+            return t
+        resid = mpmath.sqrt(mpmath.fsum((sum(mpmath.mpf(float(A[j, a])) * c[a] for a in range(3)) + 1) ** 2 for j in range(5)))
+        rho = float(resid / (mpmath.mpf(float(np.linalg.norm(A))) * cn))
+    t.normal_err = ne = normal_error_bound(cond, rho, ldlt_share(A))
+    with mpmath.workdps(50):
+        worst = max(abs(sum(mpmath.mpf(float(A[j, a])) * c[a] for a in range(3)) + 1) / cn for j in range(5))
+        t.plane_margin = float(plane_thres - worst)
+        if worst > plane_thres:
+            return t
+        nrm = [x / cn for x in c]
+        d = sum((mpmath.mpf(float(q[a])) - mpmath.mpf(float(A[0, a]))) * nrm[a] for a in range(3))  # from the nearest [quirk 2]
+        ps = np.asarray(ps, F32)[:3].astype(np.float64)
+        pn = float(np.linalg.norm(ps))
+        t.near_margin = float((mpmath.mpf(pn) - 81 * d * d) / pn) if pn > 0 else -np.inf
+        if pn < 81 * float(d) ** 2:  # body-frame norm [quirk 3]
+            return t
+    nf = np.array([float(x) for x in nrm])
+    s = 1.0 if d > 0 else -1.0
+    Rp = np.asarray(R, np.float64) @ ps
+    t.valid = True
+    t.J = np.concatenate([np.cross(Rp, nf) * s, nf * s])
+    t.ad = abs(float(d))
+    t.dJ[:3] = (np.linalg.norm(Rp) + 1.0) * (ne + 4 * EPS)
+    t.dJ[3:] = ne + 4 * EPS
+    t.dad = float(np.linalg.norm(q.astype(np.float64) - A[0])) * ne + 4 * EPS * float(np.abs(q).max())
+    return t
+
+
+def sum_bounds(J, dJ, r, dr):
+    """Per-entry bounds on H = sum J J^T and g = -sum J r of terms whose J and r are known to within dJ and dr (rows: terms),
+    plus 1e-9 of sum |J_a J_b| for the summation itself.  Returns (tol_H, tol_g)."""
+    aJ, ar = np.abs(np.asarray(J, np.float64)), np.abs(np.asarray(r, np.float64))
+    dJ, dr = np.asarray(dJ, np.float64), np.asarray(dr, np.float64)
+    tol_H = aJ.T @ dJ + dJ.T @ aJ + dJ.T @ dJ + 1e-9 * (aJ.T @ aJ)
+    tol_g = dJ.T @ ar + aJ.T @ dr + dJ.T @ dr + 1e-9 * (aJ.T @ ar)
+    return tol_H, tol_g
+
+
+@dataclass
 class PlanarPass:
     H: np.ndarray          # (6, 6) sum of J J^T over valid points
     g: np.ndarray          # (6,) sum of -J |d|
@@ -270,46 +339,12 @@ def planar_pass(map_pts, scan, T, plane_thres=0.1, res=0.5, nearby=2, max_range=
     for i in range(n):
         if kn.found[i] < 5:  # :271-273
             continue
-        A = map_pts[kn.idx[i], :3].astype(np.float64)
-        if qr_rule:
-            cq, rank[i] = colpiv_qr(A)
-            c, cond = [mpmath.mpf(float(x)) for x in cq], 0.0
-        else:
-            c, rank[i], cond = _plane_mp(A)
-        scale[i] = float(np.abs(A).max())
-        with mpmath.workdps(50):
-            cn = mpmath.sqrt(c[0] ** 2 + c[1] ** 2 + c[2] ** 2)
-            if cn == 0:
-                continue
-            resid = mpmath.sqrt(mpmath.fsum((sum(mpmath.mpf(float(A[j, a])) * c[a] for a in range(3)) + 1) ** 2 for j in range(5)))
-            rho = float(resid / (mpmath.mpf(float(np.linalg.norm(A))) * cn))
-        ne[i] = normal_error_bound(cond, rho, ldlt_share(A))
-        with mpmath.workdps(50):
-            worst = max(abs(sum(mpmath.mpf(float(A[j, a])) * c[a] for a in range(3)) + 1) / cn for j in range(5))
-            pm[i] = float(plane_thres - worst)
-            if worst > plane_thres:  # :286-293
-                continue
-            nrm = [x / cn for x in c]
-            d = sum((mpmath.mpf(float(q[i, a])) - mpmath.mpf(float(A[0, a]))) * nrm[a] for a in range(3))  # :306, from the nearest
-            ps = scan[i, :3].astype(np.float64)
-            pn = float(np.linalg.norm(ps))
-            nm[i] = float((mpmath.mpf(pn) - 81 * d * d) / pn) if pn > 0 else -np.inf
-            if pn < 81 * float(d) ** 2:  # :309 body-frame norm
-                continue
-            nf = np.array([float(x) for x in nrm])
-            s = 1.0 if d > 0 else -1.0
-            Rp = R @ ps
-            J[i] = np.concatenate([np.cross(Rp, nf) * s, nf * s])
-            ad[i] = abs(float(d))
-            valid[i] = True
-            dJ[i, :3] = (np.linalg.norm(Rp) + 1.0) * (ne[i] + 4 * EPS)
-            dJ[i, 3:] = ne[i] + 4 * EPS
-            dad[i] = float(np.linalg.norm(q[i].astype(np.float64) - A[0])) * ne[i] + 4 * EPS * float(np.abs(q[i]).max())
+        t = plane_term(map_pts[kn.idx[i], :3], q[i], scan[i, :3], R, plane_thres, qr_rule)  # :274-321
+        valid[i], J[i], ad[i], pm[i], nm[i], ne[i], rank[i], scale[i], dJ[i], dad[i] = (
+            t.valid, t.J, t.ad, t.plane_margin, t.near_margin, t.normal_err, t.rank, t.scale, t.dJ, t.dad)
     H = np.einsum("ni,nj->ij", J[valid], J[valid])
     g = -(J[valid] * ad[valid, None]).sum(0)
-    aJ = np.abs(J)
-    tol_H = aJ.T @ dJ + dJ.T @ aJ + dJ.T @ dJ + 1e-9 * (aJ.T @ aJ)
-    tol_g = dJ.T @ ad + aJ.T @ dad + dJ.T @ dad + 1e-9 * (aJ.T @ ad)
+    tol_H, tol_g = sum_bounds(J, dJ, ad, dad)
     return PlanarPass(H, g, int(valid.sum()), valid, J, ad, pm, nm, ne, rank, scale, kn, tol_H, tol_g)
 
 
