@@ -76,6 +76,19 @@ class FlsNdtVoxel(C.Structure):
                 ("mu", C.c_double * 3), ("info", C.c_double * 6)]
 
 
+class FlsGnStepCase(C.Structure):
+    _fields_ = [("method", C.c_int32), ("max_iterations", C.c_int32), ("min_effective", C.c_int32), ("iter", C.c_int32),
+                ("rot_thres", C.c_double), ("pos_thres", C.c_double), ("R", C.c_double * 9), ("t", C.c_double * 3),
+                ("last_rot", C.c_double), ("last_pos", C.c_double), ("tot", C.c_double * 31)]
+
+
+class FlsGnStepOut(C.Structure):
+    _fields_ = [("R", C.c_double * 9), ("t", C.c_double * 3), ("dx", C.c_double * 6), ("H", C.c_double * 36), ("g", C.c_double * 6),
+                ("last_rot", C.c_double), ("last_pos", C.c_double), ("published", C.c_double * 13), ("result", C.c_double * 18),
+                ("det_spd", C.c_double), ("n_valid", C.c_int64), ("iter", C.c_int32), ("converged", C.c_int32), ("failed", C.c_int32),
+                ("done", C.c_int32), ("spd", C.c_int32), ("published_ok", C.c_int32)]
+
+
 class FlsFeatureCfg(C.Structure):
     _fields_ = [("corner_threshold", C.c_float), ("planar_threshold", C.c_float), ("device", C.c_int32), ("reserved", C.c_int32)]
 

@@ -19,7 +19,7 @@ EXPORTS = [
     "fls_set_result_buffer_device", "fls_get_voxel_keys", "fls_get_map_points", "fls_ivox_add_points", "fls_preprocess", "fls_project_imu", "fls_match_batch_begin", "fls_match_batch_begin_device", "fls_match_batch_end", "fls_set_global_map", "fls_update_local_map",
     "fls_pcd_read", "fls_pcd_write", "fls_preprocess_loam", "fls_match_cluster_device", "fls_convert_cloud", "fls_preprocess_loam_device",
     "fls_preprocess_device", "fls_keyframes_create", "fls_keyframes_destroy", "fls_keyframes_add", "fls_keyframes_add_device",
-    "fls_keyframes_count", "fls_keyframes_assemble", "fls_get_ndt_voxels",
+    "fls_keyframes_count", "fls_keyframes_assemble", "fls_get_ndt_voxels", "fls_gn_step_probe",
 ]
 
 
@@ -78,6 +78,7 @@ def lib():
     L.fls_get_voxel_keys.argtypes = [vp, vp, sz, C.POINTER(sz)]
     L.fls_get_map_points.argtypes = [vp, vp, sz, C.POINTER(sz)]
     L.fls_get_ndt_voxels.argtypes = [vp, vp, sz, C.POINTER(sz)]
+    L.fls_gn_step_probe.argtypes = [vp, vp, sz, vp]
     L.fls_ivox_knn.argtypes = [vp, vp, sz, sz, C.c_int, vp, vp]
     L.fls_ivox_add_points.argtypes = [vp, vp, sz, sz]
     L.fls_voxel_grid.argtypes = [C.c_int, vp, sz, sz, f32, vp, C.POINTER(sz)]

@@ -242,6 +242,32 @@ class Registration:
         return [dict(H=np.array(b.H).reshape(6, 6), g=np.array(b.g), dx=np.array(b.dx), sum_residual=b.sum_residual, n_valid=b.n_valid)
                 for b in buf[:n]]
 
+    def gn_step_probe(self, cases):
+        """One Gauss-Newton step (solve, pose update, stop rule) per case on the handle's device: fls_gn_step_probe.  A case is a dict
+        with method, max_iterations, min_effective, iter, rot_thres, pos_thres, R (3x3), t (3), last_rot, last_pos and tot (31 totals:
+        upper-triangular H row by row, g, n_valid, sum of residuals, candidates, hits).  Returns one dict per case: the post-step
+        R, t, dx, H, g, last_rot, last_pos, n_valid, iter, converged, failed, done, the published R / t / stop word, the result record
+        (NaN where none was written), spd (the LDL^T fast path accepted the system), det_spd and published_ok."""
+        n = len(cases)
+        cin = (_abi.FlsGnStepCase * max(n, 1))()
+        for c, d in zip(cin, cases):
+            c.method, c.max_iterations, c.min_effective, c.iter = int(d["method"]), int(d["max_iterations"]), int(d["min_effective"]), int(d["iter"])
+            c.rot_thres, c.pos_thres = float(d["rot_thres"]), float(d["pos_thres"])
+            c.R[:] = [float(v) for v in np.asarray(d["R"], np.float64).reshape(9)]
+            c.t[:] = [float(v) for v in np.asarray(d["t"], np.float64).reshape(3)]
+            c.last_rot, c.last_pos = float(d["last_rot"]), float(d["last_pos"])
+            c.tot[:] = [float(v) for v in np.asarray(d["tot"], np.float64).reshape(31)]
+        cout = (_abi.FlsGnStepOut * max(n, 1))()
+        check(lib().fls_gn_step_probe(self._h, cin, n, cout), "fls_gn_step_probe")
+        out = []
+        for o in cout[:n]:
+            pub = np.array(o.published)
+            out.append(dict(R=np.array(o.R).reshape(3, 3), t=np.array(o.t), dx=np.array(o.dx), H=np.array(o.H).reshape(6, 6), g=np.array(o.g),
+                            last_rot=o.last_rot, last_pos=o.last_pos, n_valid=o.n_valid, iter=o.iter, converged=o.converged, failed=o.failed,
+                            done=o.done, published_R=pub[:9].reshape(3, 3), published_t=pub[9:12], published_stop=pub[12],
+                            result=np.array(o.result), spd=bool(o.spd), det_spd=o.det_spd, published_ok=bool(o.published_ok)))
+        return out
+
     def map_info(self) -> FlsMapInfo:
         mi = FlsMapInfo()
         check(lib().fls_get_map_info(self._h, C.byref(mi)), "fls_get_map_info")
@@ -276,6 +302,17 @@ def create_matcher(mode: str, **params) -> Registration:
     if mode not in _abi.METHOD_BY_MODE_STRING:
         raise ValueError(f"unknown registration_and_searcher_mode {mode!r}")
     return Registration(_abi.default_config(_abi.METHOD_BY_MODE_STRING[mode], **params))
+
+
+def gn_step_probe(cases, device: int = 0):
+    """Registration.gn_step_probe on a scratch handle of `device` (the step reads nothing of a handle but its device and stream)."""
+    cfg = _abi.default_config(_abi.FLS_P2PLANE_IVOX)
+    cfg.device = device
+    r = Registration(cfg)
+    try:
+        return r.gn_step_probe(cases)
+    finally:
+        r.close()
 
 
 def voxel_grid(points: np.ndarray, leaf: float, device: int = 0) -> np.ndarray:

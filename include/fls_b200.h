@@ -247,6 +247,36 @@ typedef struct {
 /* Every live voxel of the FLS_NDT map, sorted by key (x, then y, then z).  Read-only introspection for the map parity tests; writes at
  * most `capacity` records and returns the voxel count in *n.  FLS_ERR_UNSUPPORTED for other plug-ins. */
 int fls_get_ndt_voxels(fls_handle* h, fls_ndt_voxel* out, size_t capacity, size_t* n);
+
+/* Test hook: one Gauss-Newton step (the 6x6 solve, pose update and stop rule every persistent Match kernel runs after its sums) on
+ * N independent cases, one device thread per case, in one launch on the handle's device and stream.  Read-only: the handle's map
+ * and state are untouched.  A case is the pre-step state of a loop, the parameters of fls_config that the step reads, and the
+ * reduced totals of one iteration in the kernels' layout: 21 upper-triangular entries of H (row by row), 6 of g, the sum of
+ * residuals, n_valid and two traffic counters. */
+typedef struct {
+    int32_t method;         /* fls_method */
+    int32_t max_iterations;
+    int32_t min_effective;  /* NDT: ndt_min_effective_pts; the LOAM plug-ins: 50 */
+    int32_t iter;           /* iterations executed before this step */
+    double rot_thres, pos_thres;
+    double R[9];            /* row-major rotation before the step */
+    double t[3];
+    double last_rot, last_pos; /* LOAM: the dx norms of the previous iteration (0 before iteration 0) */
+    double tot[31];         /* H (21), g (6), valid count, sum of residuals, candidates, table hits */
+} fls_gn_step_case;
+typedef struct {
+    double R[9], t[3];      /* state after the step (row-major R) */
+    double dx[6], H[36], g[6];
+    double last_rot, last_pos;
+    double published[13];   /* what the step published for the other CTAs: R[9], t[3], stop word (1.0 / 0.0) */
+    double result[18];      /* the result record (fls_set_result_buffer_device layout); NaN where the step wrote none */
+    double det_spd;         /* product of the LDL^T pivots when the fast path accepted the system, else 0 */
+    int64_t n_valid;
+    int32_t iter, converged, failed, done;
+    int32_t spd;            /* the register LDL^T fast path accepted the system (else the pivoting solver ran) */
+    int32_t published_ok;   /* every published record carried the iteration's tag */
+} fls_gn_step_out;
+int fls_gn_step_probe(fls_handle* h, const fls_gn_step_case* cases, size_t n, fls_gn_step_out* out);
 /* The points the FLS_P2PLANE_IVOX map holds (packed x, y, z, intensity), in insertion order; at most `capacity` points are written, the
  * count is returned in *n.  Introspection for the map parity tests. */
 int fls_get_map_points(fls_handle* h, float* xyzi, size_t capacity, size_t* n);
