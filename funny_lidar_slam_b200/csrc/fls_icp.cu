@@ -5,11 +5,25 @@
 // nearest map point and then rejects it when d^2 > max_correspond_distance [quirk 4: squared distance against
 // an unsquared threshold].  A correspondence can therefore only survive inside radius sqrt(threshold), so a
 // uniform grid with cell >= that radius searched over its 27-cell neighbourhood returns the identical
-// correspondence for every accepted point and "nothing" exactly where upstream rejects.
+// correspondence for every accepted point and "nothing" exactly where upstream rejects.  IcpPlugin at the end is the plug-in's host
+// half: its sliding-window local map, AddCloudToLocalMap and Match.
+#include <cmath>
+
 #include "fls_gn.cuh"
-#include "fls_kernels.h"
+#include "fls_handle.h"
 
 namespace fls {
+
+static constexpr int kIcpBlock = 512;  // 64 queries x 8 lanes per CTA: few rows for the folder
+
+struct IcpArgs {
+    const float4* __restrict__ src;  // voxel-filtered scan, body frame
+    int n;
+    IvoxView map;  // floor-keyed search grid over the voxel-filtered local map
+    double max_corr;
+    GnState* state;
+};
+
 namespace {
 
 // nearest map point within the 27-cell neighbourhood; returns false when the neighbourhood is empty
@@ -195,11 +209,11 @@ __global__ void fitness_kernel(IvoxView g, const float4* __restrict__ src, int n
 
 }  // namespace
 
-int icp_grid_blocks(int n, int device) {
+static int icp_grid_blocks(int n, int device) {
     const int per_block = kIcpBlock / kIcpLanes;
     return clamp_grid((n + per_block - 1) / per_block, coresident_ctas((const void*)icp_gn_kernel<kIcpBlock>, kIcpBlock, 0, device));
 }
-void launch_icp_loop(const IcpArgs& a, const GnLoopCtl& ctl, int grid, cudaStream_t st) {
+static void launch_icp_loop(const IcpArgs& a, const GnLoopCtl& ctl, int grid, cudaStream_t st) {
     launch_cooperative(icp_gn_kernel<kIcpBlock>, grid, kIcpBlock, 0, st, a, ctl);
 }
 
@@ -211,5 +225,68 @@ void launch_fitness(const IvoxView& g, const float4* d_src, int n, const double*
     fitness_kernel<<<grid, 256, 0, st>>>(g, d_src, n, (float)T[0], (float)T[4], (float)T[8], (float)T[1], (float)T[5], (float)T[9], (float)T[2],
                                          (float)T[6], (float)T[10], (float)T[12], (float)T[13], (float)T[14], max_range, d_out2);
 }
+
+// ---- IcpOptimized ------------------------------------------------------------------------------------------------
+
+class IcpPlugin final : public Plugin {
+    WindowMap window;  // cloud_deque_ / local_map_ptr_ (icp_optimized.h:173-187, 246)
+    KeyFrameGate gate;
+    DevBuf<float4> scan;  // VoxelGridCloud of the source (:57)
+    DevBuf<float4> ins;   // Match-internal insert: the filtered scan at its final pose
+
+  public:
+    explicit IcpPlugin(Handle& handle) : Plugin(handle, kOrdered) {
+        // search grid of the bounded exact 1-NN: cell >= sqrt(max_correspond_distance)  [quirk 4]
+        const double d = h.cfg.icp_max_correspond_distance;
+        window.grid.key_mode = 1;
+        window.grid.set_resolution((float)(std::sqrt(d > 0 ? d : 1.0) * 1.001));
+    }
+
+    int add_cloud(const float4* d_cloud, size_t n, const float4*, size_t) override {
+        // icp_optimized.h:173-187: mapping mode slides a window of the last local_map_size clouds, localization mode replaces
+        // the map; both end in local_map_ptr_ = VoxelGridCloud(local_map_ptr_, map_cloud_filter_size_)
+        const int rc = window_add(window, d_cloud, n, (size_t)h.cfg.local_map_size, h.cfg.map_cloud_filter_size, true, h.cfg.localization_mode != 0,
+                                  h.scratch, h.stream, &h.launches);
+        h.set_fit_view(window.cloud.p, window.n);  // GetFitnessScore searches the same cloud
+        return rc;
+    }
+
+    int match(const float4* d_in, size_t n_in, const float4*, size_t, double* T, int* converged, fls_match_stats* st) override {
+        const fls_config& cfg = h.cfg;
+        if (n_in <= 10) return FLS_ERR_TOO_FEW_POINTS;  // CHECK_GT(ordered_cloud_.size(), 10u)  (:55)
+        if (window.grid.n_pts == 0) return FLS_ERR_NO_MAP;
+        scan.reserve(n_in);
+        const size_t n = voxel_grid_device(d_in, n_in, cfg.source_cloud_filter_size, scan.p, h.scratch, h.stream, &h.launches);  // :57
+        const int ni = (int)n;
+        const int grid = icp_grid_blocks(ni, cfg.device);
+        IcpArgs a;
+        a.src = scan.p;
+        a.n = ni;
+        a.map = h.grid_view(window.grid);
+        a.max_corr = cfg.icp_max_correspond_distance;
+        a.state = h.state.p;
+        // roofline accounting (SURVEY.md §8d, K3): 16 B source point + 27 x 16 B slot probes, 16 B per scanned map record
+        h.match_single(FLS_ICP_P2P, 0, grid, 16 + 16LL * 27, 16, scan.p, n, n, T, converged, st,
+                       [&](const GnLoopCtl& ctl) { launch_icp_loop(a, ctl, grid, h.stream); });
+        // IsNeedAddCloud (:218-236): key-frame gating on translation / RPY deltas against a persistent last_T
+        if (h.h_state->converged && !cfg.localization_mode && gate.need(T, cfg.dist_thre_add_cloud, cfg.rot_thre_add_cloud)) {
+            ins.reserve(n);
+            launch_transform_f(scan.p, n, T, ins.p, h.stream);  // :156 TransformPointCloud(source, final) in float
+            h.launches++;
+            return h.inserted(add_cloud(ins.p, n, nullptr, 0), st);
+        }
+        return FLS_OK;
+    }
+
+    void map_info(fls_map_info* out) const override {
+        const IvoxMap& g = window.grid;
+        out->n_points = (long long)g.n_pts;
+        out->n_voxels = (long long)g.n_vox;
+        out->table_slots = g.n_pts ? (long long)g.mask + 1 : 0;
+        out->bytes = (long long)g.bytes();
+    }
+};
+
+std::unique_ptr<Plugin> make_icp_plugin(Handle& h) { return std::make_unique<IcpPlugin>(h); }
 
 }  // namespace fls

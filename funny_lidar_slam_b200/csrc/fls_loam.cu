@@ -16,12 +16,43 @@
 // The loop structure is the shared persistent one (gn_handover, fls_gn.cuh): one thread per feature point, corner
 // points first then planar points (the order upstream sums them, :347-372), every class with its own persistent
 // {J, residual} record and flag byte for the "flags reset once per Match" rule [quirk 1].
+//
+// KdPlugin at the end is the host half both plug-ins share: the sliding-window planar (and LoamFull's corner) local map,
+// AddCloudToLocalMap and Match.
+#include <cmath>
+
 #include "fls_eig.cuh"
 #include "fls_gn.cuh"
-#include "fls_kernels.h"
+#include "fls_handle.h"
 #include "fls_plane.cuh"
 
 namespace fls {
+
+static constexpr int kLoamBlock = 256;
+
+// exact unbounded 5-NN over a uniform grid
+struct LoamGrid {
+    const float4* __restrict__ pts;    // cell-contiguous map points
+    const HashSlot* __restrict__ tab;  // floor-keyed occupied-cell table
+    unsigned mask;
+    float inv_cell, cell;
+    unsigned n_pts;
+};
+struct LoamArgs {
+    const float4* __restrict__ corner;  // body-frame corner features (LoamFull only)
+    int n_corner;
+    const float4* __restrict__ planar;  // body-frame planar features
+    int n_planar;
+    LoamGrid corner_map, planar_map;
+    double plane_thres;    // point_to_planar_thres
+    double search_thres;   // point_search_thres on the 5th squared distance (+inf: none)
+    double line_ratio;     // line_ratio_thres
+    float gate;            // search_thres as the search's stop bound
+    GnState* state;
+    double* __restrict__ rec;  // [n_corner + n_planar][8] persistent {J[6], residual, -}
+    unsigned char* __restrict__ flags;
+};
+
 namespace {
 
 constexpr int kMaxShell = 6;
@@ -220,15 +251,137 @@ __global__ void loam_clear_flags_kernel(unsigned char* flags, int n) {
 
 }  // namespace
 
-int loam_grid_blocks(int n, int device) {
+static int loam_grid_blocks(int n, int device) {
     const int per_block = kLoamBlock / kLoamLanes;
     return clamp_grid((n + per_block - 1) / per_block, coresident_ctas((const void*)loam_gn_kernel<kLoamBlock>, kLoamBlock, 0, device));
 }
 
-void launch_loam_loop(const LoamArgs& a, const GnLoopCtl& ctl, int grid, cudaStream_t st) {
+static void launch_loam_loop(const LoamArgs& a, const GnLoopCtl& ctl, int grid, cudaStream_t st) {
     const int n = a.n_corner + a.n_planar;
     if (n > 0) loam_clear_flags_kernel<<<(n + 255) / 256, 256, 0, st>>>(a.flags, n);
     launch_cooperative(loam_gn_kernel<kLoamBlock>, grid, kLoamBlock, 0, st, a, ctl);
 }
+
+// ---- LoamPointToPlaneKdtree / LoamFull -------------------------------------------------------------------------------
+
+static LoamGrid loam_grid_of(const WindowMap& w) {
+    LoamGrid g;
+    g.pts = w.grid.pts_sorted.p;
+    g.tab = w.grid.table.p;
+    g.mask = w.grid.mask;
+    g.inv_cell = w.grid.inv_res;
+    g.cell = w.grid.res;
+    g.n_pts = (unsigned)w.grid.n_pts;
+    return g;
+}
+
+static void window_info(const WindowMap& w, fls_map_info* out) {
+    out->n_points += (long long)w.n;
+    out->n_voxels += (long long)w.grid.n_vox;
+    out->table_slots += w.n ? (long long)w.grid.mask + 1 : 0;
+    out->bytes += (long long)(w.grid.bytes() + w.cloud.bytes());
+}
+
+class KdPlugin final : public Plugin {
+    const bool full;             // LoamFull: {planar, corner} maps and features
+    WindowMap planar;            // planar_cloud_deque_ and the search grid over it
+    std::unique_ptr<WindowMap> corner;  // corner_cloud_deque_ and its grid: LoamFull only
+    KeyFrameGate gate;
+    DevBuf<double> rec;          // persistent {J[6], residual} records
+    DevBuf<unsigned char> flags;
+    DevBuf<float4> ins, ins_corner;  // Match-internal insert: the features at their final pose
+
+  public:
+    explicit KdPlugin(Handle& handle) : Plugin(handle, handle.cfg.method == FLS_LOAM_FULL ? kPlanarCorner : kPlanar), full(reads == kPlanarCorner) {
+        const fls_config& cfg = h.cfg;
+        // exact-search grids: LoamFull only needs neighbours inside sqrt(point_search_thres), so a cell of that size settles every
+        // query in the 27-cell pass; the ungated point-to-plane variant uses ~2 map leafs
+        planar.grid.key_mode = 1;
+        if (full) {
+            const float c = (float)(std::sqrt(cfg.point_search_thres > 0 ? cfg.point_search_thres : 1.0) * 1.001);
+            planar.grid.set_resolution(c);
+            corner = std::make_unique<WindowMap>();
+            corner->grid.key_mode = 1;
+            corner->grid.set_resolution(c);
+        } else {
+            const float c = 2.0f * (cfg.map_cloud_filter_size > 0.f ? cfg.map_cloud_filter_size : 0.5f);
+            planar.grid.set_resolution(c < 0.8f ? 0.8f : c);
+        }
+    }
+
+    int add_cloud(const float4* d_planar, size_t n_planar, const float4* d_corner, size_t n_corner) override {
+        const fls_config& cfg = h.cfg;
+        if (!full) {
+            // loam_point_to_plane_kdtree.h:56-80: localization mode replaces the map, mapping mode slides a window; both
+            // end in VoxelGridCloud(local_map, map_cloud_filter_size) + kd-tree
+            const int rc = window_add(planar, d_planar, n_planar, (size_t)cfg.local_map_size, cfg.map_cloud_filter_size, true, cfg.localization_mode != 0,
+                                      h.scratch, h.stream, &h.launches);
+            if (rc == FLS_OK) h.set_fit_cloud(planar.cloud.p, planar.n);  // GetFitnessScore searches the same tree (:159-183)
+            return rc;
+        }
+        // loam_full_kdtree.h:66-104: {planar, corner}, both windows slide, filters only beyond 5 clouds
+        const int rc = window_add(planar, d_planar, n_planar, (size_t)cfg.local_map_size, cfg.map_cloud_filter_size, false, false, h.scratch, h.stream,
+                                  &h.launches);
+        if (rc != FLS_OK) return rc;
+        return window_add(*corner, d_corner, n_corner, (size_t)cfg.corner_local_map_size, cfg.corner_map_filter_size, false, false, h.scratch, h.stream,
+                          &h.launches);
+    }
+
+    int match(const float4* d_planar, size_t n_planar, const float4* d_corner, size_t n_corner, double* T, int* converged,
+              fls_match_stats* st) override {
+        const fls_config& cfg = h.cfg;
+        if (planar.n == 0) return FLS_ERR_NO_MAP;
+        const size_t n = n_planar + n_corner;
+        const int ni = (int)n;
+        const int grid = loam_grid_blocks(ni, cfg.device);
+        rec.reserve(n * 8 + 8);
+        flags.reserve(n + 1);
+        LoamArgs a;
+        a.corner = d_corner;
+        a.n_corner = (int)n_corner;
+        a.planar = d_planar;
+        a.n_planar = (int)n_planar;
+        a.planar_map = loam_grid_of(planar);
+        a.corner_map = full ? loam_grid_of(*corner) : a.planar_map;
+        a.plane_thres = cfg.point_to_planar_thres;
+        a.search_thres = full ? cfg.point_search_thres : INFINITY;
+        a.line_ratio = cfg.line_ratio_thres;
+        a.gate = full ? (float)cfg.point_search_thres * 1.0001f : INFINITY;
+        a.state = h.state.p;
+        a.rec = rec.p;
+        a.flags = flags.p;
+        // roofline accounting (K5): 16 B source point + 27 x 16 B slot probes + 56 B persistent record, 16 B per scanned map record
+        h.match_single(cfg.method, 50, grid, 16 + 16LL * 27 + 56, 16, d_planar, n_planar, n, T, converged, st, [&](const GnLoopCtl& ctl) {
+            launch_loam_loop(a, ctl, grid, h.stream);
+            h.launches++;  // the flag reset in front of the loop
+        });
+        // key-frame insertion: loam_point_to_plane_kdtree.h:146-150 (gate evaluated before the mode test), loam_full_kdtree.h:178-186
+        if (h.h_state->converged && gate.need(T, cfg.dist_thre_add_cloud, cfg.rot_thre_add_cloud) && (full || !cfg.localization_mode)) {
+            int rc2;
+            if (full) {
+                ins.reserve(n_planar);
+                ins_corner.reserve(n_corner);
+                launch_transform_d(d_planar, n_planar, T, ins.p, h.stream);  // pcl::transformPointCloud(cloud, out, T_) with the double matrix
+                launch_transform_d(d_corner, n_corner, T, ins_corner.p, h.stream);
+                h.launches += 2;
+                rc2 = add_cloud(ins.p, n_planar, ins_corner.p, n_corner);
+            } else {
+                ins.reserve(n_planar);
+                launch_transform_f(d_planar, n_planar, T, ins.p, h.stream);  // TransformPointCloud(source, final): fp32 with R, t cast to float
+                h.launches++;
+                rc2 = add_cloud(ins.p, n_planar, nullptr, 0);
+            }
+            return h.inserted(rc2, st);
+        }
+        return FLS_OK;
+    }
+
+    void map_info(fls_map_info* out) const override {  // planar map (+ corner map for LoamFull)
+        window_info(planar, out);
+        if (full) window_info(*corner, out);
+    }
+};
+
+std::unique_ptr<Plugin> make_kd_plugin(Handle& h) { return std::make_unique<KdPlugin>(h); }
 
 }  // namespace fls

@@ -1,7 +1,8 @@
 // fls_localmap.cu — the localization-mode map path around the matcher (SURVEY.md §8f-4):
 //   * Localization::LoadLocalMap, the global-map branch (src/slam/localization.cpp:364-410 upstream): the global map stays in HBM;
 //     when the pose comes within 50 m of an edge of the current local map (or there is none) a +-100 m pcl::CropBox around the
-//     pose is cut on the device (stream compaction, input order kept) and handed to AddCloudToLocalMap without leaving the GPU;
+//     pose is cut on the device (stream compaction, input order kept) and handed to the plug-in's AddCloudToLocalMap without leaving
+//     the GPU;
 //   * the PCD files behind it (pcl::io::loadPCDFile / savePCDFileBinary as used by include/common/keyframe.h:24-74 and
 //     localization.cpp:283-300): a reader / writer for x y z intensity clouds, DATA binary and ascii.
 #include <cub/cub.cuh>
@@ -32,7 +33,7 @@ __global__ void crop_flags_kernel(const float4* __restrict__ p, size_t n, float 
 }  // namespace
 
 int Handle::set_global_map(const void* pts, size_t n, size_t stride) {
-    const float4* d = upload(pts, n, stride, stage);
+    const float4* d = upload(pts, n, stride, up_cloud);
     global_map.reserve(n + 1);
     if (n) FLS_CUDA(cudaMemcpyAsync(global_map.p, d, n * sizeof(float4), cudaMemcpyDeviceToDevice, stream));
     global_n = n;
@@ -59,16 +60,16 @@ int Handle::update_local_map(const double* T, int* updated, size_t* n_local) {
     }
     have_edge = true;
     crop_keep.reserve(global_n + 1);
-    stage2.reserve(global_n + 1);
+    local_map.reserve(global_n + 1);
     scratch.num_runs.reserve(2);
     crop_flags_kernel<<<(unsigned)((global_n + 255) / 256), 256, 0, stream>>>(global_map.p, global_n, (float)local_edge[0], (float)local_edge[1],
                                                                             (float)local_edge[2], (float)local_edge[3], (float)local_edge[4],
                                                                             (float)local_edge[5], crop_keep.p);  // :401-402 .cast<float>()
     size_t tb = 0;
-    cub::DeviceSelect::Flagged(nullptr, tb, global_map.p, crop_keep.p, stage2.p, scratch.num_runs.p, (int)global_n, stream);
+    cub::DeviceSelect::Flagged(nullptr, tb, global_map.p, crop_keep.p, local_map.p, scratch.num_runs.p, (int)global_n, stream);
     scratch.cub_tmp.reserve(tb + 256);
     tb = scratch.cub_tmp.cap;
-    FLS_CUDA(cub::DeviceSelect::Flagged(scratch.cub_tmp.p, tb, global_map.p, crop_keep.p, stage2.p, scratch.num_runs.p, (int)global_n, stream));
+    FLS_CUDA(cub::DeviceSelect::Flagged(scratch.cub_tmp.p, tb, global_map.p, crop_keep.p, local_map.p, scratch.num_runs.p, (int)global_n, stream));
     FLS_CUDA(cudaMemcpyAsync(scratch.h_num_runs, scratch.num_runs.p, sizeof(int), cudaMemcpyDeviceToHost, stream));
     FLS_CUDA(cudaStreamSynchronize(stream));
     const size_t m = (size_t)*scratch.h_num_runs;
@@ -76,22 +77,9 @@ int Handle::update_local_map(const double* T, int* updated, size_t* n_local) {
     if (n_local) *n_local = m;
     if (updated) *updated = 1;
     if (m == 0) return FLS_OK;  // `local_map->empty()`: the caller gives up (:129-131); the matcher keeps its map
-    // matcher_->AddCloudToLocalMap({*local_map}) (:135, :222) — the cloud is already on the device
-    switch (cfg.method) {
-        case FLS_P2PLANE_IVOX: {
-            if (cfg.localization_mode) ivox.clear();
-            else if (ivox.n_pts != 0) return FLS_ERR_UNSUPPORTED;
-            const int rc = ivox.append_and_build(stage2.p, m, cfg.ivox_capacity, stream);
-            launches += ivox.launches;
-            ivox.launches = 0;
-            if (cfg.localization_mode) set_fit_cloud(stage2.p, m);
-            return rc;
-        }
-        case FLS_NDT: return add_cloud_ndt(stage2.p, m);
-        case FLS_ICP_P2P: return add_cloud_icp(stage2.p, m);
-        case FLS_P2PLANE_KNN: return add_cloud_kd(stage2.p, m, nullptr, 0);
-        default: return FLS_ERR_UNSUPPORTED;  // LoamFull takes {planar, corner} maps
-    }
+    // matcher_->AddCloudToLocalMap({*local_map}) (:135, :222) — the cloud is already on the device; LoamFull takes {planar, corner} maps
+    if (plugin->reads == Plugin::kPlanarCorner) return FLS_ERR_UNSUPPORTED;
+    return plugin->add_cloud(local_map.p, m, nullptr, 0);
 }
 
 // ---- PCD --------------------------------------------------------------------------------------------------------------------

@@ -7,7 +7,8 @@
 // The stable sort keeps insertion order inside a voxel, so the k-NN tie order matches a sequential insert.
 // LRU eviction (capacity_, ivox_map.cpp:133-136) is emulated exactly: every point carries its insertion stamp, the stamp of a
 // voxel's last point is its position in upstream's list, and the sequential insert of a call is simulated on the host against
-// the candidates (IvoxMap::evict_lru, lru_simulate).
+// the candidates (IvoxMap::evict_lru, lru_simulate).  window_add keeps the sliding-window local map of the ICP and kd-tree LOAM
+// plug-ins on top of such a grid.
 #include <cub/cub.cuh>
 
 #include <cstdlib>
@@ -325,7 +326,7 @@ void launch_transform_f(const float4* d_in, size_t n, const double* T, float4* d
 }
 
 // keys -> stable sort -> gather -> run-length encode -> starts: the voxel-contiguous order of the first n points of pts_all
-int IvoxMap::sort_and_runs(size_t n, cudaStream_t st, int* runs_out) {
+int IvoxMap::sort_and_runs(size_t n, cudaStream_t st, int* runs_out, int* launches) {
     BuildScratch& sc = scratch;
     sc.keys.reserve(n);
     sc.keys_sorted.reserve(n);
@@ -360,7 +361,7 @@ int IvoxMap::sort_and_runs(size_t n, cudaStream_t st, int* runs_out) {
     const int runs = *sc.h_num_runs;
     tb = sc.cub_tmp.cap;
     FLS_CUDA(cub::DeviceScan::ExclusiveSum(sc.cub_tmp.p, tb, sc.counts.p, sc.starts.p, runs, st));
-    launches += 6;
+    *launches += 6;
     *runs_out = runs;
     return FLS_OK;
 }
@@ -372,7 +373,7 @@ int IvoxMap::sort_and_runs(size_t n, cudaStream_t st, int* runs_out) {
 // redirected.  The space left behind is garbage until the next full build, which happens when the slack runs out, when a table
 // would exceed its load factor, when the garbage outweighs the live data, or when the LRU has to evict.
 // Returns 1 when the caller has to take the full path instead.
-int IvoxMap::append_incremental(const float4* d_new, size_t n_new, long long capacity, cudaStream_t st) {
+int IvoxMap::append_incremental(const float4* d_new, size_t n_new, long long capacity, cudaStream_t st, int* launches) {
     if (!incremental || n_pts == 0 || n_stencil <= 0 || n_new == 0) return 1;
     BuildScratch& sc = scratch;
     const size_t S = (size_t)n_stencil;
@@ -435,7 +436,7 @@ int IvoxMap::append_incremental(const float4* d_new, size_t n_new, long long cap
     FLS_CUDA(cudaMemcpyAsync(&last_cnt, inc_new_count.p + (T - 1), sizeof(unsigned), cudaMemcpyDeviceToHost, st));
     FLS_CUDA(cudaMemcpyAsync(&n_aff, sc.num_runs.p + 1, sizeof(int), cudaMemcpyDeviceToHost, st));
     FLS_CUDA(cudaStreamSynchronize(st));
-    launches += 9;
+    *launches += 9;
     const int n_created = hc[0];
     const size_t moved = (size_t)last_off + last_cnt;  // points of the rewritten voxels
     // has to take the full path: eviction, no room, table load
@@ -465,7 +466,7 @@ int IvoxMap::append_incremental(const float4* d_new, size_t n_new, long long cap
     const int n_new_centres = hc[0];
     unsigned long long old_records = 0;
     std::memcpy(&old_records, hc + 2, sizeof(old_records));
-    launches += 5;
+    *launches += 5;
     // From here on the point array and the occupied table are already updated; if the lists do not fit, the caller's full build
     // regenerates everything from pts_all (which it extends itself), so nothing is lost.
     if (lists_end + run_total > lists.cap || lists_end + run_total > 0xfffffff0ull) return 1;
@@ -474,7 +475,7 @@ int IvoxMap::append_incremental(const float4* d_new, size_t n_new, long long cap
     list_fill_kernel<<<grid_for((size_t)n_aff * 32, 256), 256, 0, st>>>(cuniq.p, n_aff, n_stencil, table.p, mask, pts_sorted.p, cstart.p, ccount.p, lists.p,
                                                                        ctab.p, cmask);
     FLS_CUDA(cudaGetLastError());
-    launches += 2;
+    *launches += 2;
     // bookkeeping
     pts_end += moved;
     pts_garbage += moved - n_new;  // the old copies of the rewritten voxels
@@ -488,7 +489,7 @@ int IvoxMap::append_incremental(const float4* d_new, size_t n_new, long long cap
     return FLS_OK;
 }
 
-int IvoxMap::append_and_build(const float4* d_new, size_t n_new, long long capacity, cudaStream_t st) {
+int IvoxMap::append_and_build(const float4* d_new, size_t n_new, long long capacity, cudaStream_t st, int* launches) {
     // mapping mode: append without touching the rest of the map whenever that is possible
     if (incremental && n_pts > 0 && n_new > 0 && (lists_garbage < n_list + (n_list >> 1)) && (pts_garbage < 2 * n_pts)) {
         // pts_all / stamp_all first (the full path and the LRU read them)
@@ -499,17 +500,18 @@ int IvoxMap::append_and_build(const float4* d_new, size_t n_new, long long capac
                 ++call_no;
                 ivox_stamp_kernel<<<grid_for(n_new, 256), 256, 0, st>>>(stamp_all.p + n_old0, n_new, call_no << 32);
             }
-            const int rc = append_incremental(d_new, n_new, capacity, st);
+            const int rc = append_incremental(d_new, n_new, capacity, st, launches);
             if (rc == FLS_OK) return FLS_OK;
             if (rc < 0) return rc;
             // full path below: pts_all / stamp_all already hold the new points
-            return build_full(n_old0, n0, capacity, st, /*appended=*/true);
+            return build_full(n_old0, n0, capacity, st, launches, /*appended=*/true);
         }
     }
-    return build_full(n_pts, n_pts + n_new, capacity, st, false, d_new, n_new);
+    return build_full(n_pts, n_pts + n_new, capacity, st, launches, false, d_new, n_new);
 }
 
-int IvoxMap::build_full(size_t n_old, size_t n_in, long long capacity, cudaStream_t st, bool appended, const float4* d_new, size_t n_new) {
+int IvoxMap::build_full(size_t n_old, size_t n_in, long long capacity, cudaStream_t st, int* launches, bool appended, const float4* d_new,
+                        size_t n_new) {
     size_t n = n_in;
     if (n == 0) return FLS_OK;
     if (n > 0xfffffff0ull) return FLS_ERR_INVALID_ARG;
@@ -539,15 +541,15 @@ int IvoxMap::build_full(size_t n_old, size_t n_in, long long capacity, cudaStrea
         }
     }
     int runs = 0;
-    int rc = sort_and_runs(n, st, &runs);
+    int rc = sort_and_runs(n, st, &runs, launches);
     if (rc != FLS_OK) return rc;
     if (lru && (long long)runs >= capacity) {
         // IVoxMap::AddPoints would have evicted the LRU tail while inserting (ivox_map.cpp:133-136): drop those voxels' old points
         size_t n_after = n;
-        rc = evict_lru(n_old, n, runs, capacity, st, &n_after);
+        rc = evict_lru(n_old, n, runs, capacity, st, &n_after, launches);
         if (rc != FLS_OK) return rc;
         n = n_after;
-        rc = sort_and_runs(n, st, &runs);
+        rc = sort_and_runs(n, st, &runs, launches);
         if (rc != FLS_OK) return rc;
     }
     size_t slots = 1024;
@@ -562,16 +564,16 @@ int IvoxMap::build_full(size_t n_old, size_t n_in, long long capacity, cudaStrea
     n_vox = (size_t)runs;
     pts_end = n;
     pts_garbage = 0;
-    launches += 2;
+    *launches += 2;
     ++n_full;
-    if (n_stencil > 0) return build_stencil_lists(st);
+    if (n_stencil > 0) return build_stencil_lists(st, launches);
     return FLS_OK;
 }
 
 // Exact LRU of IVoxMap::AddPoints for this call (see lru_simulate): a voxel's position in upstream's list is the insertion time of
 // its last point, so the stamps of the points are all the state there is.  Victims lose every point they held before the call;
 // one that is touched again later in the call keeps this call's points (it is created anew).  Compacts pts_all / stamp_all.
-int IvoxMap::evict_lru(size_t n_old, size_t n, int runs, long long capacity, cudaStream_t st, size_t* n_after) {
+int IvoxMap::evict_lru(size_t n_old, size_t n, int runs, long long capacity, cudaStream_t st, size_t* n_after, int* launches) {
     BuildScratch& sc = scratch;
     if (n_vox == 0) return FLS_ERR_CAPACITY;  // the first cloud alone overflows the capacity
     lru_old.reserve((size_t)runs + 1);
@@ -607,7 +609,7 @@ int IvoxMap::evict_lru(size_t n_old, size_t n, int runs, long long capacity, cud
     std::vector<unsigned> victims;
     std::vector<unsigned char> recreated;
     if (!lru_simulate(n_vox, (size_t)capacity, cand, creat, victims, recreated)) return FLS_ERR_CAPACITY;
-    launches += 4;
+    *launches += 4;
     *n_after = n;
     if (victims.empty()) return FLS_OK;
     // flags: 1 = keep; the victims' points from before this call go
@@ -632,7 +634,7 @@ int IvoxMap::evict_lru(size_t n_old, size_t n, int runs, long long capacity, cud
     const size_t kept = (size_t)*sc.h_num_runs;
     FLS_CUDA(cudaMemcpyAsync(pts_all.p, pts_sorted.p, kept * sizeof(float4), cudaMemcpyDeviceToDevice, st));
     FLS_CUDA(cudaMemcpyAsync(stamp_all.p, sc.keys.p, kept * sizeof(unsigned long long), cudaMemcpyDeviceToDevice, st));
-    launches += 4;
+    *launches += 4;
     *n_after = kept;
     return FLS_OK;
 }
@@ -653,7 +655,7 @@ size_t IvoxMap::dump_keys(unsigned long long* h_out, size_t cap, cudaStream_t st
     return m;
 }
 
-int IvoxMap::build_stencil_lists(cudaStream_t st) {
+int IvoxMap::build_stencil_lists(cudaStream_t st, int* launches) {
     BuildScratch& sc = scratch;
     const size_t S = (size_t)n_stencil;
     const size_t n_keys = n_vox * S;
@@ -702,13 +704,50 @@ int IvoxMap::build_stencil_lists(cudaStream_t st) {
     n_list = total;
     lists_end = total;
     lists_garbage = 0;
-    launches += 7;
+    *launches += 7;
     // the transient key arrays are the largest buffers of the build; give them back
     if (!incremental) {
         ckeys.release();
         ckeys_sorted.release();
     }
     return FLS_OK;
+}
+
+int window_add(WindowMap& w, const float4* d_cloud, size_t n, size_t window, float leaf, bool filter_always, bool replace, BuildScratch& sc,
+               cudaStream_t st, int* launches) {
+    const float4* merged = d_cloud;
+    size_t n_merged = n;
+    size_t depth = 1;
+    if (!replace) {
+        std::unique_ptr<WindowMap::Cloud> c(new WindowMap::Cloud());
+        c->buf.reserve(n);
+        if (n) FLS_CUDA(cudaMemcpyAsync(c->buf.p, d_cloud, n * sizeof(float4), cudaMemcpyDeviceToDevice, st));
+        c->n = n;
+        w.deque.push_back(std::move(c));
+        if (w.deque.size() > window) {
+            FLS_CUDA(cudaStreamSynchronize(st));  // the evicted buffer may still feed a copy in flight
+            w.deque.pop_front();
+        }
+        n_merged = 0;
+        for (auto& q : w.deque) n_merged += q->n;
+        w.merged.reserve(n_merged);
+        size_t off = 0;
+        for (auto& q : w.deque) {
+            if (q->n) FLS_CUDA(cudaMemcpyAsync(w.merged.p + off, q->buf.p, q->n * sizeof(float4), cudaMemcpyDeviceToDevice, st));
+            off += q->n;
+        }
+        merged = w.merged.p;
+        depth = w.deque.size();
+    }
+    w.cloud.reserve(n_merged);
+    if (filter_always || depth > 5) {
+        w.n = voxel_grid_device(merged, n_merged, leaf, w.cloud.p, sc, st, launches);
+    } else {
+        if (n_merged) FLS_CUDA(cudaMemcpyAsync(w.cloud.p, merged, n_merged * sizeof(float4), cudaMemcpyDeviceToDevice, st));
+        w.n = n_merged;
+    }
+    w.grid.clear();
+    return w.grid.append_and_build(w.cloud.p, w.n, 0, st, launches);
 }
 
 }  // namespace fls

@@ -1,5 +1,7 @@
-// fls_maps.h — host-side owners of the device-resident map structures.
+// fls_maps.h — host-side owners of the device-resident map structures.  Every builder adds the kernels it launches to `*launches`.
 #pragma once
+#include <deque>
+#include <memory>
 #include <vector>
 
 #include "fls_common.cuh"
@@ -67,27 +69,27 @@ struct IvoxMap {
     DevBuf<unsigned long long> ckeys, ckeys_sorted, cuniq;
     DevBuf<unsigned> ccount, cstart;
     BuildScratch scratch;
-    int launches = 0;
 
     void set_resolution(float r) {
         res = r;
         inv_res = 1.0f / r;
     }
     void clear() { n_pts = n_vox = n_centers = n_list = 0; }
-    int sort_and_runs(size_t n, cudaStream_t st, int* runs_out);
-    int evict_lru(size_t n_old, size_t n, int runs, long long capacity, cudaStream_t st, size_t* n_after);
+    int sort_and_runs(size_t n, cudaStream_t st, int* runs_out, int* launches);
+    int evict_lru(size_t n_old, size_t n, int runs, long long capacity, cudaStream_t st, size_t* n_after, int* launches);
     size_t dump_keys(unsigned long long* h_out, size_t cap, cudaStream_t st);  // packed keys of the occupied voxels (tests)
     // append n points that are already on the device (packed float4) and rebuild; returns fls_status
-    int append_and_build(const float4* d_new, size_t n_new, long long capacity, cudaStream_t st);
-    int build_full(size_t n_old, size_t n_in, long long capacity, cudaStream_t st, bool appended, const float4* d_new = nullptr, size_t n_new = 0);
-    int append_incremental(const float4* d_new, size_t n_new, long long capacity, cudaStream_t st);
+    int append_and_build(const float4* d_new, size_t n_new, long long capacity, cudaStream_t st, int* launches);
+    int build_full(size_t n_old, size_t n_in, long long capacity, cudaStream_t st, int* launches, bool appended, const float4* d_new = nullptr,
+                   size_t n_new = 0);
+    int append_incremental(const float4* d_new, size_t n_new, long long capacity, cudaStream_t st, int* launches);
     // log-structured state of the incremental path (mapping mode)
     bool incremental = false;          // set by the owner: the map grows by small inserts (mapping mode)
     size_t pts_end = 0, pts_garbage = 0;      // used part of pts_sorted, dead records in it
     size_t lists_end = 0, lists_garbage = 0;  // used part of lists, dead records in it
     size_t n_incremental = 0, n_full = 0;     // how many inserts took which path
     DevBuf<unsigned> inc_old_start, inc_old_count, inc_new_count, inc_new_off;
-    int build_stencil_lists(cudaStream_t st);
+    int build_stencil_lists(cudaStream_t st, int* launches);
     size_t bytes() const { return pts_all.bytes() + pts_sorted.bytes() + table.bytes() + lists.bytes() + ctab.bytes(); }
 };
 
@@ -140,17 +142,16 @@ struct NdtMap {
     DevBuf<unsigned> lru_vals, lru_vals_sorted;
     std::vector<int> h_buf;
     BuildScratch scratch;
-    int launches = 0;
 
     void configure(double voxel_size, int min_points, int max_points, long long cap);
     // evict the LRU tail exactly as upstream's sequential insert would (incremental_ndt.h:203-206); called by add_cloud
-    int evict_lru(int runs, int n_new, int n_touched, cudaStream_t st, int* n_victims, int* n_recreated);
+    int evict_lru(int runs, int n_new, int n_touched, cudaStream_t st, int* n_victims, int* n_recreated, int* launches);
     // packed voxel keys of the live voxels (tests); returns how many
     size_t dump_keys(unsigned long long* h_out, size_t cap, cudaStream_t st);
     // every live voxel with its mean, information and counters, in device order (tests)
     void dump_voxels(std::vector<fls_ndt_voxel>& out, cudaStream_t st);
     // VoxelGridCloud(cloud, leaf) then insert/update voxels; `first_scan` = flag_first_scan_ upstream
-    int add_cloud(const float4* d_cloud, size_t n, float leaf, bool first_scan, cudaStream_t st);
+    int add_cloud(const float4* d_cloud, size_t n, float leaf, bool first_scan, cudaStream_t st, int* launches);
     NdtView view() const {
         NdtView v;
         v.tab = table.p;
@@ -161,6 +162,24 @@ struct NdtMap {
     }
     size_t bytes() const { return table.bytes() + hot.bytes() + cold.bytes() + carry.bytes(); }
 };
+
+// Sliding window of clouds -> VoxelGrid -> exact search grid: the local map of IcpOptimized (cloud_deque_ / local_map_ptr_,
+// icp_optimized.h:173-187, 246) and of the kd-tree LOAM plug-ins (planar_cloud_deque_ / corner_cloud_deque_)
+struct WindowMap {
+    struct Cloud {
+        DevBuf<float4> buf;
+        size_t n = 0;
+    };
+    std::deque<std::unique_ptr<Cloud>> deque;
+    DevBuf<float4> merged;  // concatenation of the window
+    DevBuf<float4> cloud;   // what upstream builds the kd-tree on
+    size_t n = 0;
+    IvoxMap grid;           // floor-keyed uniform grid over `cloud`
+};
+// Adds a device cloud to w (replace: the window is that cloud alone) and rebuilds it.  filter_always false: VoxelGrid(leaf) only
+// once the window holds more than 5 clouds (loam_full_kdtree.h:91-99).
+int window_add(WindowMap& w, const float4* d_cloud, size_t n, size_t window, float leaf, bool filter_always, bool replace, BuildScratch& sc,
+               cudaStream_t st, int* launches);
 
 // K4: LOAM feature extraction on the projector's arrays (host in / host out); see fls_features.cu
 int extract_features_device(int device, const float* depth, const int* col, size_t n, const int* row_start, const int* row_end, int n_rows,

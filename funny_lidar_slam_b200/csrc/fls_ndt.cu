@@ -7,15 +7,36 @@
 //   * cold   : sigma, counters and a carry buffer of <= min_points_in_voxel pending points per voxel, touched only
 //              by AddCloudToLocalMap / UpdateVoxel (:130-227)
 // LRU eviction at `capacity` (:203-206) is emulated exactly: stamps per voxel + a host simulation of the sequential insert
-// (NdtMap::evict_lru, lru_simulate in fls_map.cu).
+// (NdtMap::evict_lru, lru_simulate in fls_map.cu).  NdtPlugin at the end is the plug-in's host half: its map, AddCloudToLocalMap and
+// the single and batch Match.
 #include <cub/cub.cuh>
+
+#include <cstring>
 
 #include "fls_gn.cuh"
 #include "fls_eig.cuh"
-#include "fls_kernels.h"
+#include "fls_handle.h"
 #include "fls_maps.h"
 
 namespace fls {
+
+static constexpr int kNdtBlock = 512;  // few CTA rows for the folder: a dense scan fills the device with ~150-300 CTAs instead of > 1000
+
+struct NdtArgs {
+    const float4* __restrict__ src;  // voxel-filtered scan, body frame
+    int n;
+    NdtView map;
+    double outlier_thres;
+    GnState* state;
+};
+// batch of scans in one launch: scan s is served by CTAs [cta0, cta0 + ncta) of the grid (its own persistent loop)
+struct __align__(16) NdtBatchItem {
+    NdtArgs a;
+    GnLoopCtl ctl;
+    int cta0, ncta;
+    int pad[2];
+};
+
 namespace {
 
 inline unsigned grid_for(size_t n, int block) { return (unsigned)((n + block - 1) / block); }
@@ -432,15 +453,15 @@ __global__ void __launch_bounds__(BLOCK) ndt_gn_batch_kernel(const NdtBatchItem*
 
 }  // namespace
 
-int ndt_grid(int n, int device) {
+static int ndt_grid(int n, int device) {
     return clamp_grid((n + kNdtBlock - 1) / kNdtBlock, coresident_ctas((const void*)ndt_gn_kernel<kNdtBlock>, kNdtBlock, 0, device));
 }
-void launch_ndt_loop(const NdtArgs& a, const GnLoopCtl& ctl, int grid, cudaStream_t st) {
+static void launch_ndt_loop(const NdtArgs& a, const GnLoopCtl& ctl, int grid, cudaStream_t st) {
     launch_cooperative(ndt_gn_kernel<kNdtBlock>, grid, kNdtBlock, 0, st, a, ctl);
 }
 
-int ndt_max_grid(int device) { return coresident_ctas((const void*)ndt_gn_batch_kernel<kNdtBlock>, kNdtBlock, 0, device); }
-void launch_ndt_batch(const NdtBatchItem* d_items, int n_scans, int grid, cudaStream_t st) {
+static int ndt_max_grid(int device) { return coresident_ctas((const void*)ndt_gn_batch_kernel<kNdtBlock>, kNdtBlock, 0, device); }
+static void launch_ndt_batch(const NdtBatchItem* d_items, int n_scans, int grid, cudaStream_t st) {
     launch_cooperative(ndt_gn_batch_kernel<kNdtBlock>, grid, kNdtBlock, 0, st, d_items, n_scans);
 }
 
@@ -452,12 +473,10 @@ void NdtMap::configure(double voxel_size, int min_points, int max_points, long l
     capacity = cap;
 }
 
-int NdtMap::add_cloud(const float4* d_cloud, size_t n, float leaf, bool first_scan, cudaStream_t st) {
+int NdtMap::add_cloud(const float4* d_cloud, size_t n, float leaf, bool first_scan, cudaStream_t st, int* launches) {
     if (n == 0) return FLS_OK;
     filtered.reserve(n);
-    int l = 0;
-    const size_t nf = voxel_grid_device(d_cloud, n, leaf, filtered.p, scratch, st, &l);  // :186
-    launches += l;
+    const size_t nf = voxel_grid_device(d_cloud, n, leaf, filtered.p, scratch, st, launches);  // :186
     if (nf == 0) return FLS_OK;
     if (slots == 0) {  // first use: size everything by the configured capacity
         size_t want = 1024;
@@ -470,7 +489,7 @@ int NdtMap::add_cloud(const float4* d_cloud, size_t n, float leaf, bool first_sc
         carry.reserve((size_t)capacity * (size_t)(min_pts > 0 ? min_pts : 1) * 3);
         counter.reserve(8);
         ndt_table_clear_kernel<<<grid_for(slots, 256), 256, 0, st>>>(table.p, slots, counter.p);
-        launches++;
+        ++*launches;
     }
     BuildScratch& sc = scratch;
     sc.keys.reserve(nf);
@@ -509,13 +528,13 @@ int NdtMap::add_cloud(const float4* d_cloud, size_t n, float leaf, bool first_sc
     int hc[8] = {0, 0, 0, 0, 0, 0, 0, 0};
     FLS_CUDA(cudaMemcpyAsync(hc, counter.p, 8 * sizeof(int), cudaMemcpyDeviceToHost, st));
     FLS_CUDA(cudaStreamSynchronize(st));
-    launches += 1;
+    *launches += 1;
     const int n_new = hc[3], n_touched = hc[4];
     ++call_no;
     int n_victims = 0, n_recreated = 0;
     // upstream: after every creation `if (data_.size() >= capacity_) pop_back()` (:203-206) — the list never holds `capacity` voxels
     if ((long long)n_vox + n_new >= capacity) {
-        const int rc = evict_lru(runs, n_new, n_touched, st, &n_victims, &n_recreated);
+        const int rc = evict_lru(runs, n_new, n_touched, st, &n_victims, &n_recreated, launches);
         if (rc != FLS_OK) return rc;
     }
     NdtUpdateArgs ua;
@@ -544,7 +563,7 @@ int NdtMap::add_cloud(const float4* d_cloud, size_t n, float leaf, bool first_sc
     int h[3] = {0, 0, 0};
     FLS_CUDA(cudaMemcpyAsync(h, counter.p, 3 * sizeof(int), cudaMemcpyDeviceToHost, st));
     FLS_CUDA(cudaStreamSynchronize(st));
-    launches += 6;
+    *launches += 6;
     hi_water = h[0];
     n_free -= h[2] < n_free ? h[2] : n_free;  // the creations popped that many indices off the free stack
     n_vox = n_vox + (size_t)n_new + (size_t)n_recreated - (size_t)n_victims;
@@ -554,7 +573,7 @@ int NdtMap::add_cloud(const float4* d_cloud, size_t n, float leaf, bool first_sc
 
 // Evicts what upstream's sequential insert would evict during this call (exact, including a victim that is touched again later in
 // the call): candidates = live voxels by ascending stamp, simulated on the host against the creation times of the new voxels.
-int NdtMap::evict_lru(int runs, int n_new, int n_touched, cudaStream_t st, int* n_victims, int* n_recreated) {
+int NdtMap::evict_lru(int runs, int n_new, int n_touched, cudaStream_t st, int* n_victims, int* n_recreated, int* launches) {
     BuildScratch& sc = scratch;
     const int hw = hi_water;
     const size_t n_live = n_vox;
@@ -582,7 +601,7 @@ int NdtMap::evict_lru(int runs, int n_new, int n_touched, cudaStream_t st, int* 
     FLS_CUDA(cudaMemcpyAsync(cand.data(), sc.k32a.p, sizeof(unsigned) * K, cudaMemcpyDeviceToHost, st));
     if (n_new) FLS_CUDA(cudaMemcpyAsync(creat.data(), sc.k32b.p, sizeof(unsigned) * (size_t)n_new, cudaMemcpyDeviceToHost, st));
     FLS_CUDA(cudaStreamSynchronize(st));
-    launches += 5;
+    *launches += 5;
     std::vector<unsigned> victims;
     std::vector<unsigned char> recreated;
     if (!lru_simulate(n_live, (size_t)capacity, cand, creat, victims, recreated)) return FLS_ERR_CAPACITY;
@@ -601,7 +620,7 @@ int NdtMap::evict_lru(int runs, int n_new, int n_touched, cudaStream_t st, int* 
     ndt_table_clear_only_kernel<<<grid_for(slots, 256), 256, 0, st>>>(table.p, slots);
     ndt_table_rebuild_kernel<<<grid_for(hw, 256), 256, 0, st>>>(cold.p, hw, table.p, mask);
     FLS_CUDA(cudaStreamSynchronize(st));  // the host vectors above are read by the copies
-    launches += 3;
+    *launches += 3;
     return FLS_OK;
 }
 
@@ -631,5 +650,156 @@ void NdtMap::dump_voxels(std::vector<fls_ndt_voxel>& out, cudaStream_t st) {
     out.resize((size_t)n);
     if (n) FLS_CUDA(cudaMemcpy(out.data(), d.p, sizeof(fls_ndt_voxel) * (size_t)n, cudaMemcpyDeviceToHost));
 }
+
+// ---- IncrementalNDT ----------------------------------------------------------------------------------------------
+
+class NdtPlugin final : public Plugin {
+    NdtMap map;
+    bool first_scan = true;  // flag_first_scan_ (incremental_ndt.h:394)
+    DevBuf<float4> scan;     // VoxelGridCloud of the source(s) (:232)
+    DevBuf<float4> ins;      // Match-internal insert: the filtered scan moved by the input guess
+
+  public:
+    explicit NdtPlugin(Handle& handle) : Plugin(handle, kOrdered) {
+        map.configure(h.cfg.ndt_voxel_size, h.cfg.ndt_min_points_in_voxel, h.cfg.ndt_max_points_in_voxel, h.cfg.ndt_capacity);
+    }
+
+    int add_cloud(const float4* d_cloud, size_t n, const float4*, size_t) override {
+        const fls_config& cfg = h.cfg;
+        const int rc = map.add_cloud(d_cloud, n, cfg.source_cloud_filter_size, first_scan, h.stream, &h.launches);
+        if (cfg.localization_mode && rc == FLS_OK) {
+            // kdtree_flann_.setInputCloud(cloud_world) — the voxel-filtered cloud (incremental_ndt.h:188-190)
+            const size_t nf = voxel_grid_device(d_cloud, n, cfg.source_cloud_filter_size, map.filtered.p, map.scratch, h.stream, &h.launches);
+            h.set_fit_cloud(map.filtered.p, nf);
+        }
+        first_scan = cfg.localization_mode != 0;  // :222-226
+        return rc;
+    }
+
+    int match(const float4* d_in, size_t n_in, const float4*, size_t, double* T, int* converged, fls_match_stats* st) override {
+        const fls_config& cfg = h.cfg;
+        if (map.n_vox == 0) return FLS_ERR_NO_MAP;  // CHECK(!grids_.empty())
+        scan.reserve(n_in);
+        const size_t n = voxel_grid_device(d_in, n_in, cfg.source_cloud_filter_size, scan.p, h.scratch, h.stream, &h.launches);  // :232
+        const int ni = (int)n;
+        const int grid = ndt_grid(ni, cfg.device);
+        double T_in[16];
+        std::memcpy(T_in, T, sizeof(T_in));
+        NdtArgs a;
+        a.src = scan.p;
+        a.n = ni;
+        a.map = map.view();
+        a.outlier_thres = cfg.ndt_outlier_thres;
+        a.state = h.state.p;
+        // roofline accounting (SURVEY.md §8d, K2): 16 B source point + 7 x 16 B slot probes per point-iteration,
+        // 80 B voxel record per estimated voxel hit; the 6x6 sums are fused (no per-point output).
+        h.match_single(FLS_NDT, cfg.ndt_min_effective_pts, grid, 16 + 16LL * 7, 80, scan.p, n, n, T, converged, st,
+                       [&](const GnLoopCtl& ctl) { launch_ndt_loop(a, ctl, grid, h.stream); });
+        if (!h.h_state->failed && !cfg.localization_mode) {
+            // :326-330 — the scan enters the map transformed by the INPUT guess T, not the optimised pose  [quirk 6]
+            ins.reserve(n);
+            launch_transform_f(scan.p, n, T_in, ins.p, h.stream);
+            h.launches++;
+            return h.inserted(add_cloud(ins.p, n, nullptr, 0), st);
+        }
+        return FLS_OK;
+    }
+
+    // n_scans independent IncrementalNDT::Match calls against the same (static) map in ONE cooperative launch (ndt_gn_batch_kernel —
+    // one sub-grid and one persistent Gauss-Newton loop per scan).  Localization semantics only: the map is not modified
+    // (incremental_ndt.h:222-226, flag_first_scan_ stays set).
+    int match_batch(int B, const void* const* scans, const size_t* n_in, size_t host_stride, double* T, int* converged,
+                    fls_match_stats* st) override {
+        const float4* d_scans[kMaxBatch];
+        const int rc = h.begin_batch(B, scans, n_in, host_stride, d_scans, st);
+        if (rc != FLS_OK) return rc;
+        if (B == 1) return match(d_scans[0], n_in[0], nullptr, 0, T, converged, st);
+        const fls_config& cfg = h.cfg;
+        if (map.n_vox == 0) return FLS_ERR_NO_MAP;
+        size_t total_in = 0;
+        for (int s = 0; s < B; ++s) total_in += n_in[s];
+        scan.reserve(total_in + 1);
+        // VoxelGridCloud of every source (incremental_ndt.h:232), back to back in one buffer
+        size_t off[kMaxBatch + 1];
+        off[0] = 0;
+        for (int s = 0; s < B; ++s) {
+            const size_t nf = voxel_grid_device(d_scans[s], n_in[s], cfg.source_cloud_filter_size, scan.p + off[s], h.scratch, h.stream, &h.launches);
+            if (nf > 0x3fffffffull) return FLS_ERR_INVALID_ARG;
+            off[s + 1] = off[s] + nf;
+        }
+        // sub-grids: every scan gets the CTAs its points need, scaled down together when the device cannot hold them all
+        const int cap = ndt_max_grid(cfg.device);
+        int need[kMaxBatch], tot_need = 0;
+        for (int s = 0; s < B; ++s) {
+            need[s] = (int)((off[s + 1] - off[s] + kNdtBlock - 1) / kNdtBlock);
+            if (need[s] < 1) need[s] = 1;
+            tot_need += need[s];
+        }
+        if (B > cap) return FLS_ERR_INVALID_ARG;
+        int ncta[kMaxBatch], grid = 0;
+        for (int s = 0; s < B; ++s) {
+            ncta[s] = tot_need <= cap ? need[s] : (int)((long long)need[s] * (cap - B) / tot_need) + 1;
+            grid += ncta[s];
+        }
+        const unsigned tag_base = h.next_ll_epoch((size_t)grid * 32 + (size_t)B * kLlPoseLen);
+        const size_t tbl_bytes = sizeof(NdtBatchItem) * (size_t)B;
+        NdtBatchItem* items = reinterpret_cast<NdtBatchItem*>(h.batch_table(tbl_bytes));
+        uint4* pose_base = h.ll_rows.p + (size_t)grid * 32;
+        size_t ns[kMaxBatch];
+        int cta0 = 0;
+        for (int s = 0; s < B; ++s) {
+            launch_gn_init(h.state.p + s, T + 16 * s, h.stream);
+            h.launches++;
+            ns[s] = off[s + 1] - off[s];
+            NdtBatchItem& it = items[s];
+            std::memset(&it, 0, sizeof(it));
+            it.a.src = scan.p + off[s];
+            it.a.n = (int)ns[s];
+            it.a.map = map.view();
+            it.a.outlier_thres = cfg.ndt_outlier_thres;
+            it.a.state = h.state.p + s;
+            it.ctl.state = h.state.p + s;
+            it.ctl.ll_rows = h.ll_rows.p + (size_t)cta0 * 32;
+            it.ctl.ll_pose = pose_base + (size_t)s * kLlPoseLen;
+            it.ctl.tag_base = tag_base;
+            it.ctl.gp = h.gn_params(FLS_NDT, cfg.ndt_min_effective_pts);
+            it.ctl.log = h.scan_log(s);
+            it.ctl.log_cap = h.log_cap;
+            it.ctl.result = h.scan_result(s);
+            it.cta0 = cta0;
+            it.ncta = ncta[s];
+            cta0 += ncta[s];
+        }
+        h.send_batch_table(tbl_bytes);
+        h.gn_launch(16 + 16LL * 7, 80, scan.p, ns[0],
+                    [&] { launch_ndt_batch(reinterpret_cast<const NdtBatchItem*>(h.d_batch.p), B, grid, h.stream); });
+        h.read_back(B);
+        h.end_call(st);
+        h.unpack(B, ns, T, converged, st);
+        return FLS_OK;
+    }
+
+    void map_info(fls_map_info* out) const override {
+        out->n_voxels = (long long)map.n_vox;
+        out->table_slots = (long long)map.slots;
+        out->bytes = (long long)map.bytes();
+    }
+
+    int voxel_keys(std::vector<unsigned long long>& packed, size_t cap, size_t* n) override {
+        FLS_CUDA(cudaSetDevice(h.cfg.device));
+        packed.resize(cap + 1);
+        packed.resize(map.dump_keys(packed.data(), cap, h.stream));
+        *n = map.n_vox;
+        return FLS_OK;
+    }
+
+    int ndt_voxels(std::vector<fls_ndt_voxel>& out) override {
+        FLS_CUDA(cudaSetDevice(h.cfg.device));
+        map.dump_voxels(out, h.stream);
+        return FLS_OK;
+    }
+};
+
+std::unique_ptr<Plugin> make_ndt_plugin(Handle& h) { return std::make_unique<NdtPlugin>(h); }
 
 }  // namespace fls

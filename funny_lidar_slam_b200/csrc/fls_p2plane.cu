@@ -1,7 +1,8 @@
 // fls_p2plane.cu — K1 (+ fused K6), generation 8: the whole LoamPointToPlaneIVOX Gauss-Newton loop of ONE scan as one persistent
 // kernel with a CTA barrier per iteration.  It serves the single Match (fls_match / fls_match_device); batches run on generation 9
 // (fls_p2plane_v9.cu), which shares the per-point arithmetic (fls_knn.cuh, fls_plane.cuh).  This file also holds the per-batch query
-// preparation (one kernel: state init + tile-local locality sort), the Match-internal insertion rule of mapping mode and the k-NN test entry.
+// preparation (one kernel: state init + tile-local locality sort), the Match-internal insertion rule of mapping mode, the k-NN test entry
+// and the plug-in's host half (IvoxPlugin: its iVox map, AddCloudToLocalMap, and the single and batch Match on v8 / v9).
 //
 // Per source point and iteration it fuses what LoamPointToPlaneIVOX::PlanerMatch / ::SumCoefficient do
 // (include/registration/loam_point_to_plane_ivox.h:256-340 upstream): transform with the current pose, bounded
@@ -31,12 +32,35 @@
 #include <cub/cub.cuh>
 
 #include "fls_gn.cuh"
+#include "fls_handle.h"
 #include "fls_ivox.cuh"
-#include "fls_kernels.h"
 #include "fls_knn.cuh"
 #include "fls_plane.cuh"
 
 namespace fls {
+
+static constexpr int kP2PlaneBlock = 768;  // shape of the single-scan kernel: one 24-warp CTA per SM
+
+struct PoseArg {
+    double R[9];  // row-major
+    double t[3];
+};
+
+// whole-loop arguments of the single-scan kernel (generation 8)
+struct P2PlaneArgs {
+    IvoxView map;
+    double plane_thres;
+    const float4* src;  // body-frame scan in Morton order of the query voxel (prepare_queries), packed float4
+    int n;
+    float4* rec0;  // persistent per-point record: J0..J3
+    float4* rec1;  //                              J4, J5, |d|, 1
+    unsigned char* flags;
+};
+
+// queries of a batch are put in locality order in tiles of this many consecutive points; a tile never spans two scans
+static constexpr int kOrderTile = 8192;
+inline int order_tiles(int n) { return (n + kOrderTile - 1) / kOrderTile; }
+
 namespace {
 
 // IVoxMap::GetClosestPoint through the stencil lists: one probe of the centre table, then a streaming scan of the
@@ -413,32 +437,35 @@ size_t p2plane_smem() { return (size_t)(kP2PlaneBlock / 32) * 32 * kRecW * sizeo
 
 }  // namespace
 
-int p2plane_chunks(int n) { return (n + 31) / 32; }
-
-int p2plane_grid(int n, int device) {
+// CTAs that serve a scan of n points: its warp-sized (32-point) chunks / warps per CTA, + the folder, <= co-resident
+static int p2plane_grid(int n, int device) {
     const int W = kP2PlaneBlock / 32;
-    const int need = (p2plane_chunks(n) + W - 1) / W;
+    const int need = ((n + 31) / 32 + W - 1) / W;
     // + the folding CTA (stays without chunks when there is room)
     return clamp_grid(need + 1, coresident_ctas((const void*)p2plane_gn_kernel<kP2PlaneBlock, kMinB>, kP2PlaneBlock, p2plane_smem(), device));
 }
 
-void launch_p2plane_loop(const P2PlaneArgs& a, const GnLoopCtl& ctl, int grid, cudaStream_t st) {
+static void launch_p2plane_loop(const P2PlaneArgs& a, const GnLoopCtl& ctl, int grid, cudaStream_t st) {
     launch_cooperative(p2plane_gn_kernel<kP2PlaneBlock, kMinB>, grid, kP2PlaneBlock, p2plane_smem(), st, a, ctl);
 }
 
 // Per-batch preparation: state init, flag and ticket reset and the locality order of every scan, in one launch of one block per
-// tile (one block for an empty batch).
-void prepare_queries(const float4* const* d_scan_ptrs, const int* d_offsets, const int* d_tile_off, int n_tiles, int n_scans,
-                     const PoseArg* d_poses, GnState* d_states, const IvoxView& map, unsigned char* d_flags, float4* d_sorted,
-                     unsigned* d_zero, int n_zero, cudaStream_t st, int* launches) {
+// tile (one block for an empty batch).  d_scan_ptrs[n_scans]: device pointers of the scans; d_offsets[n_scans + 1]: their positions
+// in the batch; d_tile_off[n_scans + 1]: prefix sums of order_tiles(n) over the scans; d_zero[n_zero]: words zeroed on the way (v9
+// tickets).
+static void prepare_queries(const float4* const* d_scan_ptrs, const int* d_offsets, const int* d_tile_off, int n_tiles, int n_scans,
+                            const PoseArg* d_poses, GnState* d_states, const IvoxView& map, unsigned char* d_flags, float4* d_sorted,
+                            unsigned* d_zero, int n_zero, cudaStream_t st, int* launches) {
     p2plane_prep_kernel<<<n_tiles > 0 ? n_tiles : 1, kOrdThreads, 0, st>>>(d_scan_ptrs, d_offsets, d_tile_off, n_scans, d_poses, map.inv_res, d_zero,
                                                                           n_zero, d_flags, d_states, d_sorted, map.ctab, map.cmask, map.lists);
     if (launches) *launches += 1;
 }
 
-// Returns the number of points selected for insertion (class 1 then class 2, input order) in d_out; synchronises the stream.
-size_t select_ivox_inserts(const IvoxView& map, const float4* d_src, int n, const double* R_prev, const double* t_prev, const double* R_fin,
-                           const double* t_fin, double filter, float4* d_world, float4* d_out, BuildScratch& sc, cudaStream_t st, int* launches) {
+// The Match-internal AddCloudToLocalMap of mapping mode: classifies and compacts the points that enter the map (d_world, d_out: n
+// records).  Returns the number of points selected for insertion (class 1 then class 2, input order) in d_out; synchronises the stream.
+static size_t select_ivox_inserts(const IvoxView& map, const float4* d_src, int n, const double* R_prev, const double* t_prev, const double* R_fin,
+                                  const double* t_fin, double filter, float4* d_world, float4* d_out, BuildScratch& sc, cudaStream_t st,
+                                  int* launches) {
     if (n <= 0) return 0;
     PoseArg prev, fin;
     for (int k = 0; k < 9; ++k) {
@@ -470,9 +497,270 @@ size_t select_ivox_inserts(const IvoxView& map, const float4* d_src, int n, cons
     return (size_t)(total & 0xffffffffull) + (size_t)(total >> 32);
 }
 
-void launch_ivox_knn_test(const IvoxView& map, const float4* d_q, int n, float4* d_out, int* d_found, cudaStream_t st) {
-    if (n <= 0) return;
-    ivox_knn_test_kernel<<<(n + 127) / 128, 128, 0, st>>>(map, d_q, n, d_out, d_found);
-}
+// ---- LoamPointToPlaneIVOX ------------------------------------------------------------------------------------
+
+class IvoxPlugin final : public Plugin {
+    IvoxMap map;
+    DevBuf<float4> queries;     // the scans of the batch in locality order (prepare_queries)
+    DevBuf<float4> rec0, rec1;  // persistent per-point {J, |d|} records
+    DevBuf<unsigned char> flags;
+    DevBuf<unsigned> tickets;   // chunk ticket counters of the v9 kernel (dynamic work distribution)
+    DevBuf<float4> ins_world, ins;  // Match-internal insert: the scan at its final pose, the points that enter the map
+    std::vector<size_t> pend_n;     // scans of the batch in flight (empty: none)
+    bool pend_v9 = false;
+
+    IvoxView view() const { return h.grid_view(map); }
+    int append(const float4* d, size_t n) { return map.append_and_build(d, n, h.cfg.ivox_capacity, h.stream, &h.launches); }
+
+    // everything of a batch up to the asynchronous read-back of the states: nothing here waits for the device
+    int enqueue(int B, const float4* const* d_scans, const size_t* n, const double* T) {
+        if (map.n_pts == 0) return FLS_ERR_NO_MAP;
+        const int device = h.cfg.device;
+        cudaStream_t stream = h.stream;
+        int off[kMaxBatch + 1];
+        off[0] = 0;
+        int grid = 1;
+        // K1 generations: the dataflow kernel (v9: TMA-staged runs, work ring, DMMA sums — fls_p2plane_v9.cu) serves batches; a single
+        // Match runs on the barrier kernel (v8, this file) whose one-chunk-per-warp round has the shorter hand-over (DESIGN.md §3.1 has
+        // the H100 numbers)
+        const bool use_v9 = B > 1;
+        for (int s = 0; s < B; ++s) {
+            if (n[s] > 0x3fffffffull || (long long)off[s] + (long long)n[s] > 0x7ffffff0ll) return FLS_ERR_INVALID_ARG;
+            off[s + 1] = off[s] + (int)n[s];
+            const int g = use_v9 ? p2plane_v9_grid((int)n[s], device) : p2plane_grid((int)n[s], device);
+            if (g > grid) grid = g;
+        }
+        const int n_total = off[B];
+        const size_t nt = (size_t)n_total;
+        rec0.reserve(nt + 1);
+        rec1.reserve(nt + 1);
+        flags.reserve(nt + 1);
+        queries.reserve(nt + 1);
+        // one LL row per CTA + one LL pose record per scan (+ the group rows of v9)
+        const unsigned tag_base = h.next_ll_epoch((size_t)B * grid * 32 + (size_t)B * kLlPoseLen + (size_t)B * 16 * 32);
+        // ---- per-batch tables, staged in one pinned block and sent with one copy -------------------------------------------
+        const size_t o_pose = 0, o_off = o_pose + sizeof(PoseArg) * kMaxBatch, o_toff = o_off + sizeof(int) * (kMaxBatch + 4),
+                     o_desc = o_toff + sizeof(int) * (kMaxBatch + 4), o_ptr = o_desc + sizeof(P2PlaneScan) * kMaxBatch;
+        const size_t tbl_bytes = o_ptr + sizeof(void*) * kMaxBatch;
+        unsigned char* const tbl = h.batch_table(tbl_bytes);
+        PoseArg* hp = reinterpret_cast<PoseArg*>(tbl + o_pose);
+        int* ho = reinterpret_cast<int*>(tbl + o_off);
+        int* ht = reinterpret_cast<int*>(tbl + o_toff);
+        ht[0] = 0;
+        P2PlaneScan* hd = reinterpret_cast<P2PlaneScan*>(tbl + o_desc);
+        const float4** hq = reinterpret_cast<const float4**>(tbl + o_ptr);
+        uint4* pose_base = h.ll_rows.p + (size_t)B * grid * 32;
+        for (int s = 0; s < B; ++s) {
+            const double* Ts = T + 16 * s;
+            for (int r = 0; r < 3; ++r) {
+                for (int c = 0; c < 3; ++c) hp[s].R[r * 3 + c] = Ts[c * 4 + r];
+                hp[s].t[r] = Ts[12 + r];
+            }
+            ho[s] = off[s];
+            ht[s + 1] = ht[s] + order_tiles((int)n[s]);
+            hq[s] = d_scans[s];
+            P2PlaneScan& d = hd[s];
+            d.src = queries.p + off[s];
+            d.n = (int)n[s];
+            d.tag_base = tag_base;
+            d.state = h.state.p + s;
+            d.rec0 = rec0.p + off[s];
+            d.rec1 = rec1.p + off[s];
+            d.flags = flags.p + off[s];
+            d.rows = h.ll_rows.p + (size_t)s * grid * 32;
+            d.ll_pose = pose_base + (size_t)s * kLlPoseLen;
+            d.log = h.scan_log(s);
+            d.result = h.scan_result(s);
+            d.grows = pose_base + (size_t)B * kLlPoseLen + (size_t)s * 16 * 32;
+        }
+        ho[B] = off[B];
+        h.send_batch_table(tbl_bytes);
+        const unsigned char* d_batch = h.d_batch.p;
+        const PoseArg* d_poses = reinterpret_cast<const PoseArg*>(d_batch + o_pose);
+        const int* d_off = reinterpret_cast<const int*>(d_batch + o_off);
+        const int* d_toff = reinterpret_cast<const int*>(d_batch + o_toff);
+        const P2PlaneScan* d_desc = reinterpret_cast<const P2PlaneScan*>(d_batch + o_desc);
+        const float4* const* d_ptrs = reinterpret_cast<const float4* const*>(d_batch + o_ptr);
+        // chunk tickets of v9's dynamic work distribution: one counter per (scan, iteration) + the watchdog's abort word, zeroed by
+        // the prep kernel
+        const int ticket_stride = h.cfg.max_iterations + 2;
+        const int n_tickets = use_v9 ? B * ticket_stride + 4 : 0;
+        if (use_v9) tickets.reserve((size_t)n_tickets);
+        // ONE prep kernel for the whole batch (state init, flag and ticket reset): every tile of a scan ends up in Morton order of the
+        // voxel its points fall into at the initial pose (locality only: the sums are order-free up to fp64 rounding, and the
+        // persistent per-point records live in the same order for the whole Match)
+        prepare_queries(d_ptrs, d_off, d_toff, ht[B], B, d_poses, h.state.p, view(), flags.p, queries.p, use_v9 ? tickets.p : nullptr, n_tickets,
+                        stream, &h.launches);
+        P2PlaneLoopArgs a;
+        a.map = view();
+        a.plane_thres = h.cfg.point_to_planar_thres;
+        a.gp = h.gn_params(FLS_P2PLANE_IVOX, 50);
+        a.log_cap = h.log_cap;
+        a.scans = d_desc;
+        a.n_scans = B;
+        a.tickets = nullptr;
+        a.ticket_stride = 0;
+        a.abort_word = nullptr;
+        // roofline accounting (SURVEY.md §8d, K1 — the REFERENCE algorithm's traffic): 16 B source point + n_stencil x 16 B
+        // slot probes + 32 B persistent record per point-iteration, 16 B per map record resident in the stencil voxels.
+        h.gn_launch(16 + 16LL * a.map.n_stencil + 32, 16, d_scans[0], n[0], [&] {
+            if (use_v9) {
+                a.ticket_stride = ticket_stride;
+                a.tickets = tickets.p;
+                a.abort_word = tickets.p + (size_t)B * a.ticket_stride;
+                launch_p2plane_v9(a, grid, stream);
+            } else {  // the single scan: the same buffers as scan 0's descriptor above
+                const P2PlaneArgs one{a.map, a.plane_thres, queries.p, (int)n[0], rec0.p, rec1.p, flags.p};
+                GnLoopCtl ctl;
+                ctl.state = h.state.p;
+                ctl.ll_rows = h.ll_rows.p;
+                ctl.ll_pose = pose_base;
+                ctl.tag_base = tag_base;
+                ctl.gp = a.gp;
+                ctl.log = h.scan_log(0);
+                ctl.log_cap = h.log_cap;
+                ctl.result = h.scan_result(0);
+                launch_p2plane_loop(one, ctl, grid, stream);
+            }
+        });
+        // ---- read back: every scan's state (+ its iteration log) ----------------------------------------------------------
+        h.read_back(B);
+        *h.h_abort = 0;
+        if (use_v9) FLS_CUDA(cudaMemcpyAsync(h.h_abort, a.abort_word, sizeof(unsigned), cudaMemcpyDeviceToHost, stream));
+        pend_n.assign(n, n + B);
+        pend_v9 = use_v9;
+        return FLS_OK;
+    }
+
+    // waits for the batch enqueued last and unpacks its results
+    int finish(double* T, int* converged, fls_match_stats* st) {
+        const int B = (int)pend_n.size();
+        if (B < 1) return FLS_ERR_INVALID_ARG;
+        h.end_call(st);
+        if (pend_v9 && *h.h_abort) {
+            pend_n.clear();
+            set_last_error("p2plane_v9_kernel: watchdog — a wait loop gave up after 4 s (hand-over protocol error)");
+            return FLS_ERR_CUDA;
+        }
+        h.unpack(B, pend_n.data(), T, converged, st);
+        pend_n.clear();
+        return FLS_OK;
+    }
+
+    // The whole LoamPointToPlaneIVOX Match of `B` independent scans in one persistent launch; a single Match is the batch of one.
+    int run(int B, const float4* const* d_scans, const size_t* n, double* T, int* converged, fls_match_stats* st) {
+        const int rc = enqueue(B, d_scans, n, T);
+        if (rc != FLS_OK) return rc;
+        return finish(T, converged, st);
+    }
+
+  public:
+    explicit IvoxPlugin(Handle& handle) : Plugin(handle, kPlanar) {
+        static const int counts[4] = {1, 7, 19, 27};
+        map.set_resolution(h.cfg.ivox_resolution);
+        map.key_mode = 0;
+        map.incremental = !h.cfg.localization_mode;  // mapping mode: the map grows by small inserts
+        map.n_stencil = counts[h.cfg.ivox_nearby];
+    }
+
+    // external non-first insert in mapping mode: relies on Match-internal caches upstream
+    int add_check() const override { return !h.cfg.localization_mode && map.n_pts != 0 ? FLS_ERR_UNSUPPORTED : FLS_OK; }
+
+    int add_cloud(const float4* d, size_t n, const float4*, size_t) override {
+        const int chk = add_check();
+        if (chk != FLS_OK) return chk;
+        if (h.cfg.localization_mode) map.clear();  // loam_point_to_plane_ivox.h:64-69 upstream: map re-created per call
+        const int rc = append(d, n);
+        if (h.cfg.localization_mode) h.set_fit_cloud(d, n);  // :134-138 kd-tree over the raw planar cloud
+        return rc;
+    }
+
+    int match(const float4* d_src, size_t n, const float4*, size_t, double* T, int* converged, fls_match_stats* st) override {
+        const float4* scans[1] = {d_src};
+        const size_t ns[1] = {n};
+        int conv = 0;
+        const int rc = run(1, scans, ns, T, &conv, st);
+        if (rc != FLS_OK) return rc;
+        if (converged) *converged = conv;
+        const GnState& s = *h.h_state;
+        if (s.converged && !h.cfg.localization_mode) {
+            // :205-206 — the scan enters the map through the cached-5-NN rule (body-frame points, final pose)  [quirk 8]
+            ins.reserve(n + 1);
+            ins_world.reserve(n + 1);
+            const size_t n_add = select_ivox_inserts(view(), d_src, (int)n, s.Rprev, s.tprev, s.R, s.t, 0.5 /* filter_size_map_min_ (:351) */,
+                                                     ins_world.p, ins.p, h.scratch, h.stream, &h.launches);
+            return h.inserted(append(ins.p, n_add), st);
+        }
+        return FLS_OK;
+    }
+
+    int match_batch(int B, const void* const* scans, const size_t* n, size_t host_stride, double* T, int* converged,
+                    fls_match_stats* st) override {
+        const float4* ptrs[kMaxBatch];
+        const int rc = h.begin_batch(B, scans, n, host_stride, ptrs, st);
+        if (rc != FLS_OK) return rc;
+        return B == 1 ? match(ptrs[0], n[0], nullptr, 0, T, converged, st) : run(B, ptrs, n, T, converged, st);
+    }
+
+    int batch_begin(int B, const void* const* scans, const size_t* n, size_t host_stride, const double* T) override {
+        const float4* ptrs[kMaxBatch];
+        const int rc = h.begin_batch(B, scans, n, host_stride, ptrs, nullptr);
+        if (rc != FLS_OK) return rc;
+        return enqueue(B, ptrs, n, T);
+    }
+    int batch_end(double* T, int* converged, fls_match_stats* st) override { return finish(T, converged, st); }
+    int batch_pending() const override { return (int)pend_n.size(); }
+
+    void map_info(fls_map_info* out) const override {
+        out->n_points = (long long)map.n_pts;
+        out->n_voxels = (long long)map.n_vox;
+        out->table_slots = map.n_pts ? (long long)map.mask + 1 : 0;
+        out->bytes = (long long)map.bytes();
+        out->incremental_inserts = (long long)map.n_incremental;
+        out->full_builds = (long long)map.n_full;
+    }
+
+    int voxel_keys(std::vector<unsigned long long>& packed, size_t cap, size_t* n) override {
+        FLS_CUDA(cudaSetDevice(h.cfg.device));
+        packed.resize(cap + 1);
+        packed.resize(map.dump_keys(packed.data(), cap, h.stream));
+        *n = map.n_vox;
+        return FLS_OK;
+    }
+
+    int map_points(float* xyzi, size_t cap, size_t* n) override {
+        FLS_CUDA(cudaSetDevice(h.cfg.device));
+        FLS_CUDA(cudaStreamSynchronize(h.stream));
+        const size_t m = map.n_pts < cap ? map.n_pts : cap;
+        if (m) FLS_CUDA(cudaMemcpy(xyzi, map.pts_all.p, m * sizeof(float4), cudaMemcpyDeviceToHost));
+        *n = map.n_pts;
+        return FLS_OK;
+    }
+
+    int ivox_knn(const void* queries_in, size_t n, size_t stride, float* out_pts, int32_t* out_count) override {
+        if (map.n_pts == 0) return FLS_ERR_NO_MAP;
+        h.begin_call();
+        const float4* dq = h.upload(queries_in, n, stride, h.src);
+        DevBuf<float4> d_out;
+        DevBuf<int> d_found;
+        d_out.reserve(n * 5);
+        d_found.reserve(n);
+        if (n > 0) ivox_knn_test_kernel<<<(unsigned)((n + 127) / 128), 128, 0, h.stream>>>(view(), dq, (int)n, d_out.p, d_found.p);
+        FLS_CUDA(cudaMemcpyAsync(out_pts, d_out.p, n * 5 * sizeof(float4), cudaMemcpyDeviceToHost, h.stream));
+        FLS_CUDA(cudaMemcpyAsync(out_count, d_found.p, n * sizeof(int), cudaMemcpyDeviceToHost, h.stream));
+        h.end_call(nullptr);
+        return FLS_OK;
+    }
+
+    // fls_ivox_add_points: IVoxMap::AddPoints on the map as it is (no localization-mode re-creation)
+    int ivox_add_points(const void* pts, size_t n, size_t stride) override {
+        h.begin_call();
+        const int rc = append(h.upload(pts, n, stride, h.up_cloud), n);
+        h.end_call(nullptr);
+        return rc;
+    }
+};
+
+std::unique_ptr<Plugin> make_ivox_plugin(Handle& h) { return std::make_unique<IvoxPlugin>(h); }
 
 }  // namespace fls
