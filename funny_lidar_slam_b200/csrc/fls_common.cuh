@@ -109,6 +109,39 @@ struct DevBuf {
     size_t bytes() const { return cap * sizeof(T); }
 };
 
+// ---- CUB device passes ----------------------------------------------------------------------------------
+// A pass is one CUB device call with its arguments bound, as a callable cudaError_t(void* tmp, size_t& bytes): with tmp null it
+// only writes the temporary storage it needs to `bytes`, otherwise it runs in the `bytes` of storage at tmp.  Sizing from the
+// same callable that runs keeps the two argument lists from drifting apart.
+// cub_reserve grows tmp (grow-only, 256 bytes of slack) to what the largest of `passes` needs.  A pipeline sizes all its passes
+// before the first one runs, so that its buffer is not reallocated between two of them.
+template <class... P>
+void cub_reserve(DevBuf<unsigned char>& tmp, P&&... passes) {
+    size_t need = 0;
+    auto size = [&need](auto&& pass) {
+        size_t bytes = 0;
+        pass(nullptr, bytes);
+        if (bytes > need) need = bytes;
+    };
+    (size(passes), ...);
+    tmp.reserve(need + 256);
+}
+// runs a pass in tmp, which cub_reserve has sized for it
+template <class P>
+void cub_run(DevBuf<unsigned char>& tmp, P&& pass) {
+    size_t bytes = tmp.cap;
+    FLS_CUDA(pass(tmp.p, bytes));
+}
+// sizes tmp for one pass and runs it
+template <class P>
+void cub_pass(DevBuf<unsigned char>& tmp, P&& pass) {
+    cub_reserve(tmp, pass);
+    cub_run(tmp, pass);
+}
+
+// blocks of `block` threads that cover n items
+inline unsigned grid_for(size_t n, int block) { return (unsigned)((n + block - 1) / block); }
+
 // ---- pinned host buffer (grow-only): staging whose copies do not make the enqueue wait ------------------
 template <typename T>
 struct PinnedBuf {

@@ -399,9 +399,11 @@ int convert_cloud_device(const fls_convert_cfg& c, const fls_pointcloud2& m, flo
         FLS_CUDA(cudaMemsetAsync(d_go, 0, sizeof(int), st));
         const unsigned g = (unsigned)((n + 255) / 256);
         conv_flag_kernel<<<g, 256, 0, st>>>(p, w.flag.p, d_first_kept);
-        size_t tb = 0;
-        cub::DeviceScan::ExclusiveSum(nullptr, tb, w.flag.p, w.pos.p, (int)n, st);
-        size_t need = tb;
+        auto positions = [&](void* tmp, size_t& bytes) { return cub::DeviceScan::ExclusiveSum(tmp, bytes, w.flag.p, w.pos.p, (int)n, st); };
+        auto sort = [&](void* tmp, size_t& bytes) {
+            return cub::DeviceRadixSort::SortPairs(tmp, bytes, w.key.p, w.key_sorted.p, w.idx.p, w.idx_sorted.p, (int)n, 0, 9, st);
+        };
+        auto compose = [&](void* tmp, size_t& bytes) { return cub::DeviceScan::InclusiveScan(tmp, bytes, w.map.p, w.state.p, ComposeMaps(), (int)n, st); };
         if (offsets) {
             w.key.reserve(n);
             w.key_sorted.reserve(n);
@@ -410,14 +412,11 @@ int convert_cloud_device(const fls_convert_cfg& c, const fls_pointcloud2& m, flo
             w.yaw.reserve(n);
             w.map.reserve(n);
             w.state.reserve(n);
-            size_t t1 = 0, t2 = 0;
-            cub::DeviceRadixSort::SortPairs(nullptr, t1, w.key.p, w.key_sorted.p, w.idx.p, w.idx_sorted.p, (int)n, 0, 9, st);
-            cub::DeviceScan::InclusiveScan(nullptr, t2, w.map.p, w.state.p, ComposeMaps(), (int)n, st);
-            need = std::max(need, std::max(t1, t2));
+            cub_reserve(w.cub_tmp, positions, sort, compose);
+        } else {
+            cub_reserve(w.cub_tmp, positions);
         }
-        w.cub_tmp.reserve(need + 256);
-        tb = w.cub_tmp.cap;
-        FLS_CUDA(cub::DeviceScan::ExclusiveSum(w.cub_tmp.p, tb, w.flag.p, w.pos.p, (int)n, st));
+        cub_run(w.cub_tmp, positions);
         conv_emit_kernel<<<g, 256, 0, st>>>(p, w.flag.p, w.pos.p, d_first_kept, ox, orr, ot, d_count);
         launches += 3;
         if (offsets) {  // ComputePointOffsetTime(cloud, 10.0): the kernels run, the last one writes only when the condition holds
@@ -426,12 +425,10 @@ int convert_cloud_device(const fls_convert_cfg& c, const fls_pointcloud2& m, flo
             q.two_pi = 2.0 * M_PI;
             q.period = static_cast<float>(2.0 * M_PI / q.omega);  // :547
             off_prep_kernel<<<g, 256, 0, st>>>(ox, orr, ot, d_count, (int)n, c.n_rows, w.yaw.p, w.key.p, w.idx.p, d_go);
-            tb = w.cub_tmp.cap;
-            FLS_CUDA(cub::DeviceRadixSort::SortPairs(w.cub_tmp.p, tb, w.key.p, w.key_sorted.p, w.idx.p, w.idx_sorted.p, (int)n, 0, 9, st));
+            cub_run(w.cub_tmp, sort);
             off_heads_kernel<<<1, 256, 0, st>>>(w.key_sorted.p, w.idx_sorted.p, (int)n, d_first);
             off_map_kernel<<<g, 256, 0, st>>>(q, w.key_sorted.p, w.idx_sorted.p, w.yaw.p, d_first, (int)n, w.map.p);
-            tb = w.cub_tmp.cap;
-            FLS_CUDA(cub::DeviceScan::InclusiveScan(w.cub_tmp.p, tb, w.map.p, w.state.p, ComposeMaps(), (int)n, st));
+            cub_run(w.cub_tmp, compose);
             off_write_kernel<<<g, 256, 0, st>>>(q, w.key_sorted.p, w.idx_sorted.p, w.yaw.p, d_first, w.state.p, d_go, (int)n, ot);
             launches += 6;
         }

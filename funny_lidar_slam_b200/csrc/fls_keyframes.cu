@@ -7,14 +7,12 @@
 //   kf_bbox_kernel      per-segment bounding boxes (tiles of kTile points, one atomicMin / atomicMax per block and axis)
 //   kf_keys_kernel      per-segment grid parameters (inv, min_b, div_b, the INT_MAX fallback) derived on the device from those boxes;
 //                       key = segment << 32 | cell id (a segment that overflows keys its points by input position instead)
-//   CUB                 stable radix sort of (key, arena index), run-length encode, exclusive scan — plumbing only
+//   voxel-runs pass     stable radix sort of (key, arena index), run-length encode, exclusive scan (BuildScratch, CUB) — plumbing only
 //   kf_centroid_kernel  one centroid per run (fp32 sums in input order), transformed by its segment's pose as it is written
 // The sort is stable and the segment is the key's high half, so the output is segment-major with cells ascending inside each
 // segment — the order of upstream's `+=` loop — and every centroid is summed in input order, as fls_voxelgrid.cu does (both share
 // fls_voxel.cuh).  The host waits once for the run count and once at the end, plus the two waits of the final voxel_grid_device pass
 // when there is one: the count does not depend on the number of keyframes.
-#include <cub/cub.cuh>
-
 #include <algorithm>
 #include <cstring>
 #include <mutex>
@@ -110,7 +108,6 @@ __global__ void kf_centroid_kernel(const float4* __restrict__ arena, const KfSeg
                          xform_row_f(q[6], q[7], q[8], q[11], p.x, p.y, p.z), p.w);
 }
 
-inline unsigned grid_for(size_t n, int block) { return (unsigned)((n + block - 1) / block); }
 inline size_t align16(size_t n) { return (n + 15) & ~size_t(15); }
 
 }  // namespace
@@ -235,36 +232,17 @@ struct KeyframeStore {
             d_mm = mm;
             const KfTile* d_tiles = reinterpret_cast<const KfTile*>(table.p + off_tiles);
 
-            sc.keys.reserve(N);
-            sc.keys_sorted.reserve(N);
-            sc.uniq.reserve(N);
-            sc.idx.reserve(N);
-            sc.idx_sorted.reserve(N);
-            sc.counts.reserve(N);
-            sc.starts.reserve(N);
-            sc.num_runs.reserve(2);
+            sc.reserve_runs<unsigned long long>(N);
             kf_bbox_kernel<<<(unsigned)n_tiles, kThreads, 0, stream>>>(arena, d_segs, d_tiles, mm);
             kf_keys_kernel<<<(unsigned)n_tiles, kThreads, 0, stream>>>(arena, d_segs, d_tiles, mm, inv, sc.keys.p, sc.idx.p);
             FLS_CUDA(cudaGetLastError());
             // the cell id takes the low 32 bits, the segment the next 16 (all 32 beyond 65536 keyframes): a fixed bit range keeps the
             // sort's passes, and so the launches, the same for every selection size
-            const int end_bit = K <= 65536 ? 48 : 64;
-            size_t t1 = 0, t2 = 0, t3 = 0;
-            cub::DeviceRadixSort::SortPairs(nullptr, t1, sc.keys.p, sc.keys_sorted.p, sc.idx.p, sc.idx_sorted.p, (int)N, 0, end_bit, stream);
-            cub::DeviceRunLengthEncode::Encode(nullptr, t2, sc.keys_sorted.p, sc.uniq.p, sc.counts.p, sc.num_runs.p, (int)N, stream);
-            cub::DeviceScan::ExclusiveSum(nullptr, t3, sc.counts.p, sc.starts.p, (int)N, stream);
-            sc.cub_tmp.reserve(std::max(t1, std::max(t2, t3)) + 256);
-            size_t tb = sc.cub_tmp.cap;
-            FLS_CUDA(cub::DeviceRadixSort::SortPairs(sc.cub_tmp.p, tb, sc.keys.p, sc.keys_sorted.p, sc.idx.p, sc.idx_sorted.p, (int)N, 0, end_bit,
-                                                     stream));
-            tb = sc.cub_tmp.cap;
-            FLS_CUDA(cub::DeviceRunLengthEncode::Encode(sc.cub_tmp.p, tb, sc.keys_sorted.p, sc.uniq.p, sc.counts.p, sc.num_runs.p, (int)N, stream));
-            FLS_CUDA(cudaMemcpyAsync(sc.h_num_runs, sc.num_runs.p, sizeof(int), cudaMemcpyDeviceToHost, stream));
-            FLS_CUDA(cudaStreamSynchronize(stream));
+            sc.sort_pairs<unsigned long long>(N, K <= 65536 ? 48 : 64, stream);
+            runs = (size_t)sc.encode_runs<unsigned long long>(N, stream);
             d2h += (long long)sizeof(int);
             launches += 4;
             ++waits;
-            runs = (size_t)*sc.h_num_runs;
         }
         const size_t R = n_base + runs;
         if (!final_pass && R > capacity_out) {
@@ -275,8 +253,7 @@ struct KeyframeStore {
         float4* catp = (!final_pass && d_out) ? d_out : cat.reserve(std::max<size_t>(R, 1));
         if (n_base) FLS_CUDA(cudaMemcpyAsync(catp, d_base, n_base * sizeof(float4), cudaMemcpyDeviceToDevice, stream));
         if (runs) {
-            size_t tb = sc.cub_tmp.cap;
-            FLS_CUDA(cub::DeviceScan::ExclusiveSum(sc.cub_tmp.p, tb, sc.counts.p, sc.starts.p, (int)runs, stream));
+            sc.run_starts((int)runs, stream);
             kf_centroid_kernel<<<grid_for(runs, 128), 128, 0, stream>>>(arena, d_segs, d_mm, inv, sc.uniq.p, sc.idx_sorted.p, sc.starts.p,
                                                                         sc.counts.p, (int)runs, catp + n_base);
             FLS_CUDA(cudaGetLastError());

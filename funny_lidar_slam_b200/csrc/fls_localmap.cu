@@ -65,11 +65,9 @@ int Handle::update_local_map(const double* T, int* updated, size_t* n_local) {
     crop_flags_kernel<<<(unsigned)((global_n + 255) / 256), 256, 0, stream>>>(global_map.p, global_n, (float)local_edge[0], (float)local_edge[1],
                                                                             (float)local_edge[2], (float)local_edge[3], (float)local_edge[4],
                                                                             (float)local_edge[5], crop_keep.p);  // :401-402 .cast<float>()
-    size_t tb = 0;
-    cub::DeviceSelect::Flagged(nullptr, tb, global_map.p, crop_keep.p, local_map.p, scratch.num_runs.p, (int)global_n, stream);
-    scratch.cub_tmp.reserve(tb + 256);
-    tb = scratch.cub_tmp.cap;
-    FLS_CUDA(cub::DeviceSelect::Flagged(scratch.cub_tmp.p, tb, global_map.p, crop_keep.p, local_map.p, scratch.num_runs.p, (int)global_n, stream));
+    cub_pass(scratch.cub_tmp, [&](void* tmp, size_t& bytes) {
+        return cub::DeviceSelect::Flagged(tmp, bytes, global_map.p, crop_keep.p, local_map.p, scratch.num_runs.p, (int)global_n, stream);
+    });
     FLS_CUDA(cudaMemcpyAsync(scratch.h_num_runs, scratch.num_runs.p, sizeof(int), cudaMemcpyDeviceToHost, stream));
     FLS_CUDA(cudaStreamSynchronize(stream));
     const size_t m = (size_t)*scratch.h_num_runs;

@@ -46,6 +46,12 @@ bool lru_simulate(size_t size0, size_t capacity, const std::vector<unsigned>& ca
     return true;
 }
 
+size_t lru_candidate_bound(size_t n_vox, int n_new, int n_touched, long long capacity, size_t n_cand) {
+    const long long e0 = (long long)n_vox + n_new - (capacity - 1);
+    const size_t K = (size_t)(e0 > 0 ? e0 : 0) + 2 * (size_t)n_touched + 64;
+    return K < n_cand ? K : n_cand;
+}
+
 BuildScratch::BuildScratch() {
     if (cudaMallocHost(&h_num_runs, sizeof(int)) != cudaSuccess) {  // no device / out of pinned memory: a plain allocation still works as a copy target
         cudaGetLastError();
@@ -62,7 +68,67 @@ BuildScratch::~BuildScratch() {
 
 namespace {
 
-inline unsigned grid_for(size_t n, int block) { return (unsigned)((n + block - 1) / block); }
+// the key arrays of the voxel-runs pass by key type: unsorted, sorted, one per run
+template <class K>
+struct RunKeys {
+    DevBuf<K>&in, &sorted, &uniq;
+};
+RunKeys<unsigned long long> run_keys(BuildScratch& sc, unsigned long long) { return {sc.keys, sc.keys_sorted, sc.uniq}; }
+RunKeys<unsigned> run_keys(BuildScratch& sc, unsigned) { return {sc.k32a, sc.k32b, sc.uniq32}; }
+template <class K>
+auto encode_pass(BuildScratch& sc, int n, cudaStream_t st) {
+    return [&sc, n, st](void* tmp, size_t& bytes) {
+        const RunKeys<K> k = run_keys(sc, K());
+        return cub::DeviceRunLengthEncode::Encode(tmp, bytes, k.sorted.p, k.uniq.p, sc.counts.p, sc.num_runs.p, n, st);
+    };
+}
+auto starts_pass(BuildScratch& sc, int n, cudaStream_t st) {
+    return [&sc, n, st](void* tmp, size_t& bytes) { return cub::DeviceScan::ExclusiveSum(tmp, bytes, sc.counts.p, sc.starts.p, n, st); };
+}
+
+}  // namespace
+
+template <class K>
+void BuildScratch::reserve_runs(size_t n) {
+    const RunKeys<K> k = run_keys(*this, K());
+    k.in.reserve(n);
+    k.sorted.reserve(n);
+    k.uniq.reserve(n);
+    idx.reserve(n);
+    idx_sorted.reserve(n);
+    counts.reserve(n);
+    starts.reserve(n);
+    num_runs.reserve(2);
+}
+
+template <class K>
+void BuildScratch::sort_pairs(size_t n, int end_bit, cudaStream_t st) {
+    const RunKeys<K> k = run_keys(*this, K());
+    auto sort = [&](void* tmp, size_t& bytes) {
+        return cub::DeviceRadixSort::SortPairs(tmp, bytes, k.in.p, k.sorted.p, idx.p, idx_sorted.p, (int)n, 0, end_bit, st);
+    };
+    cub_reserve(cub_tmp, sort, encode_pass<K>(*this, (int)n, st), starts_pass(*this, (int)n, st));
+    cub_run(cub_tmp, sort);
+}
+
+template <class K>
+int BuildScratch::encode_runs(size_t n, cudaStream_t st) {
+    cub_run(cub_tmp, encode_pass<K>(*this, (int)n, st));
+    FLS_CUDA(cudaMemcpyAsync(h_num_runs, num_runs.p, sizeof(int), cudaMemcpyDeviceToHost, st));
+    FLS_CUDA(cudaStreamSynchronize(st));
+    return *h_num_runs;
+}
+
+void BuildScratch::run_starts(int runs, cudaStream_t st) { cub_run(cub_tmp, starts_pass(*this, runs, st)); }
+
+template void BuildScratch::reserve_runs<unsigned long long>(size_t);
+template void BuildScratch::reserve_runs<unsigned>(size_t);
+template void BuildScratch::sort_pairs<unsigned long long>(size_t, int, cudaStream_t);
+template void BuildScratch::sort_pairs<unsigned>(size_t, int, cudaStream_t);
+template int BuildScratch::encode_runs<unsigned long long>(size_t, cudaStream_t);
+template int BuildScratch::encode_runs<unsigned>(size_t, cudaStream_t);
+
+namespace {
 
 __global__ void ivox_keys_kernel(const float4* __restrict__ pts, size_t n, float inv_res, int key_mode, unsigned long long* __restrict__ keys,
                                  unsigned* __restrict__ idx) {
@@ -328,14 +394,7 @@ void launch_transform_f(const float4* d_in, size_t n, const double* T, float4* d
 // keys -> stable sort -> gather -> run-length encode -> starts: the voxel-contiguous order of the first n points of pts_all
 int IvoxMap::sort_and_runs(size_t n, cudaStream_t st, int* runs_out, int* launches) {
     BuildScratch& sc = scratch;
-    sc.keys.reserve(n);
-    sc.keys_sorted.reserve(n);
-    sc.uniq.reserve(n);
-    sc.idx.reserve(n);
-    sc.idx_sorted.reserve(n);
-    sc.counts.reserve(n);
-    sc.starts.reserve(n);
-    sc.num_runs.reserve(2);
+    sc.reserve_runs<unsigned long long>(n);
     // mapping mode: room for the voxels the incremental inserts rewrite; buffers grow geometrically (a cudaFree + cudaMalloc of a
     // few hundred MB costs milliseconds — more than the build itself)
     if (incremental) {
@@ -344,23 +403,10 @@ int IvoxMap::sort_and_runs(size_t n, cudaStream_t st, int* runs_out, int* launch
         pts_sorted.reserve(n);
     }
     ivox_keys_kernel<<<grid_for(n, 256), 256, 0, st>>>(pts_all.p, n, inv_res, key_mode, sc.keys.p, sc.idx.p);
-    size_t tmp1 = 0, tmp2 = 0, tmp3 = 0;
-    cub::DeviceRadixSort::SortPairs(nullptr, tmp1, sc.keys.p, sc.keys_sorted.p, sc.idx.p, sc.idx_sorted.p, (int)n, 0, 63, st);
-    cub::DeviceRunLengthEncode::Encode(nullptr, tmp2, sc.keys_sorted.p, sc.uniq.p, sc.counts.p, sc.num_runs.p, (int)n, st);
-    cub::DeviceScan::ExclusiveSum(nullptr, tmp3, sc.counts.p, sc.starts.p, (int)n, st);
-    size_t tmp = tmp1 > tmp2 ? tmp1 : tmp2;
-    tmp = tmp > tmp3 ? tmp : tmp3;
-    sc.cub_tmp.reserve(tmp + 256);
-    size_t tb = sc.cub_tmp.cap;
-    FLS_CUDA(cub::DeviceRadixSort::SortPairs(sc.cub_tmp.p, tb, sc.keys.p, sc.keys_sorted.p, sc.idx.p, sc.idx_sorted.p, (int)n, 0, 63, st));
+    sc.sort_pairs<unsigned long long>(n, 63, st);
     gather_kernel<<<grid_for(n, 256), 256, 0, st>>>(pts_all.p, sc.idx_sorted.p, n, pts_sorted.p);
-    tb = sc.cub_tmp.cap;
-    FLS_CUDA(cub::DeviceRunLengthEncode::Encode(sc.cub_tmp.p, tb, sc.keys_sorted.p, sc.uniq.p, sc.counts.p, sc.num_runs.p, (int)n, st));
-    FLS_CUDA(cudaMemcpyAsync(sc.h_num_runs, sc.num_runs.p, sizeof(int), cudaMemcpyDeviceToHost, st));
-    FLS_CUDA(cudaStreamSynchronize(st));
-    const int runs = *sc.h_num_runs;
-    tb = sc.cub_tmp.cap;
-    FLS_CUDA(cub::DeviceScan::ExclusiveSum(sc.cub_tmp.p, tb, sc.counts.p, sc.starts.p, runs, st));
+    const int runs = sc.encode_runs<unsigned long long>(n, st);
+    sc.run_starts(runs, st);
     *launches += 6;
     *runs_out = runs;
     return FLS_OK;
@@ -378,31 +424,12 @@ int IvoxMap::append_incremental(const float4* d_new, size_t n_new, long long cap
     BuildScratch& sc = scratch;
     const size_t S = (size_t)n_stencil;
     // new points -> voxel runs (stable: input order inside a voxel)
-    sc.keys.reserve(n_new);
-    sc.keys_sorted.reserve(n_new);
-    sc.uniq.reserve(n_new);
-    sc.idx.reserve(n_new);
-    sc.idx_sorted.reserve(n_new);
-    sc.counts.reserve(n_new);
-    sc.starts.reserve(n_new);
+    sc.reserve_runs<unsigned long long>(n_new);
     sc.num_runs.reserve(4);
     ivox_keys_kernel<<<grid_for(n_new, 256), 256, 0, st>>>(d_new, n_new, inv_res, key_mode, sc.keys.p, sc.idx.p);
-    size_t t1 = 0, t2 = 0, t3 = 0;
-    cub::DeviceRadixSort::SortPairs(nullptr, t1, sc.keys.p, sc.keys_sorted.p, sc.idx.p, sc.idx_sorted.p, (int)n_new, 0, 63, st);
-    cub::DeviceRunLengthEncode::Encode(nullptr, t2, sc.keys_sorted.p, sc.uniq.p, sc.counts.p, sc.num_runs.p, (int)n_new, st);
-    cub::DeviceScan::ExclusiveSum(nullptr, t3, sc.counts.p, sc.starts.p, (int)n_new, st);
-    size_t tmp = t1 > t2 ? t1 : t2;
-    tmp = tmp > t3 ? tmp : t3;
-    sc.cub_tmp.reserve(tmp + 256);
-    size_t tb = sc.cub_tmp.cap;
-    FLS_CUDA(cub::DeviceRadixSort::SortPairs(sc.cub_tmp.p, tb, sc.keys.p, sc.keys_sorted.p, sc.idx.p, sc.idx_sorted.p, (int)n_new, 0, 63, st));
-    tb = sc.cub_tmp.cap;
-    FLS_CUDA(cub::DeviceRunLengthEncode::Encode(sc.cub_tmp.p, tb, sc.keys_sorted.p, sc.uniq.p, sc.counts.p, sc.num_runs.p, (int)n_new, st));
-    FLS_CUDA(cudaMemcpyAsync(sc.h_num_runs, sc.num_runs.p, sizeof(int), cudaMemcpyDeviceToHost, st));
-    FLS_CUDA(cudaStreamSynchronize(st));
-    const int T = *sc.h_num_runs;  // touched voxels
-    tb = sc.cub_tmp.cap;
-    FLS_CUDA(cub::DeviceScan::ExclusiveSum(sc.cub_tmp.p, tb, sc.counts.p, sc.starts.p, T, st));
+    sc.sort_pairs<unsigned long long>(n_new, 63, st);
+    const int T = sc.encode_runs<unsigned long long>(n_new, st);  // touched voxels
+    sc.run_starts(T, st);
     // plan: old location / length of every touched voxel, how many are created
     inc_old_start.reserve((size_t)T + 1);
     inc_old_count.reserve((size_t)T + 1);
@@ -412,22 +439,21 @@ int IvoxMap::append_incremental(const float4* d_new, size_t n_new, long long cap
     FLS_CUDA(cudaMemsetAsync(lru_cnt.p, 0, 8 * sizeof(int), st));
     inc_plan_kernel<<<grid_for((size_t)T, 256), 256, 0, st>>>(sc.uniq.p, sc.counts.p, T, table.p, mask, inc_old_start.p, inc_old_count.p, inc_new_count.p,
                                                             lru_cnt.p);
-    tb = sc.cub_tmp.cap;
-    FLS_CUDA(cub::DeviceScan::ExclusiveSum(sc.cub_tmp.p, tb, inc_new_count.p, inc_new_off.p, T, st));
+    // sized by sort_pairs: the same scan over n_new >= T items
+    cub_run(sc.cub_tmp, [&](void* tmp, size_t& bytes) { return cub::DeviceScan::ExclusiveSum(tmp, bytes, inc_new_count.p, inc_new_off.p, T, st); });
     // affected centres: every centre whose stencil contains a touched voxel
     const size_t n_keys = (size_t)T * S;
     ckeys.reserve(n_keys);
     ckeys_sorted.reserve(n_keys);
     cuniq.reserve(n_keys);
     center_keys_kernel<<<grid_for(n_keys, 256), 256, 0, st>>>(sc.uniq.p, T, n_stencil, ckeys.p);
-    size_t u1 = 0, u2 = 0;
-    cub::DeviceRadixSort::SortKeys(nullptr, u1, ckeys.p, ckeys_sorted.p, (int)n_keys, 0, 63, st);
-    cub::DeviceSelect::Unique(nullptr, u2, ckeys_sorted.p, cuniq.p, sc.num_runs.p + 1, (int)n_keys, st);
-    sc.cub_tmp.reserve((u1 > u2 ? u1 : u2) + 256);
-    tb = sc.cub_tmp.cap;
-    FLS_CUDA(cub::DeviceRadixSort::SortKeys(sc.cub_tmp.p, tb, ckeys.p, ckeys_sorted.p, (int)n_keys, 0, 63, st));
-    tb = sc.cub_tmp.cap;
-    FLS_CUDA(cub::DeviceSelect::Unique(sc.cub_tmp.p, tb, ckeys_sorted.p, cuniq.p, sc.num_runs.p + 1, (int)n_keys, st));
+    auto sort = [&](void* tmp, size_t& bytes) { return cub::DeviceRadixSort::SortKeys(tmp, bytes, ckeys.p, ckeys_sorted.p, (int)n_keys, 0, 63, st); };
+    auto unique = [&](void* tmp, size_t& bytes) {
+        return cub::DeviceSelect::Unique(tmp, bytes, ckeys_sorted.p, cuniq.p, sc.num_runs.p + 1, (int)n_keys, st);
+    };
+    cub_reserve(sc.cub_tmp, sort, unique);
+    cub_run(sc.cub_tmp, sort);
+    cub_run(sc.cub_tmp, unique);
     int hc[8];
     unsigned last_off = 0, last_cnt = 0;
     int n_aff = 0;
@@ -452,11 +478,7 @@ int IvoxMap::append_incremental(const float4* d_new, size_t n_new, long long cap
     list_count_kernel<<<grid_for((size_t)n_aff, 128), 128, 0, st>>>(cuniq.p, n_aff, n_stencil, table.p, mask, ccount.p);
     FLS_CUDA(cudaMemsetAsync(lru_cnt.p, 0, 8 * sizeof(int), st));
     inc_new_centres_kernel<<<grid_for((size_t)n_aff, 256), 256, 0, st>>>(cuniq.p, n_aff, ctab.p, cmask, ccount.p, lru_cnt.p);
-    size_t t4 = 0;
-    cub::DeviceScan::ExclusiveSum(nullptr, t4, ccount.p, cstart.p, n_aff, st);
-    sc.cub_tmp.reserve(t4 + 256);
-    tb = sc.cub_tmp.cap;
-    FLS_CUDA(cub::DeviceScan::ExclusiveSum(sc.cub_tmp.p, tb, ccount.p, cstart.p, n_aff, st));
+    cub_pass(sc.cub_tmp, [&](void* tmp, size_t& bytes) { return cub::DeviceScan::ExclusiveSum(tmp, bytes, ccount.p, cstart.p, n_aff, st); });
     unsigned l_off = 0, l_cnt = 0;
     FLS_CUDA(cudaMemcpyAsync(hc, lru_cnt.p, 8 * sizeof(int), cudaMemcpyDeviceToHost, st));
     FLS_CUDA(cudaMemcpyAsync(&l_off, cstart.p + (n_aff - 1), sizeof(unsigned), cudaMemcpyDeviceToHost, st));
@@ -592,14 +614,10 @@ int IvoxMap::evict_lru(size_t n_old, size_t n, int runs, long long capacity, cud
     FLS_CUDA(cudaStreamSynchronize(st));
     const int n_cand = hc[0], n_create = hc[1], n_touched = hc[2];
     if (n_cand == 0) return FLS_ERR_CAPACITY;
-    size_t tb = 0;
-    cub::DeviceRadixSort::SortPairs(nullptr, tb, lru_keys.p, lru_keys_sorted.p, lru_vals.p, lru_vals_sorted.p, n_cand, 0, 64, st);
-    sc.cub_tmp.reserve(tb + 256);
-    tb = sc.cub_tmp.cap;
-    FLS_CUDA(cub::DeviceRadixSort::SortPairs(sc.cub_tmp.p, tb, lru_keys.p, lru_keys_sorted.p, lru_vals.p, lru_vals_sorted.p, n_cand, 0, 64, st));
-    const long long e0 = (long long)n_vox + n_create - (capacity - 1);
-    size_t K = (size_t)(e0 > 0 ? e0 : 0) + 2 * (size_t)n_touched + 64;
-    if (K > (size_t)n_cand) K = (size_t)n_cand;
+    cub_pass(sc.cub_tmp, [&](void* tmp, size_t& bytes) {
+        return cub::DeviceRadixSort::SortPairs(tmp, bytes, lru_keys.p, lru_keys_sorted.p, lru_vals.p, lru_vals_sorted.p, n_cand, 0, 64, st);
+    });
+    const size_t K = lru_candidate_bound(n_vox, n_create, n_touched, capacity, (size_t)n_cand);
     sc.k32a.reserve(K + 1);
     ivox_cand_kernel<<<grid_for(K, 256), 256, 0, st>>>(lru_vals_sorted.p, (int)K, lru_first.p, sc.k32a.p);
     std::vector<unsigned> cand(K), creat((size_t)n_create);
@@ -621,14 +639,15 @@ int IvoxMap::evict_lru(size_t n_old, size_t n, int runs, long long capacity, cud
                                                                         sc.idx_sorted.p, lru_flags.p);
     // stable compaction of the points and their stamps (pts_sorted / keys are rebuilt by the second sort anyway: use them as targets)
     sc.keys.reserve(n + 1);
-    size_t t1 = 0, t2 = 0;
-    cub::DeviceSelect::Flagged(nullptr, t1, pts_all.p, lru_flags.p, pts_sorted.p, sc.num_runs.p, (int)n, st);
-    cub::DeviceSelect::Flagged(nullptr, t2, stamp_all.p, lru_flags.p, sc.keys.p, sc.num_runs.p, (int)n, st);
-    sc.cub_tmp.reserve((t1 > t2 ? t1 : t2) + 256);
-    tb = sc.cub_tmp.cap;
-    FLS_CUDA(cub::DeviceSelect::Flagged(sc.cub_tmp.p, tb, pts_all.p, lru_flags.p, pts_sorted.p, sc.num_runs.p, (int)n, st));
-    tb = sc.cub_tmp.cap;
-    FLS_CUDA(cub::DeviceSelect::Flagged(sc.cub_tmp.p, tb, stamp_all.p, lru_flags.p, sc.keys.p, sc.num_runs.p, (int)n, st));
+    auto keep_pts = [&](void* tmp, size_t& bytes) {
+        return cub::DeviceSelect::Flagged(tmp, bytes, pts_all.p, lru_flags.p, pts_sorted.p, sc.num_runs.p, (int)n, st);
+    };
+    auto keep_stamps = [&](void* tmp, size_t& bytes) {
+        return cub::DeviceSelect::Flagged(tmp, bytes, stamp_all.p, lru_flags.p, sc.keys.p, sc.num_runs.p, (int)n, st);
+    };
+    cub_reserve(sc.cub_tmp, keep_pts, keep_stamps);
+    cub_run(sc.cub_tmp, keep_pts);
+    cub_run(sc.cub_tmp, keep_stamps);
     FLS_CUDA(cudaMemcpyAsync(sc.h_num_runs, sc.num_runs.p, sizeof(int), cudaMemcpyDeviceToHost, st));
     FLS_CUDA(cudaStreamSynchronize(st));  // also: the host vectors above are read by the copies
     const size_t kept = (size_t)*sc.h_num_runs;
@@ -665,25 +684,20 @@ int IvoxMap::build_stencil_lists(cudaStream_t st, int* launches) {
     ckeys_sorted.reserve(n_keys);
     cuniq.reserve(n_keys);
     center_keys_kernel<<<grid_for(n_keys, 256), 256, 0, st>>>(sc.uniq.p, (int)n_vox, n_stencil, ckeys.p);
-    size_t t1 = 0, t2 = 0;
-    cub::DeviceRadixSort::SortKeys(nullptr, t1, ckeys.p, ckeys_sorted.p, (int)n_keys, 0, 63, st);
-    cub::DeviceSelect::Unique(nullptr, t2, ckeys_sorted.p, cuniq.p, sc.num_runs.p, (int)n_keys, st);
-    sc.cub_tmp.reserve((t1 > t2 ? t1 : t2) + 256);
-    size_t tb = sc.cub_tmp.cap;
-    FLS_CUDA(cub::DeviceRadixSort::SortKeys(sc.cub_tmp.p, tb, ckeys.p, ckeys_sorted.p, (int)n_keys, 0, 63, st));
-    tb = sc.cub_tmp.cap;
-    FLS_CUDA(cub::DeviceSelect::Unique(sc.cub_tmp.p, tb, ckeys_sorted.p, cuniq.p, sc.num_runs.p, (int)n_keys, st));
+    auto sort = [&](void* tmp, size_t& bytes) { return cub::DeviceRadixSort::SortKeys(tmp, bytes, ckeys.p, ckeys_sorted.p, (int)n_keys, 0, 63, st); };
+    auto unique = [&](void* tmp, size_t& bytes) {
+        return cub::DeviceSelect::Unique(tmp, bytes, ckeys_sorted.p, cuniq.p, sc.num_runs.p, (int)n_keys, st);
+    };
+    cub_reserve(sc.cub_tmp, sort, unique);
+    cub_run(sc.cub_tmp, sort);
+    cub_run(sc.cub_tmp, unique);
     FLS_CUDA(cudaMemcpyAsync(sc.h_num_runs, sc.num_runs.p, sizeof(int), cudaMemcpyDeviceToHost, st));
     FLS_CUDA(cudaStreamSynchronize(st));
     const int nc = *sc.h_num_runs;
     ccount.reserve((size_t)nc);
     cstart.reserve((size_t)nc);
     list_count_kernel<<<grid_for((size_t)nc, 128), 128, 0, st>>>(cuniq.p, nc, n_stencil, table.p, mask, ccount.p);
-    size_t t3 = 0;
-    cub::DeviceScan::ExclusiveSum(nullptr, t3, ccount.p, cstart.p, nc, st);
-    sc.cub_tmp.reserve(t3 + 256);
-    tb = sc.cub_tmp.cap;
-    FLS_CUDA(cub::DeviceScan::ExclusiveSum(sc.cub_tmp.p, tb, ccount.p, cstart.p, nc, st));
+    cub_pass(sc.cub_tmp, [&](void* tmp, size_t& bytes) { return cub::DeviceScan::ExclusiveSum(tmp, bytes, ccount.p, cstart.p, nc, st); });
     // load factor <= 0.25: the centre table is probed once per point-iteration and a long linear-probing chain stalls
     // a whole warp, so it is kept sparser than the occupied table
     size_t slots = 1024;

@@ -19,7 +19,21 @@ namespace fls {
 bool lru_simulate(size_t size0, size_t capacity, const std::vector<unsigned>& cand_first_touch, std::vector<unsigned> create_times,
                   std::vector<unsigned>& victims, std::vector<unsigned char>& recreated);
 
-// scratch shared by the sort / run-length passes of every map build and of the voxel-grid filter
+// How many of the n_cand oldest candidates lru_simulate needs for a call that creates n_new voxels in a map of n_vox, n_touched
+// of the candidates being touched by the call.  Without cascades n_vox + n_new - (capacity - 1) voxels go; every candidate the
+// simulation skips was touched in this call, and each touched victim is re-created and can push out one more, so 2 * n_touched
+// (plus a margin) covers both.  Capped at n_cand.
+size_t lru_candidate_bound(size_t n_vox, int n_new, int n_touched, long long capacity, size_t n_cand);
+
+// Scratch shared by the sort / run-length passes of every map build and of the voxel-grid filter.
+// The voxel-runs pass puts n keyed points in voxel-contiguous order: a stable radix sort of (key, point index) over key bits
+// [0, end_bit), a run-length encode of the sorted keys, and the exclusive sum of the run lengths (each run's first sorted
+// position).  Keys K = unsigned long long go keys -> keys_sorted -> uniq, keys K = unsigned go k32a -> k32b -> uniq32; both
+// sort idx -> idx_sorted and write counts and starts.  It is split in steps so that a caller can work between them:
+//   reserve_runs<K>(n)          the arrays, before the caller's key kernel fills the keys and idx
+//   sort_pairs<K>(n, end_bit)   sizes cub_tmp once for sort, encode and sum over n, then sorts
+//   encode_runs<K>(n)           encodes and returns the run count, read through h_num_runs after one stream wait
+//   run_starts(runs)            the exclusive sum of the run lengths
 struct BuildScratch {
     DevBuf<unsigned long long> keys, keys_sorted, uniq;
     DevBuf<unsigned> idx, idx_sorted, counts, starts, k32a, k32b, uniq32;
@@ -30,6 +44,13 @@ struct BuildScratch {
     bool pinned = true;
     BuildScratch();
     ~BuildScratch();
+    template <class K>
+    void reserve_runs(size_t n);
+    template <class K>
+    void sort_pairs(size_t n, int end_bit, cudaStream_t st);
+    template <class K>
+    int encode_runs(size_t n, cudaStream_t st);
+    void run_starts(int runs, cudaStream_t st);
 };
 
 // K7: VoxelGridCloud on the device.  d_out must hold n records; returns the output count.  `waits` (optional) counts the

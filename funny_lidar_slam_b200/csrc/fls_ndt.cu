@@ -39,8 +39,6 @@ struct __align__(16) NdtBatchItem {
 
 namespace {
 
-inline unsigned grid_for(size_t n, int block) { return (unsigned)((n + block - 1) / block); }
-
 __device__ __forceinline__ int ndt_coord(double v, double inv) { return (int)__dmul_rn(v, inv); }  // cast<int>() truncates
 
 __global__ void ndt_keys_kernel(const float4* __restrict__ pts, size_t n, double inv, unsigned long long* __restrict__ keys,
@@ -492,31 +490,11 @@ int NdtMap::add_cloud(const float4* d_cloud, size_t n, float leaf, bool first_sc
         ++*launches;
     }
     BuildScratch& sc = scratch;
-    sc.keys.reserve(nf);
-    sc.keys_sorted.reserve(nf);
-    sc.uniq.reserve(nf);
-    sc.idx.reserve(nf);
-    sc.idx_sorted.reserve(nf);
-    sc.counts.reserve(nf);
-    sc.starts.reserve(nf);
-    sc.num_runs.reserve(2);
+    sc.reserve_runs<unsigned long long>(nf);
     ndt_keys_kernel<<<grid_for(nf, 256), 256, 0, st>>>(filtered.p, nf, inv_voxel, sc.keys.p, sc.idx.p);
-    size_t t1 = 0, t2 = 0, t3 = 0;
-    cub::DeviceRadixSort::SortPairs(nullptr, t1, sc.keys.p, sc.keys_sorted.p, sc.idx.p, sc.idx_sorted.p, (int)nf, 0, 63, st);
-    cub::DeviceRunLengthEncode::Encode(nullptr, t2, sc.keys_sorted.p, sc.uniq.p, sc.counts.p, sc.num_runs.p, (int)nf, st);
-    cub::DeviceScan::ExclusiveSum(nullptr, t3, sc.counts.p, sc.starts.p, (int)nf, st);
-    size_t tmp = t1 > t2 ? t1 : t2;
-    tmp = tmp > t3 ? tmp : t3;
-    sc.cub_tmp.reserve(tmp + 256);
-    size_t tb = sc.cub_tmp.cap;
-    FLS_CUDA(cub::DeviceRadixSort::SortPairs(sc.cub_tmp.p, tb, sc.keys.p, sc.keys_sorted.p, sc.idx.p, sc.idx_sorted.p, (int)nf, 0, 63, st));
-    tb = sc.cub_tmp.cap;
-    FLS_CUDA(cub::DeviceRunLengthEncode::Encode(sc.cub_tmp.p, tb, sc.keys_sorted.p, sc.uniq.p, sc.counts.p, sc.num_runs.p, (int)nf, st));
-    FLS_CUDA(cudaMemcpyAsync(sc.h_num_runs, sc.num_runs.p, sizeof(int), cudaMemcpyDeviceToHost, st));
-    FLS_CUDA(cudaStreamSynchronize(st));
-    const int runs = *sc.h_num_runs;
-    tb = sc.cub_tmp.cap;
-    FLS_CUDA(cub::DeviceScan::ExclusiveSum(sc.cub_tmp.p, tb, sc.counts.p, sc.starts.p, runs, st));
+    sc.sort_pairs<unsigned long long>(nf, 63, st);
+    const int runs = sc.encode_runs<unsigned long long>(nf, st);
+    sc.run_starts(runs, st);
     // ---- LRU bookkeeping: which touched voxels exist, how many are created, who has to go first --------------------------------
     const int hi_water0 = hi_water;
     run_vi.reserve((size_t)runs + 1);
@@ -583,15 +561,10 @@ int NdtMap::evict_lru(int runs, int n_new, int n_touched, cudaStream_t st, int* 
     lru_vals.reserve(n_live + 1);
     lru_vals_sorted.reserve(n_live + 1);
     ndt_live_kernel<<<grid_for(hw, 256), 256, 0, st>>>(cold.p, hw, lru_keys.p, lru_vals.p, counter.p);
-    size_t tb = 0;
-    cub::DeviceRadixSort::SortPairs(nullptr, tb, lru_keys.p, lru_keys_sorted.p, lru_vals.p, lru_vals_sorted.p, (int)n_live, 0, 64, st);
-    sc.cub_tmp.reserve(tb + 256);
-    tb = sc.cub_tmp.cap;
-    FLS_CUDA(cub::DeviceRadixSort::SortPairs(sc.cub_tmp.p, tb, lru_keys.p, lru_keys_sorted.p, lru_vals.p, lru_vals_sorted.p, (int)n_live, 0, 64, st));
-    // the eviction count without cascades is n_vox + n_new - (capacity - 1); every skipped candidate was touched in this call
-    const long long e0 = (long long)n_live + n_new - (capacity - 1);
-    size_t K = (size_t)(e0 > 0 ? e0 : 0) + 2 * (size_t)n_touched + 64;
-    if (K > n_live) K = n_live;
+    cub_pass(sc.cub_tmp, [&](void* tmp, size_t& bytes) {
+        return cub::DeviceRadixSort::SortPairs(tmp, bytes, lru_keys.p, lru_keys_sorted.p, lru_vals.p, lru_vals_sorted.p, (int)n_live, 0, 64, st);
+    });
+    const size_t K = lru_candidate_bound(n_live, n_new, n_touched, capacity, n_live);
     sc.k32a.reserve(K + 1);
     sc.k32b.reserve((size_t)n_new + 1);
     ndt_cand_kernel<<<grid_for(K, 256), 256, 0, st>>>(lru_vals_sorted.p, (int)K, touch_run.p, sc.starts.p, sc.idx_sorted.p, sc.k32a.p);

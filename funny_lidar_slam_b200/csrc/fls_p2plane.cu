@@ -483,11 +483,7 @@ static size_t select_ivox_inserts(const IvoxView& map, const float4* d_src, int 
     const int g = (n + 127) / 128;
     ivox_insert_rule_kernel<<<g, 128, 0, st>>>(map, d_src, n, prev, fin, filter, cls, d_world);
     ivox_insert_keys_kernel<<<(n + 255) / 256, 256, 0, st>>>(cls, n, sc.keys.p);
-    size_t tb = 0;
-    cub::DeviceScan::ExclusiveSum(nullptr, tb, sc.keys.p, sc.keys_sorted.p, n, st);
-    sc.cub_tmp.reserve(tb + 256);
-    tb = sc.cub_tmp.cap;
-    FLS_CUDA(cub::DeviceScan::ExclusiveSum(sc.cub_tmp.p, tb, sc.keys.p, sc.keys_sorted.p, n, st));
+    cub_pass(sc.cub_tmp, [&](void* tmp, size_t& bytes) { return cub::DeviceScan::ExclusiveSum(tmp, bytes, sc.keys.p, sc.keys_sorted.p, n, st); });
     unsigned long long* d_total = sc.keys.p + n;  // spare slot
     ivox_insert_scatter_kernel<<<(n + 255) / 256, 256, 0, st>>>(cls, sc.keys_sorted.p, n, d_world, d_out, d_total);
     unsigned long long total = 0;

@@ -131,13 +131,11 @@ int run_preprocess(int device, const float* xyzi, const float* time, bool src_on
         }
         const unsigned g = (unsigned)((n + 255) / 256);
         pp_point_kernel<<<g, 256, 0, st>>>(px, xs, pt, ts, (int)n, dv, min_d, max_d, jump_span, w.corrected.p, w.f_ord.p, w.f_pl.p);
-        size_t tb = 0;
-        cub::DeviceScan::ExclusiveSum(nullptr, tb, w.f_ord.p, w.e_ord.p, (int)n, st);
-        w.cub_tmp.reserve(tb + 256);
-        tb = w.cub_tmp.cap;
-        FLS_CUDA(cub::DeviceScan::ExclusiveSum(w.cub_tmp.p, tb, w.f_ord.p, w.e_ord.p, (int)n, st));
-        tb = w.cub_tmp.cap;
-        FLS_CUDA(cub::DeviceScan::ExclusiveSum(w.cub_tmp.p, tb, w.f_pl.p, w.e_pl.p, (int)n, st));
+        auto scan_ord = [&](void* tmp, size_t& bytes) { return cub::DeviceScan::ExclusiveSum(tmp, bytes, w.f_ord.p, w.e_ord.p, (int)n, st); };
+        auto scan_pl = [&](void* tmp, size_t& bytes) { return cub::DeviceScan::ExclusiveSum(tmp, bytes, w.f_pl.p, w.e_pl.p, (int)n, st); };
+        cub_reserve(w.cub_tmp, scan_ord, scan_pl);
+        cub_run(w.cub_tmp, scan_ord);
+        cub_run(w.cub_tmp, scan_pl);
         pp_scatter_kernel<<<g, 256, 0, st>>>(w.corrected.p, (int)n, w.f_ord.p, w.e_ord.p, ord);
         pp_scatter_kernel<<<g, 256, 0, st>>>(w.corrected.p, (int)n, w.f_pl.p, w.e_pl.p, w.planar.p);
         unsigned last[4] = {0, 0, 0, 0};

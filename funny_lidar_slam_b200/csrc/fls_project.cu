@@ -120,11 +120,7 @@ int enqueue_project(ProjStage& w, const void* raw, const int* ring, const float*
     proj_clear_kernel<<<gc, 256, 0, st>>>(w.winner.p, cells);
     if (n) proj_claim_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(d_raw, d_ring, d_time, dv, (int)n, V, H, h_res, min_d, max_d, w.winner.p);
     proj_flags_kernel<<<gc, 256, 0, st>>>(w.winner.p, cells, w.flag.p);
-    size_t tb = 0;
-    cub::DeviceScan::ExclusiveSum(nullptr, tb, w.flag.p, w.excl.p, (int)cells, st);
-    w.cub_tmp.reserve(tb + 256);
-    tb = w.cub_tmp.cap;
-    FLS_CUDA(cub::DeviceScan::ExclusiveSum(w.cub_tmp.p, tb, w.flag.p, w.excl.p, (int)cells, st));
+    cub_pass(w.cub_tmp, [&](void* tmp, size_t& bytes) { return cub::DeviceScan::ExclusiveSum(tmp, bytes, w.flag.p, w.excl.p, (int)cells, st); });
     // upstream leaves the tails of depth / col as they were (resize to V*H, col zero-filled): zero both
     FLS_CUDA(cudaMemsetAsync(w.depth.p, 0, cells * sizeof(float), st));
     FLS_CUDA(cudaMemsetAsync(w.col.p, 0, cells * sizeof(int), st));

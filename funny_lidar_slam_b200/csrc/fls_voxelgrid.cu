@@ -4,8 +4,6 @@
 //   (xyz AND intensity) per occupied cell, cells in ascending id; dx*dy*dz > INT_MAX returns the input unchanged.
 // The radix sort is stable, so every centroid is summed in input order — the order the oracle pins.  The key and centroid
 // arithmetic lives in fls_voxel.cuh, shared with the keyframe store's segmented pass (fls_keyframes.cu).
-#include <cub/cub.cuh>
-
 #include "fls_maps.h"
 #include "fls_voxel.cuh"
 
@@ -60,8 +58,6 @@ __global__ void vg_centroid_kernel(const float4* __restrict__ pts, const unsigne
     out[r] = acc.mean(c);
 }
 
-inline unsigned grid_for(size_t n, int block) { return (unsigned)((n + block - 1) / block); }
-
 }  // namespace
 
 // Returns the number of output points; d_out must hold n records.  Synchronises the stream twice
@@ -71,7 +67,6 @@ size_t voxel_grid_device(const float4* d_pts, size_t n, float leaf, float4* d_ou
     const float inv = 1.0f / leaf;
     sc.minmax.reserve(16);
     MinMaxOrd* d_mm = reinterpret_cast<MinMaxOrd*>(sc.minmax.p);
-    sc.num_runs.reserve(2);
     minmax_init_kernel<<<1, 1, 0, st>>>(d_mm);
     const unsigned nb = grid_for(n, 256) < 592 ? grid_for(n, 256) : 592;
     minmax_kernel<<<nb, 256, 0, st>>>(d_pts, n, d_mm);
@@ -85,36 +80,17 @@ size_t voxel_grid_device(const float4* d_pts, size_t n, float leaf, float4* d_ou
         FLS_CUDA(cudaMemcpyAsync(d_out, d_pts, n * sizeof(float4), cudaMemcpyDeviceToDevice, st));
         return n;
     }
-    sc.idx.reserve(n);
-    sc.idx_sorted.reserve(n);
-    sc.counts.reserve(n);
-    sc.starts.reserve(n);
-    sc.k32a.reserve(n);
-    sc.k32b.reserve(n);
-    sc.uniq32.reserve(n);
+    sc.reserve_runs<unsigned>(n);
     vg_keys_kernel<<<grid_for(n, 256), 256, 0, st>>>(d_pts, n, inv, g, sc.k32a.p, sc.idx.p);
     int end_bit = 1;
     {
         const long long maxid = (long long)g.divb[0] * g.divb[1] * g.divb[2];
         while ((1LL << end_bit) < maxid && end_bit < 32) ++end_bit;
     }
-    size_t t1 = 0, t2 = 0, t3 = 0;
-    cub::DeviceRadixSort::SortPairs(nullptr, t1, sc.k32a.p, sc.k32b.p, sc.idx.p, sc.idx_sorted.p, (int)n, 0, end_bit, st);
-    cub::DeviceRunLengthEncode::Encode(nullptr, t2, sc.k32b.p, sc.uniq32.p, sc.counts.p, sc.num_runs.p, (int)n, st);
-    cub::DeviceScan::ExclusiveSum(nullptr, t3, sc.counts.p, sc.starts.p, (int)n, st);
-    size_t tmp = t1 > t2 ? t1 : t2;
-    tmp = tmp > t3 ? tmp : t3;
-    sc.cub_tmp.reserve(tmp + 256);
-    size_t tb = sc.cub_tmp.cap;
-    FLS_CUDA(cub::DeviceRadixSort::SortPairs(sc.cub_tmp.p, tb, sc.k32a.p, sc.k32b.p, sc.idx.p, sc.idx_sorted.p, (int)n, 0, end_bit, st));
-    tb = sc.cub_tmp.cap;
-    FLS_CUDA(cub::DeviceRunLengthEncode::Encode(sc.cub_tmp.p, tb, sc.k32b.p, sc.uniq32.p, sc.counts.p, sc.num_runs.p, (int)n, st));
-    FLS_CUDA(cudaMemcpyAsync(sc.h_num_runs, sc.num_runs.p, sizeof(int), cudaMemcpyDeviceToHost, st));
-    FLS_CUDA(cudaStreamSynchronize(st));
+    sc.sort_pairs<unsigned>(n, end_bit, st);
+    const int runs = sc.encode_runs<unsigned>(n, st);
     if (waits) *waits += 1;
-    const int runs = *sc.h_num_runs;
-    tb = sc.cub_tmp.cap;
-    FLS_CUDA(cub::DeviceScan::ExclusiveSum(sc.cub_tmp.p, tb, sc.counts.p, sc.starts.p, runs, st));
+    sc.run_starts(runs, st);
     vg_centroid_kernel<<<grid_for(runs, 128), 128, 0, st>>>(d_pts, sc.idx_sorted.p, sc.starts.p, sc.counts.p, runs, d_out);
     FLS_CUDA(cudaGetLastError());
     if (launches) *launches += 6;
