@@ -59,7 +59,6 @@ void Handle::init() {
     *h_abort = 0;
     state.reserve(kMaxBatch);
     fit_out.reserve(2);
-    fit_grid.key_mode = 1;
     switch (cfg.method) {
         case FLS_P2PLANE_IVOX: plugin = make_ivox_plugin(*this); break;
         case FLS_NDT: plugin = make_ndt_plugin(*this); break;
@@ -115,24 +114,6 @@ int Handle::begin_batch(int B, const void* const* scans, const size_t* n, size_t
         off += n[s];
     }
     return FLS_OK;
-}
-
-IvoxView Handle::grid_view(const IvoxMap& g) const {
-    IvoxView v;
-    v.pts = g.pts_sorted.p;
-    v.tab = g.table.p;
-    v.mask = g.mask;
-    v.inv_res = g.inv_res;
-    v.max_range2 = cfg.ivox_max_range * cfg.ivox_max_range;
-    static const int counts[4] = {1, 7, 19, 27};
-    v.n_stencil = counts[cfg.ivox_nearby];
-    v.lists = g.lists.p;
-    v.ctab = g.ctab.p;
-    v.cmask = g.cmask;
-    // a query and a candidate of its stencil differ by at most 2*res per axis with a non-zero offset and res otherwise:
-    // d^2 <= 12 res^2 for the full 26-neighbourhood
-    v.fast_knn = 12.0 * 1.01 * (double)g.res * (double)g.res < (double)v.max_range2 ? 1u : 0u;
-    return v;
 }
 
 void Handle::begin_call() {
@@ -283,14 +264,13 @@ int Handle::fitness(float max_range, float* score) {
     if (fit_cloud_n == 0 || last_src == nullptr || last_src_n == 0 || !(max_range > 0.f)) return FLS_OK;
     begin_call();
     if (fit_grid_version != fit_cloud_version || fit_grid_range != max_range) {
-        fit_grid.set_resolution(std::sqrt(max_range) * 1.001f);
-        fit_grid.clear();
-        const int rc = fit_grid.append_and_build(fit_pts, fit_cloud_n, 0, stream, &launches);
+        fit_grid.res = std::sqrt(max_range) * 1.001f;
+        const int rc = fit_grid.build(fit_pts, fit_cloud_n, scratch, stream, &launches);
         if (rc != FLS_OK) return rc;
         fit_grid_version = fit_cloud_version;
         fit_grid_range = max_range;
     }
-    launch_fitness(grid_view(fit_grid), last_src, (int)last_src_n, T_final, max_range, fit_out.p, stream);
+    launch_fitness(fit_grid.view(), last_src, (int)last_src_n, T_final, max_range, fit_out.p, stream);
     launches++;
     double h[2] = {0, 0};
     FLS_CUDA(cudaMemcpyAsync(h, fit_out.p, sizeof(h), cudaMemcpyDeviceToHost, stream));

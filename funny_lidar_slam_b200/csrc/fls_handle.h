@@ -113,7 +113,7 @@ struct Handle {
     size_t fit_cloud_n = 0;
     unsigned long long fit_cloud_version = 0, fit_grid_version = ~0ull;
     float fit_grid_range = -1.f;
-    IvoxMap fit_grid;
+    SearchGrid fit_grid;
     DevBuf<double> fit_out;
 
     explicit Handle(const fls_config& c);
@@ -130,7 +130,6 @@ struct Handle {
     // begin_call of a batch Match (clearing st[n_scans] when given) and its scans as device pointers: host records of `host_stride`
     // bytes go back to back into src, device scans as they are
     int begin_batch(int n_scans, const void* const* scans, const size_t* n, size_t host_stride, const float4** ptrs, fls_match_stats* st);
-    IvoxView grid_view(const IvoxMap& g) const;
     void set_fit_cloud(const float4* d, size_t n);  // copies
     void set_fit_view(const float4* d, size_t n);   // refers to d until the next call
 

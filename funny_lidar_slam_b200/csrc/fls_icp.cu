@@ -19,7 +19,7 @@ static constexpr int kIcpBlock = 512;  // 64 queries x 8 lanes per CTA: few rows
 struct IcpArgs {
     const float4* __restrict__ src;  // voxel-filtered scan, body frame
     int n;
-    IvoxView map;  // floor-keyed search grid over the voxel-filtered local map
+    GridView map;  // search grid over the voxel-filtered local map
     double max_corr;
     GnState* state;
 };
@@ -27,15 +27,15 @@ struct IcpArgs {
 namespace {
 
 // nearest map point within the 27-cell neighbourhood; returns false when the neighbourhood is empty
-__device__ __forceinline__ bool grid_nn1(const IvoxView& g, float qx, float qy, float qz, float& best_d, unsigned& best_j, unsigned& n_cand,
+__device__ __forceinline__ bool grid_nn1(const GridView& g, float qx, float qy, float qz, float& best_d, unsigned& best_j, unsigned& n_cand,
                                          unsigned& n_hits) {
     best_d = INFINITY;
     best_j = 0xffffffffu;
     n_cand = 0;
     n_hits = 0;
-    const float ux = __fmul_rn(qx, g.inv_res), uy = __fmul_rn(qy, g.inv_res), uz = __fmul_rn(qz, g.inv_res);
+    const float ux = __fmul_rn(qx, g.inv_cell), uy = __fmul_rn(qy, g.inv_cell), uz = __fmul_rn(qz, g.inv_cell);
     const int kx = (int)floorf(ux), ky = (int)floorf(uy), kz = (int)floorf(uz);
-    const float cell = 1.0f / g.inv_res;
+    const float cell = 1.0f / g.inv_cell;  // not g.cell: the two can differ in the last bit
 #pragma unroll 1
     for (int s = 0; s < 27; ++s) {
         const int cx = kx + c_stencil[s][0], cy = ky + c_stencil[s][1], cz = kz + c_stencil[s][2];
@@ -66,14 +66,14 @@ __device__ __forceinline__ bool grid_nn1(const IvoxView& g, float qx, float qy, 
 // sub, sub+kIcpLanes, ...; the winner is the lexicographic minimum of (d2, stencil position, point index) — the same
 // point the sequential scan above keeps (strict '<' in visit order).  All lanes of the group return the result.
 static constexpr int kIcpLanes = 8;
-__device__ __forceinline__ bool grid_nn1_coop(const IvoxView& g, int sub, unsigned group_mask, float qx, float qy, float qz, float& best_d,
+__device__ __forceinline__ bool grid_nn1_coop(const GridView& g, int sub, unsigned group_mask, float qx, float qy, float qz, float& best_d,
                                               unsigned& best_j, unsigned& n_cand, unsigned& n_hits) {
     best_d = INFINITY;
     best_j = 0xffffffffu;
     unsigned best_s = 0xffffu;
     n_cand = 0;
     n_hits = 0;
-    const float ux = __fmul_rn(qx, g.inv_res), uy = __fmul_rn(qy, g.inv_res), uz = __fmul_rn(qz, g.inv_res);
+    const float ux = __fmul_rn(qx, g.inv_cell), uy = __fmul_rn(qy, g.inv_cell), uz = __fmul_rn(qz, g.inv_cell);
     const int kx = (int)floorf(ux), ky = (int)floorf(uy), kz = (int)floorf(uz);
 #pragma unroll 1
     for (int s = sub; s < 27; s += kIcpLanes) {
@@ -170,7 +170,7 @@ __global__ void __launch_bounds__(BLOCK) icp_gn_kernel(IcpArgs a, GnLoopCtl ctl)
 }
 
 // GetFitnessScore (icp_optimized.h:191-215 upstream): mean squared 1-NN distance over points with d2 <= max_range
-__global__ void fitness_kernel(IvoxView g, const float4* __restrict__ src, int n, float r0, float r1, float r2, float r3, float r4, float r5,
+__global__ void fitness_kernel(GridView g, const float4* __restrict__ src, int n, float r0, float r1, float r2, float r3, float r4, float r5,
                                float r6, float r7, float r8, float t0, float t1, float t2, float max_range, double* __restrict__ out /*sum, count*/) {
     __shared__ double s_sum[8], s_cnt[8];
     double sum = 0, cnt = 0;
@@ -217,7 +217,7 @@ static void launch_icp_loop(const IcpArgs& a, const GnLoopCtl& ctl, int grid, cu
     launch_cooperative(icp_gn_kernel<kIcpBlock>, grid, kIcpBlock, 0, st, a, ctl);
 }
 
-void launch_fitness(const IvoxView& g, const float4* d_src, int n, const double* T, float max_range, double* d_out2, cudaStream_t st) {
+void launch_fitness(const GridView& g, const float4* d_src, int n, const double* T, float max_range, double* d_out2, cudaStream_t st) {
     cudaMemsetAsync(d_out2, 0, 2 * sizeof(double), st);
     if (n <= 0) return;
     int grid = (n + 255) / 256;
@@ -238,8 +238,7 @@ class IcpPlugin final : public Plugin {
     explicit IcpPlugin(Handle& handle) : Plugin(handle, kOrdered) {
         // search grid of the bounded exact 1-NN: cell >= sqrt(max_correspond_distance)  [quirk 4]
         const double d = h.cfg.icp_max_correspond_distance;
-        window.grid.key_mode = 1;
-        window.grid.set_resolution((float)(std::sqrt(d > 0 ? d : 1.0) * 1.001));
+        window.grid.res = (float)(std::sqrt(d > 0 ? d : 1.0) * 1.001);
     }
 
     int add_cloud(const float4* d_cloud, size_t n, const float4*, size_t) override {
@@ -262,7 +261,7 @@ class IcpPlugin final : public Plugin {
         IcpArgs a;
         a.src = scan.p;
         a.n = ni;
-        a.map = h.grid_view(window.grid);
+        a.map = window.grid.view();
         a.max_corr = cfg.icp_max_correspond_distance;
         a.state = h.state.p;
         // roofline accounting (SURVEY.md §8d, K3): 16 B source point + 27 x 16 B slot probes, 16 B per scanned map record
@@ -279,7 +278,7 @@ class IcpPlugin final : public Plugin {
     }
 
     void map_info(fls_map_info* out) const override {
-        const IvoxMap& g = window.grid;
+        const SearchGrid& g = window.grid;
         out->n_points = (long long)g.n_pts;
         out->n_voxels = (long long)g.n_vox;
         out->table_slots = g.n_pts ? (long long)g.mask + 1 : 0;

@@ -36,7 +36,6 @@ static __device__ __constant__ signed char c_stencil[27][4] = {
 __device__ __forceinline__ int ivox_coord(float v, float inv_res) { return (int)roundf(__fmul_rn(v, inv_res)); }
 // uniform search grid (bounded exact NN): floor(p * inv_cell)
 __device__ __forceinline__ int floor_coord(float v, float inv_res) { return (int)floorf(__fmul_rn(v, inv_res)); }
-__device__ __forceinline__ int grid_coord(float v, float inv_res, int key_mode) { return key_mode ? floor_coord(v, inv_res) : ivox_coord(v, inv_res); }
 
 __host__ __device__ __forceinline__ unsigned compact21(unsigned long long x) {  // inverse of spread21
     x &= 0x1249249249249249ULL;

@@ -44,6 +44,6 @@ int p2plane_v9_grid(int n_max, int device);  // also raises the kernel's shared-
 void launch_p2plane_v9(const P2PlaneLoopArgs& a, int grid, cudaStream_t st);
 
 // d_out2[0] = sum of squared NN distances <= max_range, d_out2[1] = how many; T column-major (cast to float inside)
-void launch_fitness(const IvoxView& g, const float4* d_src, int n, const double* T_colmajor, float max_range, double* d_out2, cudaStream_t st);
+void launch_fitness(const GridView& g, const float4* d_src, int n, const double* T_colmajor, float max_range, double* d_out2, cudaStream_t st);
 
 }  // namespace fls

@@ -30,20 +30,12 @@ namespace fls {
 
 static constexpr int kLoamBlock = 256;
 
-// exact unbounded 5-NN over a uniform grid
-struct LoamGrid {
-    const float4* __restrict__ pts;    // cell-contiguous map points
-    const HashSlot* __restrict__ tab;  // floor-keyed occupied-cell table
-    unsigned mask;
-    float inv_cell, cell;
-    unsigned n_pts;
-};
 struct LoamArgs {
     const float4* __restrict__ corner;  // body-frame corner features (LoamFull only)
     int n_corner;
     const float4* __restrict__ planar;  // body-frame planar features
     int n_planar;
-    LoamGrid corner_map, planar_map;
+    GridView corner_map, planar_map;  // exact unbounded 5-NN over these
     double plane_thres;    // point_to_planar_thres
     double search_thres;   // point_search_thres on the 5th squared distance (+inf: none)
     double line_ratio;     // line_ratio_thres
@@ -57,7 +49,7 @@ namespace {
 
 constexpr int kMaxShell = 6;
 
-__device__ __forceinline__ void scan_cell(const LoamGrid& g, int cx, int cy, int cz, float qx, float qy, float qz, Top5& nn, unsigned& n_cand) {
+__device__ __forceinline__ void scan_cell(const GridView& g, int cx, int cy, int cz, float qx, float qy, float qz, Top5& nn, unsigned& n_cand) {
     unsigned start, count;
     if (!table_find(g.tab, g.mask, pack_key(cx, cy, cz), start, count)) return;
     n_cand += count;
@@ -89,7 +81,7 @@ __device__ __forceinline__ void merge_group(Top5& m, unsigned group_mask) {
 
 // exact 5-NN; `gate` = squared distance beyond which the caller rejects the point anyway (INFINITY: none).
 // Called by all lanes of a group with the same query; every lane returns the group's merged result in `nn`.
-__device__ __noinline__ void grid_knn5(const LoamGrid& g, int sub, unsigned group_mask, float qx, float qy, float qz, float gate, Top5& nn,
+__device__ __noinline__ void grid_knn5(const GridView& g, int sub, unsigned group_mask, float qx, float qy, float qz, float gate, Top5& nn,
                                        unsigned& n_cand) {
     nn.init();
     n_cand = 0;
@@ -202,7 +194,7 @@ __global__ void __launch_bounds__(BLOCK) loam_gn_kernel(LoamArgs a, GnLoopCtl ct
             const float qx = xform_row_d(s_pose[0], s_pose[1], s_pose[2], s_pose[9], (double)sp.x, (double)sp.y, (double)sp.z);
             const float qy = xform_row_d(s_pose[3], s_pose[4], s_pose[5], s_pose[10], (double)sp.x, (double)sp.y, (double)sp.z);
             const float qz = xform_row_d(s_pose[6], s_pose[7], s_pose[8], s_pose[11], (double)sp.x, (double)sp.y, (double)sp.z);
-            const LoamGrid& g = is_corner ? a.corner_map : a.planar_map;
+            const GridView& g = is_corner ? a.corner_map : a.planar_map;
             Top5 nn;
             unsigned n_cand;
             grid_knn5(g, sub, group_mask, qx, qy, qz, a.gate, nn, n_cand);
@@ -264,17 +256,6 @@ static void launch_loam_loop(const LoamArgs& a, const GnLoopCtl& ctl, int grid, 
 
 // ---- LoamPointToPlaneKdtree / LoamFull -------------------------------------------------------------------------------
 
-static LoamGrid loam_grid_of(const WindowMap& w) {
-    LoamGrid g;
-    g.pts = w.grid.pts_sorted.p;
-    g.tab = w.grid.table.p;
-    g.mask = w.grid.mask;
-    g.inv_cell = w.grid.inv_res;
-    g.cell = w.grid.res;
-    g.n_pts = (unsigned)w.grid.n_pts;
-    return g;
-}
-
 static void window_info(const WindowMap& w, fls_map_info* out) {
     out->n_points += (long long)w.n;
     out->n_voxels += (long long)w.grid.n_vox;
@@ -296,16 +277,14 @@ class KdPlugin final : public Plugin {
         const fls_config& cfg = h.cfg;
         // exact-search grids: LoamFull only needs neighbours inside sqrt(point_search_thres), so a cell of that size settles every
         // query in the 27-cell pass; the ungated point-to-plane variant uses ~2 map leafs
-        planar.grid.key_mode = 1;
         if (full) {
             const float c = (float)(std::sqrt(cfg.point_search_thres > 0 ? cfg.point_search_thres : 1.0) * 1.001);
-            planar.grid.set_resolution(c);
+            planar.grid.res = c;
             corner = std::make_unique<WindowMap>();
-            corner->grid.key_mode = 1;
-            corner->grid.set_resolution(c);
+            corner->grid.res = c;
         } else {
             const float c = 2.0f * (cfg.map_cloud_filter_size > 0.f ? cfg.map_cloud_filter_size : 0.5f);
-            planar.grid.set_resolution(c < 0.8f ? 0.8f : c);
+            planar.grid.res = c < 0.8f ? 0.8f : c;
         }
     }
 
@@ -341,8 +320,8 @@ class KdPlugin final : public Plugin {
         a.n_corner = (int)n_corner;
         a.planar = d_planar;
         a.n_planar = (int)n_planar;
-        a.planar_map = loam_grid_of(planar);
-        a.corner_map = full ? loam_grid_of(*corner) : a.planar_map;
+        a.planar_map = planar.grid.view();
+        a.corner_map = full ? corner->grid.view() : a.planar_map;
         a.plane_thres = cfg.point_to_planar_thres;
         a.search_thres = full ? cfg.point_search_thres : INFINITY;
         a.line_ratio = cfg.line_ratio_thres;

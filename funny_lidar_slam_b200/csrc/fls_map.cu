@@ -1,14 +1,14 @@
-// fls_map.cu — device-side construction of the point grids (iVox map, ICP / fitness search grids): K8, batch form.
+// fls_map.cu — device-side construction of the point grids (iVox map IvoxMap, search grid SearchGrid): K8, batch form.
 //
 // IVoxMap::AddPoints (src/ivox_map/ivox_map.cpp:122-143 upstream) inserts points one by one into an
 // unordered_map of std::list nodes.  Here a whole cloud is inserted at once:
-//   key (Morton of round(p/res)) -> stable radix sort -> gather -> run-length encode -> scan -> hash insert,
-// then (iVox only) the per-centre stencil lists are materialised (see fls_ivox.cuh).
+//   key (Morton of round(p/res); floor(p/res) in a SearchGrid) -> stable radix sort -> gather -> run-length encode -> scan -> hash insert,
+// then the iVox map materialises its per-centre stencil lists (see fls_ivox.cuh).
 // The stable sort keeps insertion order inside a voxel, so the k-NN tie order matches a sequential insert.
 // LRU eviction (capacity_, ivox_map.cpp:133-136) is emulated exactly: every point carries its insertion stamp, the stamp of a
 // voxel's last point is its position in upstream's list, and the sequential insert of a call is simulated on the host against
 // the candidates (IvoxMap::evict_lru, lru_simulate).  window_add keeps the sliding-window local map of the ICP and kd-tree LOAM
-// plug-ins on top of such a grid.
+// plug-ins on top of a SearchGrid.
 #include <cub/cub.cuh>
 
 #include <cstdlib>
@@ -130,12 +130,15 @@ template int BuildScratch::encode_runs<unsigned>(size_t, cudaStream_t);
 
 namespace {
 
-__global__ void ivox_keys_kernel(const float4* __restrict__ pts, size_t n, float inv_res, int key_mode, unsigned long long* __restrict__ keys,
-                                 unsigned* __restrict__ idx) {
+// Morton keys of the voxels of round(p * inv_res) (iVox) or floor(p * inv_res) (search grid)
+template <bool kFloor>
+__global__ void voxel_keys_kernel(const float4* __restrict__ pts, size_t n, float inv_res, unsigned long long* __restrict__ keys,
+                                  unsigned* __restrict__ idx) {
     const size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
     if (i >= n) return;
     const float4 p = pts[i];
-    keys[i] = morton_key(grid_coord(p.x, inv_res, key_mode), grid_coord(p.y, inv_res, key_mode), grid_coord(p.z, inv_res, key_mode));
+    keys[i] = kFloor ? morton_key(floor_coord(p.x, inv_res), floor_coord(p.y, inv_res), floor_coord(p.z, inv_res))
+                     : morton_key(ivox_coord(p.x, inv_res), ivox_coord(p.y, inv_res), ivox_coord(p.z, inv_res));
     idx[i] = (unsigned)i;
 }
 
@@ -391,24 +394,42 @@ void launch_transform_f(const float4* d_in, size_t n, const double* T, float4* d
                                                         (float)T[2], (float)T[6], (float)T[10], (float)T[12], (float)T[13], (float)T[14], d_out);
 }
 
-// keys -> stable sort -> gather -> run-length encode -> starts: the voxel-contiguous order of the first n points of pts_all
-int IvoxMap::sort_and_runs(size_t n, cudaStream_t st, int* runs_out, int* launches) {
-    BuildScratch& sc = scratch;
+// The build steps IvoxMap and SearchGrid share.  keys -> stable sort -> gather into dst (room for n) -> run-length encode ->
+// starts: the n points at pts in voxel-contiguous order; returns the voxel count.
+template <bool kFloor>
+static int sorted_runs(const float4* pts, size_t n, float inv_res, float4* dst, BuildScratch& sc, cudaStream_t st, int* launches) {
     sc.reserve_runs<unsigned long long>(n);
-    // mapping mode: room for the voxels the incremental inserts rewrite; buffers grow geometrically (a cudaFree + cudaMalloc of a
-    // few hundred MB costs milliseconds — more than the build itself)
-    if (incremental) {
-        if (n + n / 2 + 65536 > pts_sorted.cap) pts_sorted.reserve(3 * n + 65536);
-    } else {
-        pts_sorted.reserve(n);
-    }
-    ivox_keys_kernel<<<grid_for(n, 256), 256, 0, st>>>(pts_all.p, n, inv_res, key_mode, sc.keys.p, sc.idx.p);
+    voxel_keys_kernel<kFloor><<<grid_for(n, 256), 256, 0, st>>>(pts, n, inv_res, sc.keys.p, sc.idx.p);
     sc.sort_pairs<unsigned long long>(n, 63, st);
-    gather_kernel<<<grid_for(n, 256), 256, 0, st>>>(pts_all.p, sc.idx_sorted.p, n, pts_sorted.p);
+    gather_kernel<<<grid_for(n, 256), 256, 0, st>>>(pts, sc.idx_sorted.p, n, dst);
     const int runs = sc.encode_runs<unsigned long long>(n, st);
     sc.run_starts(runs, st);
     *launches += 6;
-    *runs_out = runs;
+    return runs;
+}
+
+// the table of `slots` (a power of two) slots over the runs of sorted_runs; returns its mask
+static unsigned fill_table(DevBuf<HashSlot>& table, size_t slots, int runs, const BuildScratch& sc, cudaStream_t st, int* launches) {
+    const unsigned mask = (unsigned)(slots - 1);
+    table.reserve(slots);
+    table_clear_kernel<<<grid_for(slots, 256), 256, 0, st>>>(table.p, slots);
+    ivox_insert_kernel<<<grid_for(runs, 256), 256, 0, st>>>(sc.uniq.p, sc.starts.p, sc.counts.p, runs, table.p, mask);
+    FLS_CUDA(cudaGetLastError());
+    *launches += 2;
+    return mask;
+}
+
+int SearchGrid::build(const float4* d_cloud, size_t n, BuildScratch& sc, cudaStream_t st, int* launches) {
+    n_pts = n_vox = 0;
+    if (n == 0) return FLS_OK;
+    if (n > 0xfffffff0ull) return FLS_ERR_INVALID_ARG;
+    pts_sorted.reserve(n);
+    const int runs = sorted_runs<true>(d_cloud, n, 1.0f / res, pts_sorted.p, sc, st, launches);
+    size_t slots = 1024;
+    while (slots < 2 * (size_t)runs) slots <<= 1;
+    mask = fill_table(table, slots, runs, sc, st, launches);
+    n_pts = n;
+    n_vox = (size_t)runs;
     return FLS_OK;
 }
 
@@ -420,13 +441,13 @@ int IvoxMap::sort_and_runs(size_t n, cudaStream_t st, int* runs_out, int* launch
 // would exceed its load factor, when the garbage outweighs the live data, or when the LRU has to evict.
 // Returns 1 when the caller has to take the full path instead.
 int IvoxMap::append_incremental(const float4* d_new, size_t n_new, long long capacity, cudaStream_t st, int* launches) {
-    if (!incremental || n_pts == 0 || n_stencil <= 0 || n_new == 0) return 1;
+    if (!incremental || n_pts == 0 || n_new == 0) return 1;
     BuildScratch& sc = scratch;
     const size_t S = (size_t)n_stencil;
     // new points -> voxel runs (stable: input order inside a voxel)
     sc.reserve_runs<unsigned long long>(n_new);
     sc.num_runs.reserve(4);
-    ivox_keys_kernel<<<grid_for(n_new, 256), 256, 0, st>>>(d_new, n_new, inv_res, key_mode, sc.keys.p, sc.idx.p);
+    voxel_keys_kernel<false><<<grid_for(n_new, 256), 256, 0, st>>>(d_new, n_new, inv_res, sc.keys.p, sc.idx.p);
     sc.sort_pairs<unsigned long long>(n_new, 63, st);
     const int T = sc.encode_runs<unsigned long long>(n_new, st);  // touched voxels
     sc.run_starts(T, st);
@@ -537,7 +558,7 @@ int IvoxMap::build_full(size_t n_old, size_t n_in, long long capacity, cudaStrea
     size_t n = n_in;
     if (n == 0) return FLS_OK;
     if (n > 0xfffffff0ull) return FLS_ERR_INVALID_ARG;
-    const bool lru = capacity > 0;  // the iVox map proper (the search grids have no capacity)
+    const bool lru = capacity > 0;
     // grow pts_all (and the insertion stamps) preserving the old contents
     if (n > pts_all.cap) {
         DevBuf<float4> bigger;
@@ -562,34 +583,32 @@ int IvoxMap::build_full(size_t n_old, size_t n_in, long long capacity, cudaStrea
             ivox_stamp_kernel<<<grid_for(n_new, 256), 256, 0, st>>>(stamp_all.p + n_old, n_new, call_no << 32);
         }
     }
-    int runs = 0;
-    int rc = sort_and_runs(n, st, &runs, launches);
-    if (rc != FLS_OK) return rc;
+    // mapping mode: room for the voxels the incremental inserts rewrite; buffers grow geometrically (a cudaFree + cudaMalloc of a
+    // few hundred MB costs milliseconds — more than the build itself)
+    if (incremental) {
+        if (n + n / 2 + 65536 > pts_sorted.cap) pts_sorted.reserve(3 * n + 65536);
+    } else {
+        pts_sorted.reserve(n);
+    }
+    int runs = sorted_runs<false>(pts_all.p, n, inv_res, pts_sorted.p, scratch, st, launches);
     if (lru && (long long)runs >= capacity) {
         // IVoxMap::AddPoints would have evicted the LRU tail while inserting (ivox_map.cpp:133-136): drop those voxels' old points
         size_t n_after = n;
-        rc = evict_lru(n_old, n, runs, capacity, st, &n_after, launches);
+        const int rc = evict_lru(n_old, n, runs, capacity, st, &n_after, launches);
         if (rc != FLS_OK) return rc;
         n = n_after;
-        rc = sort_and_runs(n, st, &runs, launches);
-        if (rc != FLS_OK) return rc;
+        runs = sorted_runs<false>(pts_all.p, n, inv_res, pts_sorted.p, scratch, st, launches);  // n only shrank: pts_sorted has room
     }
     size_t slots = 1024;
     while (slots < (incremental ? 4 : 2) * (size_t)runs) slots <<= 1;  // mapping mode: room for the voxels to come
     if (incremental && slots <= (size_t)mask + 1 && table.cap >= (size_t)mask + 1 && (size_t)mask + 1 >= 2 * (size_t)runs) slots = (size_t)mask + 1;  // keep the table while it is big enough
-    table.reserve(slots);
-    mask = (unsigned)(slots - 1);
-    table_clear_kernel<<<grid_for(slots, 256), 256, 0, st>>>(table.p, slots);
-    ivox_insert_kernel<<<grid_for(runs, 256), 256, 0, st>>>(scratch.uniq.p, scratch.starts.p, scratch.counts.p, runs, table.p, mask);
-    FLS_CUDA(cudaGetLastError());
+    mask = fill_table(table, slots, runs, scratch, st, launches);
     n_pts = n;
     n_vox = (size_t)runs;
     pts_end = n;
     pts_garbage = 0;
-    *launches += 2;
     ++n_full;
-    if (n_stencil > 0) return build_stencil_lists(st, launches);
-    return FLS_OK;
+    return build_stencil_lists(st, launches);
 }
 
 // Exact LRU of IVoxMap::AddPoints for this call (see lru_simulate): a voxel's position in upstream's list is the insertion time of
@@ -760,8 +779,7 @@ int window_add(WindowMap& w, const float4* d_cloud, size_t n, size_t window, flo
         if (n_merged) FLS_CUDA(cudaMemcpyAsync(w.cloud.p, merged, n_merged * sizeof(float4), cudaMemcpyDeviceToDevice, st));
         w.n = n_merged;
     }
-    w.grid.clear();
-    return w.grid.append_and_build(w.cloud.p, w.n, 0, st, launches);
+    return w.grid.build(w.cloud.p, w.n, sc, st, launches);
 }
 
 }  // namespace fls

@@ -1,4 +1,5 @@
-// fls_maps.h — host-side owners of the device-resident map structures.  Every builder adds the kernels it launches to `*launches`.
+// fls_maps.h — host-side owners of the device-resident map structures (SearchGrid, IvoxMap, NdtMap, WindowMap).  Every builder adds
+// the kernels it launches to `*launches`.
 #pragma once
 #include <deque>
 #include <memory>
@@ -58,19 +59,38 @@ struct BuildScratch {
 size_t voxel_grid_device(const float4* d_pts, size_t n, float leaf, float4* d_out, BuildScratch& sc, cudaStream_t st, int* launches,
                          int* waits = nullptr);
 
-// Point grid: voxel-contiguous float4 points + open-addressing table of {key, start, count} (see fls_ivox.cuh).
-// key_mode 0: round(p/res)  — IVoxMap::Pos2Grid (iVox map of the LOAM plug-in)
-// key_mode 1: floor(p/res)  — uniform search grid under the bounded exact 1-NN of IcpOptimized / GetFitnessScore
+// Uniform search grid over a cloud for the exact 1-NN of IcpOptimized / GetFitnessScore and the exact 5-NN of the kd-tree LOAM
+// plug-ins: cells of floor(p/res), the cloud in cell-contiguous order and an open-addressing table of {key, start, count}.
+struct GridView {  // what the search kernels read
+    const float4* __restrict__ pts;    // cell-contiguous points
+    const HashSlot* __restrict__ tab;  // floor-keyed occupied-cell table
+    unsigned mask;
+    float inv_cell, cell;
+    unsigned n_pts;
+};
+struct SearchGrid {
+    float res = 0.5f;
+    size_t n_pts = 0, n_vox = 0;
+    unsigned mask = 0;
+    DevBuf<float4> pts_sorted;
+    DevBuf<HashSlot> table;
+    // rebuilds the grid over the n points at d_cloud (an empty cloud leaves it empty and launches nothing); returns fls_status
+    int build(const float4* d_cloud, size_t n, BuildScratch& sc, cudaStream_t st, int* launches);
+    GridView view() const { return {pts_sorted.p, table.p, mask, 1.0f / res, res, (unsigned)n_pts}; }
+    size_t bytes() const { return pts_sorted.bytes() + table.bytes(); }
+};
+
+// iVox map: voxels of round(p/res) (IVoxMap::Pos2Grid), voxel-contiguous float4 points + open-addressing table of
+// {key, start, count} (see fls_ivox.cuh).
 //
-// With n_stencil > 0 the build also materialises, for every "centre" voxel (occupied, or within the stencil of an
+// The build also materialises, for every "centre" voxel (occupied, or within the stencil of an
 // occupied voxel), the concatenation of the points of its stencil voxels in the reference's visit order — the exact
 // candidate sequence IVoxMap::GetClosestPoint walks — as one contiguous float4 run, plus a second table
 // {centre key -> run start, run length}.  A k-NN query is then ONE table probe and ONE streaming scan
 // (HBM is spent to buy bandwidth-friendly access: ~n_stencil x the point array).
 struct IvoxMap {
     float res = 0.5f, inv_res = 2.0f;
-    int key_mode = 0;
-    int n_stencil = 0;  // 0: no stencil lists (ICP / fitness grids)
+    int n_stencil = 1;  // voxels per stencil: 1, 7, 19 or 27
     size_t n_pts = 0, n_vox = 0;
     unsigned mask = 0;
     DevBuf<float4> pts_all;     // insertion order (kept so incremental adds can rebuild)
@@ -96,7 +116,6 @@ struct IvoxMap {
         inv_res = 1.0f / r;
     }
     void clear() { n_pts = n_vox = n_centers = n_list = 0; }
-    int sort_and_runs(size_t n, cudaStream_t st, int* runs_out, int* launches);
     int evict_lru(size_t n_old, size_t n, int runs, long long capacity, cudaStream_t st, size_t* n_after, int* launches);
     size_t dump_keys(unsigned long long* h_out, size_t cap, cudaStream_t st);  // packed keys of the occupied voxels (tests)
     // append n points that are already on the device (packed float4) and rebuild; returns fls_status
@@ -195,7 +214,7 @@ struct WindowMap {
     DevBuf<float4> merged;  // concatenation of the window
     DevBuf<float4> cloud;   // what upstream builds the kd-tree on
     size_t n = 0;
-    IvoxMap grid;           // floor-keyed uniform grid over `cloud`
+    SearchGrid grid;        // over `cloud`
 };
 // Adds a device cloud to w (replace: the window is that cloud alone) and rebuilds it.  filter_always false: VoxelGrid(leaf) only
 // once the window holds more than 5 clouds (loam_full_kdtree.h:91-99).

@@ -505,7 +505,13 @@ class IvoxPlugin final : public Plugin {
     std::vector<size_t> pend_n;     // scans of the batch in flight (empty: none)
     bool pend_v9 = false;
 
-    IvoxView view() const { return h.grid_view(map); }
+    IvoxView view() const {
+        const float max_range2 = h.cfg.ivox_max_range * h.cfg.ivox_max_range;
+        // a query and a candidate of its stencil differ by at most 2*res per axis with a non-zero offset and res otherwise:
+        // d^2 <= 12 res^2 for the full 26-neighbourhood
+        const unsigned fast_knn = 12.0 * 1.01 * (double)map.res * (double)map.res < (double)max_range2 ? 1u : 0u;
+        return {map.pts_sorted.p, map.table.p, map.mask, map.inv_res, max_range2, map.n_stencil, map.lists.p, map.ctab.p, map.cmask, fast_knn};
+    }
     int append(const float4* d, size_t n) { return map.append_and_build(d, n, h.cfg.ivox_capacity, h.stream, &h.launches); }
 
     // everything of a batch up to the asynchronous read-back of the states: nothing here waits for the device
@@ -654,7 +660,6 @@ class IvoxPlugin final : public Plugin {
     explicit IvoxPlugin(Handle& handle) : Plugin(handle, kPlanar) {
         static const int counts[4] = {1, 7, 19, 27};
         map.set_resolution(h.cfg.ivox_resolution);
-        map.key_mode = 0;
         map.incremental = !h.cfg.localization_mode;  // mapping mode: the map grows by small inserts
         map.n_stencil = counts[h.cfg.ivox_nearby];
     }
