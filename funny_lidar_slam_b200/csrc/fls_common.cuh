@@ -232,6 +232,13 @@ __host__ __device__ __forceinline__ unsigned long long morton_key(int x, int y, 
 }
 
 #ifdef __CUDACC__
+// static_cast<int64_t> of a double as x86-64's cvttsd2si does it: toward zero, and INT64_MIN for NaN and for values outside the
+// int64 range.  C++ leaves those cases undefined, so the rule is written out here rather than left to what a plain conversion
+// happens to return.  Every time product of the pre-processing path (the scan window, the de-skew's point time) goes through it.
+__device__ __forceinline__ long long trunc_i64(double v) {
+    return (v >= -9.2233720368547758e18 && v < 9.2233720368547758e18) ? __double2ll_rz(v) : (long long)0x8000000000000000ull;
+}
+
 __device__ __forceinline__ bool table_find(const HashSlot* __restrict__ tab, unsigned mask, unsigned long long key, unsigned& start,
                                            unsigned& count) {
     unsigned h = hash_key(key) & mask;

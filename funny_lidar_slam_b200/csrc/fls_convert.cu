@@ -257,11 +257,6 @@ __global__ void off_write_kernel(OffsetParams q, const unsigned short* __restric
 }
 
 // ---- time window and stamps ------------------------------------------------------------------------------------------------
-// x86-64's cvttsd2si: NaN and values outside the int64 range give INT64_MIN (what upstream's static_cast<int64_t> does there)
-__device__ __forceinline__ long long trunc_i64(double v) {
-    return (v >= -9.2233720368547758e18 && v < 9.2233720368547758e18) ? __double2ll_rz(v) : (long long)0x8000000000000000ull;
-}
-
 constexpr int kWinThreads = 1024;
 
 // GetLidarPointMinMaxOffsetTime (:554-571): a NaN first time stays; otherwise the earliest point equal to the extreme (which decides the

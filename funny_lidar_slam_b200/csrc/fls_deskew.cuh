@@ -19,7 +19,7 @@ struct DeskewView {
 
 #ifdef __CUDACC__
 __device__ __forceinline__ bool deskew_point(const DeskewView& d, float x, float y, float z, float rel_time, float& xo, float& yo, float& zo) {
-    const unsigned long long t = (unsigned long long)((long long)d.ref_time + (long long)__dmul_rn((double)rel_time, 1.0e6));
+    const unsigned long long t = (unsigned long long)((long long)d.ref_time + trunc_i64(__dmul_rn((double)rel_time, 1.0e6)));
     const int m = d.m;
     if (m < 2 || d.t[0] > t || d.t[m - 1] < t) return false;
     int l;
@@ -43,8 +43,13 @@ __device__ __forceinline__ bool deskew_point(const DeskewView& d, float x, float
     double qy = __dadd_rn(__dmul_rn(a[1], u), __dmul_rn(b[1], s));
     double qz = __dadd_rn(__dmul_rn(a[2], u), __dmul_rn(b[2], s));
     double qw = __dadd_rn(__dmul_rn(a[3], u), __dmul_rn(b[3], s));
-    const double n = __dsqrt_rn(__dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(qx, qx), __dmul_rn(qy, qy)), __dmul_rn(qz, qz)), __dmul_rn(qw, qw)));
-    qx = __ddiv_rn(qx, n); qy = __ddiv_rn(qy, n); qz = __ddiv_rn(qz, n); qw = __ddiv_rn(qw, n);
+    // q.normalized(): Eigen 3.3.7 leaves the coefficients as they are unless the squared norm is > 0 (q(t) = 0 between q and -q;
+    // NaN from a 0 / 0 ratio)
+    const double sq = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(qx, qx), __dmul_rn(qy, qy)), __dmul_rn(qz, qz)), __dmul_rn(qw, qw));
+    if (sq > 0.0) {
+        const double n = __dsqrt_rn(sq);
+        qx = __ddiv_rn(qx, n); qy = __ddiv_rn(qy, n); qz = __ddiv_rn(qz, n); qw = __ddiv_rn(qw, n);
+    }
     // q = q_ref^-1 * q(t)
     const double ax = d.qri[0], ay = d.qri[1], az = d.qri[2], aw = d.qri[3];
     const double px = __dsub_rn(__dadd_rn(__dadd_rn(__dmul_rn(aw, qx), __dmul_rn(ax, qw)), __dmul_rn(ay, qz)), __dmul_rn(az, qy));

@@ -28,13 +28,22 @@ bool deskew_ref_inverse(const unsigned long long* t, const double* q, size_t m, 
     const double u = 1.0 - s;
     volatile double qx = q[4 * l] * u + q[4 * r] * s, qy = q[4 * l + 1] * u + q[4 * r + 1] * s, qz = q[4 * l + 2] * u + q[4 * r + 2] * s,
                     qw = q[4 * l + 3] * u + q[4 * r + 3] * s;
-    const double n = std::sqrt(((qx * qx + qy * qy) + qz * qz) + qw * qw);
-    const double nx = qx / n, ny = qy / n, nz = qz / n, nw = qw / n;
+    // Eigen 3.3.7's guards: normalized() leaves a quaternion whose squared norm is not > 0 as it is, inverse() of one returns zero
+    const double sq = ((qx * qx + qy * qy) + qz * qz) + qw * qw;
+    double nx = qx, ny = qy, nz = qz, nw = qw;
+    if (sq > 0.0) {
+        const double n = std::sqrt(sq);
+        nx = qx / n, ny = qy / n, nz = qz / n, nw = qw / n;
+    }
     const double n2 = ((nx * nx + ny * ny) + nz * nz) + nw * nw;
-    qri[0] = -nx / n2;
-    qri[1] = -ny / n2;
-    qri[2] = -nz / n2;
-    qri[3] = nw / n2;
+    if (n2 > 0.0) {
+        qri[0] = -nx / n2;
+        qri[1] = -ny / n2;
+        qri[2] = -nz / n2;
+        qri[3] = nw / n2;
+    } else {
+        qri[0] = qri[1] = qri[2] = qri[3] = 0.0;
+    }
     return true;
 }
 
@@ -78,13 +87,22 @@ struct PpWorkspace : Workspace {
 
 }  // namespace
 
-// uploads the IMU samples and fills the view; returns FLS_ERR_INVALID_ARG when ref_time is outside the buffer (SetRefTime fails)
-int make_deskew_view(const fls_imu_buffer* imu, DevBuf<unsigned long long>& d_t, DevBuf<double>& d_q, cudaStream_t st, DeskewView& v) {
+// uploads the IMU samples and fills the view.  ref_outside: ref_time is outside the buffer (SetRefTime fails; the view stays the
+// identity).  Returns FLS_ERR_INVALID_ARG for a null array, more than 2^31 - 1 samples, or a stamp followed by a smaller one:
+// deskew_point finds the interval by bisection, upstream by a downward scan (data_searcher.h:100-134), and the two pick the same
+// pair only on ascending stamps (equal ones allowed).
+int make_deskew_view(const fls_imu_buffer* imu, DevBuf<unsigned long long>& d_t, DevBuf<double>& d_q, cudaStream_t st, DeskewView& v,
+                     bool& ref_outside) {
     std::memset(&v, 0, sizeof(v));
+    ref_outside = false;
     if (!imu || imu->n_imu == 0) return FLS_OK;  // identity
     if (!imu->imu_time_us || !imu->imu_quat_xyzw || imu->n_imu > 0x7fffffffull) return FLS_ERR_INVALID_ARG;
-    if (!deskew_ref_inverse(reinterpret_cast<const unsigned long long*>(imu->imu_time_us), imu->imu_quat_xyzw, imu->n_imu, imu->ref_time_us, v.qri))
-        return FLS_ERR_INVALID_ARG;
+    for (size_t k = 1; k < imu->n_imu; ++k)
+        if (imu->imu_time_us[k] < imu->imu_time_us[k - 1]) return FLS_ERR_INVALID_ARG;
+    if (!deskew_ref_inverse(reinterpret_cast<const unsigned long long*>(imu->imu_time_us), imu->imu_quat_xyzw, imu->n_imu, imu->ref_time_us, v.qri)) {
+        ref_outside = true;
+        return FLS_OK;
+    }
     d_t.reserve(imu->n_imu);
     d_q.reserve(imu->n_imu * 4);
     FLS_CUDA(cudaMemcpyAsync(d_t.p, imu->imu_time_us, imu->n_imu * sizeof(unsigned long long), cudaMemcpyHostToDevice, st));
@@ -110,8 +128,10 @@ int run_preprocess(int device, const float* xyzi, const float* time, bool src_on
     return with_workspace<PpWorkspace>(device, [&](PpWorkspace& w) -> int {
         cudaStream_t st = w.st;
         DeskewView dv;
-        const int rc = make_deskew_view(imu, w.imu_t, w.imu_q, st, dv);
-        if (rc != FLS_OK) return rc == FLS_ERR_INVALID_ARG && imu && imu->n_imu ? FLS_OK : rc;  // SetRefTime failed: upstream drops the scan (:178-183) -> empty clouds
+        bool ref_outside;
+        const int rc = make_deskew_view(imu, w.imu_t, w.imu_q, st, dv, ref_outside);
+        if (rc != FLS_OK) return rc;
+        if (ref_outside) return FLS_OK;  // SetRefTime failed: upstream drops the scan (:178-183) -> empty clouds
         w.corrected.reserve(n);
         float4* ord = d_ordered ? reinterpret_cast<float4*>(d_ordered) : w.ordered.reserve(n);
         w.planar.reserve(n);

@@ -37,7 +37,7 @@ __global__ void proj_claim_kernel(const float4* __restrict__ raw, const int* __r
     if (col >= H) col -= H;
     if (row >= V || row < 0 || col < 0 || col >= H) return;  // :81-82
     if (dv.m > 0) {  // ProcessPoint fails for a time outside the IMU buffer: the point returns without claiming its cell (:100-103)
-        const unsigned long long t = (unsigned long long)((long long)dv.ref_time + (long long)__dmul_rn((double)time[k], 1.0e6));
+        const unsigned long long t = (unsigned long long)((long long)dv.ref_time + trunc_i64(__dmul_rn((double)time[k], 1.0e6)));
         if (dv.m < 2 || dv.t[0] > t || dv.t[dv.m - 1] < t) return;
     }
     atomicMin(&winner[(size_t)row * H + col], (unsigned)k);  // :86-87 first hit wins
@@ -80,18 +80,19 @@ struct ProjWorkspace : Workspace {
 
 }  // namespace
 
-int make_deskew_view(const fls_imu_buffer* imu, DevBuf<unsigned long long>& d_t, DevBuf<double>& d_q, cudaStream_t st, DeskewView& v);
+int make_deskew_view(const fls_imu_buffer* imu, DevBuf<unsigned long long>& d_t, DevBuf<double>& d_q, cudaStream_t st, DeskewView& v,
+                     bool& ref_outside);
 
 int enqueue_project(ProjStage& w, const void* raw, const int* ring, const float* time, const fls_imu_buffer* imu, size_t n, size_t stride, int V, int H,
                     float h_res, float min_d, float max_d, cudaStream_t st, long long* h2d, int* launches, bool src_on_device) {
     const size_t cells = (size_t)V * H;
     DeskewView dv;
     const bool use_imu = imu && imu->n_imu && time;
-    int rc = make_deskew_view(use_imu ? imu : nullptr, w.imu_t, w.imu_q, st, dv);
-    const bool ref_failed = rc == FLS_ERR_INVALID_ARG && use_imu && imu->imu_time_us && imu->imu_quat_xyzw;  // SetRefTime failed: no point is accepted
-    if (rc != FLS_OK && !ref_failed) return rc;
+    bool ref_outside;
+    const int rc = make_deskew_view(use_imu ? imu : nullptr, w.imu_t, w.imu_q, st, dv, ref_outside);
+    if (rc != FLS_OK) return rc;
     if (dv.m > 0) *h2d += (long long)(imu->n_imu * (sizeof(unsigned long long) + 4 * sizeof(double)));
-    if (ref_failed) n = 0;
+    if (ref_outside) n = 0;  // SetRefTime failed: no point is accepted
     w.raw.reserve(n + 1);
     w.ring.reserve(n + 1);
     w.time.reserve(n + 1);

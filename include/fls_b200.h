@@ -329,8 +329,9 @@ int fls_pcd_read(const char* path, float* xyzi, size_t capacity, size_t* n);
 int fls_pcd_write(const char* path, const float* xyzi, size_t n);
 
 /* IMU orientation samples around a scan — what LidarDistortionCorrector reads through its DataSearcher<IMUData>
- * (include/lidar/lidar_distortion_corrector.h:11-48, src/lidar/lidar_distortion_corrector.cpp:19-64): time stamps in microseconds
- * (ascending), unit quaternions in Eigen coefficient order x, y, z, w, the reference time of the scan (SetRefTime) and the
+ * (include/lidar/lidar_distortion_corrector.h:11-48, src/lidar/lidar_distortion_corrector.cpp:19-64): time stamps in microseconds,
+ * ascending (equal neighbours allowed; a stamp followed by a smaller one is rejected with FLS_ERR_INVALID_ARG, where upstream's
+ * downward scan would pick some pair anyway; so is a null time or quaternion array when n_imu > 0), unit quaternions in Eigen coefficient order x, y, z, w, the reference time of the scan (SetRefTime) and the
  * lidar -> imu extrinsic (column-major 4x4).  n_imu == 0 (or a NULL pointer to the struct): no de-skew, points pass unchanged. */
 typedef struct {
     const uint64_t* imu_time_us;

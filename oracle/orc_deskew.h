@@ -26,6 +26,12 @@ struct ImuBuffer {
     double T_li[16];  // lidar -> imu, column-major 4x4
 };
 
+// int64_t(rel_time * 1.0e6) of ProcessPoint (:41) as x86-64's cvttsd2si computes it: toward zero, INT64_MIN for NaN and for
+// values outside the int64 range (a plain conversion is undefined behaviour there).  The device uses the same rule (trunc_i64).
+inline int64_t time_to_i64(double v) {
+    return (v >= -9.2233720368547758e18 && v < 9.2233720368547758e18) ? int64_t(v) : std::numeric_limits<int64_t>::min();
+}
+
 // data_searcher.h:100-134
 inline bool search_two(const ImuBuffer& b, uint64_t t, size_t& l, size_t& r) {
     const size_t m = b.t.size();
@@ -41,19 +47,24 @@ inline bool search_two(const ImuBuffer& b, uint64_t t, size_t& l, size_t& r) {
     return true;
 }
 
-// motion_interpolator.h:27-35: normalised linear interpolation of the coefficients (no hemisphere alignment)
+// motion_interpolator.h:27-35: normalised linear interpolation of the coefficients (no hemisphere alignment).  Eigen 3.3.7's
+// normalized() returns the coefficients unchanged when the squared norm is not > 0 (q and -q at ratio 0.5: zero; a NaN ratio).
 inline Quat lerp(const Quat& a, const Quat& b, double s) {
     const double u = 1.0 - s;
     Quat q{a.x * u + b.x * s, a.y * u + b.y * s, a.z * u + b.z * s, a.w * u + b.w * s};
-    const double n = std::sqrt(((q.x * q.x + q.y * q.y) + q.z * q.z) + q.w * q.w);
+    const double sq = ((q.x * q.x + q.y * q.y) + q.z * q.z) + q.w * q.w;
+    if (!(sq > 0.0)) return q;
+    const double n = std::sqrt(sq);
     return Quat{q.x / n, q.y / n, q.z / n, q.w / n};
 }
 inline Quat qmul(const Quat& a, const Quat& b) {
     return Quat{((a.w * b.x + a.x * b.w) + a.y * b.z) - a.z * b.y, ((a.w * b.y + a.y * b.w) + a.z * b.x) - a.x * b.z,
                 ((a.w * b.z + a.z * b.w) + a.x * b.y) - a.y * b.x, ((a.w * b.w - a.x * b.x) - a.y * b.y) - a.z * b.z};
 }
+// Eigen 3.3.7 Quaternion::inverse(): zero when the squared norm is not > 0
 inline Quat qinv(const Quat& a) {
     const double n2 = ((a.x * a.x + a.y * a.y) + a.z * a.z) + a.w * a.w;
+    if (!(n2 > 0.0)) return Quat{0.0, 0.0, 0.0, 0.0};
     return Quat{-a.x / n2, -a.y / n2, -a.z / n2, a.w / n2};
 }
 // Eigen QuaternionBase::_transformVector: v + w * (2 q x v) + q x (2 q x v)
@@ -75,7 +86,7 @@ inline bool ref_inverse(const ImuBuffer& b, Quat& q_ref_inv) {
 }
 // lidar_distortion_corrector.cpp:37-64
 inline bool process_point(const ImuBuffer& b, const Quat& q_ref_inv, float x, float y, float z, float rel_time, float* out) {
-    const uint64_t t = uint64_t(int64_t(b.ref_time) + int64_t(rel_time * 1.0e6));
+    const uint64_t t = b.ref_time + uint64_t(time_to_i64(double(rel_time) * 1.0e6));  // the int64 sum, in unsigned arithmetic
     size_t l, r;
     if (!search_two(b, t, l, r)) return false;
     const double ratio = double(t - b.t[l]) / double(b.t[r] - b.t[l]);

@@ -5,31 +5,7 @@ import pytest
 from scipy.spatial import cKDTree
 
 from oracle import pyoracle as orc
-
-
-def _voxel_grid_numpy(pts, leaf):
-    """Independent restatement of pcl::VoxelGrid (PCL 1.10): float32 cell maths, stable order, sequential fp32 sums."""
-    inv = np.float32(1.0) / np.float32(leaf)
-    mn = pts[:, :3].min(0)
-    mx = pts[:, :3].max(0)
-    minb = np.floor(mn * inv).astype(np.int64)
-    maxb = np.floor(mx * inv).astype(np.int64)
-    div = maxb - minb + 1
-    ijk = (np.floor(pts[:, :3] * inv) - minb.astype(np.float32)).astype(np.int64)
-    lin = ijk[:, 0] + ijk[:, 1] * div[0] + ijk[:, 2] * div[0] * div[1]
-    order = np.argsort(lin, kind="stable")
-    out = []
-    s = 0
-    while s < len(order):
-        e = s
-        while e < len(order) and lin[order[e]] == lin[order[s]]:
-            e += 1
-        acc = np.zeros(4, np.float32)
-        for k in order[s:e]:
-            acc = (acc + pts[k]).astype(np.float32)
-        out.append(acc / np.float32(e - s))
-        s = e
-    return np.array(out, np.float32)
+from tests import frontend_ref
 
 
 def test_voxel_grid_matches_independent_restatement():
@@ -37,7 +13,7 @@ def test_voxel_grid_matches_independent_restatement():
     pts = np.concatenate([rng.uniform(-6, 6, (3000, 3)), rng.uniform(0, 100, (3000, 1))], 1).astype(np.float32)
     for leaf in (0.3, 0.5, 1.0):
         got = orc.voxel_grid(pts, leaf)
-        want = _voxel_grid_numpy(pts, leaf)
+        want, _ = frontend_ref.voxel_grid(pts, leaf)
         assert got.shape == want.shape
         assert np.array_equal(got.view(np.uint32), want.view(np.uint32))
 

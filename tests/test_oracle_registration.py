@@ -9,6 +9,7 @@ import pytest
 from funny_lidar_slam_b200 import FLS_ICP_P2P, FLS_NDT, FLS_P2PLANE_IVOX, default_config, synth
 from funny_lidar_slam_b200._abi import FLS_FLAG_ITER_LOG
 from oracle import pyoracle as orc
+from tests import frontend_ref
 
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 
@@ -147,78 +148,6 @@ def test_feature_extractor_properties(world, traj):
     assert len(ci2) <= len(ci)
 
 
-def _features_literal(depth, col, n, row_start, row_end, corner_thr, planar_thr):
-    """Loop-for-loop Python restatement of FeatureExtractor::{SelectValidPoints, ComputeRoughness, SelectFeatures}
-    (src/loam/feature_extractor.cpp:46-222 upstream) written from the reference text, sharing nothing with oracle/.
-    fp32 arithmetic where upstream has float, double comparisons where it promotes.  Sort ties are broken by position
-    (upstream's std::sort is unstable; inputs of the test have no ties)."""
-    f32 = np.float32
-    depth = depth.astype(f32)
-    valid = np.ones(n + 8, bool)
-    corner = np.zeros(n + 8, bool)
-    valid[:5] = False
-    valid[n - 6:n] = False
-    for i in range(5, n - 6):
-        d1, d2 = depth[i], depth[i + 1]
-        if abs(int(col[i + 1]) - int(col[i])) < 10:
-            if float(f32(d1 - d2)) > 0.3:
-                valid[i - 5:i + 1] = False
-            elif float(f32(d2 - d1)) > 0.3:
-                valid[i + 1:i + 7] = False
-        a, b = abs(f32(depth[i - 1] - depth[i])), abs(f32(depth[i + 1] - depth[i]))
-        if float(a) > 0.02 * float(depth[i]) and float(b) > 0.02 * float(depth[i]):
-            valid[i] = False
-    rough = np.zeros(n, f32)
-    index = np.arange(n)
-    for i in range(5, n - 5):
-        s = f32(0)
-        for k in (-5, -4, -3, -2, -1, 1, 2, 3, 4, 5):
-            s = f32(s + depth[i + k])
-        s = f32(s - f32(f32(10.0) * depth[i]))
-        rough[i] = f32(s * s)
-    feat_r, feat_i = rough.copy(), index.copy()  # point_features_: sorted in place block by block
-
-    def suppress(idx):
-        for k in range(1, 6):
-            if abs(int(col[idx + k]) - int(col[idx + k - 1])) > 10:
-                break
-            valid[idx + k] = False
-        for k in range(-1, -6, -1):
-            if abs(int(col[idx + k]) - int(col[idx + k + 1])) > 10:
-                break
-            valid[idx + k] = False
-
-    corners, planars = [], []
-    for rs, re in zip(row_start, row_end):
-        for b in range(6):
-            t = int((int(re) - int(rs)) / 6)  # C integer division (truncation)
-            bs, be = int(rs) + b * t, int(rs) + (b + 1) * t
-            if bs >= be:
-                continue
-            order = sorted(range(bs, be), key=lambda j: (feat_r[j], feat_i[j]))
-            feat_r[bs:be], feat_i[bs:be] = feat_r[order].copy(), feat_i[order].copy()
-            picked = 0
-            for j in range(be, bs - 1, -1):
-                idx = int(feat_i[j])
-                if feat_r[j] > f32(corner_thr) and valid[idx]:
-                    picked += 1
-                    if picked <= 20:
-                        corner[idx] = True
-                        corners.append(idx)
-                    else:
-                        break
-                    valid[idx] = False
-                    suppress(idx)
-            for j in range(bs, be + 1):
-                idx = int(feat_i[j])
-                if valid[idx] and feat_r[j] < f32(planar_thr):
-                    valid[idx] = False
-                    suppress(idx)
-                if not corner[idx]:
-                    planars.append(idx)
-    return np.array(corners, np.int32), np.array(planars, np.int32)
-
-
 @pytest.mark.parametrize("seed", [0, 1, 2])
 def test_feature_extractor_against_literal_python_restatement(seed):
     rng = np.random.default_rng(seed)
@@ -240,7 +169,7 @@ def test_feature_extractor_against_literal_python_restatement(seed):
     re = (ends - 6).astype(np.int32)
     for ct, pt in ((1.0, 0.1), (0.05, 0.01), (0.2, 5.0)):
         oc, op, _ = orc.extract_features(depth, col, n, rs, re, ct, pt)
-        lc, lp = _features_literal(depth, col, n, rs, re, ct, pt)
+        lc, lp, _ = frontend_ref.features(depth, col, n, rs, re, ct, pt)
         assert np.array_equal(oc, lc), (seed, ct, pt)
         assert np.array_equal(op, lp), (seed, ct, pt)
     assert len(oc) > 0 and len(op) > 100
