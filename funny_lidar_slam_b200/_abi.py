@@ -89,6 +89,17 @@ class FlsGnStepOut(C.Structure):
                 ("done", C.c_int32), ("spd", C.c_int32), ("published_ok", C.c_int32)]
 
 
+class FlsRelocCfg(C.Structure):
+    _fields_ = [("xy_radius", C.c_double), ("xy_step", C.c_double), ("yaw_range", C.c_double), ("yaw_step", C.c_double),
+                ("coarse_leaf", C.c_float), ("max_range", C.c_float), ("accept_fitness", C.c_float), ("n_refine", C.c_int32)]
+
+
+class FlsRelocResult(C.Structure):
+    _fields_ = [("n_hypotheses", C.c_int64), ("best_hypothesis", C.c_int64), ("n_refined", C.c_int32), ("best_rank", C.c_int32),
+                ("converged", C.c_int32), ("accepted", C.c_int32), ("fitness", C.c_float), ("coarse_score", C.c_float),
+                ("host_waits", C.c_int32), ("gpu_launches", C.c_int32)]
+
+
 class FlsFeatureCfg(C.Structure):
     _fields_ = [("corner_threshold", C.c_float), ("planar_threshold", C.c_float), ("device", C.c_int32), ("reserved", C.c_int32)]
 

@@ -6,7 +6,7 @@ import ctypes as C
 import os
 
 from ._abi import (FlsConfig, FlsConvertCfg, FlsConvertResult, FlsFeatureCfg, FlsIterLog, FlsLoamFrontendCfg, FlsMapInfo, FlsMatchStats,
-                   FlsPointCloud2)
+                   FlsPointCloud2, FlsRelocCfg, FlsRelocResult)
 
 _PKG = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_PKG, "libfls_b200.so")
@@ -20,6 +20,7 @@ EXPORTS = [
     "fls_pcd_read", "fls_pcd_write", "fls_preprocess_loam", "fls_match_cluster_device", "fls_convert_cloud", "fls_preprocess_loam_device",
     "fls_preprocess_device", "fls_keyframes_create", "fls_keyframes_destroy", "fls_keyframes_add", "fls_keyframes_add_device",
     "fls_keyframes_count", "fls_keyframes_assemble", "fls_get_ndt_voxels", "fls_gn_step_probe",
+    "fls_relocalize", "fls_relocalize_device",
 ]
 
 
@@ -72,6 +73,9 @@ def lib():
     L.fls_pcd_write.argtypes = [C.c_char_p, vp, sz]
     L.fls_match_batch_end.argtypes = [vp, vp, C.POINTER(C.c_int), C.POINTER(FlsMatchStats)]
     L.fls_fitness.argtypes = [vp, f32, C.POINTER(f32)]
+    reloc_outs = [C.POINTER(FlsRelocCfg), vp, C.POINTER(FlsRelocResult), vp, vp, vp, vp, vp, sz]
+    L.fls_relocalize.argtypes = [vp, vp, sz, sz] + reloc_outs
+    L.fls_relocalize_device.argtypes = [vp, vp, sz] + reloc_outs
     L.fls_get_iter_log.argtypes = [vp, C.POINTER(FlsIterLog), C.c_int]
     L.fls_get_iter_log_scan.argtypes = [vp, C.c_int, C.POINTER(FlsIterLog), C.c_int]
     L.fls_get_map_info.argtypes = [vp, C.POINTER(FlsMapInfo)]

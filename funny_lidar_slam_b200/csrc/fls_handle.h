@@ -63,13 +63,22 @@ struct KeyFrameGate {
     bool need(const double* T, double dist_thre, double rot_thre);
 };
 
+// the hypothesis grid of fls_relocalize (fls_b200.h): offsets -I..I in x and y, yaw offsets k0..K (n_yaw of them), P hypotheses
+static constexpr long long kRelocMaxHypotheses = 1LL << 20;
+struct RelocGrid {
+    int I = 0, K = 0, k0 = 0, n_yaw = 1;
+    long long P = 1;
+};
+// checks a relocalization configuration and sizes its grid (FLS_ERR_INVALID_ARG: see fls_relocalize)
+int reloc_grid(const fls_reloc_cfg& c, RelocGrid* g);
+
 struct Handle {
     fls_config cfg;
     cudaStream_t stream = nullptr;
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
 
-    // per-call accounting (fls_match_stats)
-    int launches = 0;
+    // per-call accounting (fls_match_stats; waits: stream synchronisations of end_call / inserted and of the filters that count them)
+    int launches = 0, waits = 0;
     long long h2d_bytes = 0, d2h_bytes = 0;
 
     // upload staging
@@ -107,14 +116,21 @@ struct Handle {
     std::unique_ptr<Plugin> plugin;
 
     // GetFitnessScore support: cloud the upstream kd-tree is built on (fit_pts: fit_cloud, or a cloud the plug-in keeps) + a search
-    // grid sized for max_range
+    // grid sized for max_range; the poses scored, per-tile partials and per-pose {sum, count} of the scoring kernel (fls_reloc.cu)
     DevBuf<float4> fit_cloud;
     const float4* fit_pts = nullptr;
     size_t fit_cloud_n = 0;
     unsigned long long fit_cloud_version = 0, fit_grid_version = ~0ull;
     float fit_grid_range = -1.f;
     SearchGrid fit_grid;
-    DevBuf<double> fit_out;
+    DevBuf<double> fit_pose, fit_part_sum, fit_out;
+    DevBuf<unsigned> fit_part_cnt, fit_cnt;
+    // relocalization: the coarse cloud, the hypotheses, their partials, scores and sort keys / indices (in and out), the picks
+    DevBuf<float4> reloc_coarse;
+    DevBuf<double> reloc_poses, reloc_part_sum, reloc_score;
+    DevBuf<unsigned> reloc_part_cnt, reloc_idx;
+    DevBuf<unsigned long long> reloc_key;
+    DevBuf<unsigned char> reloc_pick;
 
     explicit Handle(const fls_config& c);
     ~Handle();
@@ -181,6 +197,11 @@ struct Handle {
     int inserted(int rc, fls_match_stats* st);
 
     int fitness(float max_range, float* score);
+    int fit_grid_for(float max_range, int* waits);  // (re)builds fit_grid for max_range when needed; counts its wait
+    void fitness_enqueue(const float4* d_src, size_t n, int P, float max_range);  // P poses of fit_pose -> fit_out / fit_cnt
+    // fls_relocalize on a device scan (the call has begun; g from reloc_grid)
+    int relocalize(const float4* d_scan, size_t n, const fls_reloc_cfg& c, const RelocGrid& g, double* T, fls_reloc_result* out, double* refined_T,
+                   int32_t* refined_converged, float* refined_fitness, int64_t* refined_index, double* coarse_scores, size_t coarse_cap);
 
     // localization-mode map path (fls_localmap.cu): resident global map, +-100 m crop around the pose when needed
     DevBuf<float4> global_map;

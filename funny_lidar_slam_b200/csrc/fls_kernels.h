@@ -1,5 +1,5 @@
 // fls_kernels.h — launch interfaces that more than one file uses: the LOAM-iVox batch kernel (generation 9, whose host half lives
-// with generation 8 in fls_p2plane.cu) and GetFitnessScore.  Each plug-in's own argument structs and launchers sit in its file.
+// with generation 8 in fls_p2plane.cu).  Each plug-in's own argument structs and launchers sit in its file.
 #pragma once
 #include "fls_common.cuh"
 #include "fls_gn.cuh"
@@ -42,8 +42,5 @@ struct P2PlaneLoopArgs {
 // generation 9 (fls_p2plane_v9.cu), batches: barrier-free dataflow, TMA-staged candidate runs, DMMA sums
 int p2plane_v9_grid(int n_max, int device);  // also raises the kernel's shared-memory limit on `device`
 void launch_p2plane_v9(const P2PlaneLoopArgs& a, int grid, cudaStream_t st);
-
-// d_out2[0] = sum of squared NN distances <= max_range, d_out2[1] = how many; T column-major (cast to float inside)
-void launch_fitness(const GridView& g, const float4* d_src, int n, const double* T_colmajor, float max_range, double* d_out2, cudaStream_t st);
 
 }  // namespace fls

@@ -41,6 +41,38 @@ def _cloud(a):
     return a.ctypes.data_as(C.c_void_p), a.shape[0], a.shape[1] * 4, a
 
 
+@dataclass
+class RelocResult:
+    """What Registration.relocalize returns: the chosen pose T (4,4) and fls_reloc_result's fields; the per-refined arrays are in
+    refinement rank order (rank 0 = best coarse score) and coarse_scores in hypothesis index order (None unless asked for)."""
+    T: np.ndarray
+    accepted: bool
+    converged: bool
+    fitness: float
+    coarse_score: float
+    n_hypotheses: int
+    best_hypothesis: int
+    best_rank: int
+    n_refined: int
+    host_waits: int
+    gpu_launches: int
+    refined_T: np.ndarray
+    refined_converged: np.ndarray
+    refined_fitness: np.ndarray
+    refined_index: np.ndarray
+    coarse_scores: np.ndarray | None = None
+
+
+def reloc_cfg(xy_radius=10.0, xy_step=1.0, yaw_range=np.pi, yaw_step=np.deg2rad(10.0), coarse_leaf=1.0, max_range=2.0, accept_fitness=1.0,
+              n_refine=64) -> _abi.FlsRelocCfg:
+    """fls_reloc_cfg; the defaults search +-10 m at 1 m and the full circle at 10 deg around the guess, with Localization::Init's
+    GetFitnessScore(2.0) < 1.0 as the acceptance rule (src/slam/localization.cpp:135-140 upstream)."""
+    c = _abi.FlsRelocCfg()
+    c.xy_radius, c.xy_step, c.yaw_range, c.yaw_step = float(xy_radius), float(xy_step), float(yaw_range), float(yaw_step)
+    c.coarse_leaf, c.max_range, c.accept_fitness, c.n_refine = float(coarse_leaf), float(max_range), float(accept_fitness), int(n_refine)
+    return c
+
+
 def _batch_poses(Ts):
     return np.ascontiguousarray(np.transpose(np.asarray(Ts, np.float64), (0, 2, 1))).copy()  # Eigen column-major per pose
 
@@ -191,6 +223,44 @@ class Registration:
         T[...] = Tc.T
         self.last_stats = st
         return bool(conv.value)
+
+    # -- relocalization from a coarse pose (Localization::Init upstream) -----------------------------------
+    def _relocalize(self, call, T_guess, coarse_scores, cfg):
+        c = cfg if isinstance(cfg, _abi.FlsRelocCfg) else reloc_cfg(**cfg)
+        k = max(1, int(c.n_refine))
+        Tc = np.ascontiguousarray(np.asarray(T_guess, np.float64).T).copy()
+        res = _abi.FlsRelocResult()
+        rT = np.zeros((k, 4, 4), np.float64)
+        rconv = np.zeros(k, np.int32)
+        rfit = np.zeros(k, np.float32)
+        ridx = np.zeros(k, np.int64)
+        cs = np.zeros(max(int(coarse_scores), 1), np.float64)
+        vp = lambda a: a.ctypes.data_as(C.c_void_p)
+        check(call(C.byref(c), vp(Tc), C.byref(res), vp(rT), vp(rconv), vp(rfit), vp(ridx), vp(cs) if coarse_scores else None, int(coarse_scores)),
+              "fls_relocalize")
+        n = res.n_refined
+        ncs = min(int(coarse_scores), int(res.n_hypotheses)) if res.n_refined else 0
+        return RelocResult(T=Tc.T.copy(), accepted=bool(res.accepted), converged=bool(res.converged), fitness=float(res.fitness),
+                           coarse_score=float(res.coarse_score), n_hypotheses=int(res.n_hypotheses), best_hypothesis=int(res.best_hypothesis),
+                           best_rank=int(res.best_rank), n_refined=int(n), host_waits=int(res.host_waits), gpu_launches=int(res.gpu_launches),
+                           refined_T=np.transpose(rT[:n], (0, 2, 1)).copy(), refined_converged=rconv[:n].astype(bool), refined_fitness=rfit[:n].copy(),
+                           refined_index=ridx[:n].copy(), coarse_scores=cs[:ncs].copy() if coarse_scores else None)
+
+    def relocalize(self, cloud_or_cluster, T_guess, coarse_scores: int = 0, cfg=None, **kw) -> RelocResult:
+        """fls_relocalize: score an x-y-yaw grid of hypotheses around T_guess (4,4), refine the best n_refine in one batch Match and
+        return the pose Localization::Init's rule would pick.  cloud_or_cluster: the cloud Match reads ((n,4)/(n,8) float32; the
+        planar cloud for LOAM-iVox, the ordered cloud for NDT) or a PointcloudCluster.  cfg: an FlsRelocCfg, else reloc_cfg(**kw).
+        coarse_scores: how many coarse scores (index order) to return."""
+        c = cloud_or_cluster
+        if isinstance(c, PointcloudCluster):
+            c = c.ordered_cloud if self.cfg.method == _abi.FLS_NDT else c.planar_cloud
+        p, n, s, keep = _cloud(c)
+        return self._relocalize(lambda *a: lib().fls_relocalize(self._h, p, n, s, *a), T_guess, coarse_scores, cfg if cfg is not None else kw)
+
+    def relocalize_device(self, d_ptr: int, n: int, T_guess, coarse_scores: int = 0, cfg=None, **kw) -> RelocResult:
+        """relocalize with a device-resident packed float4 scan (it must stay valid until the next Match, as in match_device)."""
+        return self._relocalize(lambda *a: lib().fls_relocalize_device(self._h, C.c_void_p(int(d_ptr)) if d_ptr else None, int(n), *a), T_guess,
+                                coarse_scores, cfg if cfg is not None else kw)
 
     # -- localization-mode map path (Localization::LoadLocalMap upstream) ---------------------------------
     def set_global_map(self, cloud: np.ndarray) -> None:

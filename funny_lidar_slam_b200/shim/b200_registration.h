@@ -79,6 +79,24 @@ public:
         return score;
     }
 
+    // Localization::Init from the RViz "2D Pose Estimate" (localization.cpp:114-169): searches an x-y-yaw grid around T, refines the
+    // best poses and picks one by Init's own rule.  T receives the chosen pose (also when false is returned, as upstream writes it);
+    // *fitness its GetFitnessScore(cfg.max_range).  Returns whether it is accepted (converged and fitness < cfg.accept_fitness).
+    // PointToPlane_IVOX and IncrementalNDT in localization mode, after fls_update_local_map at the guess.
+    bool Relocalize(const PointcloudClusterPtr& source_cloud_cluster, Mat4d& T, const fls_reloc_cfg& cfg, float* fitness) {
+        const auto& cloud = method_ == FLS_NDT ? source_cloud_cluster->ordered_cloud_.points : source_cloud_cluster->planar_cloud_.points;
+        fls_reloc_result res;
+        const int rc = fls_relocalize(handle_, cloud.data(), cloud.size(), sizeof(PCLPointXYZI), &cfg, T.data(), &res, nullptr, nullptr, nullptr,
+                                      nullptr, nullptr, 0);
+        if (fitness) *fitness = rc == FLS_OK ? res.fitness : FloatNaN;
+        if (rc != FLS_OK) {
+            LOG(WARNING) << "fls_relocalize: " << fls_strerror(rc) << " " << fls_last_error();
+            return false;
+        }
+        DLOG(INFO) << "B200 Relocalize hypotheses=" << res.n_hypotheses << " rank=" << res.best_rank << " fitness=" << res.fitness;
+        return res.accepted != 0;
+    }
+
     // Convenience: the factory branch a maintainer adds to FrontEnd::InitMatcher / Localization::InitMatcher.
     static std::shared_ptr<RegistrationInterface> Create(const std::string& mode, const fls_config& overrides_applied) {
         return std::make_shared<B200Registration>(overrides_applied);

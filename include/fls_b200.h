@@ -27,6 +27,8 @@
  *   fls_keyframes_*            <- the keyframe-map loops of System::SaveMap (src/slam/system.cpp:299-341),
  *                                 System::VisualizeGlobalMap (src/slam/system.cpp:847-896) and
  *                                 LoopClosure::GetSubMap (src/slam/loop_closure.cpp:179-231)
+ *   fls_relocalize / _device   <- Localization::Init's Match + GetFitnessScore(2.0) < 1.0 (src/slam/localization.cpp:135-140),
+ *                                 searching an x-y-yaw grid around the given pose
  *
  * Conventions
  *   * Points are read from caller memory as {float x, y, z, <pad>, intensity ...} records `stride_bytes`
@@ -213,6 +215,67 @@ int fls_match_batch_begin_device(fls_handle* h, int n_scans, const void* const* 
 int fls_match_batch_end(fls_handle* h, double* T_colmajor, int* converged, fls_match_stats* stats);
 int fls_match_batch_device(fls_handle* h, int n_scans, const void* const* d_planar, const size_t* n, double* T_colmajor, int* converged,
                            fls_match_stats* stats);
+
+/* Relocalization from a coarse pose (Localization::Init's "2D Pose Estimate", src/slam/localization.cpp:114-169 upstream, which runs
+ * one Match from the clicked pose and accepts it when it converges and GetFitnessScore(2.0) < 1.0).
+ *
+ * Hypotheses.  With I = floor(xy_radius / xy_step + 1e-9) (0 when xy_radius == 0) and K = floor(min(yaw_range, pi) / yaw_step + 1e-9)
+ * (0 when yaw_range == 0), the yaw offsets are psi_k = k * yaw_step for k = -K..K, except that k = -K is left out when yaw_range >= pi
+ * and 2 K yaw_step >= 2 pi - 1e-9 (it would repeat +K: the full circle without a duplicate).  Hypothesis (j, i, k) is, in fp64,
+ *   R = Rz(psi_k) * R_guess   (row 0: c*g0 - s*g1, row 1: s*g0 + c*g1, row 2: g2, no fused multiply-add)
+ *   t = t_guess + (i * xy_step, j * xy_step, 0)        for i, j = -I..I,
+ * so z, roll and pitch stay those of the guess.  Index order: yaw fastest, then x (i), then y (j): index = ((j+I)*(2I+1) + (i+I))*n_yaw + k'.
+ * Coarse score.  C = VoxelGridCloud(scan, coarse_leaf) with m points; d2 = the fp32 squared distance of each point, moved by the
+ * hypothesis cast to float (as fls_fitness moves it), to its nearest fit-cloud point; a point is an inlier when d2 <= max_range.
+ * score = (sum of inlier d2 + (m - inliers) * max_range) / m: GetFitnessScore's sum with every outlier counted at the gate.
+ * Selection: the n_refine smallest scores, ties to the lower index.  Refinement: one fls_match_batch_device of those poses, the same
+ * device scan n_refine times (n_refine == 1: a plain Match).  Fitness: GetFitnessScore(max_range) of each refined pose on the cloud
+ * fls_fitness reads after that Match.  Choice: the converged refined pose with the lowest fitness (ties: the better coarse rank), or
+ * the lowest fitness when none converged; accepted = converged && fitness < accept_fitness.  T receives the chosen pose even when it
+ * is not accepted, as upstream (:160-163).  Afterwards fls_fitness(max_range) returns the reported fitness and a Match behaves as
+ * after a plain Match; the map is not modified.  Every score is reproducible bit for bit from call to call.
+ *
+ * `scan` is the cloud the plug-in's Match reads (planar for FLS_P2PLANE_IVOX, ordered for FLS_NDT), host records of stride_bytes;
+ * fls_relocalize_device takes packed float4 device records, which must stay valid until the next Match (as in fls_match_device).
+ * Optional outputs, in refinement rank order (rank 0 = best coarse score): refined_T [n_refine*16] column-major poses after the
+ * Match, refined_converged, refined_fitness and refined_index (grid index of the start pose) [n_refine]; coarse_scores receives
+ * the first min(coarse_cap, n_hypotheses) scores in index order.  An empty scan (or an empty coarse cloud) refines nothing: T is
+ * left as given, fitness = FLT_MAX, accepted = 0.  out->host_waits and out->gpu_launches count the call's stream synchronisations
+ * and launches: 5 waits for FLS_P2PLANE_IVOX and 7 for FLS_NDT, one more when the fit grid is rebuilt for a new map or max_range.
+ * FLS_P2PLANE_IVOX and FLS_NDT in localization mode; FLS_ERR_UNSUPPORTED (no side effect) otherwise; FLS_ERR_NO_MAP before a map;
+ * FLS_ERR_INVALID_ARG for a NaN, zero or negative step, leaf or range where it is used, n_refine outside 1..64, more than 2^20
+ * hypotheses, or while a batch from fls_match_batch_begin is in flight on the handle.  The step must lie inside the convergence
+ * basin of the plug-in's Match: about 1 m and 10 degrees for FLS_P2PLANE_IVOX, 0.5 m and 5 degrees or finer for FLS_NDT. */
+typedef struct {
+    double xy_radius;      /* hypotheses at guess + (i*xy_step, j*xy_step, 0), |i|,|j| <= floor(xy_radius/xy_step) */
+    double xy_step;        /* > 0 (ignored when xy_radius == 0) */
+    double yaw_range;      /* yaw offsets k*yaw_step, |k*yaw_step| <= yaw_range; >= pi: the full circle, no duplicate offset */
+    double yaw_step;       /* > 0 (ignored when yaw_range == 0) */
+    float coarse_leaf;     /* VoxelGridCloud leaf of the scan used for the coarse scores (> 0) */
+    float max_range;       /* GetFitnessScore's max_range, for both stages: 2.0 in Localization::Init (:138) */
+    float accept_fitness;  /* accepted = converged && fitness < accept_fitness: 1.0 upstream (:140) */
+    int32_t n_refine;      /* 1..64 best coarse hypotheses refined by one batch Match */
+} fls_reloc_cfg;
+
+typedef struct {
+    int64_t n_hypotheses;     /* hypotheses scored */
+    int64_t best_hypothesis;  /* grid index of the returned pose's start hypothesis (-1 when nothing was refined) */
+    int32_t n_refined;
+    int32_t best_rank;        /* its rank among the refined (0 = best coarse score) */
+    int32_t converged;
+    int32_t accepted;
+    float fitness;            /* GetFitnessScore(max_range) at the returned pose */
+    float coarse_score;       /* its coarse score */
+    int32_t host_waits;       /* stream synchronisations of the call */
+    int32_t gpu_launches;
+} fls_reloc_result;
+
+int fls_relocalize(fls_handle* h, const void* scan, size_t n, size_t stride_bytes, const fls_reloc_cfg* cfg, double T_colmajor[16],
+                   fls_reloc_result* out, double* refined_T, int32_t* refined_converged, float* refined_fitness, int64_t* refined_index,
+                   double* coarse_scores, size_t coarse_cap);
+int fls_relocalize_device(fls_handle* h, const void* d_scan, size_t n, const fls_reloc_cfg* cfg, double T_colmajor[16], fls_reloc_result* out,
+                          double* refined_T, int32_t* refined_converged, float* refined_fitness, int64_t* refined_index, double* coarse_scores,
+                          size_t coarse_cap);
 
 /* Device-side results for a consumer that lives on the GPU (the per-batch NCCL all-gather of poses, SURVEY.md §8e): once set,
  * every Match additionally writes, for scan s of the call, 18 doubles at d_results + 18*s — the column-major Mat4d pose
