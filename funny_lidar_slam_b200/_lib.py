@@ -20,7 +20,7 @@ EXPORTS = [
     "fls_pcd_read", "fls_pcd_write", "fls_preprocess_loam", "fls_match_cluster_device", "fls_convert_cloud", "fls_preprocess_loam_device",
     "fls_preprocess_device", "fls_keyframes_create", "fls_keyframes_destroy", "fls_keyframes_add", "fls_keyframes_add_device",
     "fls_keyframes_count", "fls_keyframes_assemble", "fls_get_ndt_voxels", "fls_gn_step_probe",
-    "fls_relocalize", "fls_relocalize_device",
+    "fls_relocalize", "fls_relocalize_device", "fls_relocalize_wide", "fls_relocalize_wide_device", "fls_relocalize_wide_levels",
 ]
 
 
@@ -76,6 +76,10 @@ def lib():
     reloc_outs = [C.POINTER(FlsRelocCfg), vp, C.POINTER(FlsRelocResult), vp, vp, vp, vp, vp, sz]
     L.fls_relocalize.argtypes = [vp, vp, sz, sz] + reloc_outs
     L.fls_relocalize_device.argtypes = [vp, vp, sz] + reloc_outs
+    wide_outs = [C.POINTER(FlsRelocCfg), vp, C.POINTER(FlsRelocResult), vp, vp, vp, vp, C.POINTER(C.c_int64)]
+    L.fls_relocalize_wide.argtypes = [vp, vp, sz, sz] + wide_outs
+    L.fls_relocalize_wide_device.argtypes = [vp, vp, sz] + wide_outs
+    L.fls_relocalize_wide_levels.argtypes = [vp, vp, C.c_int]
     L.fls_get_iter_log.argtypes = [vp, C.POINTER(FlsIterLog), C.c_int]
     L.fls_get_iter_log_scan.argtypes = [vp, C.c_int, C.POINTER(FlsIterLog), C.c_int]
     L.fls_get_map_info.argtypes = [vp, C.POINTER(FlsMapInfo)]

@@ -65,12 +65,14 @@ struct KeyFrameGate {
 
 // the hypothesis grid of fls_relocalize (fls_b200.h): offsets -I..I in x and y, yaw offsets k0..K (n_yaw of them), P hypotheses
 static constexpr long long kRelocMaxHypotheses = 1LL << 20;
+static constexpr long long kRelocWideMaxHypotheses = 1LL << 31;  // and I <= 32767: fls_relocalize_wide
 struct RelocGrid {
-    int I = 0, K = 0, k0 = 0, n_yaw = 1;
-    long long P = 1;
+    int I = 0, K = 0, k0 = 0;
+    long long n_yaw = 1, P = 1;  // n_yaw reaches 2^31 on the full circle of the wide cap
 };
-// checks a relocalization configuration and sizes its grid (FLS_ERR_INVALID_ARG: see fls_relocalize)
-int reloc_grid(const fls_reloc_cfg& c, RelocGrid* g);
+// checks a relocalization configuration and sizes its grid (FLS_ERR_INVALID_ARG: see fls_relocalize, and fls_relocalize_wide's caps
+// when wide)
+int reloc_grid(const fls_reloc_cfg& c, RelocGrid* g, bool wide = false);
 
 struct Handle {
     fls_config cfg;
@@ -131,6 +133,20 @@ struct Handle {
     DevBuf<unsigned> reloc_part_cnt, reloc_idx;
     DevBuf<unsigned long long> reloc_key;
     DevBuf<unsigned char> reloc_pick;
+    // fls_relocalize_wide: the lower-bound distance lattice of the fit cloud (fls_reloc.cu; rebuilt like fit_grid), the node lists of
+    // a level and the next, sort keys, child counts and offsets, and U's sort key
+    struct {
+        int nx = 0, ny = 0, nz = 0;
+        double ox = 0, oy = 0, oz = 0, h = 0, q = 0;  // origin, pitch, quantum
+    } lat;
+    DevBuf<unsigned short> lat_v;
+    unsigned long long lat_version = ~0ull;
+    float lat_range = -1.f;
+    DevBuf<float4> wide_pts;  // the coarse cloud with each point's node-independent slack term
+    DevBuf<long long> wide_nodes, wide_next;
+    std::vector<long long> wide_levels;  // nodes evaluated per level of the last call, from its start level down to 0
+    DevBuf<unsigned long long> wide_key, wide_u;
+    DevBuf<int> wide_count;
 
     explicit Handle(const fls_config& c);
     ~Handle();
@@ -202,6 +218,10 @@ struct Handle {
     // fls_relocalize on a device scan (the call has begun; g from reloc_grid)
     int relocalize(const float4* d_scan, size_t n, const fls_reloc_cfg& c, const RelocGrid& g, double* T, fls_reloc_result* out, double* refined_T,
                    int32_t* refined_converged, float* refined_fitness, int64_t* refined_index, double* coarse_scores, size_t coarse_cap);
+    int lattice_for(float max_range, int* waits);  // (re)builds the lattice of the fit cloud for max_range when needed; counts its wait
+    // fls_relocalize_wide on a device scan (the call has begun; g from reloc_grid(wide))
+    int relocalize_wide(const float4* d_scan, size_t n, const fls_reloc_cfg& c, const RelocGrid& g, double* T, fls_reloc_result* out, double* refined_T,
+                        int32_t* refined_converged, float* refined_fitness, int64_t* refined_index, int64_t* evaluations);
 
     // localization-mode map path (fls_localmap.cu): resident global map, +-100 m crop around the pose when needed
     DevBuf<float4> global_map;

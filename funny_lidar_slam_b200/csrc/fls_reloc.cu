@@ -10,8 +10,10 @@
 #include <cfloat>
 #include <cmath>
 #include <cstring>
+#include <string>
 
 #include <cub/device/device_radix_sort.cuh>
+#include <cub/device/device_scan.cuh>
 
 #include "fls_handle.h"
 
@@ -151,17 +153,15 @@ __global__ void pose_score_reduce_kernel(const double* __restrict__ part_sum, co
 struct RelocGridArgs {
     double R[9], t[3];  // the guess
     double xy_step, yaw_step;
-    int I, K, k0, n_yaw;  // yaw offsets k0 .. K
-    int P;
+    int I, K, k0;  // yaw offsets k0 .. K
+    long long n_yaw, P;
 };
-__global__ void reloc_poses_kernel(RelocGridArgs g, double* __restrict__ poses) {
-    const int p = blockIdx.x * blockDim.x + threadIdx.x;
-    if (p >= g.P) return;
-    const int nx = 2 * g.I + 1;
-    const int ky = p % g.n_yaw, ix = (p / g.n_yaw) % nx, jy = p / (g.n_yaw * nx);
+// hypothesis p of the grid: the one formula of both searches, so that a leaf has the same bits in each
+__device__ __forceinline__ void reloc_leaf_pose(const RelocGridArgs& g, long long p, double* o) {
+    const long long nx = 2LL * g.I + 1;
+    const long long ky = p % g.n_yaw, ix = (p / g.n_yaw) % nx, jy = p / (g.n_yaw * nx);
     const double psi = __dmul_rn((double)(g.k0 + ky), g.yaw_step);
     const double c = cos(psi), s = sin(psi);
-    double* o = poses + (size_t)p * 12;
     for (int j = 0; j < 3; ++j) {
         const double a = g.R[j], b = g.R[3 + j];
         o[j] = __dsub_rn(__dmul_rn(c, a), __dmul_rn(s, b));
@@ -171,6 +171,11 @@ __global__ void reloc_poses_kernel(RelocGridArgs g, double* __restrict__ poses) 
     o[9] = __dadd_rn(g.t[0], __dmul_rn((double)(ix - g.I), g.xy_step));
     o[10] = __dadd_rn(g.t[1], __dmul_rn((double)(jy - g.I), g.xy_step));
     o[11] = g.t[2];
+}
+__global__ void reloc_poses_kernel(RelocGridArgs g, double* __restrict__ poses) {
+    const int p = blockIdx.x * blockDim.x + threadIdx.x;
+    if (p >= g.P) return;
+    reloc_leaf_pose(g, p, poses + (size_t)p * 12);
 }
 
 // the selected hypotheses: {index, coarse score, pose} records, read back in one copy
@@ -265,7 +270,9 @@ int Handle::fitness(float max_range, float* score) {
 }
 
 // ---- relocalization ------------------------------------------------------------------------------------------------------------
-int reloc_grid(const fls_reloc_cfg& c, RelocGrid* g) {
+int reloc_grid(const fls_reloc_cfg& c, RelocGrid* g, bool wide) {
+    const double max_i = wide ? 32767.0 : 1024.0;
+    const long long max_p = wide ? kRelocWideMaxHypotheses : kRelocMaxHypotheses;
     auto bad = [](double v) { return !(v > 0.0) || !std::isfinite(v); };
     if (!(c.xy_radius >= 0.0) || !std::isfinite(c.xy_radius) || !(c.yaw_range >= 0.0) || !std::isfinite(c.yaw_range)) return FLS_ERR_INVALID_ARG;
     if ((c.xy_radius > 0.0 && bad(c.xy_step)) || (c.yaw_range > 0.0 && bad(c.yaw_step))) return FLS_ERR_INVALID_ARG;
@@ -273,55 +280,130 @@ int reloc_grid(const fls_reloc_cfg& c, RelocGrid* g) {
     const double kPi = 3.14159265358979323846;
     const double fi = c.xy_radius > 0.0 ? std::floor(c.xy_radius / c.xy_step + 1e-9) : 0.0;
     const double fk = c.yaw_range > 0.0 ? std::floor(std::fmin(c.yaw_range, kPi) / c.yaw_step + 1e-9) : 0.0;
-    if (fi > 1024.0 || fk > (double)kRelocMaxHypotheses) return FLS_ERR_INVALID_ARG;
+    if (fi > max_i || fk > (double)(max_p / 2)) return FLS_ERR_INVALID_ARG;  // K > max_p / 2 gives more than max_p yaws
     g->I = (int)fi;
     g->K = (int)fk;
     g->k0 = -g->K;
     if (c.yaw_range >= kPi && g->K > 0 && 2.0 * g->K * c.yaw_step >= 2.0 * kPi - 1e-9) g->k0 = -g->K + 1;  // -K would repeat +K
-    g->n_yaw = g->K - g->k0 + 1;
+    g->n_yaw = (long long)g->K - g->k0 + 1;
     const long long nx = 2LL * g->I + 1;
+    if (nx * nx > max_p / g->n_yaw) return FLS_ERR_INVALID_ARG;  // P > max_p, without overflow
     const long long P = nx * nx * g->n_yaw;
-    if (P > kRelocMaxHypotheses) return FLS_ERR_INVALID_ARG;
     g->P = P;
     return FLS_OK;
 }
 
-int Handle::relocalize(const float4* d_scan, size_t n, const fls_reloc_cfg& c, const RelocGrid& gr, double* T, fls_reloc_result* out, double* refined_T,
-                       int32_t* refined_converged, float* refined_fitness, int64_t* refined_index, double* coarse_scores, size_t coarse_cap) {
+// The tail of both searches: the plug-in's batch Match of the nr picks, GetFitnessScore of every refined pose and Init's choice
+// rule.  L and W are the launches and waits of the call so far; out has its prelude.
+static int reloc_refine(Handle& h, const float4* d_scan, size_t n, const fls_reloc_cfg& c, const RelocPick* pick, int nr, int L, int W, double* T,
+                        fls_reloc_result* out, double* refined_T, int32_t* refined_converged, float* refined_fitness, int64_t* refined_index) {
+    // ---- refinement: the plug-in's batch Match of the picks, the same scan nr times ------------------------------------------------
+    double Tr[kMaxBatch * 16];
+    int conv[kMaxBatch];
+    const void* scans[kMaxBatch];
+    size_t ns[kMaxBatch];
+    for (int r = 0; r < nr; ++r) {
+        double* Ts = Tr + 16 * r;
+        for (int i = 0; i < 3; ++i) {
+            for (int j = 0; j < 3; ++j) Ts[j * 4 + i] = pick[r].pose[i * 3 + j];
+            Ts[12 + i] = pick[r].pose[9 + i];
+        }
+        Ts[3] = Ts[7] = Ts[11] = 0.0;
+        Ts[15] = 1.0;
+        scans[r] = d_scan;
+        ns[r] = n;
+    }
+    L += h.launches;
+    const int rc = h.plugin->match_batch(nr, scans, ns, 0, Tr, conv, nullptr);  // begins its own call
+    L += h.launches;
+    W += h.waits;
+    h.launches = 0;
+    if (rc != FLS_OK) return rc;
+    // ---- fitness of every refined pose on the cloud fls_fitness reads after that Match, in one launch -------------------------------
+    double rows[kMaxBatch * 12];
+    for (int r = 0; r < nr; ++r) pose_rows(Tr + 16 * r, rows + 12 * r);
+    h.fit_pose.reserve((size_t)nr * 12);
+    FLS_CUDA(cudaMemcpyAsync(h.fit_pose.p, rows, sizeof(double) * 12 * (size_t)nr, cudaMemcpyHostToDevice, h.stream));
+    float fit[kMaxBatch];
+    for (int r = 0; r < nr; ++r) fit[r] = FLT_MAX;
+    if (h.last_src && h.last_src_n) {
+        h.fitness_enqueue(h.last_src, h.last_src_n, nr, c.max_range);
+        double sums[kMaxBatch];
+        unsigned cnts[kMaxBatch];
+        FLS_CUDA(cudaMemcpyAsync(sums, h.fit_out.p, sizeof(double) * (size_t)nr, cudaMemcpyDeviceToHost, h.stream));
+        FLS_CUDA(cudaMemcpyAsync(cnts, h.fit_cnt.p, sizeof(unsigned) * (size_t)nr, cudaMemcpyDeviceToHost, h.stream));
+        FLS_CUDA(cudaStreamSynchronize(h.stream));
+        ++W;
+        for (int r = 0; r < nr; ++r) fit[r] = fitness_of(sums[r], cnts[r]);
+    }
+    // ---- choice: the converged pose of lowest fitness (ties: rank), else the lowest fitness -----------------------------------------
+    int best = -1;
+    for (int pass = 0; pass < 2 && best < 0; ++pass)
+        for (int r = 0; r < nr; ++r)
+            if ((pass == 1 || conv[r]) && (best < 0 || fit[r] < fit[best])) best = r;
+    std::memcpy(T, Tr + 16 * best, 16 * sizeof(double));
+    std::memcpy(h.T_final, T, sizeof(h.T_final));  // a later fls_fitness scores the chosen pose on last_src
+    out->n_refined = nr;
+    out->best_rank = best;
+    out->best_hypothesis = pick[best].index;
+    out->converged = conv[best] ? 1 : 0;
+    out->fitness = fit[best];
+    out->coarse_score = (float)pick[best].score;
+    out->accepted = (conv[best] && fit[best] < c.accept_fitness) ? 1 : 0;
+    for (int r = 0; r < nr; ++r) {
+        if (refined_T) std::memcpy(refined_T + 16 * r, Tr + 16 * r, 16 * sizeof(double));
+        if (refined_converged) refined_converged[r] = conv[r];
+        if (refined_fitness) refined_fitness[r] = fit[r];
+        if (refined_index) refined_index[r] = pick[r].index;
+    }
+    out->gpu_launches = L + h.launches;  // h.launches: the fitness launches since the Match
+    out->host_waits = W;
+    return FLS_OK;
+}
+
+// The head of both searches: out's defaults, the coarse cloud (*m points) and the fit grid, and the grid's arguments.  An empty
+// coarse cloud (*m == 0) has finished the call: nothing to score or refine, and a later fls_fitness scores the empty cloud.
+static int reloc_prelude(Handle& h, const float4* d_scan, size_t n, const fls_reloc_cfg& c, const RelocGrid& gr, const double* T,
+                         fls_reloc_result* out, int& W, size_t* m, RelocGridArgs* ga) {
     std::memset(out, 0, sizeof(*out));
     out->n_hypotheses = gr.P;
     out->best_hypothesis = -1;
     out->fitness = FLT_MAX;
     out->coarse_score = FLT_MAX;
-    int L = 0, W = 0;  // launches and waits of the whole call
-    auto account = [&] {
-        out->gpu_launches = L + launches;
-        out->host_waits = W;
-    };
     // ---- coarse cloud and the fit grid ---------------------------------------------------------------------------------------------
-    reloc_coarse.reserve(n + 1);
-    const size_t m = voxel_grid_device(d_scan, n, c.coarse_leaf, reloc_coarse.p, scratch, stream, &launches, &W);
-    if (m == 0) {  // an empty scan: nothing to score or refine, and a later fls_fitness scores the empty cloud
-        last_src = d_scan;
-        last_src_n = 0;
-        account();
+    h.reloc_coarse.reserve(n + 1);
+    *m = voxel_grid_device(d_scan, n, c.coarse_leaf, h.reloc_coarse.p, h.scratch, h.stream, &h.launches, &W);
+    if (*m == 0) {
+        h.last_src = d_scan;
+        h.last_src_n = 0;
+        out->gpu_launches = h.launches;
+        out->host_waits = W;
         return FLS_OK;
     }
-    int rc = fit_grid_for(c.max_range, &W);
+    const int rc = h.fit_grid_for(c.max_range, &W);
     if (rc != FLS_OK) return rc;
+    pose_rows(T, ga->R);
+    for (int k = 0; k < 3; ++k) ga->t[k] = T[12 + k];
+    ga->xy_step = gr.I ? c.xy_step : 0.0;  // an unused step may be anything
+    ga->yaw_step = gr.K ? c.yaw_step : 0.0;
+    ga->I = gr.I;
+    ga->K = gr.K;
+    ga->k0 = gr.k0;
+    ga->n_yaw = gr.n_yaw;
+    ga->P = gr.P;
+    return FLS_OK;
+}
+
+int Handle::relocalize(const float4* d_scan, size_t n, const fls_reloc_cfg& c, const RelocGrid& gr, double* T, fls_reloc_result* out, double* refined_T,
+                       int32_t* refined_converged, float* refined_fitness, int64_t* refined_index, double* coarse_scores, size_t coarse_cap) {
+    int L = 0, W = 0;  // launches and waits of the whole call
+    size_t m = 0;
+    RelocGridArgs ga;
+    const int rc = reloc_prelude(*this, d_scan, n, c, gr, T, out, W, &m, &ga);
+    if (rc != FLS_OK || m == 0) return rc;
     // ---- the hypotheses, their coarse scores and the n_refine best -----------------------------------------------------------------
     const int P = (int)gr.P;
     const int nr = P < c.n_refine ? P : c.n_refine;
-    RelocGridArgs ga;
-    pose_rows(T, ga.R);
-    for (int k = 0; k < 3; ++k) ga.t[k] = T[12 + k];
-    ga.xy_step = gr.I ? c.xy_step : 0.0;  // an unused step may be anything
-    ga.yaw_step = gr.K ? c.yaw_step : 0.0;
-    ga.I = gr.I;
-    ga.K = gr.K;
-    ga.k0 = gr.k0;
-    ga.n_yaw = gr.n_yaw;
-    ga.P = P;
     const size_t tiles = (m + kCoarseTile - 1) / kCoarseTile;
     reloc_poses.reserve((size_t)P * 12);
     reloc_part_sum.reserve((size_t)P * tiles);
@@ -350,67 +432,494 @@ int Handle::relocalize(const float4* d_scan, size_t n, const fls_reloc_cfg& c, c
     if (n_cs) FLS_CUDA(cudaMemcpyAsync(coarse_scores, reloc_score.p, sizeof(double) * n_cs, cudaMemcpyDeviceToHost, stream));
     FLS_CUDA(cudaStreamSynchronize(stream));
     ++W;
-    // ---- refinement: the plug-in's batch Match of the picks, the same scan nr times ------------------------------------------------
-    double Tr[kMaxBatch * 16];
-    int conv[kMaxBatch];
-    const void* scans[kMaxBatch];
-    size_t ns[kMaxBatch];
-    for (int r = 0; r < nr; ++r) {
-        double* Ts = Tr + 16 * r;
-        for (int i = 0; i < 3; ++i) {
-            for (int j = 0; j < 3; ++j) Ts[j * 4 + i] = pick[r].pose[i * 3 + j];
-            Ts[12 + i] = pick[r].pose[9 + i];
+    return reloc_refine(*this, d_scan, n, c, pick, nr, L, W, T, out, refined_T, refined_converged, refined_fitness, refined_index);
+}
+
+namespace {
+
+// ---- fls_relocalize_wide: exact branch and bound over the hypothesis grid ------------------------------------------------------
+// A node of level l is an aligned block of 2^l x 2^l x 2^l leaves (hypotheses) in (x, y, yaw) index space, clipped at the grid's
+// edges; its id orders the blocks as the leaves are ordered (yaw fastest, then x, then y), so a level-0 node is a leaf.  A node is
+// evaluated at one representative leaf: the one 2^(l-1) past its low corner in each index, or the last one where the block is clipped.
+//
+// The bound.  Let q_i be scan point p_i moved by the representative as the score kernel moves it (the fp64 pose cast to float,
+// xform_row_f), and b_i a lower bound on the distance from q_i to the fit cloud (the lattice below).  A leaf of the node moves p_i to
+// q'_i with |q'_i - q_i| <= delta_i = dt + dpsi * |(R_guess p_i)_xy| + eps_i, where dt = xy_step * sqrt(hx^2 + hy^2) bounds the
+// translation offset (hx, hy, hk: the largest index offsets from the representative to a leaf of the node), and dpsi = hk * yaw_step
+// bounds the turn: the leaves share z, roll and pitch, and |Rz(a) v - Rz(b) v| = 2 |sin((a - b) / 2)| |v_xy| <= |a - b| |v_xy|.
+// eps_i covers the floats.  A transform row is ((r0 x + r1 y) + r2 z) + t in fp32 with r and t the fp64 pose rounded once: with
+// u = 2^-24, |r| <= 1 and the rotation rows of the leaves rounded in fp64 (2^-53, far below u), each of the five roundings and the
+// two casts is at most u (|p|_1 + |t|) to first order, so a coordinate is within 7u (|p|_1 + |t|_inf) of the exact value and the
+// point within 7 sqrt(3) u (...) < 13u (...); for two poses 26u, taken as 32u (|p_i|_1 + tau) with tau the largest |t| coordinate of
+// any leaf.  dist2_ref's three roundings on differences and three on products and sums give d2_f >= d^2 (1 - 6u) to first order,
+// so sqrt(d2_f) >= d - 3u d; the term below only differs from max_range when d < sqrt(max_range) (1 + 4u), so 8u sqrt(max_range)
+// covers it.  The lattice lookup and the bound itself run in fp64, whose roundings (2^-53 relative) the factor 32 absorbs.  So
+// every leaf's fp32 squared 1-NN distance of p_i is at least max(0, b_i - delta_i)^2, and GetFitnessScore's gated sum of the leaf,
+// sum_i min(d2_i, max_range) (an outlier or a point without a neighbour counts max_range), is at least
+//   LB = sum_i min(max(0, b_i - delta_i)^2, max_range)        (in fp64).
+// Both sums are fp64 sums of up to 2^30 non-negative terms in different orders: their rounding is below m 2^-53 < 1.2e-7 of the
+// sum, so a node is pruned only when LB / m > U (1 + kPruneMargin).
+//
+// U is the n-th smallest exact score among the distinct leaves scored so far: the representatives of the start level (the lowest
+// level with at most 2^20 nodes) are all scored exactly, and no later level scores any (those reps would repeat leaves already
+// scored or be scored again at level 0; the start level's U already comes from up to 2^20 leaves spread over the whole grid).  A
+// node is kept iff LB / m <= U (1 + margin): every leaf scoring <= U keeps all its ancestors, so the n best leaves of the whole grid,
+// and every tie at the n-th score, reach level 0, where all survivors are scored exactly and sorted on (score bits, leaf index).
+constexpr long long kWideChunk = 1LL << 20;  // nodes of the start level, and of one launch at any level
+constexpr long long kWideCap = 1LL << 23;    // survivors of one level; more is FLS_ERR_CAPACITY
+constexpr double kPruneMargin = 1e-6;
+constexpr double kU = 1.0 / 16777216.0;  // unit roundoff of fp32
+constexpr size_t kLatticeCells = 1u << 25;
+constexpr int kLatticeLine = 65535;  // cells per axis at most: the per-line stacks of the transform are 16-bit
+constexpr unsigned kEdtInf = 0xffffffffu;
+
+struct LatticeView {
+    const unsigned short* v;
+    int nx, ny, nz;
+    double ox, oy, oz, h, inv_h, q;
+};
+
+// blocks per axis of n leaves at level l
+__host__ __device__ inline long long level_blocks(long long n, int l) { return (n + (1LL << l) - 1) >> l; }
+
+// representative index and largest offset to any index of block b at level l of an axis of n leaves
+__device__ inline long long block_rep(long long b, int l, long long n, int& h) {
+    const long long lo = b << l, hi = min(lo + (1LL << l), n) - 1;
+    const long long r = l ? min(lo + (1LL << (l - 1)), hi) : lo;
+    h = (int)max(r - lo, hi - r);
+    return r;
+}
+
+struct NodeRep {
+    long long leaf;
+    int hx, hy, hk;
+};
+__device__ inline NodeRep node_rep(long long id, int l, long long nx, long long nk) {
+    const long long nbk = level_blocks(nk, l), nbx = level_blocks(nx, l);
+    const long long bk = id % nbk, bx = (id / nbk) % nbx, by = id / (nbk * nbx);
+    NodeRep r;
+    const long long rk = block_rep(bk, l, nk, r.hk), rx = block_rep(bx, l, nx, r.hx), ry = block_rep(by, l, nx, r.hy);
+    r.leaf = (ry * nx + rx) * nk + rk;
+    return r;
+}
+
+__global__ void reloc_iota_kernel(long long* __restrict__ out, long long n) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) out[i] = i;
+}
+
+// poses of the representatives of N nodes of level l
+__global__ void reloc_rep_poses_kernel(RelocGridArgs g, const long long* __restrict__ nodes, int N, int l, double* __restrict__ poses) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= N) return;
+    reloc_leaf_pose(g, node_rep(nodes[i], l, 2LL * g.I + 1, g.n_yaw).leaf, poses + (size_t)i * 12);
+}
+
+struct BoundArgs {
+    LatticeView lat;
+    RelocGridArgs g;
+    const float4* __restrict__ src;  // the coarse cloud with w = |(R_guess p)_xy| rounded up (reloc_slack_points_kernel)
+    int n;
+    const long long* __restrict__ nodes;
+    int N, level, n_tiles;
+    double eps0, eps1, max_range;  // eps_i = eps0 + eps1 |p_i|_1
+    double* __restrict__ part;     // [N][n_tiles]
+};
+
+// grid (ceil(N / 8), min(n_tiles, 65535)): pose_score_kernel<8, 2048>'s tiling; per (node, tile) the partial of LB
+__global__ void __launch_bounds__(kScoreBlock) reloc_bound_kernel(BoundArgs a) {
+    constexpr int PPC = kCoarsePoses, TILE = kCoarseTile, TPP = kScoreBlock / PPC;
+    __shared__ float4 s_pts[TILE];
+    __shared__ double s_sum[kScoreBlock];
+    const int sub = threadIdx.x % TPP;
+    const int node = blockIdx.x * PPC + threadIdx.x / TPP;
+    float r[12];
+    double dt = 0.0, dpsi = 0.0;
+    if (node < a.N) {
+        const NodeRep nr = node_rep(a.nodes[node], a.level, 2LL * a.g.I + 1, a.g.n_yaw);
+        double pose[12];
+        reloc_leaf_pose(a.g, nr.leaf, pose);
+#pragma unroll
+        for (int k = 0; k < 12; ++k) r[k] = (float)pose[k];
+        dt = a.g.xy_step * sqrt((double)nr.hx * nr.hx + (double)nr.hy * nr.hy);
+        dpsi = (double)nr.hk * a.g.yaw_step;
+    }
+    const LatticeView& L = a.lat;
+    const double ex = L.ox + L.nx * L.h, ey = L.oy + L.ny * L.h, ez = L.oz + L.nz * L.h;
+    for (int tile = blockIdx.y; tile < a.n_tiles; tile += gridDim.y) {  // uniform across the CTA
+        const size_t base = (size_t)tile * TILE;
+        const int m = (int)min((size_t)TILE, (size_t)a.n - base);
+        for (int i = threadIdx.x; i < m; i += kScoreBlock) s_pts[i] = a.src[base + i];
+        double sum = 0.0;
+        __syncthreads();
+        if (node < a.N) {
+#pragma unroll 1
+            for (int i = sub; i < m; i += TPP) {
+                const float4 sp = s_pts[i];
+                const double qx = xform_row_f(r[0], r[1], r[2], r[9], sp.x, sp.y, sp.z);
+                const double qy = xform_row_f(r[3], r[4], r[5], r[10], sp.x, sp.y, sp.z);
+                const double qz = xform_row_f(r[6], r[7], r[8], r[11], sp.x, sp.y, sp.z);
+                // b_i: the distance to the lattice's box, and the lattice value of the cell of q's projection onto the box (the
+                // projection onto a convex set: |q - p|^2 >= |q - q*|^2 + |q* - p|^2 for every fit point p in the box)
+                const double dx = fmax(0.0, fmax(L.ox - qx, qx - ex)), dy = fmax(0.0, fmax(L.oy - qy, qy - ey)), dz = fmax(0.0, fmax(L.oz - qz, qz - ez));
+                const int cx = (int)fmin(fmax((qx - L.ox) * L.inv_h, 0.0), L.nx - 1.0);
+                const int cy = (int)fmin(fmax((qy - L.oy) * L.inv_h, 0.0), L.ny - 1.0);
+                const int cz = (int)fmin(fmax((qz - L.oz) * L.inv_h, 0.0), L.nz - 1.0);
+                const double lv = (double)__ldg(L.v + ((size_t)cz * L.ny + cy) * L.nx + cx) * L.q;
+                const double b = sqrt(dx * dx + dy * dy + dz * dz + lv * lv);
+                const double delta = dt + dpsi * (double)sp.w + a.eps0 + a.eps1 * ((double)fabsf(sp.x) + (double)fabsf(sp.y) + (double)fabsf(sp.z));
+                const double e = fmax(0.0, b - delta);
+                sum += fmin(e * e, a.max_range);
+            }
         }
-        Ts[3] = Ts[7] = Ts[11] = 0.0;
-        Ts[15] = 1.0;
-        scans[r] = d_scan;
-        ns[r] = n;
+        s_sum[threadIdx.x] = sum;
+        __syncthreads();
+#pragma unroll
+        for (int o = TPP / 2; o > 0; o >>= 1) {
+            if (sub < o) s_sum[threadIdx.x] += s_sum[threadIdx.x + o];
+            __syncthreads();
+        }
+        if (sub == 0 && node < a.N) a.part[(size_t)node * a.n_tiles + tile] = s_sum[threadIdx.x];
     }
-    L += launches;
-    rc = plugin->match_batch(nr, scans, ns, 0, Tr, conv, nullptr);  // begins its own call
-    L += launches;
-    W += waits;
-    launches = 0;
-    if (rc != FLS_OK) return rc;
-    // ---- fitness of every refined pose on the cloud fls_fitness reads after that Match, in one launch -------------------------------
-    double rows[kMaxBatch * 12];
-    for (int r = 0; r < nr; ++r) pose_rows(Tr + 16 * r, rows + 12 * r);
-    fit_pose.reserve((size_t)nr * 12);
-    FLS_CUDA(cudaMemcpyAsync(fit_pose.p, rows, sizeof(double) * 12 * (size_t)nr, cudaMemcpyHostToDevice, stream));
-    float fit[kMaxBatch];
-    for (int r = 0; r < nr; ++r) fit[r] = FLT_MAX;
-    if (last_src && last_src_n) {
-        fitness_enqueue(last_src, last_src_n, nr, c.max_range);
-        double sums[kMaxBatch];
-        unsigned cnts[kMaxBatch];
-        FLS_CUDA(cudaMemcpyAsync(sums, fit_out.p, sizeof(double) * (size_t)nr, cudaMemcpyDeviceToHost, stream));
-        FLS_CUDA(cudaMemcpyAsync(cnts, fit_cnt.p, sizeof(unsigned) * (size_t)nr, cudaMemcpyDeviceToHost, stream));
-        FLS_CUDA(cudaStreamSynchronize(stream));
-        ++W;
-        for (int r = 0; r < nr; ++r) fit[r] = fitness_of(sums[r], cnts[r]);
+}
+
+// per node: LB / m against U (the n-th smallest sorted score bits at *u_key) -> how many children it passes to level l - 1
+__global__ void reloc_keep_kernel(const double* __restrict__ part, int N, int n_tiles, int m, const unsigned long long* __restrict__ u_key,
+                                  const long long* __restrict__ nodes, int l, long long nx, long long nk, int* __restrict__ n_children) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= N) return;
+    double lb = 0.0;
+    for (int t = 0; t < n_tiles; ++t) lb += part[(size_t)i * n_tiles + t];
+    const double U = __longlong_as_double((long long)*u_key);
+    int k = 0;
+    if (lb / (double)m <= U * (1.0 + kPruneMargin)) {
+        const long long id = nodes[i], nbk = level_blocks(nk, l), nbx = level_blocks(nx, l);
+        const long long bk = id % nbk, bx = (id / nbk) % nbx, by = id / (nbk * nbx);
+        const long long ck = level_blocks(nk, l - 1), cx = level_blocks(nx, l - 1);
+        k = (int)((min(2 * bk + 2, ck) - 2 * bk) * (min(2 * bx + 2, cx) - 2 * bx) * (min(2 * by + 2, cx) - 2 * by));
     }
-    // ---- choice: the converged pose of lowest fitness (ties: rank), else the lowest fitness -----------------------------------------
-    int best = -1;
-    for (int pass = 0; pass < 2 && best < 0; ++pass)
-        for (int r = 0; r < nr; ++r)
-            if ((pass == 1 || conv[r]) && (best < 0 || fit[r] < fit[best])) best = r;
-    std::memcpy(T, Tr + 16 * best, 16 * sizeof(double));
-    std::memcpy(T_final, T, sizeof(T_final));  // a later fls_fitness scores the chosen pose on last_src
-    out->n_refined = nr;
-    out->best_rank = best;
-    out->best_hypothesis = pick[best].index;
-    out->converged = conv[best] ? 1 : 0;
-    out->fitness = fit[best];
-    out->coarse_score = (float)pick[best].score;
-    out->accepted = (conv[best] && fit[best] < c.accept_fitness) ? 1 : 0;
-    for (int r = 0; r < nr; ++r) {
-        if (refined_T) std::memcpy(refined_T + 16 * r, Tr + 16 * r, 16 * sizeof(double));
-        if (refined_converged) refined_converged[r] = conv[r];
-        if (refined_fitness) refined_fitness[r] = fit[r];
-        if (refined_index) refined_index[r] = pick[r].index;
+    n_children[i] = k;
+}
+
+// the children of the kept nodes of level l, at their offsets in the level l - 1 list
+__global__ void reloc_children_kernel(const long long* __restrict__ nodes, const int* __restrict__ n_children, const int* __restrict__ offset, int N,
+                                      int l, long long nx, long long nk, long long* __restrict__ out) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= N || n_children[i] == 0) return;
+    const long long id = nodes[i], nbk = level_blocks(nk, l), nbx = level_blocks(nx, l);
+    const long long bk = id % nbk, bx = (id / nbk) % nbx, by = id / (nbk * nbx);
+    const long long ck = level_blocks(nk, l - 1), cx = level_blocks(nx, l - 1);
+    long long* o = out + offset[i];
+    for (long long y = 2 * by; y < min(2 * by + 2, cx); ++y)
+        for (long long x = 2 * bx; x < min(2 * bx + 2, cx); ++x)
+            for (long long k = 2 * bk; k < min(2 * bk + 2, ck); ++k) *o++ = (y * cx + x) * ck + k;
+}
+
+// the n best after the sort: {leaf index, score, pose}
+__global__ void reloc_pick_wide_kernel(const unsigned long long* __restrict__ key_sorted, const long long* __restrict__ leaf_sorted, RelocGridArgs g,
+                                       int n, RelocPick* __restrict__ out) {
+    const int r = threadIdx.x;
+    if (r >= n) return;
+    out[r].index = leaf_sorted[r];
+    out[r].score = __longlong_as_double((long long)key_sorted[r]);
+    reloc_leaf_pose(g, leaf_sorted[r], out[r].pose);
+}
+
+// ---- the lower-bound distance lattice -------------------------------------------------------------------------------------------
+// Cells of pitch h over the fit cloud's bounding box.  An exact squared Euclidean distance transform between cell centres (in cells,
+// three separable passes of Meijster's integer lower envelope, one thread per line) gives D(c) to the nearest occupied cell.  A point
+// x of cell c and a fit point p of cell c' are at least the distance between the two cell boxes apart, h sqrt(sum_k max(0, |c_k -
+// c'_k| - 1)^2) = h min over the 27 neighbours c + s (s in {-1, 0, 1}^3) of |c + s - c'|, and the neighbour that attains it lies
+// between c and c', inside the box; so the cell stores h sqrt(min_s D(c + s)), rounded down to quanta of h / 64 in 16 bits.  Values
+// saturate at 1024 h, which covers sqrt(max_range) (<= 4 h) plus a slack of about 1000 cells; a larger slack makes its term zero
+// anyway.  h = sqrt(max_range) / 4, doubled until the box has at most 2^25 cells and at most 65535 along each axis.
+
+// one block: the bounding box of the fit cloud, as {min x, y, z, max x, y, z}
+__global__ void lattice_bbox_kernel(const float4* __restrict__ pts, size_t n, float* __restrict__ box) {
+    __shared__ float s[6][256];
+    float v[6] = {INFINITY, INFINITY, INFINITY, -INFINITY, -INFINITY, -INFINITY};
+    for (size_t i = threadIdx.x; i < n; i += blockDim.x) {
+        const float4 p = pts[i];
+        v[0] = fminf(v[0], p.x), v[1] = fminf(v[1], p.y), v[2] = fminf(v[2], p.z);
+        v[3] = fmaxf(v[3], p.x), v[4] = fmaxf(v[4], p.y), v[5] = fmaxf(v[5], p.z);
     }
-    account();
+    for (int k = 0; k < 6; ++k) s[k][threadIdx.x] = v[k];
+    __syncthreads();
+    for (int o = blockDim.x / 2; o > 0; o >>= 1) {
+        if (threadIdx.x < o)
+            for (int k = 0; k < 6; ++k) s[k][threadIdx.x] = k < 3 ? fminf(s[k][threadIdx.x], s[k][threadIdx.x + o]) : fmaxf(s[k][threadIdx.x], s[k][threadIdx.x + o]);
+        __syncthreads();
+    }
+    if (threadIdx.x < 6) box[threadIdx.x] = s[threadIdx.x][0];
+}
+
+__global__ void lattice_mark_kernel(const float4* __restrict__ pts, size_t n, LatticeView L, unsigned* __restrict__ d) {
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const float4 p = pts[i];
+    const int cx = (int)fmin(fmax(floor(((double)p.x - L.ox) * L.inv_h), 0.0), L.nx - 1.0);
+    const int cy = (int)fmin(fmax(floor(((double)p.y - L.oy) * L.inv_h), 0.0), L.ny - 1.0);
+    const int cz = (int)fmin(fmax(floor(((double)p.z - L.oz) * L.inv_h), 0.0), L.nz - 1.0);
+    d[((size_t)cz * L.ny + cy) * L.nx + cx] = 0u;
+}
+
+// one pass of the separable transform along `axis`: out(u) = min_i (u - i)^2 + in(i) on every line, exact in integers (kEdtInf: no
+// fit point yet; a finite value saturates below it, which keeps it a lower bound).  s and t: per-line stacks at the line's own cells.
+__global__ void lattice_edt_kernel(const unsigned* __restrict__ in, unsigned* __restrict__ out, unsigned short* __restrict__ s,
+                                   unsigned short* __restrict__ t, int nx, int ny, int nz, int axis) {
+    const long long line = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    long long base, stride;
+    int n;
+    if (axis == 0) {
+        if (line >= (long long)ny * nz) return;
+        base = line * nx, stride = 1, n = nx;
+    } else if (axis == 1) {
+        if (line >= (long long)nx * nz) return;
+        base = (line / nx) * nx * ny + line % nx, stride = nx, n = ny;
+    } else {
+        if (line >= (long long)nx * ny) return;
+        base = line, stride = (long long)nx * ny, n = nz;
+    }
+    constexpr long long kInf = 1LL << 40;
+    auto g = [&](long long i) -> long long {
+        const unsigned v = in[base + i * stride];
+        return v == kEdtInf ? kInf : (long long)v;
+    };
+    auto f = [&](long long x, long long i) { return (x - i) * (x - i) + g(i); };
+    auto S = [&](long long k) -> unsigned short& { return s[base + k * stride]; };
+    auto Tt = [&](long long k) -> unsigned short& { return t[base + k * stride]; };
+    long long q = 0;
+    S(0) = 0;
+    Tt(0) = 0;
+    for (long long u = 1; u < n; ++u) {
+        while (q >= 0 && f(Tt(q), S(q)) > f(Tt(q), u)) --q;
+        if (q < 0) {
+            q = 0;
+            S(0) = (unsigned short)u;
+        } else {
+            const long long i = S(q), num = u * u - i * i + g(u) - g(i), den = 2 * (u - i);
+            const long long w = 1 + (num >= 0 ? num / den : -((-num + den - 1) / den));  // 1 + floor(num / den)
+            if (w < n) {
+                ++q;
+                S(q) = (unsigned short)u;
+                Tt(q) = (unsigned short)w;
+            }
+        }
+    }
+    for (long long u = n - 1; u >= 0; --u) {
+        const long long d = f(u, S(q));
+        out[base + u * stride] = d >= kInf ? kEdtInf : (unsigned)min(d, (long long)kEdtInf - 1);
+        if (u == Tt(q)) --q;
+    }
+}
+
+__global__ void lattice_store_kernel(const unsigned* __restrict__ d, int nx, int ny, int nz, double h, double q, unsigned short* __restrict__ v) {
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= (size_t)nx * ny * nz) return;
+    const int x = (int)(i % nx), y = (int)((i / nx) % ny), z = (int)(i / ((size_t)nx * ny));
+    unsigned m = kEdtInf;
+    for (int dz = max(z - 1, 0); dz <= min(z + 1, nz - 1); ++dz)
+        for (int dy = max(y - 1, 0); dy <= min(y + 1, ny - 1); ++dy)
+            for (int dx = max(x - 1, 0); dx <= min(x + 1, nx - 1); ++dx) m = min(m, d[((size_t)dz * ny + dy) * nx + dx]);
+    // fp64 roundings of the square root and the products: taken off with a relative 2^-40 before rounding down
+    const double b = sqrt((double)m) * h * (1.0 - 0x1p-40);
+    v[i] = (unsigned short)fmin(floor(b / q), 65535.0);
+}
+
+// per scan point: its coordinates and |(R_guess p)_xy| rounded up, the node-independent part of the slack
+__global__ void reloc_slack_points_kernel(const float4* __restrict__ src, int n, RelocGridArgs g, float4* __restrict__ out) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const float4 p = src[i];
+    const double vx = g.R[0] * p.x + g.R[1] * p.y + g.R[2] * p.z, vy = g.R[3] * p.x + g.R[4] * p.y + g.R[5] * p.z;
+    out[i] = make_float4(p.x, p.y, p.z, __double2float_ru(sqrt(vx * vx + vy * vy)));
+}
+
+}  // namespace
+
+// The lattice of the current fit cloud and max_range, rebuilt like fit_grid (two waits when it is: the bounding box, and the end of
+// the build before its scratch is freed).
+int Handle::lattice_for(float max_range, int* waits) {
+    if (lat_version == fit_cloud_version && lat_range == max_range) return FLS_OK;
+    DevBuf<float> box;
+    box.reserve(6);
+    lattice_bbox_kernel<<<1, 256, 0, stream>>>(fit_pts, fit_cloud_n, box.p);
+    float b[6];
+    FLS_CUDA(cudaMemcpyAsync(b, box.p, sizeof(b), cudaMemcpyDeviceToHost, stream));
+    FLS_CUDA(cudaStreamSynchronize(stream));
+    if (waits) ++*waits;
+    double h = std::sqrt((double)max_range) / 4.0;
+    long long n[3];
+    for (;; h *= 2.0) {
+        for (int k = 0; k < 3; ++k) n[k] = (long long)std::floor(((double)b[3 + k] - (double)b[k]) / h) + 1;
+        if (n[0] * n[1] * n[2] <= (long long)kLatticeCells && n[0] <= kLatticeLine && n[1] <= kLatticeLine && n[2] <= kLatticeLine) break;
+    }
+    lat.nx = (int)n[0], lat.ny = (int)n[1], lat.nz = (int)n[2];
+    lat.ox = b[0], lat.oy = b[1], lat.oz = b[2];
+    lat.h = h;
+    lat.q = h / 64.0;
+    const size_t cells = (size_t)(n[0] * n[1] * n[2]);
+    LatticeView L{nullptr, lat.nx, lat.ny, lat.nz, lat.ox, lat.oy, lat.oz, h, 1.0 / h, lat.q};
+    DevBuf<unsigned> d0, d1;
+    DevBuf<unsigned short> s, t;
+    d0.reserve(cells), d1.reserve(cells), s.reserve(cells), t.reserve(cells);
+    lat_v.reserve(cells);
+    FLS_CUDA(cudaMemsetAsync(d0.p, 0xff, cells * sizeof(unsigned), stream));
+    lattice_mark_kernel<<<grid_for(fit_cloud_n, 256), 256, 0, stream>>>(fit_pts, fit_cloud_n, L, d0.p);
+    const long long lines[3] = {n[1] * n[2], n[0] * n[2], n[0] * n[1]};
+    lattice_edt_kernel<<<grid_for((size_t)lines[0], 128), 128, 0, stream>>>(d0.p, d1.p, s.p, t.p, lat.nx, lat.ny, lat.nz, 0);
+    lattice_edt_kernel<<<grid_for((size_t)lines[1], 128), 128, 0, stream>>>(d1.p, d0.p, s.p, t.p, lat.nx, lat.ny, lat.nz, 1);
+    lattice_edt_kernel<<<grid_for((size_t)lines[2], 128), 128, 0, stream>>>(d0.p, d1.p, s.p, t.p, lat.nx, lat.ny, lat.nz, 2);
+    lattice_store_kernel<<<grid_for(cells, 256), 256, 0, stream>>>(d1.p, lat.nx, lat.ny, lat.nz, h, lat.q, lat_v.p);
+    FLS_CUDA(cudaGetLastError());
+    FLS_CUDA(cudaStreamSynchronize(stream));  // the scratch above is freed on return
+    if (waits) ++*waits;
+    launches += 6;
+    lat_version = fit_cloud_version;
+    lat_range = max_range;
     return FLS_OK;
+}
+
+int Handle::relocalize_wide(const float4* d_scan, size_t n, const fls_reloc_cfg& c, const RelocGrid& gr, double* T, fls_reloc_result* out,
+                            double* refined_T, int32_t* refined_converged, float* refined_fitness, int64_t* refined_index, int64_t* evaluations) {
+    int L = 0, W = 0;  // launches and waits of the whole call
+    long long evals = 0;
+    if (evaluations) *evaluations = 0;
+    wide_levels.clear();
+    size_t m = 0;
+    RelocGridArgs ga;
+    int rc = reloc_prelude(*this, d_scan, n, c, gr, T, out, W, &m, &ga);
+    if (rc != FLS_OK || m == 0) return rc;
+    const long long P = gr.P, nx = 2LL * gr.I + 1, nk = gr.n_yaw;
+    const int nr = P < c.n_refine ? (int)P : c.n_refine;
+    int ls = 0;
+    while (level_blocks(nx, ls) * level_blocks(nx, ls) * level_blocks(nk, ls) > kWideChunk) ++ls;
+    long long N = level_blocks(nx, ls) * level_blocks(nx, ls) * level_blocks(nk, ls);
+    const size_t tiles = (m + kCoarseTile - 1) / kCoarseTile;
+    auto reserve_chunk = [&](size_t k) {  // a launch's poses, partials and scores
+        reloc_poses.reserve(k * 12);
+        reloc_part_sum.reserve(k * tiles);
+        reloc_part_cnt.reserve(k * tiles);
+        reloc_score.reserve(k);
+        reloc_idx.reserve(k);
+    };
+    reloc_pick.reserve(sizeof(RelocPick) * kMaxBatch);
+    wide_nodes.reserve((size_t)N);
+    reloc_iota_kernel<<<grid_for((size_t)N, 256), 256, 0, stream>>>(wide_nodes.p, N);
+    ++L;
+    // exact scores of the representatives of N nodes of level l -> their sort keys
+    auto exact = [&](const long long* nodes, long long N_, int l, unsigned long long* keys) {
+        for (long long o = 0; o < N_; o += kWideChunk) {
+            const int k = (int)(N_ - o < kWideChunk ? N_ - o : kWideChunk);
+            reserve_chunk((size_t)k);
+            reloc_rep_poses_kernel<<<grid_for((size_t)k, 128), 128, 0, stream>>>(ga, nodes + o, k, l, reloc_poses.p);
+            pose_score_launch(true, fit_grid.view(), reloc_coarse.p, (int)m, reloc_poses.p, k, c.max_range, reloc_part_sum.p, reloc_part_cnt.p, stream);
+            pose_score_reduce_kernel<<<grid_for((size_t)k, 128), 128, 0, stream>>>(reloc_part_sum.p, reloc_part_cnt.p, k, (int)tiles, (int)m, c.max_range,
+                                                                                   nullptr, nullptr, reloc_score.p, keys + o, reloc_idx.p);
+            L += 3;
+        }
+        evals += N_;
+    };
+    if (ls > 0) {
+        rc = lattice_for(c.max_range, &W);
+        if (rc != FLS_OK) return rc;
+        // U: the nr-th smallest score of the start level's representatives
+        wide_key.reserve((size_t)N * 2);
+        exact(wide_nodes.p, N, ls, wide_key.p);
+        cub_pass(scratch.cub_tmp, [&](void* tmp, size_t& bytes) {
+            return cub::DeviceRadixSort::SortKeys(tmp, bytes, wide_key.p, wide_key.p + N, (int)N, 0, 64, stream);
+        });
+        ++L;
+        wide_u.reserve(1);
+        FLS_CUDA(cudaMemcpyAsync(wide_u.p, wide_key.p + N + nr - 1, sizeof(unsigned long long), cudaMemcpyDeviceToDevice, stream));
+        // the slack's float terms (derivation above): tau, the largest translation coordinate of any leaf
+        const double tau = std::fmax(std::fmax(std::fabs(ga.t[0]), std::fabs(ga.t[1])) + gr.I * ga.xy_step, std::fabs(ga.t[2]));
+        BoundArgs ba{};
+        ba.lat = {lat_v.p, lat.nx, lat.ny, lat.nz, lat.ox, lat.oy, lat.oz, lat.h, 1.0 / lat.h, lat.q};
+        ba.g = ga;
+        wide_pts.reserve(m);
+        reloc_slack_points_kernel<<<grid_for(m, 256), 256, 0, stream>>>(reloc_coarse.p, (int)m, ga, wide_pts.p);
+        ++L;
+        ba.src = wide_pts.p;
+        ba.n = (int)m;
+        ba.n_tiles = (int)tiles;
+        ba.eps0 = 32.0 * kU * tau + 8.0 * kU * std::sqrt((double)c.max_range);
+        ba.eps1 = 32.0 * kU;
+        ba.max_range = c.max_range;
+        for (int l = ls; l >= 1; --l) {
+            wide_count.reserve((size_t)N * 2);
+            int* cnt = wide_count.p;
+            int* off = wide_count.p + N;
+            for (long long o = 0; o < N; o += kWideChunk) {
+                const int k = (int)(N - o < kWideChunk ? N - o : kWideChunk);
+                reserve_chunk((size_t)k);
+                ba.nodes = wide_nodes.p + o;
+                ba.N = k;
+                ba.level = l;
+                ba.part = reloc_part_sum.p;
+                const dim3 grid((unsigned)((k + kCoarsePoses - 1) / kCoarsePoses), (unsigned)(tiles < 65535 ? tiles : 65535));
+                reloc_bound_kernel<<<grid, kScoreBlock, 0, stream>>>(ba);
+                reloc_keep_kernel<<<grid_for((size_t)k, 128), 128, 0, stream>>>(reloc_part_sum.p, k, (int)tiles, (int)m, wide_u.p, wide_nodes.p + o, l, nx,
+                                                                                 nk, cnt + o);
+                L += 2;
+            }
+            evals += N;
+            wide_levels.push_back(N);
+            cub_pass(scratch.cub_tmp, [&](void* tmp, size_t& bytes) { return cub::DeviceScan::ExclusiveSum(tmp, bytes, cnt, off, (int)N, stream); });
+            int last[2];
+            FLS_CUDA(cudaMemcpyAsync(last, cnt + N - 1, sizeof(int), cudaMemcpyDeviceToHost, stream));
+            FLS_CUDA(cudaMemcpyAsync(last + 1, off + N - 1, sizeof(int), cudaMemcpyDeviceToHost, stream));
+            FLS_CUDA(cudaStreamSynchronize(stream));
+            ++W;
+            ++L;
+            const long long next = (long long)last[0] + last[1];
+            if (next > kWideCap) {
+                set_last_error("fls_relocalize_wide: " + std::to_string(next) + " nodes survive at level " + std::to_string(l - 1));
+                out->gpu_launches = L + launches;
+                out->host_waits = W;
+                return FLS_ERR_CAPACITY;
+            }
+            wide_next.reserve((size_t)next);
+            reloc_children_kernel<<<grid_for((size_t)N, 128), 128, 0, stream>>>(wide_nodes.p, cnt, off, (int)N, l, nx, nk, wide_next.p);
+            ++L;
+            std::swap(wide_nodes.p, wide_next.p);
+            std::swap(wide_nodes.cap, wide_next.cap);
+            N = next;
+        }
+    }
+    // ---- level 0: every surviving leaf scored exactly, a stable sort on (score bits, leaf index), the n best -------------------------
+    wide_key.reserve((size_t)N * 2);
+    wide_next.reserve((size_t)N * 2);
+    exact(wide_nodes.p, N, 0, wide_key.p);
+    wide_levels.push_back(N);
+    int bits = 1;
+    while ((1LL << bits) < P) ++bits;
+    unsigned long long* key2 = wide_key.p + N;
+    long long* leaf2 = wide_next.p;
+    long long* leaf3 = wide_next.p + N;
+    cub_reserve(
+        scratch.cub_tmp,
+        [&](void* tmp, size_t& bytes) {
+            return cub::DeviceRadixSort::SortPairs(tmp, bytes, (const unsigned long long*)wide_nodes.p, (unsigned long long*)leaf2, wide_key.p, key2, (int)N,
+                                                   0, bits, stream);
+        },
+        [&](void* tmp, size_t& bytes) { return cub::DeviceRadixSort::SortPairs(tmp, bytes, key2, wide_key.p, leaf2, leaf3, (int)N, 0, 64, stream); });
+    cub_run(scratch.cub_tmp, [&](void* tmp, size_t& bytes) {
+        return cub::DeviceRadixSort::SortPairs(tmp, bytes, (const unsigned long long*)wide_nodes.p, (unsigned long long*)leaf2, wide_key.p, key2, (int)N, 0,
+                                               bits, stream);
+    });
+    cub_run(scratch.cub_tmp,
+            [&](void* tmp, size_t& bytes) { return cub::DeviceRadixSort::SortPairs(tmp, bytes, key2, wide_key.p, leaf2, leaf3, (int)N, 0, 64, stream); });
+    RelocPick* d_pick = reinterpret_cast<RelocPick*>(reloc_pick.p);
+    reloc_pick_wide_kernel<<<1, kMaxBatch, 0, stream>>>(wide_key.p, leaf3, ga, nr, d_pick);
+    FLS_CUDA(cudaGetLastError());
+    L += 3;
+    RelocPick pick[kMaxBatch];
+    FLS_CUDA(cudaMemcpyAsync(pick, d_pick, sizeof(RelocPick) * (size_t)nr, cudaMemcpyDeviceToHost, stream));
+    FLS_CUDA(cudaStreamSynchronize(stream));
+    ++W;
+    if (evaluations) *evaluations = evals;
+    return reloc_refine(*this, d_scan, n, c, pick, nr, L, W, T, out, refined_T, refined_converged, refined_fitness, refined_index);
 }
 
 }  // namespace fls

@@ -225,7 +225,7 @@ class Registration:
         return bool(conv.value)
 
     # -- relocalization from a coarse pose (Localization::Init upstream) -----------------------------------
-    def _relocalize(self, call, T_guess, coarse_scores, cfg):
+    def _relocalize(self, call, T_guess, coarse_scores, cfg, wide=False):
         c = cfg if isinstance(cfg, _abi.FlsRelocCfg) else reloc_cfg(**cfg)
         k = max(1, int(c.n_refine))
         Tc = np.ascontiguousarray(np.asarray(T_guess, np.float64).T).copy()
@@ -236,15 +236,20 @@ class Registration:
         ridx = np.zeros(k, np.int64)
         cs = np.zeros(max(int(coarse_scores), 1), np.float64)
         vp = lambda a: a.ctypes.data_as(C.c_void_p)
-        check(call(C.byref(c), vp(Tc), C.byref(res), vp(rT), vp(rconv), vp(rfit), vp(ridx), vp(cs) if coarse_scores else None, int(coarse_scores)),
-              "fls_relocalize")
+        evals = C.c_int64(-1)
+        if wide:
+            check(call(C.byref(c), vp(Tc), C.byref(res), vp(rT), vp(rconv), vp(rfit), vp(ridx), C.byref(evals)), "fls_relocalize_wide")
+        else:
+            check(call(C.byref(c), vp(Tc), C.byref(res), vp(rT), vp(rconv), vp(rfit), vp(ridx), vp(cs) if coarse_scores else None, int(coarse_scores)),
+                  "fls_relocalize")
         n = res.n_refined
         ncs = min(int(coarse_scores), int(res.n_hypotheses)) if res.n_refined else 0
-        return RelocResult(T=Tc.T.copy(), accepted=bool(res.accepted), converged=bool(res.converged), fitness=float(res.fitness),
+        r = RelocResult(T=Tc.T.copy(), accepted=bool(res.accepted), converged=bool(res.converged), fitness=float(res.fitness),
                            coarse_score=float(res.coarse_score), n_hypotheses=int(res.n_hypotheses), best_hypothesis=int(res.best_hypothesis),
                            best_rank=int(res.best_rank), n_refined=int(n), host_waits=int(res.host_waits), gpu_launches=int(res.gpu_launches),
                            refined_T=np.transpose(rT[:n], (0, 2, 1)).copy(), refined_converged=rconv[:n].astype(bool), refined_fitness=rfit[:n].copy(),
                            refined_index=ridx[:n].copy(), coarse_scores=cs[:ncs].copy() if coarse_scores else None)
+        return (r, int(evals.value)) if wide else r
 
     def relocalize(self, cloud_or_cluster, T_guess, coarse_scores: int = 0, cfg=None, **kw) -> RelocResult:
         """fls_relocalize: score an x-y-yaw grid of hypotheses around T_guess (4,4), refine the best n_refine in one batch Match and
@@ -261,6 +266,28 @@ class Registration:
         """relocalize with a device-resident packed float4 scan (it must stay valid until the next Match, as in match_device)."""
         return self._relocalize(lambda *a: lib().fls_relocalize_device(self._h, C.c_void_p(int(d_ptr)) if d_ptr else None, int(n), *a), T_guess,
                                 coarse_scores, cfg if cfg is not None else kw)
+
+    def relocalize_wide(self, cloud_or_cluster, T_guess, cfg=None, **kw):
+        """fls_relocalize_wide: relocalize's results on the same grid without its 2^20 cap (up to 2^31 hypotheses), searched by exact
+        branch and bound.  Returns (RelocResult without coarse_scores, the number of pose evaluations the search ran)."""
+        c = cloud_or_cluster
+        if isinstance(c, PointcloudCluster):
+            c = c.ordered_cloud if self.cfg.method == _abi.FLS_NDT else c.planar_cloud
+        p, n, s, keep = _cloud(c)
+        return self._relocalize(lambda *a: lib().fls_relocalize_wide(self._h, p, n, s, *a), T_guess, 0, cfg if cfg is not None else kw, wide=True)
+
+    def relocalize_wide_device(self, d_ptr: int, n: int, T_guess, cfg=None, **kw):
+        """relocalize_wide with a device-resident packed float4 scan (it must stay valid until the next Match)."""
+        return self._relocalize(lambda *a: lib().fls_relocalize_wide_device(self._h, C.c_void_p(int(d_ptr)) if d_ptr else None, int(n), *a), T_guess, 0,
+                                cfg if cfg is not None else kw, wide=True)
+
+    def relocalize_wide_levels(self) -> list:
+        """fls_relocalize_wide_levels: the nodes the last relocalize_wide reached per level, from its start level down to 0."""
+        buf = (C.c_int64 * 64)()
+        n = lib().fls_relocalize_wide_levels(self._h, buf, 64)
+        if n < 0:
+            check(n, "fls_relocalize_wide_levels")
+        return [int(v) for v in buf[:n]]
 
     # -- localization-mode map path (Localization::LoadLocalMap upstream) ---------------------------------
     def set_global_map(self, cloud: np.ndarray) -> None:

@@ -97,6 +97,23 @@ public:
         return res.accepted != 0;
     }
 
+    // Relocalize over a whole local map (fls_relocalize_wide): the same grid and the same result without the 2^20 hypothesis cap,
+    // searched by exact branch and bound; for a click tens of metres or any angle off.
+    bool RelocalizeWide(const PointcloudClusterPtr& source_cloud_cluster, Mat4d& T, const fls_reloc_cfg& cfg, float* fitness) {
+        const auto& cloud = method_ == FLS_NDT ? source_cloud_cluster->ordered_cloud_.points : source_cloud_cluster->planar_cloud_.points;
+        fls_reloc_result res;
+        int64_t evaluations = 0;
+        const int rc = fls_relocalize_wide(handle_, cloud.data(), cloud.size(), sizeof(PCLPointXYZI), &cfg, T.data(), &res, nullptr, nullptr, nullptr,
+                                           nullptr, &evaluations);
+        if (fitness) *fitness = rc == FLS_OK ? res.fitness : FloatNaN;
+        if (rc != FLS_OK) {
+            LOG(WARNING) << "fls_relocalize_wide: " << fls_strerror(rc) << " " << fls_last_error();
+            return false;
+        }
+        DLOG(INFO) << "B200 RelocalizeWide hypotheses=" << res.n_hypotheses << " evaluations=" << evaluations << " fitness=" << res.fitness;
+        return res.accepted != 0;
+    }
+
     // Convenience: the factory branch a maintainer adds to FrontEnd::InitMatcher / Localization::InitMatcher.
     static std::shared_ptr<RegistrationInterface> Create(const std::string& mode, const fls_config& overrides_applied) {
         return std::make_shared<B200Registration>(overrides_applied);

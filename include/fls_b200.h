@@ -29,6 +29,8 @@
  *                                 LoopClosure::GetSubMap (src/slam/loop_closure.cpp:179-231)
  *   fls_relocalize / _device   <- Localization::Init's Match + GetFitnessScore(2.0) < 1.0 (src/slam/localization.cpp:135-140),
  *                                 searching an x-y-yaw grid around the given pose
+ *   fls_relocalize_wide /      <- the same over a whole local map (up to 2^31 hypotheses), by exact branch and bound
+ *   _wide_device
  *
  * Conventions
  *   * Points are read from caller memory as {float x, y, z, <pad>, intensity ...} records `stride_bytes`
@@ -62,7 +64,7 @@ typedef enum {
     FLS_ERR_NO_DEVICE = -3,     /* no sm_90 device visible — the product has NO CPU fallback */
     FLS_ERR_UNSUPPORTED = -4,   /* method / mode not implemented by this build */
     FLS_ERR_NO_MAP = -5,        /* Match before AddCloudToLocalMap (reference: CHECK(!grids_.empty())) */
-    FLS_ERR_CAPACITY = -6,      /* voxel count would exceed the LRU capacity (eviction not emulated on device) */
+    FLS_ERR_CAPACITY = -6,      /* voxel count would exceed the LRU capacity (eviction not emulated on device); also fls_relocalize_wide */
     FLS_ERR_TOO_FEW_POINTS = -7 /* reference: CHECK_GT(ordered_cloud_.size(), 10u) icp_optimized.h:55 */
 } fls_status;
 
@@ -276,6 +278,37 @@ int fls_relocalize(fls_handle* h, const void* scan, size_t n, size_t stride_byte
 int fls_relocalize_device(fls_handle* h, const void* d_scan, size_t n, const fls_reloc_cfg* cfg, double T_colmajor[16], fls_reloc_result* out,
                           double* refined_T, int32_t* refined_converged, float* refined_fitness, int64_t* refined_index, double* coarse_scores,
                           size_t coarse_cap);
+
+/* Relocalization over a whole local map: the hypotheses of fls_relocalize's grid searched by exact branch and bound on the device.
+ * It takes the same fls_reloc_cfg, defines the same grid and returns what fls_relocalize would return for that cfg without its
+ * 2^20 cap: T, every field of *out, and the refined arrays (the same n_refine hypotheses in the same order, hence the same Match,
+ * fitness and choice).  In place of coarse_scores, *evaluations (optional) receives the number of pose evaluations the search ran:
+ * lower bounds plus exact scores, against out->n_hypotheses for the exhaustive search.
+ *
+ * The search.  Aligned blocks of 2^l x 2^l x 2^l hypotheses (x, y, yaw indices) are evaluated at one representative each, from the
+ * lowest level with at most 2^20 blocks down to single hypotheses; all representatives of that start level are scored exactly,
+ * and U is the n_refine-th smallest of those scores.  A block is dropped when a lower bound on the coarse score of every hypothesis
+ * in it exceeds U by a relative 1e-6: the score at the representative, with each point's distance to the fit cloud read from a
+ * lower-bound distance lattice and reduced by how far the block's other hypotheses can move that point (plus fp32 rounding).  Every
+ * hypothesis that scores at most U survives, so the selection is exact, ties included.  Grids of at most 2^20 hypotheses start at
+ * single hypotheses and score every one, as fls_relocalize does.  DESIGN.md §3.11 gives the bound and the lattice.
+ *
+ * Caps: at most 2^31 hypotheses and floor(xy_radius / xy_step) <= 32767 (else FLS_ERR_INVALID_ARG).  FLS_ERR_CAPACITY when more
+ * than 2^23 blocks survive one level, before any Match runs (T, the map and fls_fitness are then as before the call): a map and scan
+ * so featureless that most of a very large grid cannot be told apart from the best.  The lattice is built by the first call past 2^20
+ * hypotheses after the map or max_range changes (two more waits); its pitch is sqrt(max_range) / 4, coarser when the map's bounding box would exceed
+ * 2^25 cells.  Waits: those of fls_relocalize, plus one per level above the start of the descent; launches grow with the number of
+ * levels and of 2^20-block chunks.  Everything else — plug-ins, modes, argument checks, the empty scan, the state left for
+ * fls_fitness and Match — is fls_relocalize's. */
+int fls_relocalize_wide(fls_handle* h, const void* scan, size_t n, size_t stride_bytes, const fls_reloc_cfg* cfg, double T_colmajor[16],
+                        fls_reloc_result* out, double* refined_T, int32_t* refined_converged, float* refined_fitness, int64_t* refined_index,
+                        int64_t* evaluations);
+int fls_relocalize_wide_device(fls_handle* h, const void* d_scan, size_t n, const fls_reloc_cfg* cfg, double T_colmajor[16], fls_reloc_result* out,
+                               double* refined_T, int32_t* refined_converged, float* refined_fitness, int64_t* refined_index, int64_t* evaluations);
+/* The nodes the last fls_relocalize_wide call on h reached at each level, from its start level down to single hypotheses (the start
+ * level: all its blocks; below: the children of the blocks kept one level up; 0 levels after an empty scan or a failed call before
+ * the search).  Writes min(capacity, levels) values and returns the number of levels, or FLS_ERR_INVALID_ARG. */
+int fls_relocalize_wide_levels(const fls_handle* h, int64_t* nodes, int capacity);
 
 /* Device-side results for a consumer that lives on the GPU (the per-batch NCCL all-gather of poses, SURVEY.md §8e): once set,
  * every Match additionally writes, for scan s of the call, 18 doubles at d_results + 18*s — the column-major Mat4d pose
