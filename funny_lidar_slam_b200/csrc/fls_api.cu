@@ -569,15 +569,15 @@ int fls_fitness(fls_handle* hh, float max_range, float* score) {
     FLS_CATCH
 }
 
-// fls_relocalize of a host scan of `host_stride` bytes per record or (0) a device scan: the checks that need no device first, then the
-// plug-ins and modes without a batch Match in localization mode, which answer with no side effect
-static int relocalize(fls_handle* hh, const void* scan, size_t n, size_t host_stride, const fls_reloc_cfg* cfg, double* T, fls_reloc_result* out,
-                      double* refined_T, int32_t* refined_converged, float* refined_fitness, int64_t* refined_index, double* coarse_scores,
-                      size_t coarse_cap) {
+// fls_relocalize (wide: fls_relocalize_wide) of a host scan of `host_stride` bytes per record or (0) a device scan: the checks that need
+// no device first, then the plug-ins and modes without a batch Match in localization mode, which answer with no side effect
+static int relocalize(fls_handle* hh, bool wide, const void* scan, size_t n, size_t host_stride, const fls_reloc_cfg* cfg, double* T,
+                      fls_reloc_result* out, double* refined_T, int32_t* refined_converged, float* refined_fitness, int64_t* refined_index,
+                      double* coarse_scores, size_t coarse_cap, int64_t* evaluations) {
     Handle* h = reinterpret_cast<Handle*>(hh);
     if (!h || !cfg || !T || !out || (!scan && n) || (coarse_cap && !coarse_scores) || n > 0x3fffffffull) return FLS_ERR_INVALID_ARG;
     fls::RelocGrid g;
-    const int v = fls::reloc_grid(*cfg, &g);
+    const int v = fls::reloc_grid(*cfg, &g, wide);
     if (v != FLS_OK) return v;
     if (!h->cfg.localization_mode || (h->cfg.method != FLS_P2PLANE_IVOX && h->cfg.method != FLS_NDT)) return FLS_ERR_UNSUPPORTED;
     if (h->plugin->batch_pending()) return FLS_ERR_INVALID_ARG;  // one batch in flight per handle (fls_match_batch_begin)
@@ -585,7 +585,8 @@ static int relocalize(fls_handle* hh, const void* scan, size_t n, size_t host_st
     FLS_TRY
     h->begin_call();
     const float4* d = host_stride ? h->upload(scan, n, host_stride, h->src) : static_cast<const float4*>(scan);
-    return h->relocalize(d, n, *cfg, g, T, out, refined_T, refined_converged, refined_fitness, refined_index, coarse_scores, coarse_cap);
+    return h->relocalize(d, n, *cfg, g, wide, T, out, refined_T, refined_converged, refined_fitness, refined_index, coarse_scores, coarse_cap,
+                         evaluations);
     FLS_CATCH
 }
 
@@ -593,50 +594,32 @@ int fls_relocalize(fls_handle* hh, const void* scan, size_t n, size_t stride, co
                    double* refined_T, int32_t* refined_converged, float* refined_fitness, int64_t* refined_index, double* coarse_scores,
                    size_t coarse_cap) {
     if (!stride_ok(stride)) return FLS_ERR_INVALID_ARG;
-    return relocalize(hh, scan, n, stride, cfg, T, out, refined_T, refined_converged, refined_fitness, refined_index, coarse_scores, coarse_cap);
+    return relocalize(hh, false, scan, n, stride, cfg, T, out, refined_T, refined_converged, refined_fitness, refined_index, coarse_scores, coarse_cap,
+                      nullptr);
 }
 
 int fls_relocalize_device(fls_handle* hh, const void* d_scan, size_t n, const fls_reloc_cfg* cfg, double T[16], fls_reloc_result* out,
                           double* refined_T, int32_t* refined_converged, float* refined_fitness, int64_t* refined_index, double* coarse_scores,
                           size_t coarse_cap) {
-    return relocalize(hh, d_scan, n, 0, cfg, T, out, refined_T, refined_converged, refined_fitness, refined_index, coarse_scores, coarse_cap);
-}
-
-// fls_relocalize_wide of a host scan of `host_stride` bytes per record or (0) a device scan, through relocalize()'s checks
-static int relocalize_wide(fls_handle* hh, const void* scan, size_t n, size_t host_stride, const fls_reloc_cfg* cfg, double* T, fls_reloc_result* out,
-                           double* refined_T, int32_t* refined_converged, float* refined_fitness, int64_t* refined_index, int64_t* evaluations) {
-    Handle* h = reinterpret_cast<Handle*>(hh);
-    if (!h || !cfg || !T || !out || (!scan && n) || n > 0x3fffffffull) return FLS_ERR_INVALID_ARG;
-    fls::RelocGrid g;
-    const int v = fls::reloc_grid(*cfg, &g, true);
-    if (v != FLS_OK) return v;
-    if (!h->cfg.localization_mode || (h->cfg.method != FLS_P2PLANE_IVOX && h->cfg.method != FLS_NDT)) return FLS_ERR_UNSUPPORTED;
-    if (h->plugin->batch_pending()) return FLS_ERR_INVALID_ARG;
-    if (h->fit_cloud_n == 0) return FLS_ERR_NO_MAP;
-    FLS_TRY
-    h->begin_call();
-    const float4* d = host_stride ? h->upload(scan, n, host_stride, h->src) : static_cast<const float4*>(scan);
-    return h->relocalize_wide(d, n, *cfg, g, T, out, refined_T, refined_converged, refined_fitness, refined_index, evaluations);
-    FLS_CATCH
+    return relocalize(hh, false, d_scan, n, 0, cfg, T, out, refined_T, refined_converged, refined_fitness, refined_index, coarse_scores, coarse_cap,
+                      nullptr);
 }
 
 int fls_relocalize_wide(fls_handle* hh, const void* scan, size_t n, size_t stride, const fls_reloc_cfg* cfg, double T[16], fls_reloc_result* out,
                         double* refined_T, int32_t* refined_converged, float* refined_fitness, int64_t* refined_index, int64_t* evaluations) {
     if (!stride_ok(stride)) return FLS_ERR_INVALID_ARG;
-    return relocalize_wide(hh, scan, n, stride, cfg, T, out, refined_T, refined_converged, refined_fitness, refined_index, evaluations);
+    return relocalize(hh, true, scan, n, stride, cfg, T, out, refined_T, refined_converged, refined_fitness, refined_index, nullptr, 0, evaluations);
 }
 
 int fls_relocalize_wide_device(fls_handle* hh, const void* d_scan, size_t n, const fls_reloc_cfg* cfg, double T[16], fls_reloc_result* out,
                                double* refined_T, int32_t* refined_converged, float* refined_fitness, int64_t* refined_index, int64_t* evaluations) {
-    return relocalize_wide(hh, d_scan, n, 0, cfg, T, out, refined_T, refined_converged, refined_fitness, refined_index, evaluations);
+    return relocalize(hh, true, d_scan, n, 0, cfg, T, out, refined_T, refined_converged, refined_fitness, refined_index, nullptr, 0, evaluations);
 }
 
 int fls_relocalize_wide_levels(const fls_handle* hh, int64_t* nodes, int capacity) {
     const Handle* h = reinterpret_cast<const Handle*>(hh);
     if (!h || capacity < 0 || (capacity && !nodes)) return FLS_ERR_INVALID_ARG;
-    const int n = (int)h->wide_levels.size();
-    for (int i = 0; i < n && i < capacity; ++i) nodes[i] = h->wide_levels[i];
-    return n;
+    return h->relocalize_levels(nodes, capacity);
 }
 
 int fls_set_result_buffer_device(fls_handle* hh, double* d_results, size_t capacity_scans) {

@@ -73,6 +73,10 @@ struct RelocGrid {
 // checks a relocalization configuration and sizes its grid (FLS_ERR_INVALID_ARG: see fls_relocalize, and fls_relocalize_wide's caps
 // when wide)
 int reloc_grid(const fls_reloc_cfg& c, RelocGrid* g, bool wide = false);
+struct Reloc;  // relocalization's state on a handle (fls_reloc.cu)
+struct RelocFree {
+    void operator()(Reloc* r) const;
+};
 
 struct Handle {
     fls_config cfg;
@@ -127,26 +131,8 @@ struct Handle {
     SearchGrid fit_grid;
     DevBuf<double> fit_pose, fit_part_sum, fit_out;
     DevBuf<unsigned> fit_part_cnt, fit_cnt;
-    // relocalization: the coarse cloud, the hypotheses, their partials, scores and sort keys / indices (in and out), the picks
-    DevBuf<float4> reloc_coarse;
-    DevBuf<double> reloc_poses, reloc_part_sum, reloc_score;
-    DevBuf<unsigned> reloc_part_cnt, reloc_idx;
-    DevBuf<unsigned long long> reloc_key;
-    DevBuf<unsigned char> reloc_pick;
-    // fls_relocalize_wide: the lower-bound distance lattice of the fit cloud (fls_reloc.cu; rebuilt like fit_grid), the node lists of
-    // a level and the next, sort keys, child counts and offsets, and U's sort key
-    struct {
-        int nx = 0, ny = 0, nz = 0;
-        double ox = 0, oy = 0, oz = 0, h = 0, q = 0;  // origin, pitch, quantum
-    } lat;
-    DevBuf<unsigned short> lat_v;
-    unsigned long long lat_version = ~0ull;
-    float lat_range = -1.f;
-    DevBuf<float4> wide_pts;  // the coarse cloud with each point's node-independent slack term
-    DevBuf<long long> wide_nodes, wide_next;
-    std::vector<long long> wide_levels;  // nodes evaluated per level of the last call, from its start level down to 0
-    DevBuf<unsigned long long> wide_key, wide_u;
-    DevBuf<int> wide_count;
+    // relocalization's buffers, lattice and level record (fls_reloc.cu), made by its first call
+    std::unique_ptr<Reloc, RelocFree> reloc;
 
     explicit Handle(const fls_config& c);
     ~Handle();
@@ -215,13 +201,12 @@ struct Handle {
     int fitness(float max_range, float* score);
     int fit_grid_for(float max_range, int* waits);  // (re)builds fit_grid for max_range when needed; counts its wait
     void fitness_enqueue(const float4* d_src, size_t n, int P, float max_range);  // P poses of fit_pose -> fit_out / fit_cnt
-    // fls_relocalize on a device scan (the call has begun; g from reloc_grid)
-    int relocalize(const float4* d_scan, size_t n, const fls_reloc_cfg& c, const RelocGrid& g, double* T, fls_reloc_result* out, double* refined_T,
-                   int32_t* refined_converged, float* refined_fitness, int64_t* refined_index, double* coarse_scores, size_t coarse_cap);
-    int lattice_for(float max_range, int* waits);  // (re)builds the lattice of the fit cloud for max_range when needed; counts its wait
-    // fls_relocalize_wide on a device scan (the call has begun; g from reloc_grid(wide))
-    int relocalize_wide(const float4* d_scan, size_t n, const fls_reloc_cfg& c, const RelocGrid& g, double* T, fls_reloc_result* out, double* refined_T,
-                        int32_t* refined_converged, float* refined_fitness, int64_t* refined_index, int64_t* evaluations);
+    // fls_relocalize, or fls_relocalize_wide when wide, on a device scan (the call has begun; g from reloc_grid(c, &g, wide)); coarse_scores
+    // and coarse_cap are fls_relocalize's, evaluations fls_relocalize_wide's
+    int relocalize(const float4* d_scan, size_t n, const fls_reloc_cfg& c, const RelocGrid& g, bool wide, double* T, fls_reloc_result* out, double* refined_T,
+                   int32_t* refined_converged, float* refined_fitness, int64_t* refined_index, double* coarse_scores, size_t coarse_cap,
+                   int64_t* evaluations);
+    int relocalize_levels(int64_t* nodes, int capacity) const;  // fls_relocalize_wide_levels (0 levels before a wide call)
 
     // localization-mode map path (fls_localmap.cu): resident global map, +-100 m crop around the pose when needed
     DevBuf<float4> global_map;

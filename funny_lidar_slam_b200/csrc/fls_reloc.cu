@@ -1,12 +1,14 @@
-// fls_reloc.cu — GetFitnessScore of many poses of one cloud, and relocalization from a coarse pose (fls_relocalize).
+// fls_reloc.cu — GetFitnessScore of many poses of one cloud, and relocalization from a coarse pose (fls_relocalize, and its exact
+// branch and bound over a whole local map, fls_relocalize_wide).
 //
-// pose_score_kernel is the one fitness path of the library: for P poses of one cloud it returns, per pose, the sum of the fp32 squared
-// 1-NN distances <= max_range (in fp64) and how many there are.  A CTA stages a tile of the cloud in shared memory once and sweeps
-// PPC poses over it; each pose's partial of that tile is reduced in a fixed tree, written to its own slot, and a second kernel adds
-// the tiles of every pose in index order.  No atomics: every result is reproducible bit for bit and independent of scheduling.
-// GetFitnessScore (Handle::fitness) is its one-pose-per-CTA form; relocalization scores its whole hypothesis grid with 8 poses per
-// CTA, keeps the best by a stable radix sort of the scores, refines them with the plug-in's batch Match and scores the refined poses
-// with the same one-pose-per-CTA form that a later fls_fitness runs.
+// pose_score_kernel sweeps P poses over one cloud: a CTA stages a tile of the cloud in shared memory once and sweeps PPC poses over
+// it; each pose's partial of that tile is reduced in a fixed tree and written to its own slot.  What a point adds is its term's:
+// FitTerm makes it the one fitness path of the library (per pose the sum of the fp32 squared 1-NN distances <= max_range, in fp64,
+// and how many there are; a second kernel adds the tiles of every pose in index order), BoundTerm the lower bound of the branch and
+// bound.  No atomics: every result is reproducible bit for bit and independent of scheduling.  GetFitnessScore (Handle::fitness) is
+// the one-pose-per-CTA form; relocalization scores hypotheses with 8 poses per CTA, keeps the best by a stable radix sort of the
+// scores, refines them with the plug-in's batch Match and scores the refined poses with the same one-pose-per-CTA form that a later
+// fls_fitness runs.
 #include <cfloat>
 #include <cmath>
 #include <cstring>
@@ -59,31 +61,29 @@ __device__ __forceinline__ bool grid_nn1(const GridView& g, float qx, float qy, 
     return best_j != 0xffffffffu;
 }
 
-struct ScoreArgs {
-    GridView g;
+// A term of pose_score_kernel: pose(p) reads what slot p (< P) needs, add(pose, point, sum, cnt) adds one point's contribution;
+// only a term with kCounts counts points, and only its kernel keeps counts in shared memory.
+template <class Term>
+struct SweepArgs {
+    Term t;
     const float4* __restrict__ src;
-    int n;
-    const double* __restrict__ poses;  // [P][12]: row-major R, then t (fp64; cast to float here, as TransformPointCloud does)
-    int P;
-    float max_range;
-    int n_tiles;
-    double* __restrict__ part_sum;  // [P][n_tiles]
-    unsigned* __restrict__ part_cnt;
+    int n, P, n_tiles;
+    double* __restrict__ part_sum;    // [P][n_tiles]
+    unsigned* __restrict__ part_cnt;  // [P][n_tiles] when Term::kCounts
 };
 
-// grid (ceil(P / PPC), min(n_tiles, 65535)): CTA (x, y) scores poses x*PPC .. x*PPC+PPC-1 on tiles y, y + gridDim.y, ... of TILE
+// grid (ceil(P / PPC), min(n_tiles, 65535)): CTA (x, y) sweeps poses x*PPC .. x*PPC+PPC-1 over tiles y, y + gridDim.y, ... of TILE
 // points each, one partial per (pose, tile)
-template <int PPC, int TILE>
-__global__ void __launch_bounds__(kScoreBlock) pose_score_kernel(ScoreArgs a) {
+template <int PPC, int TILE, class Term>
+__global__ void __launch_bounds__(kScoreBlock) pose_score_kernel(SweepArgs<Term> a) {
     constexpr int TPP = kScoreBlock / PPC;  // threads per pose
     __shared__ float4 s_pts[TILE];
     __shared__ double s_sum[kScoreBlock];
-    __shared__ unsigned s_cnt[kScoreBlock];
+    __shared__ unsigned s_cnt[Term::kCounts ? kScoreBlock : 1];
     const int sub = threadIdx.x % TPP;
     const int pose = blockIdx.x * PPC + threadIdx.x / TPP;
-    float r[12];
-#pragma unroll
-    for (int k = 0; k < 12; ++k) r[k] = pose < a.P ? (float)__ldg(a.poses + (size_t)pose * 12 + k) : 0.f;
+    typename Term::Pose q;
+    if (pose < a.P) q = a.t.pose(pose);
     for (int tile = blockIdx.y; tile < a.n_tiles; tile += gridDim.y) {  // uniform across the CTA
         const size_t base = (size_t)tile * TILE;
         const int m = (int)min((size_t)TILE, (size_t)a.n - base);
@@ -93,42 +93,62 @@ __global__ void __launch_bounds__(kScoreBlock) pose_score_kernel(ScoreArgs a) {
         __syncthreads();
         if (pose < a.P) {
 #pragma unroll 1
-            for (int i = sub; i < m; i += TPP) {
-                const float4 sp = s_pts[i];
-                const float qx = xform_row_f(r[0], r[1], r[2], r[9], sp.x, sp.y, sp.z);
-                const float qy = xform_row_f(r[3], r[4], r[5], r[10], sp.x, sp.y, sp.z);
-                const float qz = xform_row_f(r[6], r[7], r[8], r[11], sp.x, sp.y, sp.z);
-                float d2;
-                unsigned j, nc, nh;
-                if (grid_nn1(a.g, qx, qy, qz, d2, j, nc, nh) && d2 <= a.max_range) {
-                    sum += (double)d2;
-                    cnt += 1;
-                }
-            }
+            for (int i = sub; i < m; i += TPP) a.t.add(q, s_pts[i], sum, cnt);
         }
         s_sum[threadIdx.x] = sum;
-        s_cnt[threadIdx.x] = cnt;
+        if constexpr (Term::kCounts) s_cnt[threadIdx.x] = cnt;
         __syncthreads();  // also: every read of s_pts is done before the next tile overwrites it
 #pragma unroll
         for (int o = TPP / 2; o > 0; o >>= 1) {  // fixed tree inside each pose's group of threads
             if (sub < o) {
                 s_sum[threadIdx.x] += s_sum[threadIdx.x + o];
-                s_cnt[threadIdx.x] += s_cnt[threadIdx.x + o];
+                if constexpr (Term::kCounts) s_cnt[threadIdx.x] += s_cnt[threadIdx.x + o];
             }
             __syncthreads();
         }
         if (sub == 0 && pose < a.P) {
             a.part_sum[(size_t)pose * a.n_tiles + tile] = s_sum[threadIdx.x];
-            a.part_cnt[(size_t)pose * a.n_tiles + tile] = s_cnt[threadIdx.x];
+            if constexpr (Term::kCounts) a.part_cnt[(size_t)pose * a.n_tiles + tile] = s_cnt[threadIdx.x];
         }
     }
 }
 
-// per pose: the tiles in order -> {sum, count}; with keys: also the coarse score, its sort key (the bits of a non-negative double
-// order as the values do) and the identity permutation
+// GetFitnessScore's term: the pose from a row-major R | t table; a point's fp32 squared 1-NN distance, added and counted when it is
+// within max_range
+struct FitTerm {
+    static constexpr bool kCounts = true;
+    GridView g;
+    const double* __restrict__ poses;  // [P][12]: row-major R, then t (fp64; cast to float here, as TransformPointCloud does)
+    float max_range;
+    struct Pose {
+        float r[12];
+    };
+    __device__ __forceinline__ Pose pose(int p) const {
+        Pose q;
+#pragma unroll
+        for (int k = 0; k < 12; ++k) q.r[k] = (float)__ldg(poses + (size_t)p * 12 + k);
+        return q;
+    }
+    __device__ __forceinline__ void add(const Pose& q, float4 sp, double& sum, unsigned& cnt) const {
+        const float* r = q.r;
+        const float qx = xform_row_f(r[0], r[1], r[2], r[9], sp.x, sp.y, sp.z);
+        const float qy = xform_row_f(r[3], r[4], r[5], r[10], sp.x, sp.y, sp.z);
+        const float qz = xform_row_f(r[6], r[7], r[8], r[11], sp.x, sp.y, sp.z);
+        float d2;
+        unsigned j, nc, nh;
+        if (grid_nn1(g, qx, qy, qz, d2, j, nc, nh) && d2 <= max_range) {
+            sum += (double)d2;
+            cnt += 1;
+        }
+    }
+};
+
+// per pose: the tiles in order -> {sum, count} (sum_out), or the coarse score's sort key (the bits of a non-negative double order as
+// the values do) and, when ids is given, the id of the pose's node (nodes null: base + p), which at level 0 is its leaf
 __global__ void pose_score_reduce_kernel(const double* __restrict__ part_sum, const unsigned* __restrict__ part_cnt, int P, int n_tiles, int m,
-                                         float max_range, double* __restrict__ sum_out, unsigned* __restrict__ cnt_out, double* __restrict__ score,
-                                         unsigned long long* __restrict__ key, unsigned* __restrict__ idx) {
+                                         float max_range, double* __restrict__ sum_out, unsigned* __restrict__ cnt_out,
+                                         unsigned long long* __restrict__ key, const long long* __restrict__ nodes, long long base,
+                                         unsigned long long* __restrict__ ids) {
     const int p = blockIdx.x * blockDim.x + threadIdx.x;
     if (p >= P) return;
     double s = 0.0;
@@ -140,13 +160,11 @@ __global__ void pose_score_reduce_kernel(const double* __restrict__ part_sum, co
     if (sum_out) {
         sum_out[p] = s;
         cnt_out[p] = c;
+        return;
     }
-    if (score) {
-        const double v = (s + (double)(m - (int)c) * (double)max_range) / (double)m;
-        score[p] = v;
-        key[p] = (unsigned long long)__double_as_longlong(v);
-        idx[p] = (unsigned)p;
-    }
+    const double v = (s + (double)(m - (int)c) * (double)max_range) / (double)m;
+    key[p] = (unsigned long long)__double_as_longlong(v);
+    if (ids) ids[p] = (unsigned long long)(nodes ? nodes[p] : base + p);
 }
 
 // the hypothesis grid of fls_relocalize (fls_b200.h): pose p in fp64, row-major R | t
@@ -172,40 +190,32 @@ __device__ __forceinline__ void reloc_leaf_pose(const RelocGridArgs& g, long lon
     o[10] = __dadd_rn(g.t[1], __dmul_rn((double)(jy - g.I), g.xy_step));
     o[11] = g.t[2];
 }
-__global__ void reloc_poses_kernel(RelocGridArgs g, double* __restrict__ poses) {
-    const int p = blockIdx.x * blockDim.x + threadIdx.x;
-    if (p >= g.P) return;
-    reloc_leaf_pose(g, p, poses + (size_t)p * 12);
-}
-
 // the selected hypotheses: {index, coarse score, pose} records, read back in one copy
 struct RelocPick {
     long long index;
     double score;
     double pose[12];
 };
-__global__ void reloc_pick_kernel(const unsigned* __restrict__ idx_sorted, const double* __restrict__ score, const double* __restrict__ poses, int n,
-                                  RelocPick* __restrict__ out) {
+// the n best after the sort: {leaf index, score, pose}
+__global__ void reloc_pick_kernel(const unsigned long long* __restrict__ key_sorted, const unsigned long long* __restrict__ leaf_sorted,
+                                  RelocGridArgs g, int n, RelocPick* __restrict__ out) {
     const int r = threadIdx.x;
     if (r >= n) return;
-    const unsigned i = idx_sorted[r];
-    out[r].index = i;
-    out[r].score = score[i];
-    for (int k = 0; k < 12; ++k) out[r].pose[k] = poses[(size_t)i * 12 + k];
+    out[r].index = (long long)leaf_sorted[r];
+    out[r].score = __longlong_as_double((long long)key_sorted[r]);
+    reloc_leaf_pose(g, (long long)leaf_sorted[r], out[r].pose);
 }
 
 constexpr int kFitTile = kScoreBlock;  // GetFitnessScore: one pose per CTA, one point per thread
-constexpr int kCoarseTile = 2048;      // the hypothesis grid: 8 poses per CTA over 2048 staged points (32 KB)
+constexpr int kCoarseTile = 2048;      // relocalization: 8 poses per CTA over 2048 staged points (32 KB)
 constexpr int kCoarsePoses = 8;
 
-void pose_score_launch(bool coarse, const GridView& g, const float4* d_src, int n, const double* d_poses, int P, float max_range, double* part_sum,
-                       unsigned* part_cnt, cudaStream_t st) {
-    ScoreArgs a{g, d_src, n, d_poses, P, max_range, 0, part_sum, part_cnt};
-    const int tile = coarse ? kCoarseTile : kFitTile, ppc = coarse ? kCoarsePoses : 1;
-    a.n_tiles = (n + tile - 1) / tile;
+template <bool kCoarse, class Term>
+void pose_score_launch(const Term& t, const float4* d_src, int n, int P, double* part_sum, unsigned* part_cnt, cudaStream_t st) {
+    constexpr int tile = kCoarse ? kCoarseTile : kFitTile, ppc = kCoarse ? kCoarsePoses : 1;
+    const SweepArgs<Term> a{t, d_src, n, P, (n + tile - 1) / tile, part_sum, part_cnt};
     const dim3 grid((unsigned)((P + ppc - 1) / ppc), (unsigned)(a.n_tiles < 65535 ? a.n_tiles : 65535));
-    if (coarse) pose_score_kernel<kCoarsePoses, kCoarseTile><<<grid, kScoreBlock, 0, st>>>(a);
-    else pose_score_kernel<1, kFitTile><<<grid, kScoreBlock, 0, st>>>(a);
+    pose_score_kernel<ppc, tile, Term><<<grid, kScoreBlock, 0, st>>>(a);
     FLS_CUDA(cudaGetLastError());
 }
 
@@ -233,9 +243,9 @@ void Handle::fitness_enqueue(const float4* d_src, size_t n, int P, float max_ran
     fit_part_cnt.reserve((size_t)P * tiles + 1);
     fit_out.reserve((size_t)P);
     fit_cnt.reserve((size_t)P);
-    pose_score_launch(false, fit_grid.view(), d_src, (int)n, fit_pose.p, P, max_range, fit_part_sum.p, fit_part_cnt.p, stream);
+    pose_score_launch<false>(FitTerm{fit_grid.view(), fit_pose.p, max_range}, d_src, (int)n, P, fit_part_sum.p, fit_part_cnt.p, stream);
     pose_score_reduce_kernel<<<grid_for((size_t)P, 64), 64, 0, stream>>>(fit_part_sum.p, fit_part_cnt.p, P, (int)tiles, 0, max_range, fit_out.p, fit_cnt.p,
-                                                                         nullptr, nullptr, nullptr);
+                                                                         nullptr, nullptr, 0, nullptr);
     launches += 2;
 }
 
@@ -293,8 +303,8 @@ int reloc_grid(const fls_reloc_cfg& c, RelocGrid* g, bool wide) {
     return FLS_OK;
 }
 
-// The tail of both searches: the plug-in's batch Match of the nr picks, GetFitnessScore of every refined pose and Init's choice
-// rule.  L and W are the launches and waits of the call so far; out has its prelude.
+// The tail of the search: the plug-in's batch Match of the nr picks, GetFitnessScore of every refined pose and Init's choice rule.
+// L and W are the launches and waits of the call so far; out has its defaults.
 static int reloc_refine(Handle& h, const float4* d_scan, size_t n, const fls_reloc_cfg& c, const RelocPick* pick, int nr, int L, int W, double* T,
                         fls_reloc_result* out, double* refined_T, int32_t* refined_converged, float* refined_fitness, int64_t* refined_index) {
     // ---- refinement: the plug-in's batch Match of the picks, the same scan nr times ------------------------------------------------
@@ -359,80 +369,6 @@ static int reloc_refine(Handle& h, const float4* d_scan, size_t n, const fls_rel
     out->gpu_launches = L + h.launches;  // h.launches: the fitness launches since the Match
     out->host_waits = W;
     return FLS_OK;
-}
-
-// The head of both searches: out's defaults, the coarse cloud (*m points) and the fit grid, and the grid's arguments.  An empty
-// coarse cloud (*m == 0) has finished the call: nothing to score or refine, and a later fls_fitness scores the empty cloud.
-static int reloc_prelude(Handle& h, const float4* d_scan, size_t n, const fls_reloc_cfg& c, const RelocGrid& gr, const double* T,
-                         fls_reloc_result* out, int& W, size_t* m, RelocGridArgs* ga) {
-    std::memset(out, 0, sizeof(*out));
-    out->n_hypotheses = gr.P;
-    out->best_hypothesis = -1;
-    out->fitness = FLT_MAX;
-    out->coarse_score = FLT_MAX;
-    // ---- coarse cloud and the fit grid ---------------------------------------------------------------------------------------------
-    h.reloc_coarse.reserve(n + 1);
-    *m = voxel_grid_device(d_scan, n, c.coarse_leaf, h.reloc_coarse.p, h.scratch, h.stream, &h.launches, &W);
-    if (*m == 0) {
-        h.last_src = d_scan;
-        h.last_src_n = 0;
-        out->gpu_launches = h.launches;
-        out->host_waits = W;
-        return FLS_OK;
-    }
-    const int rc = h.fit_grid_for(c.max_range, &W);
-    if (rc != FLS_OK) return rc;
-    pose_rows(T, ga->R);
-    for (int k = 0; k < 3; ++k) ga->t[k] = T[12 + k];
-    ga->xy_step = gr.I ? c.xy_step : 0.0;  // an unused step may be anything
-    ga->yaw_step = gr.K ? c.yaw_step : 0.0;
-    ga->I = gr.I;
-    ga->K = gr.K;
-    ga->k0 = gr.k0;
-    ga->n_yaw = gr.n_yaw;
-    ga->P = gr.P;
-    return FLS_OK;
-}
-
-int Handle::relocalize(const float4* d_scan, size_t n, const fls_reloc_cfg& c, const RelocGrid& gr, double* T, fls_reloc_result* out, double* refined_T,
-                       int32_t* refined_converged, float* refined_fitness, int64_t* refined_index, double* coarse_scores, size_t coarse_cap) {
-    int L = 0, W = 0;  // launches and waits of the whole call
-    size_t m = 0;
-    RelocGridArgs ga;
-    const int rc = reloc_prelude(*this, d_scan, n, c, gr, T, out, W, &m, &ga);
-    if (rc != FLS_OK || m == 0) return rc;
-    // ---- the hypotheses, their coarse scores and the n_refine best -----------------------------------------------------------------
-    const int P = (int)gr.P;
-    const int nr = P < c.n_refine ? P : c.n_refine;
-    const size_t tiles = (m + kCoarseTile - 1) / kCoarseTile;
-    reloc_poses.reserve((size_t)P * 12);
-    reloc_part_sum.reserve((size_t)P * tiles);
-    reloc_part_cnt.reserve((size_t)P * tiles);
-    reloc_score.reserve((size_t)P);
-    reloc_key.reserve((size_t)P * 2);
-    reloc_idx.reserve((size_t)P * 2);
-    reloc_pick.reserve(sizeof(RelocPick) * kMaxBatch);
-    reloc_poses_kernel<<<grid_for((size_t)P, 128), 128, 0, stream>>>(ga, reloc_poses.p);
-    pose_score_launch(true, fit_grid.view(), reloc_coarse.p, (int)m, reloc_poses.p, P, c.max_range, reloc_part_sum.p, reloc_part_cnt.p, stream);
-    pose_score_reduce_kernel<<<grid_for((size_t)P, 128), 128, 0, stream>>>(reloc_part_sum.p, reloc_part_cnt.p, P, (int)tiles, (int)m, c.max_range, nullptr,
-                                                                           nullptr, reloc_score.p, reloc_key.p, reloc_idx.p);
-    // stable LSD radix sort of (score bits, index): equal scores keep index order
-    unsigned long long* keys_out = reloc_key.p + P;
-    unsigned* idx_out = reloc_idx.p + P;
-    cub_pass(scratch.cub_tmp, [&](void* tmp, size_t& bytes) {
-        return cub::DeviceRadixSort::SortPairs(tmp, bytes, reloc_key.p, keys_out, reloc_idx.p, idx_out, P, 0, 64, stream);
-    });
-    RelocPick* d_pick = reinterpret_cast<RelocPick*>(reloc_pick.p);
-    reloc_pick_kernel<<<1, kMaxBatch, 0, stream>>>(idx_out, reloc_score.p, reloc_poses.p, nr, d_pick);
-    FLS_CUDA(cudaGetLastError());
-    L += 5;
-    RelocPick pick[kMaxBatch];
-    FLS_CUDA(cudaMemcpyAsync(pick, d_pick, sizeof(RelocPick) * (size_t)nr, cudaMemcpyDeviceToHost, stream));
-    const size_t n_cs = coarse_scores ? (coarse_cap < (size_t)P ? coarse_cap : (size_t)P) : 0;
-    if (n_cs) FLS_CUDA(cudaMemcpyAsync(coarse_scores, reloc_score.p, sizeof(double) * n_cs, cudaMemcpyDeviceToHost, stream));
-    FLS_CUDA(cudaStreamSynchronize(stream));
-    ++W;
-    return reloc_refine(*this, d_scan, n, c, pick, nr, L, W, T, out, refined_T, refined_converged, refined_fitness, refined_index);
 }
 
 namespace {
@@ -508,80 +444,58 @@ __global__ void reloc_iota_kernel(long long* __restrict__ out, long long n) {
     if (i < n) out[i] = i;
 }
 
-// poses of the representatives of N nodes of level l
-__global__ void reloc_rep_poses_kernel(RelocGridArgs g, const long long* __restrict__ nodes, int N, int l, double* __restrict__ poses) {
+// poses of the representatives of N nodes of level l (nodes null: node i is base + i)
+__global__ void reloc_rep_poses_kernel(RelocGridArgs g, const long long* __restrict__ nodes, long long base, int N, int l, double* __restrict__ poses) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= N) return;
-    reloc_leaf_pose(g, node_rep(nodes[i], l, 2LL * g.I + 1, g.n_yaw).leaf, poses + (size_t)i * 12);
+    reloc_leaf_pose(g, node_rep(nodes ? nodes[i] : base + i, l, 2LL * g.I + 1, g.n_yaw).leaf, poses + (size_t)i * 12);
 }
 
-struct BoundArgs {
+// pose_score_kernel's term of LB (derived at the head of this section): the pose of a node's representative, and per point
+// min(max(0, b_i - delta_i)^2, max_range).  The points are the coarse cloud with w = |(R_guess p)_xy| rounded up
+// (reloc_slack_points_kernel).
+struct BoundTerm {
+    static constexpr bool kCounts = false;
     LatticeView lat;
     RelocGridArgs g;
-    const float4* __restrict__ src;  // the coarse cloud with w = |(R_guess p)_xy| rounded up (reloc_slack_points_kernel)
-    int n;
     const long long* __restrict__ nodes;
-    int N, level, n_tiles;
+    int level;
     double eps0, eps1, max_range;  // eps_i = eps0 + eps1 |p_i|_1
-    double* __restrict__ part;     // [N][n_tiles]
+    struct Pose {
+        float r[12];
+        double dt, dpsi, ex, ey, ez;  // delta_i's node terms, and the far corner of the lattice's box
+    };
+    __device__ __forceinline__ Pose pose(int i) const {
+        const NodeRep nr = node_rep(nodes[i], level, 2LL * g.I + 1, g.n_yaw);
+        double p[12];
+        reloc_leaf_pose(g, nr.leaf, p);
+        Pose q;
+#pragma unroll
+        for (int k = 0; k < 12; ++k) q.r[k] = (float)p[k];
+        q.dt = g.xy_step * sqrt((double)nr.hx * nr.hx + (double)nr.hy * nr.hy);
+        q.dpsi = (double)nr.hk * g.yaw_step;
+        q.ex = lat.ox + lat.nx * lat.h, q.ey = lat.oy + lat.ny * lat.h, q.ez = lat.oz + lat.nz * lat.h;
+        return q;
+    }
+    __device__ __forceinline__ void add(const Pose& q, float4 sp, double& sum, unsigned&) const {
+        const float* r = q.r;
+        const LatticeView& L = lat;
+        const double qx = xform_row_f(r[0], r[1], r[2], r[9], sp.x, sp.y, sp.z);
+        const double qy = xform_row_f(r[3], r[4], r[5], r[10], sp.x, sp.y, sp.z);
+        const double qz = xform_row_f(r[6], r[7], r[8], r[11], sp.x, sp.y, sp.z);
+        // b_i: the distance to the lattice's box, and the lattice value of the cell of q's projection onto the box (the
+        // projection onto a convex set: |q - p|^2 >= |q - q*|^2 + |q* - p|^2 for every fit point p in the box)
+        const double dx = fmax(0.0, fmax(L.ox - qx, qx - q.ex)), dy = fmax(0.0, fmax(L.oy - qy, qy - q.ey)), dz = fmax(0.0, fmax(L.oz - qz, qz - q.ez));
+        const int cx = (int)fmin(fmax((qx - L.ox) * L.inv_h, 0.0), L.nx - 1.0);
+        const int cy = (int)fmin(fmax((qy - L.oy) * L.inv_h, 0.0), L.ny - 1.0);
+        const int cz = (int)fmin(fmax((qz - L.oz) * L.inv_h, 0.0), L.nz - 1.0);
+        const double lv = (double)__ldg(L.v + ((size_t)cz * L.ny + cy) * L.nx + cx) * L.q;
+        const double b = sqrt(dx * dx + dy * dy + dz * dz + lv * lv);
+        const double delta = q.dt + q.dpsi * (double)sp.w + eps0 + eps1 * ((double)fabsf(sp.x) + (double)fabsf(sp.y) + (double)fabsf(sp.z));
+        const double e = fmax(0.0, b - delta);
+        sum += fmin(e * e, max_range);
+    }
 };
-
-// grid (ceil(N / 8), min(n_tiles, 65535)): pose_score_kernel<8, 2048>'s tiling; per (node, tile) the partial of LB
-__global__ void __launch_bounds__(kScoreBlock) reloc_bound_kernel(BoundArgs a) {
-    constexpr int PPC = kCoarsePoses, TILE = kCoarseTile, TPP = kScoreBlock / PPC;
-    __shared__ float4 s_pts[TILE];
-    __shared__ double s_sum[kScoreBlock];
-    const int sub = threadIdx.x % TPP;
-    const int node = blockIdx.x * PPC + threadIdx.x / TPP;
-    float r[12];
-    double dt = 0.0, dpsi = 0.0;
-    if (node < a.N) {
-        const NodeRep nr = node_rep(a.nodes[node], a.level, 2LL * a.g.I + 1, a.g.n_yaw);
-        double pose[12];
-        reloc_leaf_pose(a.g, nr.leaf, pose);
-#pragma unroll
-        for (int k = 0; k < 12; ++k) r[k] = (float)pose[k];
-        dt = a.g.xy_step * sqrt((double)nr.hx * nr.hx + (double)nr.hy * nr.hy);
-        dpsi = (double)nr.hk * a.g.yaw_step;
-    }
-    const LatticeView& L = a.lat;
-    const double ex = L.ox + L.nx * L.h, ey = L.oy + L.ny * L.h, ez = L.oz + L.nz * L.h;
-    for (int tile = blockIdx.y; tile < a.n_tiles; tile += gridDim.y) {  // uniform across the CTA
-        const size_t base = (size_t)tile * TILE;
-        const int m = (int)min((size_t)TILE, (size_t)a.n - base);
-        for (int i = threadIdx.x; i < m; i += kScoreBlock) s_pts[i] = a.src[base + i];
-        double sum = 0.0;
-        __syncthreads();
-        if (node < a.N) {
-#pragma unroll 1
-            for (int i = sub; i < m; i += TPP) {
-                const float4 sp = s_pts[i];
-                const double qx = xform_row_f(r[0], r[1], r[2], r[9], sp.x, sp.y, sp.z);
-                const double qy = xform_row_f(r[3], r[4], r[5], r[10], sp.x, sp.y, sp.z);
-                const double qz = xform_row_f(r[6], r[7], r[8], r[11], sp.x, sp.y, sp.z);
-                // b_i: the distance to the lattice's box, and the lattice value of the cell of q's projection onto the box (the
-                // projection onto a convex set: |q - p|^2 >= |q - q*|^2 + |q* - p|^2 for every fit point p in the box)
-                const double dx = fmax(0.0, fmax(L.ox - qx, qx - ex)), dy = fmax(0.0, fmax(L.oy - qy, qy - ey)), dz = fmax(0.0, fmax(L.oz - qz, qz - ez));
-                const int cx = (int)fmin(fmax((qx - L.ox) * L.inv_h, 0.0), L.nx - 1.0);
-                const int cy = (int)fmin(fmax((qy - L.oy) * L.inv_h, 0.0), L.ny - 1.0);
-                const int cz = (int)fmin(fmax((qz - L.oz) * L.inv_h, 0.0), L.nz - 1.0);
-                const double lv = (double)__ldg(L.v + ((size_t)cz * L.ny + cy) * L.nx + cx) * L.q;
-                const double b = sqrt(dx * dx + dy * dy + dz * dz + lv * lv);
-                const double delta = dt + dpsi * (double)sp.w + a.eps0 + a.eps1 * ((double)fabsf(sp.x) + (double)fabsf(sp.y) + (double)fabsf(sp.z));
-                const double e = fmax(0.0, b - delta);
-                sum += fmin(e * e, a.max_range);
-            }
-        }
-        s_sum[threadIdx.x] = sum;
-        __syncthreads();
-#pragma unroll
-        for (int o = TPP / 2; o > 0; o >>= 1) {
-            if (sub < o) s_sum[threadIdx.x] += s_sum[threadIdx.x + o];
-            __syncthreads();
-        }
-        if (sub == 0 && node < a.N) a.part[(size_t)node * a.n_tiles + tile] = s_sum[threadIdx.x];
-    }
-}
 
 // per node: LB / m against U (the n-th smallest sorted score bits at *u_key) -> how many children it passes to level l - 1
 __global__ void reloc_keep_kernel(const double* __restrict__ part, int N, int n_tiles, int m, const unsigned long long* __restrict__ u_key,
@@ -613,16 +527,6 @@ __global__ void reloc_children_kernel(const long long* __restrict__ nodes, const
     for (long long y = 2 * by; y < min(2 * by + 2, cx); ++y)
         for (long long x = 2 * bx; x < min(2 * bx + 2, cx); ++x)
             for (long long k = 2 * bk; k < min(2 * bk + 2, ck); ++k) *o++ = (y * cx + x) * ck + k;
-}
-
-// the n best after the sort: {leaf index, score, pose}
-__global__ void reloc_pick_wide_kernel(const unsigned long long* __restrict__ key_sorted, const long long* __restrict__ leaf_sorted, RelocGridArgs g,
-                                       int n, RelocPick* __restrict__ out) {
-    const int r = threadIdx.x;
-    if (r >= n) return;
-    out[r].index = leaf_sorted[r];
-    out[r].score = __longlong_as_double((long long)key_sorted[r]);
-    reloc_leaf_pose(g, leaf_sorted[r], out[r].pose);
 }
 
 // ---- the lower-bound distance lattice -------------------------------------------------------------------------------------------
@@ -737,13 +641,42 @@ __global__ void reloc_slack_points_kernel(const float4* __restrict__ src, int n,
 
 }  // namespace
 
+// Relocalization's state on a handle, made by its first call: the coarse cloud and its copy with each point's slack term, a launch's
+// poses and partials, sort keys and leaf ids (an unsorted and a sorted half each), the node lists of a level and the next with their
+// child counts and offsets, U's sort key, the picks, the lower-bound lattice of the fit cloud, and the levels of the last wide search.
+struct Reloc {
+    DevBuf<float4> coarse, slack_pts;
+    DevBuf<double> poses, part_sum;
+    DevBuf<unsigned> part_cnt;
+    DevBuf<unsigned long long> key, leaf, u;
+    DevBuf<long long> nodes, next;
+    DevBuf<int> count;
+    DevBuf<RelocPick> pick;
+    LatticeView lat{};
+    DevBuf<unsigned short> lat_v;
+    unsigned long long lat_version = ~0ull;
+    float lat_range = -1.f;
+    std::vector<long long> levels;  // nodes evaluated per level of the last fls_relocalize_wide call, from its start level down to 0
+
+    int lattice_for(Handle& hd, float max_range, int* waits);
+};
+
+void RelocFree::operator()(Reloc* r) const { delete r; }
+
+int Handle::relocalize_levels(int64_t* out, int capacity) const {
+    const int n = reloc ? (int)reloc->levels.size() : 0;
+    for (int i = 0; i < n && i < capacity; ++i) out[i] = reloc->levels[i];
+    return n;
+}
+
 // The lattice of the current fit cloud and max_range, rebuilt like fit_grid (two waits when it is: the bounding box, and the end of
 // the build before its scratch is freed).
-int Handle::lattice_for(float max_range, int* waits) {
-    if (lat_version == fit_cloud_version && lat_range == max_range) return FLS_OK;
+int Reloc::lattice_for(Handle& hd, float max_range, int* waits) {
+    if (lat_version == hd.fit_cloud_version && lat_range == max_range) return FLS_OK;
+    const cudaStream_t stream = hd.stream;
     DevBuf<float> box;
     box.reserve(6);
-    lattice_bbox_kernel<<<1, 256, 0, stream>>>(fit_pts, fit_cloud_n, box.p);
+    lattice_bbox_kernel<<<1, 256, 0, stream>>>(hd.fit_pts, hd.fit_cloud_n, box.p);
     float b[6];
     FLS_CUDA(cudaMemcpyAsync(b, box.p, sizeof(b), cudaMemcpyDeviceToHost, stream));
     FLS_CUDA(cudaStreamSynchronize(stream));
@@ -754,18 +687,14 @@ int Handle::lattice_for(float max_range, int* waits) {
         for (int k = 0; k < 3; ++k) n[k] = (long long)std::floor(((double)b[3 + k] - (double)b[k]) / h) + 1;
         if (n[0] * n[1] * n[2] <= (long long)kLatticeCells && n[0] <= kLatticeLine && n[1] <= kLatticeLine && n[2] <= kLatticeLine) break;
     }
-    lat.nx = (int)n[0], lat.ny = (int)n[1], lat.nz = (int)n[2];
-    lat.ox = b[0], lat.oy = b[1], lat.oz = b[2];
-    lat.h = h;
-    lat.q = h / 64.0;
     const size_t cells = (size_t)(n[0] * n[1] * n[2]);
-    LatticeView L{nullptr, lat.nx, lat.ny, lat.nz, lat.ox, lat.oy, lat.oz, h, 1.0 / h, lat.q};
     DevBuf<unsigned> d0, d1;
     DevBuf<unsigned short> s, t;
     d0.reserve(cells), d1.reserve(cells), s.reserve(cells), t.reserve(cells);
     lat_v.reserve(cells);
+    lat = {lat_v.p, (int)n[0], (int)n[1], (int)n[2], b[0], b[1], b[2], h, 1.0 / h, h / 64.0};
     FLS_CUDA(cudaMemsetAsync(d0.p, 0xff, cells * sizeof(unsigned), stream));
-    lattice_mark_kernel<<<grid_for(fit_cloud_n, 256), 256, 0, stream>>>(fit_pts, fit_cloud_n, L, d0.p);
+    lattice_mark_kernel<<<grid_for(hd.fit_cloud_n, 256), 256, 0, stream>>>(hd.fit_pts, hd.fit_cloud_n, lat, d0.p);
     const long long lines[3] = {n[1] * n[2], n[0] * n[2], n[0] * n[1]};
     lattice_edt_kernel<<<grid_for((size_t)lines[0], 128), 128, 0, stream>>>(d0.p, d1.p, s.p, t.p, lat.nx, lat.ny, lat.nz, 0);
     lattice_edt_kernel<<<grid_for((size_t)lines[1], 128), 128, 0, stream>>>(d1.p, d0.p, s.p, t.p, lat.nx, lat.ny, lat.nz, 1);
@@ -774,97 +703,114 @@ int Handle::lattice_for(float max_range, int* waits) {
     FLS_CUDA(cudaGetLastError());
     FLS_CUDA(cudaStreamSynchronize(stream));  // the scratch above is freed on return
     if (waits) ++*waits;
-    launches += 6;
-    lat_version = fit_cloud_version;
+    hd.launches += 6;
+    lat_version = hd.fit_cloud_version;
     lat_range = max_range;
     return FLS_OK;
 }
 
-int Handle::relocalize_wide(const float4* d_scan, size_t n, const fls_reloc_cfg& c, const RelocGrid& gr, double* T, fls_reloc_result* out,
-                            double* refined_T, int32_t* refined_converged, float* refined_fitness, int64_t* refined_index, int64_t* evaluations) {
+int Handle::relocalize(const float4* d_scan, size_t n, const fls_reloc_cfg& c, const RelocGrid& gr, bool wide, double* T, fls_reloc_result* out,
+                       double* refined_T, int32_t* refined_converged, float* refined_fitness, int64_t* refined_index, double* coarse_scores,
+                       size_t coarse_cap, int64_t* evaluations) {
+    if (!reloc) reloc.reset(new Reloc);
+    Reloc& s = *reloc;
     int L = 0, W = 0;  // launches and waits of the whole call
     long long evals = 0;
     if (evaluations) *evaluations = 0;
-    wide_levels.clear();
-    size_t m = 0;
+    if (wide) s.levels.clear();
+    std::memset(out, 0, sizeof(*out));
+    out->n_hypotheses = gr.P;
+    out->best_hypothesis = -1;
+    out->fitness = FLT_MAX;
+    out->coarse_score = FLT_MAX;
+    // ---- coarse cloud and the fit grid; an empty coarse cloud ends the call: nothing to score or refine, and a later fls_fitness
+    // scores the empty cloud --------------------------------------------------------------------------------------------------------
+    s.coarse.reserve(n + 1);
+    const size_t m = voxel_grid_device(d_scan, n, c.coarse_leaf, s.coarse.p, scratch, stream, &launches, &W);
+    if (m == 0) {
+        last_src = d_scan;
+        last_src_n = 0;
+        out->gpu_launches = launches;
+        out->host_waits = W;
+        return FLS_OK;
+    }
+    int rc = fit_grid_for(c.max_range, &W);
+    if (rc != FLS_OK) return rc;
     RelocGridArgs ga;
-    int rc = reloc_prelude(*this, d_scan, n, c, gr, T, out, W, &m, &ga);
-    if (rc != FLS_OK || m == 0) return rc;
+    pose_rows(T, ga.R);
+    for (int k = 0; k < 3; ++k) ga.t[k] = T[12 + k];
+    ga.xy_step = gr.I ? c.xy_step : 0.0;  // an unused step may be anything
+    ga.yaw_step = gr.K ? c.yaw_step : 0.0;
+    ga.I = gr.I;
+    ga.K = gr.K;
+    ga.k0 = gr.k0;
+    ga.n_yaw = gr.n_yaw;
+    ga.P = gr.P;
+    // ---- the start level: the lowest with at most 2^20 nodes (level 0 on every grid fls_relocalize accepts) -----------------------
     const long long P = gr.P, nx = 2LL * gr.I + 1, nk = gr.n_yaw;
     const int nr = P < c.n_refine ? (int)P : c.n_refine;
     int ls = 0;
     while (level_blocks(nx, ls) * level_blocks(nx, ls) * level_blocks(nk, ls) > kWideChunk) ++ls;
     long long N = level_blocks(nx, ls) * level_blocks(nx, ls) * level_blocks(nk, ls);
     const size_t tiles = (m + kCoarseTile - 1) / kCoarseTile;
-    auto reserve_chunk = [&](size_t k) {  // a launch's poses, partials and scores
-        reloc_poses.reserve(k * 12);
-        reloc_part_sum.reserve(k * tiles);
-        reloc_part_cnt.reserve(k * tiles);
-        reloc_score.reserve(k);
-        reloc_idx.reserve(k);
+    auto reserve_chunk = [&](size_t k) {  // a launch's poses and partials
+        s.poses.reserve(k * 12);
+        s.part_sum.reserve(k * tiles);
+        s.part_cnt.reserve(k * tiles);
     };
-    reloc_pick.reserve(sizeof(RelocPick) * kMaxBatch);
-    wide_nodes.reserve((size_t)N);
-    reloc_iota_kernel<<<grid_for((size_t)N, 256), 256, 0, stream>>>(wide_nodes.p, N);
-    ++L;
-    // exact scores of the representatives of N nodes of level l -> their sort keys
-    auto exact = [&](const long long* nodes, long long N_, int l, unsigned long long* keys) {
+    s.pick.reserve(kMaxBatch);
+    // exact scores of the representatives of N_ nodes of level l (nodes null: node i is i) -> their sort keys, and their node ids
+    // when ids is given
+    auto exact = [&](const long long* nodes, long long N_, int l, unsigned long long* keys, unsigned long long* ids) {
         for (long long o = 0; o < N_; o += kWideChunk) {
             const int k = (int)(N_ - o < kWideChunk ? N_ - o : kWideChunk);
+            const long long* chunk = nodes ? nodes + o : nullptr;
             reserve_chunk((size_t)k);
-            reloc_rep_poses_kernel<<<grid_for((size_t)k, 128), 128, 0, stream>>>(ga, nodes + o, k, l, reloc_poses.p);
-            pose_score_launch(true, fit_grid.view(), reloc_coarse.p, (int)m, reloc_poses.p, k, c.max_range, reloc_part_sum.p, reloc_part_cnt.p, stream);
-            pose_score_reduce_kernel<<<grid_for((size_t)k, 128), 128, 0, stream>>>(reloc_part_sum.p, reloc_part_cnt.p, k, (int)tiles, (int)m, c.max_range,
-                                                                                   nullptr, nullptr, reloc_score.p, keys + o, reloc_idx.p);
+            reloc_rep_poses_kernel<<<grid_for((size_t)k, 128), 128, 0, stream>>>(ga, chunk, o, k, l, s.poses.p);
+            pose_score_launch<true>(FitTerm{fit_grid.view(), s.poses.p, c.max_range}, s.coarse.p, (int)m, k, s.part_sum.p, s.part_cnt.p, stream);
+            pose_score_reduce_kernel<<<grid_for((size_t)k, 128), 128, 0, stream>>>(s.part_sum.p, s.part_cnt.p, k, (int)tiles, (int)m, c.max_range, nullptr,
+                                                                                   nullptr, keys + o, chunk, o, ids ? ids + o : nullptr);
             L += 3;
         }
         evals += N_;
     };
+    // ---- the descent from the start level to level 1 (fls_relocalize_wide past 2^20 hypotheses) ------------------------------------
     if (ls > 0) {
-        rc = lattice_for(c.max_range, &W);
+        rc = s.lattice_for(*this, c.max_range, &W);
         if (rc != FLS_OK) return rc;
+        s.nodes.reserve((size_t)N);
+        reloc_iota_kernel<<<grid_for((size_t)N, 256), 256, 0, stream>>>(s.nodes.p, N);
+        ++L;
         // U: the nr-th smallest score of the start level's representatives
-        wide_key.reserve((size_t)N * 2);
-        exact(wide_nodes.p, N, ls, wide_key.p);
+        s.key.reserve((size_t)N * 2);
+        exact(s.nodes.p, N, ls, s.key.p, nullptr);
         cub_pass(scratch.cub_tmp, [&](void* tmp, size_t& bytes) {
-            return cub::DeviceRadixSort::SortKeys(tmp, bytes, wide_key.p, wide_key.p + N, (int)N, 0, 64, stream);
+            return cub::DeviceRadixSort::SortKeys(tmp, bytes, s.key.p, s.key.p + N, (int)N, 0, 64, stream);
         });
         ++L;
-        wide_u.reserve(1);
-        FLS_CUDA(cudaMemcpyAsync(wide_u.p, wide_key.p + N + nr - 1, sizeof(unsigned long long), cudaMemcpyDeviceToDevice, stream));
+        s.u.reserve(1);
+        FLS_CUDA(cudaMemcpyAsync(s.u.p, s.key.p + N + nr - 1, sizeof(unsigned long long), cudaMemcpyDeviceToDevice, stream));
         // the slack's float terms (derivation above): tau, the largest translation coordinate of any leaf
         const double tau = std::fmax(std::fmax(std::fabs(ga.t[0]), std::fabs(ga.t[1])) + gr.I * ga.xy_step, std::fabs(ga.t[2]));
-        BoundArgs ba{};
-        ba.lat = {lat_v.p, lat.nx, lat.ny, lat.nz, lat.ox, lat.oy, lat.oz, lat.h, 1.0 / lat.h, lat.q};
-        ba.g = ga;
-        wide_pts.reserve(m);
-        reloc_slack_points_kernel<<<grid_for(m, 256), 256, 0, stream>>>(reloc_coarse.p, (int)m, ga, wide_pts.p);
+        s.slack_pts.reserve(m);
+        reloc_slack_points_kernel<<<grid_for(m, 256), 256, 0, stream>>>(s.coarse.p, (int)m, ga, s.slack_pts.p);
         ++L;
-        ba.src = wide_pts.p;
-        ba.n = (int)m;
-        ba.n_tiles = (int)tiles;
-        ba.eps0 = 32.0 * kU * tau + 8.0 * kU * std::sqrt((double)c.max_range);
-        ba.eps1 = 32.0 * kU;
-        ba.max_range = c.max_range;
+        BoundTerm bound{s.lat, ga, nullptr, 0, 32.0 * kU * tau + 8.0 * kU * std::sqrt((double)c.max_range), 32.0 * kU, c.max_range};
         for (int l = ls; l >= 1; --l) {
-            wide_count.reserve((size_t)N * 2);
-            int* cnt = wide_count.p;
-            int* off = wide_count.p + N;
+            s.count.reserve((size_t)N * 2);
+            int* cnt = s.count.p;
+            int* off = s.count.p + N;
             for (long long o = 0; o < N; o += kWideChunk) {
                 const int k = (int)(N - o < kWideChunk ? N - o : kWideChunk);
                 reserve_chunk((size_t)k);
-                ba.nodes = wide_nodes.p + o;
-                ba.N = k;
-                ba.level = l;
-                ba.part = reloc_part_sum.p;
-                const dim3 grid((unsigned)((k + kCoarsePoses - 1) / kCoarsePoses), (unsigned)(tiles < 65535 ? tiles : 65535));
-                reloc_bound_kernel<<<grid, kScoreBlock, 0, stream>>>(ba);
-                reloc_keep_kernel<<<grid_for((size_t)k, 128), 128, 0, stream>>>(reloc_part_sum.p, k, (int)tiles, (int)m, wide_u.p, wide_nodes.p + o, l, nx,
-                                                                                 nk, cnt + o);
+                bound.nodes = s.nodes.p + o;
+                bound.level = l;
+                pose_score_launch<true>(bound, s.slack_pts.p, (int)m, k, s.part_sum.p, nullptr, stream);
+                reloc_keep_kernel<<<grid_for((size_t)k, 128), 128, 0, stream>>>(s.part_sum.p, k, (int)tiles, (int)m, s.u.p, s.nodes.p + o, l, nx, nk, cnt + o);
                 L += 2;
             }
             evals += N;
-            wide_levels.push_back(N);
+            s.levels.push_back(N);
             cub_pass(scratch.cub_tmp, [&](void* tmp, size_t& bytes) { return cub::DeviceScan::ExclusiveSum(tmp, bytes, cnt, off, (int)N, stream); });
             int last[2];
             FLS_CUDA(cudaMemcpyAsync(last, cnt + N - 1, sizeof(int), cudaMemcpyDeviceToHost, stream));
@@ -879,43 +825,41 @@ int Handle::relocalize_wide(const float4* d_scan, size_t n, const fls_reloc_cfg&
                 out->host_waits = W;
                 return FLS_ERR_CAPACITY;
             }
-            wide_next.reserve((size_t)next);
-            reloc_children_kernel<<<grid_for((size_t)N, 128), 128, 0, stream>>>(wide_nodes.p, cnt, off, (int)N, l, nx, nk, wide_next.p);
+            s.next.reserve((size_t)next);
+            reloc_children_kernel<<<grid_for((size_t)N, 128), 128, 0, stream>>>(s.nodes.p, cnt, off, (int)N, l, nx, nk, s.next.p);
             ++L;
-            std::swap(wide_nodes.p, wide_next.p);
-            std::swap(wide_nodes.cap, wide_next.cap);
+            std::swap(s.nodes.p, s.next.p);
+            std::swap(s.nodes.cap, s.next.cap);
             N = next;
         }
     }
-    // ---- level 0: every surviving leaf scored exactly, a stable sort on (score bits, leaf index), the n best -------------------------
-    wide_key.reserve((size_t)N * 2);
-    wide_next.reserve((size_t)N * 2);
-    exact(wide_nodes.p, N, 0, wide_key.p);
-    wide_levels.push_back(N);
+    // ---- level 0: every leaf left scored exactly, a stable sort on (score bits, leaf index), the n best -----------------------------
+    // A descent's survivors are scored into the upper halves and first sorted into leaf order; a grid scored whole is in leaf order.
+    s.key.reserve((size_t)N * 2);
+    s.leaf.reserve((size_t)N * 2);
+    unsigned long long *key = s.key.p, *leaf = s.leaf.p, *key2 = key + N, *leaf2 = leaf + N;
+    exact(ls ? s.nodes.p : nullptr, N, 0, ls ? key2 : key, ls ? leaf2 : leaf);
+    if (wide) s.levels.push_back(N);
     int bits = 1;
     while ((1LL << bits) < P) ++bits;
-    unsigned long long* key2 = wide_key.p + N;
-    long long* leaf2 = wide_next.p;
-    long long* leaf3 = wide_next.p + N;
-    cub_reserve(
-        scratch.cub_tmp,
-        [&](void* tmp, size_t& bytes) {
-            return cub::DeviceRadixSort::SortPairs(tmp, bytes, (const unsigned long long*)wide_nodes.p, (unsigned long long*)leaf2, wide_key.p, key2, (int)N,
-                                                   0, bits, stream);
-        },
-        [&](void* tmp, size_t& bytes) { return cub::DeviceRadixSort::SortPairs(tmp, bytes, key2, wide_key.p, leaf2, leaf3, (int)N, 0, 64, stream); });
-    cub_run(scratch.cub_tmp, [&](void* tmp, size_t& bytes) {
-        return cub::DeviceRadixSort::SortPairs(tmp, bytes, (const unsigned long long*)wide_nodes.p, (unsigned long long*)leaf2, wide_key.p, key2, (int)N, 0,
-                                               bits, stream);
-    });
-    cub_run(scratch.cub_tmp,
-            [&](void* tmp, size_t& bytes) { return cub::DeviceRadixSort::SortPairs(tmp, bytes, key2, wide_key.p, leaf2, leaf3, (int)N, 0, 64, stream); });
-    RelocPick* d_pick = reinterpret_cast<RelocPick*>(reloc_pick.p);
-    reloc_pick_wide_kernel<<<1, kMaxBatch, 0, stream>>>(wide_key.p, leaf3, ga, nr, d_pick);
+    auto by_leaf = [&](void* tmp, size_t& bytes) { return cub::DeviceRadixSort::SortPairs(tmp, bytes, leaf2, leaf, key2, key, (int)N, 0, bits, stream); };
+    auto by_key = [&](void* tmp, size_t& bytes) { return cub::DeviceRadixSort::SortPairs(tmp, bytes, key, key2, leaf, leaf2, (int)N, 0, 64, stream); };
+    if (ls > 0) {
+        cub_reserve(scratch.cub_tmp, by_leaf, by_key);
+        cub_run(scratch.cub_tmp, by_leaf);
+        ++L;
+    } else {
+        cub_reserve(scratch.cub_tmp, by_key);
+    }
+    cub_run(scratch.cub_tmp, by_key);
+    reloc_pick_kernel<<<1, kMaxBatch, 0, stream>>>(key2, leaf2, ga, nr, s.pick.p);
     FLS_CUDA(cudaGetLastError());
-    L += 3;
+    L += 2;
     RelocPick pick[kMaxBatch];
-    FLS_CUDA(cudaMemcpyAsync(pick, d_pick, sizeof(RelocPick) * (size_t)nr, cudaMemcpyDeviceToHost, stream));
+    FLS_CUDA(cudaMemcpyAsync(pick, s.pick.p, sizeof(RelocPick) * (size_t)nr, cudaMemcpyDeviceToHost, stream));
+    // fls_relocalize's coarse scores: the unsorted keys hold their bits
+    const size_t n_cs = coarse_scores ? (coarse_cap < (size_t)P ? coarse_cap : (size_t)P) : 0;
+    if (n_cs) FLS_CUDA(cudaMemcpyAsync(coarse_scores, key, sizeof(double) * n_cs, cudaMemcpyDeviceToHost, stream));
     FLS_CUDA(cudaStreamSynchronize(stream));
     ++W;
     if (evaluations) *evaluations = evals;

@@ -297,9 +297,9 @@ int fls_relocalize_device(fls_handle* h, const void* d_scan, size_t n, const fls
  * than 2^23 blocks survive one level, before any Match runs (T, the map and fls_fitness are then as before the call): a map and scan
  * so featureless that most of a very large grid cannot be told apart from the best.  The lattice is built by the first call past 2^20
  * hypotheses after the map or max_range changes (two more waits); its pitch is sqrt(max_range) / 4, coarser when the map's bounding box would exceed
- * 2^25 cells.  Waits: those of fls_relocalize, plus one per level above the start of the descent; launches grow with the number of
- * levels and of 2^20-block chunks.  Everything else — plug-ins, modes, argument checks, the empty scan, the state left for
- * fls_fitness and Match — is fls_relocalize's. */
+ * 2^25 cells.  Waits: those of fls_relocalize, plus one per level above the start of the descent; launches: those of fls_relocalize
+ * on a grid of at most 2^20 hypotheses, and past it growing with the number of levels and of 2^20-block chunks.  Everything else —
+ * plug-ins, modes, argument checks, the empty scan, the state left for fls_fitness and Match — is fls_relocalize's. */
 int fls_relocalize_wide(fls_handle* h, const void* scan, size_t n, size_t stride_bytes, const fls_reloc_cfg* cfg, double T_colmajor[16],
                         fls_reloc_result* out, double* refined_T, int32_t* refined_converged, float* refined_fitness, int64_t* refined_index,
                         int64_t* evaluations);

@@ -103,7 +103,7 @@ def main():
         coarse_us, n_k = 0.0, 0
         for e in prof.events():
             k = e.name
-            if "reloc_poses_kernel" in k or "pose_score_kernel<8" in k or "RadixSort" in k or "reloc_pick_kernel" in k or "pose_score_reduce" in k:
+            if "reloc_rep_poses_kernel" in k or "pose_score_kernel<8" in k or "RadixSort" in k or "reloc_pick_kernel" in k or "pose_score_reduce" in k:
                 coarse_us += e.device_time
                 n_k += 1
         # (b) the loop a caller can write today: n_refine Matches + GetFitnessScore from the same start poses
