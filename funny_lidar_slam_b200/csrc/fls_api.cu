@@ -220,6 +220,35 @@ void Handle::unpack(int B, const size_t* n, double* T, int* converged, fls_match
     for (int s = 0; s < B; ++s) log_n[s] = h_state[s].iter < log_cap ? h_state[s].iter : log_cap;
 }
 
+int Handle::filter_batch(int B, const float4* const* d, const size_t* n, float leaf, DevBuf<float4>& dst, size_t* off, size_t* ns) {
+    // room for every distinct source: a scan that repeats an earlier (pointer, count) is filtered once (relocalization refines many
+    // poses of one scan)
+    auto first_of = [&](int s) {
+        int first = 0;
+        while (first < s && !(d[first] == d[s] && n[first] == n[s])) ++first;
+        return first;
+    };
+    size_t total_in = 0;
+    for (int s = 0; s < B; ++s)
+        if (first_of(s) == s) total_in += n[s];
+    dst.reserve(total_in + 1);
+    size_t end = 0;
+    for (int s = 0; s < B; ++s) {
+        const int first = first_of(s);
+        if (first < s) {
+            off[s] = off[first];
+            ns[s] = ns[first];
+            continue;
+        }
+        const size_t nf = voxel_grid_device(d[s], n[s], leaf, dst.p + end, scratch, stream, &launches, &waits);
+        if (nf > 0x3fffffffull) return FLS_ERR_INVALID_ARG;
+        off[s] = end;
+        ns[s] = nf;
+        end += nf;
+    }
+    return FLS_OK;
+}
+
 int Handle::inserted(int rc, fls_match_stats* st) {
     FLS_CUDA(cudaStreamSynchronize(stream));
     ++waits;

@@ -33,6 +33,16 @@ struct GnLoopCtl {
 };
 static constexpr int kResultLen = 18;  // column-major 4x4 pose, converged, iterations
 
+// One scan of a batch in one cooperative launch (NDT, ICP, kd-tree LOAM): the plug-in's kernel arguments and control block, served
+// by CTAs [cta0, cta0 + ncta) of the grid, which run their own persistent loop (gn_batch_loop)
+template <class Args>
+struct __align__(16) GnBatchItem {
+    Args a;
+    GnLoopCtl ctl;
+    int cta0, ncta;
+    int pad[2];
+};
+
 void launch_gn_init(GnState* d_state, const double* T_colmajor, cudaStream_t st);
 
 #ifdef __CUDACC__
@@ -309,6 +319,29 @@ __device__ __forceinline__ bool gn_handover(double (&acc)[kNumAcc], const GnLoop
     const unsigned tag = c.tag_base | (unsigned)(it + 1);
     gn_warp_rows<BLOCK>(acc, s_red);
     return gn_handover_rows<BLOCK>(s_red, s_stop, c, tag, s_pose, cta, ncta);
+}
+
+// A batch of independent scans against the same (static) map in ONE cooperative launch: the grid is cut into one sub-grid per
+// scan, each running its own persistent Gauss-Newton loop (own rows, pose record and state) — the ~15 us hand-over of a scan
+// overlaps with the residual passes of the others, which is what the single-scan loop cannot hide at these sizes.  Each CTA finds
+// its item (items are in cta0 order), copies it to shared memory and runs loop(args, ctl, cta, ncta) on its sub-grid.
+template <int BLOCK, class Args, class Loop>
+__device__ __forceinline__ void gn_batch_loop(const GnBatchItem<Args>* __restrict__ items, int n_scans, Loop loop) {
+    __shared__ GnBatchItem<Args> s_item;
+    __shared__ int s_which;
+    if (threadIdx.x == 0) {
+        int w = 0;
+        while (w + 1 < n_scans && (int)blockIdx.x >= items[w + 1].cta0) ++w;
+        s_which = w;
+    }
+    __syncthreads();
+    {
+        const unsigned long long* src = reinterpret_cast<const unsigned long long*>(items + s_which);
+        unsigned long long* dst = reinterpret_cast<unsigned long long*>(&s_item);
+        for (int k = threadIdx.x; k < (int)(sizeof(GnBatchItem<Args>) / 8); k += BLOCK) dst[k] = src[k];
+    }
+    __syncthreads();
+    loop(s_item.a, s_item.ctl, (int)blockIdx.x - s_item.cta0, s_item.ncta);
 }
 #endif
 

@@ -195,6 +195,59 @@ struct Handle {
         end_call(st);
         unpack(1, &n_source, T, converged, st);
     }
+    // ---- a batch Match on sub-grids of one cooperative launch (NDT, ICP, kd-tree LOAM) ----
+    // VoxelGridCloud of every distinct source of a batch, back to back in dst: scan s reads [off[s], off[s] + ns[s]), and a scan that
+    // repeats an earlier (pointer, count) reads the range of its first occurrence.  FLS_ERR_INVALID_ARG past 2^30 filtered points.
+    int filter_batch(int B, const float4* const* d, const size_t* n, float leaf, DevBuf<float4>& dst, size_t* off, size_t* ns);
+    // The Gauss-Newton half of such a batch.  Scan s (ns[s] points, also its n_source) gets one CTA per `per_cta` points, all scaled
+    // down together when the `cap` co-resident CTAs of the batch kernel cannot hold them (more scans than CTAs: FLS_ERR_INVALID_ARG).
+    // Then, per scan: its state from T, its control block and its item, whose arguments fill(s, item.a) sets; the gn_launch of
+    // launch(d_items, grid), the wait, and T / converged / stats of every scan.  src0: the source of scan 0 (GetFitnessScore).
+    template <class Args, class Fill, class Launch>
+    int match_subgrids(int method, int min_effective, int B, const size_t* ns, int per_cta, int cap, long long point_iter_bytes, long long cand_bytes,
+                       const float4* src0, double* T, int* converged, fls_match_stats* st, Fill&& fill, Launch&& launch) {
+        int need[kMaxBatch], tot_need = 0;
+        for (int s = 0; s < B; ++s) {
+            need[s] = (int)((ns[s] + per_cta - 1) / per_cta);
+            if (need[s] < 1) need[s] = 1;
+            tot_need += need[s];
+        }
+        if (B > cap) return FLS_ERR_INVALID_ARG;
+        int ncta[kMaxBatch], grid = 0;
+        for (int s = 0; s < B; ++s) {
+            ncta[s] = tot_need <= cap ? need[s] : (int)((long long)need[s] * (cap - B) / tot_need) + 1;
+            grid += ncta[s];
+        }
+        const unsigned tag_base = next_ll_epoch((size_t)grid * 32 + (size_t)B * kLlPoseLen);
+        const size_t tbl_bytes = sizeof(GnBatchItem<Args>) * (size_t)B;
+        GnBatchItem<Args>* items = reinterpret_cast<GnBatchItem<Args>*>(batch_table(tbl_bytes));
+        uint4* pose_base = ll_rows.p + (size_t)grid * 32;
+        int cta0 = 0;
+        for (int s = 0; s < B; ++s) {
+            launch_gn_init(state.p + s, T + 16 * s, stream);
+            launches++;
+            GnBatchItem<Args>& it = items[s];
+            std::memset(&it, 0, sizeof(it));
+            fill(s, it.a);
+            it.ctl.state = state.p + s;
+            it.ctl.ll_rows = ll_rows.p + (size_t)cta0 * 32;
+            it.ctl.ll_pose = pose_base + (size_t)s * kLlPoseLen;
+            it.ctl.tag_base = tag_base;
+            it.ctl.gp = gn_params(method, min_effective);
+            it.ctl.log = scan_log(s);
+            it.ctl.log_cap = log_cap;
+            it.ctl.result = scan_result(s);
+            it.cta0 = cta0;
+            it.ncta = ncta[s];
+            cta0 += ncta[s];
+        }
+        send_batch_table(tbl_bytes);
+        gn_launch(point_iter_bytes, cand_bytes, src0, ns[0], [&] { launch(reinterpret_cast<const GnBatchItem<Args>*>(d_batch.p), grid); });
+        read_back(B);
+        end_call(st);
+        unpack(B, ns, T, converged, st);
+        return FLS_OK;
+    }
     // end of a Match that added its scan to the map with status rc: waits for the insertion and counts its launches too
     int inserted(int rc, fls_match_stats* st);
 

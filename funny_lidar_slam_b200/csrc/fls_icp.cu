@@ -71,9 +71,10 @@ __device__ __forceinline__ bool grid_nn1_coop(const GridView& g, int sub, unsign
     return best_j != 0xffffffffu;
 }
 
-// One persistent launch runs every Gauss-Newton iteration of a Match (gn_handover, fls_gn.cuh).
+// One persistent launch runs every Gauss-Newton iteration of a Match (gn_handover, fls_gn.cuh), on the CTAs (cta, ncta) of the
+// sub-grid that serves the scan.
 template <int BLOCK>
-__global__ void __launch_bounds__(BLOCK) icp_gn_kernel(IcpArgs a, GnLoopCtl ctl) {
+__device__ __forceinline__ void icp_gn_loop(const IcpArgs& a, const GnLoopCtl& ctl, const int cta, const int ncta) {
     __shared__ double s_pose[12];
     __shared__ float s_posef[12];
     const int sub = threadIdx.x & (kIcpLanes - 1);
@@ -88,7 +89,7 @@ __global__ void __launch_bounds__(BLOCK) icp_gn_kernel(IcpArgs a, GnLoopCtl ctl)
 #pragma unroll
         for (int k = 0; k < kNumAcc; ++k) acc[k] = 0.0;
 
-        for (int i = blockIdx.x * kPerBlock + threadIdx.x / kIcpLanes; i < a.n; i += gridDim.x * kPerBlock) {
+        for (int i = (unsigned)cta * kPerBlock + threadIdx.x / kIcpLanes; i < a.n; i += (unsigned)ncta * kPerBlock) {
             const float4 sp = a.src[i];
             const float qx = xform_row_f(s_posef[0], s_posef[1], s_posef[2], s_posef[9], sp.x, sp.y, sp.z);
             const float qy = xform_row_f(s_posef[3], s_posef[4], s_posef[5], s_posef[10], sp.x, sp.y, sp.z);
@@ -128,8 +129,19 @@ __global__ void __launch_bounds__(BLOCK) icp_gn_kernel(IcpArgs a, GnLoopCtl ctl)
                 acc[kAccRes] += sqrt(e0 * e0 + e1 * e1 + e2 * e2);  // total_res += error.norm()  (:126)
             }
         }
-        if (gn_handover<BLOCK>(acc, ctl, it, s_pose)) break;
+        if (gn_handover<BLOCK>(acc, ctl, it, s_pose, cta, ncta)) break;
     }
+}
+
+template <int BLOCK>
+__global__ void __launch_bounds__(BLOCK) icp_gn_kernel(IcpArgs a, GnLoopCtl ctl) {
+    icp_gn_loop<BLOCK>(a, ctl, (int)blockIdx.x, (int)gridDim.x);
+}
+
+// a batch of scans, one sub-grid each (gn_batch_loop, fls_gn.cuh)
+template <int BLOCK>
+__global__ void __launch_bounds__(BLOCK) icp_gn_batch_kernel(const GnBatchItem<IcpArgs>* __restrict__ items, int n_scans) {
+    gn_batch_loop<BLOCK>(items, n_scans, [](const IcpArgs& a, const GnLoopCtl& ctl, int cta, int ncta) { icp_gn_loop<BLOCK>(a, ctl, cta, ncta); });
 }
 
 }  // namespace
@@ -140,6 +152,10 @@ static int icp_grid_blocks(int n, int device) {
 }
 static void launch_icp_loop(const IcpArgs& a, const GnLoopCtl& ctl, int grid, cudaStream_t st) {
     launch_cooperative(icp_gn_kernel<kIcpBlock>, grid, kIcpBlock, 0, st, a, ctl);
+}
+static int icp_max_grid(int device) { return coresident_ctas((const void*)icp_gn_batch_kernel<kIcpBlock>, kIcpBlock, 0, device); }
+static void launch_icp_batch(const GnBatchItem<IcpArgs>* d_items, int n_scans, int grid, cudaStream_t st) {
+    launch_cooperative(icp_gn_batch_kernel<kIcpBlock>, grid, kIcpBlock, 0, st, d_items, n_scans);
 }
 
 // ---- IcpOptimized ------------------------------------------------------------------------------------------------
@@ -191,6 +207,37 @@ class IcpPlugin final : public Plugin {
             return h.inserted(add_cloud(ins.p, n, nullptr, 0), st);
         }
         return FLS_OK;
+    }
+
+    // n_scans independent IcpOptimized::Match calls against the same (static) map in ONE cooperative launch (icp_gn_batch_kernel —
+    // one sub-grid and one persistent Gauss-Newton loop per scan).  The single Match's refusals come first, before anything is
+    // uploaded or launched; a batch of one is the single Match.
+    int match_batch(int B, const void* const* scans, const size_t* n_in, size_t host_stride, double* T, int* converged,
+                    fls_match_stats* st) override {
+        for (int s = 0; s < B; ++s)
+            if (!scans[s] && n_in[s]) return FLS_ERR_INVALID_ARG;
+        for (int s = 0; s < B; ++s)
+            if (n_in[s] <= 10) return FLS_ERR_TOO_FEW_POINTS;  // CHECK_GT(ordered_cloud_.size(), 10u)  (:55)
+        if (window.grid.n_pts == 0) return FLS_ERR_NO_MAP;
+        const float4* d_scans[kMaxBatch];
+        const int rc = h.begin_batch(B, scans, n_in, host_stride, d_scans, st);
+        if (rc != FLS_OK) return rc;
+        if (B == 1) return match(d_scans[0], n_in[0], nullptr, 0, T, converged, st);
+        const fls_config& cfg = h.cfg;
+        size_t off[kMaxBatch], ns[kMaxBatch];
+        const int rf = h.filter_batch(B, d_scans, n_in, cfg.source_cloud_filter_size, scan, off, ns);  // :57
+        if (rf != FLS_OK) return rf;
+        const GridView view = window.grid.view();
+        return h.match_subgrids<IcpArgs>(FLS_ICP_P2P, 0, B, ns, kIcpBlock / kIcpLanes, icp_max_grid(cfg.device), 16 + 16LL * 27, 16, scan.p + off[0], T,
+                                         converged, st,
+                                         [&](int s, IcpArgs& a) {
+                                             a.src = scan.p + off[s];
+                                             a.n = (int)ns[s];
+                                             a.map = view;
+                                             a.max_corr = cfg.icp_max_correspond_distance;
+                                             a.state = h.state.p + s;
+                                         },
+                                         [&](const GnBatchItem<IcpArgs>* d_items, int grid) { launch_icp_batch(d_items, B, grid, h.stream); });
     }
 
     void map_info(fls_map_info* out) const override {

@@ -174,8 +174,9 @@ __device__ __forceinline__ bool corner_term(const float4* __restrict__ P, const 
     return true;
 }
 
+// One persistent launch runs every Gauss-Newton iteration of a Match, on the CTAs (cta, ncta) of the sub-grid that serves the scan.
 template <int BLOCK>
-__global__ void __launch_bounds__(BLOCK) loam_gn_kernel(LoamArgs a, GnLoopCtl ctl) {
+__device__ __forceinline__ void loam_gn_loop(const LoamArgs a, const GnLoopCtl& ctl, const int cta, const int ncta) {
     __shared__ double s_pose[12];
     const int n_total = a.n_corner + a.n_planar;
     const int sub = threadIdx.x & (kLoamLanes - 1);
@@ -187,7 +188,7 @@ __global__ void __launch_bounds__(BLOCK) loam_gn_kernel(LoamArgs a, GnLoopCtl ct
         double acc[kNumAcc];
 #pragma unroll
         for (int k = 0; k < kNumAcc; ++k) acc[k] = 0.0;
-        for (int i = blockIdx.x * kPerBlock + threadIdx.x / kLoamLanes; i < n_total; i += gridDim.x * kPerBlock) {
+        for (int i = (unsigned)cta * kPerBlock + threadIdx.x / kLoamLanes; i < n_total; i += (unsigned)ncta * kPerBlock) {
             const bool is_corner = i < a.n_corner;
             const float4 sp = is_corner ? a.corner[i] : a.planar[i - a.n_corner];
             // pcl::transformPoint with the double transform, stored back as fp32 (:219-220, :284-285, kdtree :211-212)
@@ -232,8 +233,19 @@ __global__ void __launch_bounds__(BLOCK) loam_gn_kernel(LoamArgs a, GnLoopCtl ct
                 else acc[kAccValid] += 1.0;           // number_valid_planar_ (the < 50 failure test)
             }
         }
-        if (gn_handover<BLOCK>(acc, ctl, it, s_pose)) break;
+        if (gn_handover<BLOCK>(acc, ctl, it, s_pose, cta, ncta)) break;
     }
+}
+
+template <int BLOCK>
+__global__ void __launch_bounds__(BLOCK) loam_gn_kernel(LoamArgs a, GnLoopCtl ctl) {
+    loam_gn_loop<BLOCK>(a, ctl, (int)blockIdx.x, (int)gridDim.x);
+}
+
+// a batch of scans, one sub-grid each (gn_batch_loop, fls_gn.cuh); each scan's records and flags are its own range of one buffer
+template <int BLOCK>
+__global__ void __launch_bounds__(BLOCK) loam_gn_batch_kernel(const GnBatchItem<LoamArgs>* __restrict__ items, int n_scans) {
+    gn_batch_loop<BLOCK>(items, n_scans, [](const LoamArgs& a, const GnLoopCtl& ctl, int cta, int ncta) { loam_gn_loop<BLOCK>(a, ctl, cta, ncta); });
 }
 
 __global__ void loam_clear_flags_kernel(unsigned char* flags, int n) {
@@ -252,6 +264,13 @@ static void launch_loam_loop(const LoamArgs& a, const GnLoopCtl& ctl, int grid, 
     const int n = a.n_corner + a.n_planar;
     if (n > 0) loam_clear_flags_kernel<<<(n + 255) / 256, 256, 0, st>>>(a.flags, n);
     launch_cooperative(loam_gn_kernel<kLoamBlock>, grid, kLoamBlock, 0, st, a, ctl);
+}
+
+static int loam_max_grid(int device) { return coresident_ctas((const void*)loam_gn_batch_kernel<kLoamBlock>, kLoamBlock, 0, device); }
+// clears the flags of every scan of the batch (n of them in all) in one launch, then the batch kernel
+static void launch_loam_batch(const GnBatchItem<LoamArgs>* d_items, int n_scans, unsigned char* flags, size_t n, int grid, cudaStream_t st) {
+    if (n > 0) loam_clear_flags_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(flags, (int)n);
+    launch_cooperative(loam_gn_batch_kernel<kLoamBlock>, grid, kLoamBlock, 0, st, d_items, n_scans);
 }
 
 // ---- LoamPointToPlaneKdtree / LoamFull -------------------------------------------------------------------------------
@@ -353,6 +372,53 @@ class KdPlugin final : public Plugin {
             return h.inserted(rc2, st);
         }
         return FLS_OK;
+    }
+
+    // n_scans independent LoamPointToPlaneKdtree::Match calls on planar features against the same (static) map in ONE cooperative
+    // launch (loam_gn_batch_kernel — one sub-grid and one persistent Gauss-Newton loop per scan).  Scan s owns records and flags
+    // [off[s], off[s] + n[s]) of one buffer, cleared together.  The key-frame gate is left alone: in localization mode nothing is
+    // inserted, so its last_T cannot be observed.  A batch of one is the single Match; LoamFull reads two clouds per scan and has no
+    // batch.
+    int match_batch(int B, const void* const* scans, const size_t* n_in, size_t host_stride, double* T, int* converged,
+                    fls_match_stats* st) override {
+        if (full) return FLS_ERR_UNSUPPORTED;
+        const float4* d_scans[kMaxBatch];
+        const int rc = h.begin_batch(B, scans, n_in, host_stride, d_scans, st);
+        if (rc != FLS_OK) return rc;
+        if (B == 1) return match(d_scans[0], n_in[0], nullptr, 0, T, converged, st);
+        const fls_config& cfg = h.cfg;
+        if (planar.n == 0) return FLS_ERR_NO_MAP;
+        size_t off[kMaxBatch], total = 0;
+        for (int s = 0; s < B; ++s) {
+            if (n_in[s] > 0x3fffffffull) return FLS_ERR_INVALID_ARG;
+            off[s] = total;
+            total += n_in[s];
+        }
+        if (total > 0x7fffffffull) return FLS_ERR_INVALID_ARG;  // flags and records of the batch are indexed by int
+        rec.reserve(total * 8 + 8);
+        flags.reserve(total + 1);
+        const GridView view = planar.grid.view();
+        return h.match_subgrids<LoamArgs>(cfg.method, 50, B, n_in, kLoamBlock / kLoamLanes, loam_max_grid(cfg.device), 16 + 16LL * 27 + 56, 16,
+                                          d_scans[0], T, converged, st,
+                                          [&](int s, LoamArgs& a) {
+                                              a.corner = nullptr;
+                                              a.n_corner = 0;
+                                              a.planar = d_scans[s];
+                                              a.n_planar = (int)n_in[s];
+                                              a.planar_map = view;
+                                              a.corner_map = view;
+                                              a.plane_thres = cfg.point_to_planar_thres;
+                                              a.search_thres = INFINITY;
+                                              a.line_ratio = cfg.line_ratio_thres;
+                                              a.gate = INFINITY;
+                                              a.state = h.state.p + s;
+                                              a.rec = rec.p + off[s] * 8;
+                                              a.flags = flags.p + off[s];
+                                          },
+                                          [&](const GnBatchItem<LoamArgs>* d_items, int grid) {
+                                              launch_loam_batch(d_items, B, flags.p, total, grid, h.stream);
+                                              if (total > 0) h.launches++;  // the flag reset in front of the loop
+                                          });
     }
 
     void map_info(fls_map_info* out) const override {  // planar map (+ corner map for LoamFull)

@@ -148,15 +148,16 @@ class Registration:
         check(rc, "fls_fitness")
         return float(out.value)
 
-    # -- batched Match (throughput entry; LoamPointToPlaneIVOX in localization mode) -----------------------------
+    # -- batched Match (throughput entry; LOAM-iVox, NDT, ICP and kd-tree point-to-plane in localization mode) -----
     def _batch_results(self, conv, st, Tc):
         self.last_batch_stats = list(st)
         self.last_stats = st[0]
         return np.array(conv[:], bool), np.transpose(Tc, (0, 2, 1)).copy()
 
     def match_batch(self, scans, Ts):
-        """scans: list of (n,4)/(n,8) host clouds; Ts: (B,4,4) float64 initial poses.  Returns (converged[B], T[B,4,4]);
-        self.last_batch_stats holds the per-scan fls_match_stats (call-level timings on element 0)."""
+        """scans: list of (n,4)/(n,8) host clouds — the planar clouds for the LOAM plug-ins, the ordered clouds for NDT and ICP (LoamFull
+        has no batch); Ts: (B,4,4) float64 initial poses.  Returns (converged[B], T[B,4,4]); self.last_batch_stats holds the per-scan
+        fls_match_stats (call-level timings on element 0)."""
         B = len(scans)
         keep, arr_p, arr_n, stride, Tc = _host_batch(scans, Ts)
         conv = (C.c_int * B)()

@@ -201,11 +201,16 @@ int fls_fitness(fls_handle* h, float max_range, float* score);
 
 /* Batched Match for throughput (the benchmark entry SURVEY.md §8b names): `n_scans` (<= 64) independent scans, each with its
  * own in-out pose T[s*16 .. s*16+15], converged[s] and stats[s], matched against the same map in ONE persistent launch.
- * Implemented for FLS_P2PLANE_IVOX (one persistent work-queue kernel for the batch) and FLS_NDT (one cooperative launch, a
- * sub-grid and a Gauss-Newton loop per scan); more than one scan requires localization_mode (Match must not modify the map).
- * For the LOAM-iVox plug-in the entry reads the planar clouds, for NDT the ordered clouds of the scans.
+ * Implemented for FLS_P2PLANE_IVOX (one persistent work-queue kernel for the batch) and for FLS_NDT, FLS_ICP_P2P and
+ * FLS_P2PLANE_KNN (one cooperative launch, a sub-grid and a Gauss-Newton loop per scan); more than one scan requires
+ * localization_mode (Match must not modify the map), and a batch of one is fls_match.  The LOAM-iVox and kd-tree point-to-plane
+ * plug-ins read each scan as its planar cloud, NDT and ICP as its ordered cloud (voxel-filtered once per distinct (pointer, count)).
+ * FLS_ICP_P2P: FLS_ERR_TOO_FEW_POINTS when any scan has 10 points or fewer and FLS_ERR_NO_MAP before a map, both before anything is
+ * uploaded or launched (T untouched).  FLS_LOAM_FULL reads two clouds per scan: FLS_ERR_UNSUPPORTED for any n_scans, no side effect.
+ * After a batch, fls_fitness scores scan 0's final pose on scan 0's source.
  * Call-level figures (gpu_ms, gpu_launches, byte counts, kernel_ms) are reported in stats[0]; per-scan fields everywhere.
- * Results are identical to n_scans separate fls_match calls.  The _device variant takes device pointers to packed float4 scans. */
+ * Results equal n_scans separate fls_match calls: the same converged flag, iterations and n_valid, poses within fp64 rounding (a
+ * sub-grid folds its CTA rows in another order than a whole grid).  The _device variant takes device pointers to packed float4 scans. */
 int fls_match_batch(fls_handle* h, int n_scans, const void* const* planar, const size_t* n, size_t stride_bytes, double* T_colmajor,
                     int* converged, fls_match_stats* stats);
 /* fls_match_batch in two halves, so that a caller with two handles overlaps the host->device copy of one batch with the kernels of
@@ -319,7 +324,8 @@ int fls_set_result_buffer_device(fls_handle* h, double* d_results, size_t capaci
 
 /* per-iteration log of the last fls_match (needs FLS_FLAG_ITER_LOG; batch: scan 0); returns the number of entries written */
 int fls_get_iter_log(const fls_handle* h, fls_iter_log* out, int capacity);
-/* the same for scan `scan` of the last Match call (the batch entries of FLS_P2PLANE_IVOX and FLS_NDT keep one log per scan);
+/* the same for scan `scan` of the last Match call (the batch entries of FLS_P2PLANE_IVOX, FLS_NDT,
+ * FLS_ICP_P2P and FLS_P2PLANE_KNN keep one log per scan);
  * FLS_ERR_INVALID_ARG when `scan` is not below that call's n_scans; a Match that fails after its launch leaves no log */
 int fls_get_iter_log_scan(const fls_handle* h, int scan, fls_iter_log* out, int capacity);
 
