@@ -1,7 +1,8 @@
-// fls_gn.cu — state initialisation of a Gauss-Newton loop (NDT / ICP / kd-tree LOAM; the LOAM-iVox path initialises its
-// states in its batch prep kernel), and the per-device kernel attributes that size and prepare every persistent launch.
-// The solve / update / stop rule itself (K6) is device code in fls_gn.cuh: gn_step_pre, which every persistent kernel runs, and
-// the single-level fold around it (gn_handover / gn_handover_rows), which every one but the LOAM-iVox batch kernel uses.
+// fls_gn.cu — state initialisation of a single NDT or ICP Match's Gauss-Newton loop (a sub-grid launch starts each scan with
+// gn_start_kernel, the LOAM-iVox path in its batch prep kernel), and the per-device kernel attributes that size and prepare every
+// persistent launch.  The solve / update / stop rule itself (K6) is device code in fls_gn.cuh: gn_step_pre, which every persistent
+// kernel runs, and the single-level fold around it (gn_handover / gn_handover_rows), which every one but the LOAM-iVox batch kernel
+// uses.
 // fls_gn_step_probe runs gn_step_pre alone on constructed cases, for the tests that hold the step to a reference.
 #include <map>
 #include <utility>
@@ -13,32 +14,11 @@
 namespace fls {
 namespace {
 
-__global__ void gn_init_kernel(GnState* s, double t00, double t10, double t20, double t01, double t11, double t21, double t02, double t12,
-                               double t22, double t03, double t13, double t23) {
-    if (threadIdx.x != 0) return;
-    // arguments are the column-major Mat4d entries T(r,c) named t<r><c>
-    const double R[9] = {t00, t01, t02, t10, t11, t12, t20, t21, t22};
-    const double t[3] = {t03, t13, t23};
-    for (int i = 0; i < 9; ++i) s->R[i] = s->R0[i] = s->Rprev[i] = R[i];
-    for (int i = 0; i < 3; ++i) s->t[i] = s->t0[i] = s->tprev[i] = t[i];
-    s->last_rot = s->last_pos = 0.0;
-    for (int i = 0; i < 36; ++i) s->H[i] = 0;
-    for (int i = 0; i < 6; ++i) s->g[i] = s->dx[i] = 0;
-    s->sum_res = 0;
-    s->cand_total = s->hits_total = 0;
-    s->n_valid = 0;
-    s->iter = 0;
-    s->done = 0;
-    s->converged = 0;
-    s->failed = 0;
-}
+__global__ void gn_init_kernel(GnState* s, GnPose p) { gn_state_init(s, p); }
 
 }  // namespace
 
-void launch_gn_init(GnState* d_state, const double* T, cudaStream_t st) {
-    // T is column-major: T[c*4 + r]
-    gn_init_kernel<<<1, 32, 0, st>>>(d_state, T[0], T[1], T[2], T[4], T[5], T[6], T[8], T[9], T[10], T[12], T[13], T[14]);
-}
+void launch_gn_init(GnState* d_state, const double* T, cudaStream_t st) { gn_init_kernel<<<1, 1, 0, st>>>(d_state, gn_pose(T)); }
 
 // ---- kernel attributes per device ----------------------------------------------------------------------------------------
 // Handles on different threads size their kernels concurrently: one lock over every entry.

@@ -33,8 +33,8 @@ struct GnLoopCtl {
 };
 static constexpr int kResultLen = 18;  // column-major 4x4 pose, converged, iterations
 
-// One scan of a batch in one cooperative launch (NDT, ICP, kd-tree LOAM): the plug-in's kernel arguments and control block, served
-// by CTAs [cta0, cta0 + ncta) of the grid, which run their own persistent loop (gn_batch_loop)
+// One scan of a sub-grid launch (a batch of NDT, ICP or kd-tree LOAM; a single kd-tree LOAM Match is a batch of one): the plug-in's
+// kernel arguments and control block, served by CTAs [cta0, cta0 + ncta) of the grid, which run their own persistent loop (gn_batch_loop)
 template <class Args>
 struct __align__(16) GnBatchItem {
     Args a;
@@ -43,9 +43,52 @@ struct __align__(16) GnBatchItem {
     int pad[2];
 };
 
-void launch_gn_init(GnState* d_state, const double* T_colmajor, cudaStream_t st);
+// the pose a loop starts from
+struct GnPose {
+    double R[9], t[3];  // row-major R
+};
+inline GnPose gn_pose(const double* T_colmajor) {
+    GnPose p;
+    for (int r = 0; r < 3; ++r) {
+        for (int c = 0; c < 3; ++c) p.R[r * 3 + c] = T_colmajor[c * 4 + r];
+        p.t[r] = T_colmajor[12 + r];
+    }
+    return p;
+}
+
+void launch_gn_init(GnState* d_state, const double* T_colmajor, cudaStream_t st);  // the state alone (single NDT / ICP Match)
 
 #ifdef __CUDACC__
+// a loop's state before its first iteration
+__device__ inline void gn_state_init(GnState* s, const GnPose& p) {
+    for (int i = 0; i < 9; ++i) s->R[i] = s->R0[i] = s->Rprev[i] = p.R[i];
+    for (int i = 0; i < 3; ++i) s->t[i] = s->t0[i] = s->tprev[i] = p.t[i];
+    s->last_rot = s->last_pos = 0.0;
+    for (int i = 0; i < 36; ++i) s->H[i] = 0;
+    for (int i = 0; i < 6; ++i) s->g[i] = s->dx[i] = 0;
+    s->sum_res = 0;
+    s->cand_total = s->hits_total = 0;
+    s->n_valid = 0;
+    s->iter = 0;
+    s->done = 0;
+    s->converged = 0;
+    s->failed = 0;
+}
+
+// The start of one scan's loop in a sub-grid launch: its state (item.ctl.state) from the pose, and the item itself to `dst`, where
+// the loop kernel finds it.  The item travels as a kernel argument, so a Match needs no copy of its own to send it.
+template <class Args>
+__global__ void gn_start_kernel(GnBatchItem<Args> item, GnBatchItem<Args>* dst, GnPose p) {
+    gn_state_init(item.ctl.state, p);
+    *dst = item;
+}
+
+// one launch of gn_start_kernel; T is the column-major 4x4 pose the scan starts from
+template <class Args>
+void launch_gn_start(const GnBatchItem<Args>& item, GnBatchItem<Args>* dst, const double* T, cudaStream_t st) {
+    gn_start_kernel<Args><<<1, 1, 0, st>>>(item, dst, gn_pose(T));
+}
+
 // ---- flag-in-data hand-over ("LL" records) ---------------------------------------------------------------------------
 // A 16-byte record {lo32, tag, hi32, tag} carries one double together with the tag of the iteration that produced it.
 // Each 8-byte half is a single-copy-atomic store, so a reader that sees the expected tag in BOTH halves has the value —
@@ -321,10 +364,11 @@ __device__ __forceinline__ bool gn_handover(double (&acc)[kNumAcc], const GnLoop
     return gn_handover_rows<BLOCK>(s_red, s_stop, c, tag, s_pose, cta, ncta);
 }
 
-// A batch of independent scans against the same (static) map in ONE cooperative launch: the grid is cut into one sub-grid per
-// scan, each running its own persistent Gauss-Newton loop (own rows, pose record and state) — the ~15 us hand-over of a scan
-// overlaps with the residual passes of the others, which is what the single-scan loop cannot hide at these sizes.  Each CTA finds
-// its item (items are in cta0 order), copies it to shared memory and runs loop(args, ctl, cta, ncta) on its sub-grid.
+// Independent scans against the same (static) map in ONE cooperative launch: the grid is cut into one sub-grid per scan, each
+// running its own persistent Gauss-Newton loop (own rows, pose record and state) — the ~15 us hand-over of a scan overlaps with the
+// residual passes of the others, which is what a lone scan's loop cannot hide at these sizes.  A single kd-tree LOAM Match is one
+// scan on the whole grid.  Each CTA finds its item (items are in cta0 order), copies it to shared memory and runs loop(args, ctl, cta, ncta) on
+// its sub-grid.
 template <int BLOCK, class Args, class Loop>
 __device__ __forceinline__ void gn_batch_loop(const GnBatchItem<Args>* __restrict__ items, int n_scans, Loop loop) {
     __shared__ GnBatchItem<Args> s_item;

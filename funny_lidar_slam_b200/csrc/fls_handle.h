@@ -95,8 +95,8 @@ struct Handle {
     // Gauss-Newton state shared by the plug-ins
     DevBuf<uint4> ll_rows;      // LL hand-over records of the persistent kernels: [grid][32] rows + pose records
     unsigned match_epoch = 0;   // tag prefix of those records
-    PinnedBuf<unsigned char> h_batch;  // staging of the per-batch tables (poses, offsets, scan descriptors, CTA map, pointers)
-    DevBuf<unsigned char> d_batch;
+    PinnedBuf<unsigned char> h_batch;  // staging of the LOAM-iVox per-batch tables (poses, offsets, scan descriptors, CTA map, pointers)
+    DevBuf<unsigned char> d_batch;     // their device copy, or the items of a match_subgrids launch
     DevBuf<GnState> state;
     GnState* h_state = nullptr;  // pinned
     DevBuf<fls_iter_log> log;
@@ -195,17 +195,19 @@ struct Handle {
         end_call(st);
         unpack(1, &n_source, T, converged, st);
     }
-    // ---- a batch Match on sub-grids of one cooperative launch (NDT, ICP, kd-tree LOAM) ----
+    // ---- a Match of one or more scans on sub-grids of one cooperative launch (NDT, ICP and kd-tree LOAM batches, kd-tree LOAM Match) ----
     // VoxelGridCloud of every distinct source of a batch, back to back in dst: scan s reads [off[s], off[s] + ns[s]), and a scan that
     // repeats an earlier (pointer, count) reads the range of its first occurrence.  FLS_ERR_INVALID_ARG past 2^30 filtered points.
     int filter_batch(int B, const float4* const* d, const size_t* n, float leaf, DevBuf<float4>& dst, size_t* off, size_t* ns);
-    // The Gauss-Newton half of such a batch.  Scan s (ns[s] points, also its n_source) gets one CTA per `per_cta` points, all scaled
-    // down together when the `cap` co-resident CTAs of the batch kernel cannot hold them (more scans than CTAs: FLS_ERR_INVALID_ARG).
-    // Then, per scan: its state from T, its control block and its item, whose arguments fill(s, item.a) sets; the gn_launch of
-    // launch(d_items, grid), the wait, and T / converged / stats of every scan.  src0: the source of scan 0 (GetFitnessScore).
+    // The Gauss-Newton half of such a Match; a single kd-tree LOAM Match is B = 1, whose sub-grid is the whole grid.  Scan s (ns[s]
+    // points, also its n_source) gets one CTA per `per_cta` points, all scaled down together when the `cap` co-resident CTAs of the
+    // kernel cannot hold them (more scans than CTAs: FLS_ERR_INVALID_ARG).  Then, per scan: its control block and its item, whose arguments
+    // fill(s, item.a) sets, and one launch that starts its state from T and writes the item to d_batch; the gn_launch of
+    // launch(d_items, grid), the wait, and T / converged / stats of every scan.  fit_src / fit_n: the cloud GetFitnessScore reads
+    // afterwards.
     template <class Args, class Fill, class Launch>
     int match_subgrids(int method, int min_effective, int B, const size_t* ns, int per_cta, int cap, long long point_iter_bytes, long long cand_bytes,
-                       const float4* src0, double* T, int* converged, fls_match_stats* st, Fill&& fill, Launch&& launch) {
+                       const float4* fit_src, size_t fit_n, double* T, int* converged, fls_match_stats* st, Fill&& fill, Launch&& launch) {
         int need[kMaxBatch], tot_need = 0;
         for (int s = 0; s < B; ++s) {
             need[s] = (int)((ns[s] + per_cta - 1) / per_cta);
@@ -219,14 +221,11 @@ struct Handle {
             grid += ncta[s];
         }
         const unsigned tag_base = next_ll_epoch((size_t)grid * 32 + (size_t)B * kLlPoseLen);
-        const size_t tbl_bytes = sizeof(GnBatchItem<Args>) * (size_t)B;
-        GnBatchItem<Args>* items = reinterpret_cast<GnBatchItem<Args>*>(batch_table(tbl_bytes));
+        GnBatchItem<Args>* d_items = reinterpret_cast<GnBatchItem<Args>*>(d_batch.reserve(sizeof(GnBatchItem<Args>) * (size_t)B));
         uint4* pose_base = ll_rows.p + (size_t)grid * 32;
         int cta0 = 0;
         for (int s = 0; s < B; ++s) {
-            launch_gn_init(state.p + s, T + 16 * s, stream);
-            launches++;
-            GnBatchItem<Args>& it = items[s];
+            GnBatchItem<Args> it;
             std::memset(&it, 0, sizeof(it));
             fill(s, it.a);
             it.ctl.state = state.p + s;
@@ -240,9 +239,10 @@ struct Handle {
             it.cta0 = cta0;
             it.ncta = ncta[s];
             cta0 += ncta[s];
+            launch_gn_start(it, d_items + s, T + 16 * s, stream);
+            launches++;
         }
-        send_batch_table(tbl_bytes);
-        gn_launch(point_iter_bytes, cand_bytes, src0, ns[0], [&] { launch(reinterpret_cast<const GnBatchItem<Args>*>(d_batch.p), grid); });
+        gn_launch(point_iter_bytes, cand_bytes, fit_src, fit_n, [&] { launch(d_items, grid); });
         read_back(B);
         end_call(st);
         unpack(B, ns, T, converged, st);

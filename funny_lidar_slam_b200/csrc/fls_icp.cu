@@ -228,8 +228,8 @@ class IcpPlugin final : public Plugin {
         const int rf = h.filter_batch(B, d_scans, n_in, cfg.source_cloud_filter_size, scan, off, ns);  // :57
         if (rf != FLS_OK) return rf;
         const GridView view = window.grid.view();
-        return h.match_subgrids<IcpArgs>(FLS_ICP_P2P, 0, B, ns, kIcpBlock / kIcpLanes, icp_max_grid(cfg.device), 16 + 16LL * 27, 16, scan.p + off[0], T,
-                                         converged, st,
+        return h.match_subgrids<IcpArgs>(FLS_ICP_P2P, 0, B, ns, kIcpBlock / kIcpLanes, icp_max_grid(cfg.device), 16 + 16LL * 27, 16, scan.p + off[0],
+                                         ns[0], T, converged, st,
                                          [&](int s, IcpArgs& a) {
                                              a.src = scan.p + off[s];
                                              a.n = (int)ns[s];

@@ -176,7 +176,7 @@ __device__ __forceinline__ bool corner_term(const float4* __restrict__ P, const 
 
 // One persistent launch runs every Gauss-Newton iteration of a Match, on the CTAs (cta, ncta) of the sub-grid that serves the scan.
 template <int BLOCK>
-__device__ __forceinline__ void loam_gn_loop(const LoamArgs a, const GnLoopCtl& ctl, const int cta, const int ncta) {
+__device__ __forceinline__ void loam_gn_loop(const LoamArgs& a, const GnLoopCtl& ctl, const int cta, const int ncta) {
     __shared__ double s_pose[12];
     const int n_total = a.n_corner + a.n_planar;
     const int sub = threadIdx.x & (kLoamLanes - 1);
@@ -237,14 +237,9 @@ __device__ __forceinline__ void loam_gn_loop(const LoamArgs a, const GnLoopCtl& 
     }
 }
 
+// every scan of a Match on its own sub-grid (gn_batch_loop, fls_gn.cuh); each scan's records and flags are its own range of one buffer
 template <int BLOCK>
-__global__ void __launch_bounds__(BLOCK) loam_gn_kernel(LoamArgs a, GnLoopCtl ctl) {
-    loam_gn_loop<BLOCK>(a, ctl, (int)blockIdx.x, (int)gridDim.x);
-}
-
-// a batch of scans, one sub-grid each (gn_batch_loop, fls_gn.cuh); each scan's records and flags are its own range of one buffer
-template <int BLOCK>
-__global__ void __launch_bounds__(BLOCK) loam_gn_batch_kernel(const GnBatchItem<LoamArgs>* __restrict__ items, int n_scans) {
+__global__ void __launch_bounds__(BLOCK) loam_gn_kernel(const GnBatchItem<LoamArgs>* __restrict__ items, int n_scans) {
     gn_batch_loop<BLOCK>(items, n_scans, [](const LoamArgs& a, const GnLoopCtl& ctl, int cta, int ncta) { loam_gn_loop<BLOCK>(a, ctl, cta, ncta); });
 }
 
@@ -255,22 +250,11 @@ __global__ void loam_clear_flags_kernel(unsigned char* flags, int n) {
 
 }  // namespace
 
-static int loam_grid_blocks(int n, int device) {
-    const int per_block = kLoamBlock / kLoamLanes;
-    return clamp_grid((n + per_block - 1) / per_block, coresident_ctas((const void*)loam_gn_kernel<kLoamBlock>, kLoamBlock, 0, device));
-}
-
-static void launch_loam_loop(const LoamArgs& a, const GnLoopCtl& ctl, int grid, cudaStream_t st) {
-    const int n = a.n_corner + a.n_planar;
-    if (n > 0) loam_clear_flags_kernel<<<(n + 255) / 256, 256, 0, st>>>(a.flags, n);
-    launch_cooperative(loam_gn_kernel<kLoamBlock>, grid, kLoamBlock, 0, st, a, ctl);
-}
-
-static int loam_max_grid(int device) { return coresident_ctas((const void*)loam_gn_batch_kernel<kLoamBlock>, kLoamBlock, 0, device); }
-// clears the flags of every scan of the batch (n of them in all) in one launch, then the batch kernel
-static void launch_loam_batch(const GnBatchItem<LoamArgs>* d_items, int n_scans, unsigned char* flags, size_t n, int grid, cudaStream_t st) {
+static int loam_max_grid(int device) { return coresident_ctas((const void*)loam_gn_kernel<kLoamBlock>, kLoamBlock, 0, device); }
+// clears the flags of every scan of the Match (n of them in all) in one launch when there are any, then the loop kernel
+static void launch_loam(const GnBatchItem<LoamArgs>* d_items, int n_scans, unsigned char* flags, size_t n, int grid, cudaStream_t st) {
     if (n > 0) loam_clear_flags_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(flags, (int)n);
-    launch_cooperative(loam_gn_batch_kernel<kLoamBlock>, grid, kLoamBlock, 0, st, d_items, n_scans);
+    launch_cooperative(loam_gn_kernel<kLoamBlock>, grid, kLoamBlock, 0, st, d_items, n_scans);
 }
 
 // ---- LoamPointToPlaneKdtree / LoamFull -------------------------------------------------------------------------------
@@ -290,6 +274,50 @@ class KdPlugin final : public Plugin {
     DevBuf<double> rec;          // persistent {J[6], residual} records
     DevBuf<unsigned char> flags;
     DevBuf<float4> ins, ins_corner;  // Match-internal insert: the features at their final pose
+
+    // The Match of B scans, in ONE cooperative launch (loam_gn_kernel — one sub-grid and one persistent Gauss-Newton loop per scan).
+    // Scan s is the planar features d_planar[s] (n_planar[s] points) and, when d_corner is given (LoamFull), the corner features
+    // d_corner[s] (n_corner[s] points); it owns records and flags [off[s], off[s] + its points) of one buffer, cleared together.
+    int match_scans(int B, const float4* const* d_planar, const size_t* n_planar, const float4* const* d_corner, const size_t* n_corner, double* T,
+                    int* converged, fls_match_stats* st) {
+        const fls_config& cfg = h.cfg;
+        if (planar.n == 0) return FLS_ERR_NO_MAP;
+        size_t ns[kMaxBatch], off[kMaxBatch], total = 0;
+        for (int s = 0; s < B; ++s) {
+            ns[s] = n_planar[s] + (d_corner ? n_corner[s] : 0);
+            if (ns[s] > 0x3fffffffull) return FLS_ERR_INVALID_ARG;
+            off[s] = total;
+            total += ns[s];
+        }
+        if (total > 0x7fffffffull) return FLS_ERR_INVALID_ARG;  // flags and records of a Match are indexed by int
+        rec.reserve(total * 8 + 8);
+        flags.reserve(total + 1);
+        const GridView planar_view = planar.grid.view();
+        const GridView corner_view = full ? corner->grid.view() : planar_view;
+        // roofline accounting (K5): 16 B source point + 27 x 16 B slot probes + 56 B persistent record, 16 B per scanned map record.
+        // GetFitnessScore reads the planar features.
+        return h.match_subgrids<LoamArgs>(cfg.method, 50, B, ns, kLoamBlock / kLoamLanes, loam_max_grid(cfg.device), 16 + 16LL * 27 + 56, 16,
+                                          d_planar[0], n_planar[0], T, converged, st,
+                                          [&](int s, LoamArgs& a) {
+                                              a.corner = d_corner ? d_corner[s] : nullptr;
+                                              a.n_corner = d_corner ? (int)n_corner[s] : 0;
+                                              a.planar = d_planar[s];
+                                              a.n_planar = (int)n_planar[s];
+                                              a.planar_map = planar_view;
+                                              a.corner_map = corner_view;
+                                              a.plane_thres = cfg.point_to_planar_thres;
+                                              a.search_thres = full ? cfg.point_search_thres : INFINITY;
+                                              a.line_ratio = cfg.line_ratio_thres;
+                                              a.gate = full ? (float)cfg.point_search_thres * 1.0001f : INFINITY;
+                                              a.state = h.state.p + s;
+                                              a.rec = rec.p + off[s] * 8;
+                                              a.flags = flags.p + off[s];
+                                          },
+                                          [&](const GnBatchItem<LoamArgs>* d_items, int grid) {
+                                              launch_loam(d_items, B, flags.p, total, grid, h.stream);
+                                              if (total > 0) h.launches++;  // the flag reset in front of the loop
+                                          });
+    }
 
   public:
     explicit KdPlugin(Handle& handle) : Plugin(handle, handle.cfg.method == FLS_LOAM_FULL ? kPlanarCorner : kPlanar), full(reads == kPlanarCorner) {
@@ -328,31 +356,8 @@ class KdPlugin final : public Plugin {
     int match(const float4* d_planar, size_t n_planar, const float4* d_corner, size_t n_corner, double* T, int* converged,
               fls_match_stats* st) override {
         const fls_config& cfg = h.cfg;
-        if (planar.n == 0) return FLS_ERR_NO_MAP;
-        const size_t n = n_planar + n_corner;
-        const int ni = (int)n;
-        const int grid = loam_grid_blocks(ni, cfg.device);
-        rec.reserve(n * 8 + 8);
-        flags.reserve(n + 1);
-        LoamArgs a;
-        a.corner = d_corner;
-        a.n_corner = (int)n_corner;
-        a.planar = d_planar;
-        a.n_planar = (int)n_planar;
-        a.planar_map = planar.grid.view();
-        a.corner_map = full ? corner->grid.view() : a.planar_map;
-        a.plane_thres = cfg.point_to_planar_thres;
-        a.search_thres = full ? cfg.point_search_thres : INFINITY;
-        a.line_ratio = cfg.line_ratio_thres;
-        a.gate = full ? (float)cfg.point_search_thres * 1.0001f : INFINITY;
-        a.state = h.state.p;
-        a.rec = rec.p;
-        a.flags = flags.p;
-        // roofline accounting (K5): 16 B source point + 27 x 16 B slot probes + 56 B persistent record, 16 B per scanned map record
-        h.match_single(cfg.method, 50, grid, 16 + 16LL * 27 + 56, 16, d_planar, n_planar, n, T, converged, st, [&](const GnLoopCtl& ctl) {
-            launch_loam_loop(a, ctl, grid, h.stream);
-            h.launches++;  // the flag reset in front of the loop
-        });
+        const int rc = match_scans(1, &d_planar, &n_planar, &d_corner, &n_corner, T, converged, st);
+        if (rc != FLS_OK) return rc;
         // key-frame insertion: loam_point_to_plane_kdtree.h:146-150 (gate evaluated before the mode test), loam_full_kdtree.h:178-186
         if (h.h_state->converged && gate.need(T, cfg.dist_thre_add_cloud, cfg.rot_thre_add_cloud) && (full || !cfg.localization_mode)) {
             int rc2;
@@ -375,10 +380,8 @@ class KdPlugin final : public Plugin {
     }
 
     // n_scans independent LoamPointToPlaneKdtree::Match calls on planar features against the same (static) map in ONE cooperative
-    // launch (loam_gn_batch_kernel — one sub-grid and one persistent Gauss-Newton loop per scan).  Scan s owns records and flags
-    // [off[s], off[s] + n[s]) of one buffer, cleared together.  The key-frame gate is left alone: in localization mode nothing is
-    // inserted, so its last_T cannot be observed.  A batch of one is the single Match; LoamFull reads two clouds per scan and has no
-    // batch.
+    // launch.  The key-frame gate is left alone: in localization mode nothing is inserted, so its last_T cannot be observed.  A
+    // batch of one is the single Match; LoamFull reads two clouds per scan and has no batch.
     int match_batch(int B, const void* const* scans, const size_t* n_in, size_t host_stride, double* T, int* converged,
                     fls_match_stats* st) override {
         if (full) return FLS_ERR_UNSUPPORTED;
@@ -386,39 +389,7 @@ class KdPlugin final : public Plugin {
         const int rc = h.begin_batch(B, scans, n_in, host_stride, d_scans, st);
         if (rc != FLS_OK) return rc;
         if (B == 1) return match(d_scans[0], n_in[0], nullptr, 0, T, converged, st);
-        const fls_config& cfg = h.cfg;
-        if (planar.n == 0) return FLS_ERR_NO_MAP;
-        size_t off[kMaxBatch], total = 0;
-        for (int s = 0; s < B; ++s) {
-            if (n_in[s] > 0x3fffffffull) return FLS_ERR_INVALID_ARG;
-            off[s] = total;
-            total += n_in[s];
-        }
-        if (total > 0x7fffffffull) return FLS_ERR_INVALID_ARG;  // flags and records of the batch are indexed by int
-        rec.reserve(total * 8 + 8);
-        flags.reserve(total + 1);
-        const GridView view = planar.grid.view();
-        return h.match_subgrids<LoamArgs>(cfg.method, 50, B, n_in, kLoamBlock / kLoamLanes, loam_max_grid(cfg.device), 16 + 16LL * 27 + 56, 16,
-                                          d_scans[0], T, converged, st,
-                                          [&](int s, LoamArgs& a) {
-                                              a.corner = nullptr;
-                                              a.n_corner = 0;
-                                              a.planar = d_scans[s];
-                                              a.n_planar = (int)n_in[s];
-                                              a.planar_map = view;
-                                              a.corner_map = view;
-                                              a.plane_thres = cfg.point_to_planar_thres;
-                                              a.search_thres = INFINITY;
-                                              a.line_ratio = cfg.line_ratio_thres;
-                                              a.gate = INFINITY;
-                                              a.state = h.state.p + s;
-                                              a.rec = rec.p + off[s] * 8;
-                                              a.flags = flags.p + off[s];
-                                          },
-                                          [&](const GnBatchItem<LoamArgs>* d_items, int grid) {
-                                              launch_loam_batch(d_items, B, flags.p, total, grid, h.stream);
-                                              if (total > 0) h.launches++;  // the flag reset in front of the loop
-                                          });
+        return match_scans(B, d_scans, n_in, nullptr, nullptr, T, converged, st);
     }
 
     void map_info(fls_map_info* out) const override {  // planar map (+ corner map for LoamFull)

@@ -671,7 +671,7 @@ class NdtPlugin final : public Plugin {
         if (rf != FLS_OK) return rf;
         const NdtView view = map.view();
         return h.match_subgrids<NdtArgs>(FLS_NDT, cfg.ndt_min_effective_pts, B, ns, kNdtBlock, ndt_max_grid(cfg.device), 16 + 16LL * 7, 80,
-                                         scan.p + off[0], T, converged, st,
+                                         scan.p + off[0], ns[0], T, converged, st,
                                          [&](int s, NdtArgs& a) {
                                              a.src = scan.p + off[s];
                                              a.n = (int)ns[s];
