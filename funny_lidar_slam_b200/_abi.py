@@ -100,6 +100,15 @@ class FlsRelocResult(C.Structure):
                 ("host_waits", C.c_int32), ("gpu_launches", C.c_int32)]
 
 
+class FlsScCfg(C.Structure):
+    """fls_sc_cfg: the Scan Context descriptor's shape (include/fls_b200.h)"""
+    _fields_ = [("n_rings", C.c_int32), ("n_sectors", C.c_int32), ("max_radius", C.c_float), ("z_offset", C.c_float)]
+
+
+class FlsPlaceMatch(C.Structure):
+    _fields_ = [("id", C.c_int64), ("distance", C.c_double), ("yaw", C.c_double), ("shift", C.c_int32), ("reserved", C.c_int32)]
+
+
 class FlsFeatureCfg(C.Structure):
     _fields_ = [("corner_threshold", C.c_float), ("planar_threshold", C.c_float), ("device", C.c_int32), ("reserved", C.c_int32)]
 

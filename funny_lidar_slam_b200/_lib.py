@@ -6,7 +6,7 @@ import ctypes as C
 import os
 
 from ._abi import (FlsConfig, FlsConvertCfg, FlsConvertResult, FlsFeatureCfg, FlsIterLog, FlsLoamFrontendCfg, FlsMapInfo, FlsMatchStats,
-                   FlsPointCloud2, FlsRelocCfg, FlsRelocResult)
+                   FlsPlaceMatch, FlsPointCloud2, FlsRelocCfg, FlsRelocResult, FlsScCfg)
 
 _PKG = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_PKG, "libfls_b200.so")
@@ -21,6 +21,7 @@ EXPORTS = [
     "fls_preprocess_device", "fls_keyframes_create", "fls_keyframes_destroy", "fls_keyframes_add", "fls_keyframes_add_device",
     "fls_keyframes_count", "fls_keyframes_assemble", "fls_get_ndt_voxels", "fls_gn_step_probe",
     "fls_relocalize", "fls_relocalize_device", "fls_relocalize_wide", "fls_relocalize_wide_device", "fls_relocalize_wide_levels",
+    "fls_keyframes_scan_context", "fls_keyframes_detect_loop", "fls_keyframes_place_query", "fls_keyframes_place_query_device",
 ]
 
 
@@ -99,6 +100,11 @@ def lib():
     L.fls_keyframes_add_device.argtypes = [vp, C.c_int64, vp, sz]
     L.fls_keyframes_count.argtypes = [vp, C.POINTER(sz), C.POINTER(sz)]
     L.fls_keyframes_assemble.argtypes = [vp, vp, sz, vp, f32, f32, vp, sz, vp, vp, sz, C.POINTER(sz), C.POINTER(FlsMatchStats)]
+    sc, pm, st = C.POINTER(FlsScCfg), C.POINTER(FlsPlaceMatch), C.POINTER(FlsMatchStats)
+    L.fls_keyframes_scan_context.argtypes = [vp, sc, vp, sz, vp]
+    L.fls_keyframes_detect_loop.argtypes = [vp, sc, C.c_int64, C.c_int64, sz, pm, C.POINTER(sz), st]
+    L.fls_keyframes_place_query.argtypes = [vp, sc, vp, sz, sz, sz, pm, C.POINTER(sz), vp, st]
+    L.fls_keyframes_place_query_device.argtypes = [vp, sc, vp, sz, sz, pm, C.POINTER(sz), vp, st]
     for name in EXPORTS:
         getattr(L, name)  # AttributeError if the ABI drifted
     if L.fls_abi_version() != 1:

@@ -20,12 +20,12 @@
 #include <vector>
 
 #include "fls_maps.h"
+#include "fls_place.h"
 #include "fls_voxel.cuh"
 
 namespace fls {
 namespace {
 
-constexpr int kTile = 8192;    // points of one segment handled by one block of the bbox / key kernels
 constexpr int kThreads = 256;
 
 struct KfSeg {                    // one keyframe of the selection (64 B)
@@ -127,6 +127,9 @@ struct KeyframeStore {
     DevBuf<float4> cat, fin;
     BuildScratch sc;  // segmented pass (keys, keys_sorted, uniq, idx, idx_sorted, counts, starts, cub_tmp, num_runs)
     BuildScratch vg;  // final voxel_grid_device pass
+    PlaceIndex place;                 // Scan Context descriptors (fls_place.cu)
+    DevBuf<float4> query;             // a host scan query, uploaded
+    PinnedBuf<unsigned char> h_out;   // read-back of the place entries
 
     KeyframeStore(int dev, size_t cap) : device(dev), capacity(cap) {
         try {
@@ -143,6 +146,7 @@ struct KeyframeStore {
     ~KeyframeStore() { release(); }
     void release() {
         h_table.release();
+        h_out.release();
         if (arena) cudaFree(arena);
         if (ev0) cudaEventDestroy(ev0);
         if (ev1) cudaEventDestroy(ev1);
@@ -287,6 +291,73 @@ struct KeyframeStore {
         }
         return FLS_OK;
     }
+
+    // fls_keyframes_scan_context
+    int scan_context(const fls_sc_cfg& cfg, const int64_t* ids, size_t n_ids, float* desc) {
+        std::lock_guard<std::mutex> lk(mu);
+        for (size_t k = 0; k < n_ids; ++k)
+            if (ids[k] < 0 || ids[k] >= (int64_t)count.size()) return FLS_ERR_INVALID_ARG;
+        FLS_CUDA(cudaSetDevice(device));
+        int launches = 0;
+        long long h2d = 0;
+        place.describe(cfg, arena, begin, count, nullptr, 0, false, stream, &launches, &h2d);
+        const size_t nc = place.n_cells();
+        float* h = reinterpret_cast<float*>(h_out.reserve(std::max<size_t>(n_ids * nc * sizeof(float), 1)));
+        for (size_t k = 0; k < n_ids; ++k)
+            FLS_CUDA(cudaMemcpyAsync(h + k * nc, place.desc((size_t)ids[k]), nc * sizeof(float), cudaMemcpyDeviceToHost, stream));
+        FLS_CUDA(cudaStreamSynchronize(stream));
+        if (n_ids) std::memcpy(desc, h, n_ids * nc * sizeof(float));
+        return FLS_OK;
+    }
+
+    // fls_keyframes_detect_loop (query_id >= 0) and fls_keyframes_place_query(_device) (query_id < 0: the scan pts)
+    int place_match(const fls_sc_cfg& cfg, int64_t query_id, int64_t min_span, const void* pts, size_t n, size_t stride, bool on_device, size_t k,
+                    fls_place_match* out, size_t* n_found, float* query_desc, fls_match_stats* stats) {
+        std::lock_guard<std::mutex> lk(mu);
+        const size_t K = count.size();
+        const bool scan = query_id < 0;
+        if (!scan && query_id >= (int64_t)K) return FLS_ERR_INVALID_ARG;
+        const size_t n_cand = scan ? K : (size_t)std::max<int64_t>(0, query_id - min_span);  // ids with query_id - id > min_span
+        const size_t n_out = std::min(k, n_cand);
+        FLS_CUDA(cudaSetDevice(device));
+        int launches = 0;
+        long long h2d = 0, d2h = 0;
+        FLS_CUDA(cudaEventRecord(ev0, stream));
+        const float4* d_query = nullptr;
+        if (scan && n) {
+            if (on_device) {
+                d_query = reinterpret_cast<const float4*>(pts);
+            } else {
+                query.reserve(n);
+                upload_records(pts, n, stride, query.p, raw, stream, &h2d, &launches);
+                d_query = query.p;
+            }
+        }
+        const size_t n_read = place.describe(cfg, arena, begin, count, d_query, n, scan, stream, &launches, &h2d);
+        const size_t q = scan ? K : (size_t)query_id, nc = place.n_cells();
+        const size_t off_desc = (n_out * sizeof(fls_place_match) + 15) & ~size_t(15);
+        unsigned char* h = h_out.reserve(off_desc + nc * sizeof(float));
+        if (n_cand) {
+            place.search(q, n_cand, n_out, reinterpret_cast<fls_place_match*>(h), stream, device, &launches);
+            d2h += (long long)(n_out * sizeof(fls_place_match));
+        }
+        if (query_desc) {
+            FLS_CUDA(cudaMemcpyAsync(h + off_desc, place.desc(q), nc * sizeof(float), cudaMemcpyDeviceToHost, stream));
+            d2h += (long long)(nc * sizeof(float));
+        }
+        FLS_CUDA(cudaEventRecord(ev1, stream));
+        FLS_CUDA(cudaStreamSynchronize(stream));
+        if (n_out) std::memcpy(out, h, n_out * sizeof(fls_place_match));
+        if (query_desc) std::memcpy(query_desc, h + off_desc, nc * sizeof(float));
+        *n_found = n_out;
+        if (stats) {
+            fill_call_stats(stats, ev0, ev1, launches, h2d, d2h);
+            stats->iterations = 1;
+            stats->n_source = (int64_t)n_read;
+            stats->n_valid = (int64_t)n_cand;
+        }
+        return FLS_OK;
+    }
 };
 
 }  // namespace fls
@@ -349,6 +420,45 @@ int fls_keyframes_assemble(fls_keyframes* s, const int64_t* ids, size_t n_ids, c
     FLS_TRY
     return reinterpret_cast<fls::KeyframeStore*>(s)->assemble(ids, n_ids, T_colmajor, leaf, final_leaf, reinterpret_cast<const float4*>(d_base),
                                                               n_base, out, reinterpret_cast<float4*>(d_out), capacity, n_out, stats);
+    FLS_CATCH
+}
+
+int fls_keyframes_scan_context(fls_keyframes* s, const fls_sc_cfg* cfg, const int64_t* ids, size_t n_ids, float* desc) {
+    if (!s || !cfg || !fls::sc_cfg_ok(*cfg) || (n_ids && (!ids || !desc))) return FLS_ERR_INVALID_ARG;
+    FLS_TRY
+    return reinterpret_cast<fls::KeyframeStore*>(s)->scan_context(*cfg, ids, n_ids, desc);
+    FLS_CATCH
+}
+
+int fls_keyframes_detect_loop(fls_keyframes* s, const fls_sc_cfg* cfg, int64_t query_id, int64_t min_span, size_t k, fls_place_match* out,
+                              size_t* n_found, fls_match_stats* stats) {
+    if (!n_found) return FLS_ERR_INVALID_ARG;
+    *n_found = 0;
+    if (!s || !cfg || !fls::sc_cfg_ok(*cfg) || k < 1 || !out || query_id < 0 || min_span < 0) return FLS_ERR_INVALID_ARG;
+    FLS_TRY
+    return reinterpret_cast<fls::KeyframeStore*>(s)->place_match(*cfg, query_id, min_span, nullptr, 0, 0, false, k, out, n_found, nullptr, stats);
+    FLS_CATCH
+}
+
+int fls_keyframes_place_query(fls_keyframes* s, const fls_sc_cfg* cfg, const void* pts, size_t n, size_t stride_bytes, size_t k,
+                              fls_place_match* out, size_t* n_found, float* query_desc, fls_match_stats* stats) {
+    if (!n_found) return FLS_ERR_INVALID_ARG;
+    *n_found = 0;
+    if (!s || !cfg || !fls::sc_cfg_ok(*cfg) || k < 1 || !out || (!pts && n) || n > 0xffffffffull || !fls::stride_ok(stride_bytes))
+        return FLS_ERR_INVALID_ARG;
+    FLS_TRY
+    return reinterpret_cast<fls::KeyframeStore*>(s)->place_match(*cfg, -1, 0, pts, n, stride_bytes, false, k, out, n_found, query_desc, stats);
+    FLS_CATCH
+}
+
+int fls_keyframes_place_query_device(fls_keyframes* s, const fls_sc_cfg* cfg, const void* d_pts, size_t n, size_t k, fls_place_match* out,
+                                     size_t* n_found, float* query_desc, fls_match_stats* stats) {
+    if (!n_found) return FLS_ERR_INVALID_ARG;
+    *n_found = 0;
+    if (!s || !cfg || !fls::sc_cfg_ok(*cfg) || k < 1 || !out || (!d_pts && n) || n > 0xffffffffull) return FLS_ERR_INVALID_ARG;
+    FLS_TRY
+    return reinterpret_cast<fls::KeyframeStore*>(s)->place_match(*cfg, -1, 0, d_pts, n, FLS_LAYOUT_PACKED, true, k, out, n_found, query_desc,
+                                                                 stats);
     FLS_CATCH
 }
 

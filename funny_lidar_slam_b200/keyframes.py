@@ -10,6 +10,10 @@ The three helpers below restate the upstream sites that run this primitive: `sav
 src/slam/system.cpp:299-341), `global_map_round` (one round of System::VisualizeGlobalMap, src/slam/system.cpp:847-896) and
 `loopclosure_submap` (LoopClosure::GetSubMap, src/slam/loop_closure.cpp:179-231).  Poses are (4, 4) float64 matrices, one per
 keyframe id; clouds are (n,4) packed x,y,z,intensity or (n,8) pcl::PointXYZI float32 records.
+
+Place recognition by Scan Context (include/fls_b200.h, DESIGN.md §3.12): `detect_loop` is LoopClosure::DetectByFeature
+(src/slam/loop_closure.cpp:62-64, a stub upstream) and `place_query` finds the keyframe a scan was taken near.  Each returns
+PlaceMatch records ordered by (distance, id); `place_pose` turns one into the coarse pose T_kf @ Rz(yaw) that fls_relocalize refines.
 """
 from __future__ import annotations
 
@@ -17,9 +21,23 @@ import ctypes as C
 
 import numpy as np
 
-from ._abi import FlsMatchStats
+from ._abi import FlsMatchStats, FlsPlaceMatch, FlsScCfg
 from ._lib import check, lib
 from .registration import _batch_poses, _cloud
+
+
+def sc_cfg(n_rings: int = 20, n_sectors: int = 60, max_radius: float = 80.0, z_offset: float = 2.0) -> FlsScCfg:
+    """fls_sc_cfg; the defaults are the paper's 20 rings x 60 sectors out to 80 m, with z lifted by the sensor height."""
+    c = FlsScCfg()
+    c.n_rings, c.n_sectors, c.max_radius, c.z_offset = int(n_rings), int(n_sectors), float(max_radius), float(z_offset)
+    return c
+
+
+def place_pose(T_keyframe, yaw: float) -> np.ndarray:
+    """The coarse world pose of a query matched to a keyframe at pose T_keyframe with relative yaw `yaw`: T_keyframe @ Rz(yaw)."""
+    Rz = np.eye(4)
+    Rz[:2, :2] = [[np.cos(yaw), -np.sin(yaw)], [np.sin(yaw), np.cos(yaw)]]
+    return np.asarray(T_keyframe, np.float64) @ Rz
 
 
 class KeyFrameStore:
@@ -98,6 +116,52 @@ class KeyFrameStore:
         check(rc, "fls_keyframes_assemble")
         self.last_stats = st
         return out[:n_out.value].copy() if host_out else None
+
+    # -- place recognition (Scan Context) ---------------------------------------------------------------------------------------
+    def scan_context(self, ids, cfg: FlsScCfg | None = None) -> np.ndarray:
+        """The descriptors of keyframes `ids` as (len(ids), n_rings, n_sectors) float32."""
+        c = cfg or sc_cfg()
+        ids = np.ascontiguousarray(np.asarray(ids, np.int64).reshape(-1))
+        out = np.empty((len(ids), c.n_rings, c.n_sectors), np.float32)
+        check(lib().fls_keyframes_scan_context(self._s, C.byref(c), ids.ctypes.data_as(C.c_void_p), len(ids), out.ctypes.data_as(C.c_void_p)),
+              "fls_keyframes_scan_context")
+        return out
+
+    def _matches(self, call, k: int, where: str):
+        buf = (FlsPlaceMatch * max(int(k), 1))()
+        n = C.c_size_t(0)
+        st = FlsMatchStats()
+        check(call(int(k), buf, C.byref(n), C.byref(st)), where)
+        self.last_stats = st
+        return buf[:n.value]
+
+    def detect_loop(self, query_id: int, min_span: int, k: int = 1, cfg: FlsScCfg | None = None):
+        """LoopClosure::DetectByFeature: the k stored keyframes with query_id - id > min_span nearest to keyframe query_id, as
+        FlsPlaceMatch records ordered by (distance, id).  No distance threshold is applied."""
+        c = cfg or sc_cfg()
+        return self._matches(lambda k_, b, n, st: lib().fls_keyframes_detect_loop(self._s, C.byref(c), int(query_id), int(min_span), k_, b, n, st), k,
+                             "fls_keyframes_detect_loop")
+
+    def place_query(self, cloud, k: int = 1, cfg: FlsScCfg | None = None, return_desc: bool = False):
+        """The k stored keyframes nearest to the scan `cloud` ((n,4) or (n,8) float32, sensor frame).  With return_desc, also the
+        scan's descriptor: (matches, (n_rings, n_sectors) float32)."""
+        c = cfg or sc_cfg()
+        p, n, s, keep = _cloud(cloud)
+        desc = np.empty((c.n_rings, c.n_sectors), np.float32)
+        dp = desc.ctypes.data_as(C.c_void_p) if return_desc else None
+        m = self._matches(lambda k_, b, n_, st: lib().fls_keyframes_place_query(self._s, C.byref(c), p, n, s, k_, b, n_, dp, st), k,
+                          "fls_keyframes_place_query")
+        return (m, desc) if return_desc else m
+
+    def place_query_device(self, d_points: int, n: int, k: int = 1, cfg: FlsScCfg | None = None, return_desc: bool = False):
+        """place_query with a scan of n packed float4 records in device memory on the store's device."""
+        c = cfg or sc_cfg()
+        desc = np.empty((c.n_rings, c.n_sectors), np.float32)
+        dp = desc.ctypes.data_as(C.c_void_p) if return_desc else None
+        d = C.c_void_p(int(d_points)) if d_points else None
+        m = self._matches(lambda k_, b, n_, st: lib().fls_keyframes_place_query_device(self._s, C.byref(c), d, int(n), k_, b, n_, dp, st), k,
+                          "fls_keyframes_place_query_device")
+        return (m, desc) if return_desc else m
 
 
 def save_map_cloud(store: KeyFrameStore, poses, leaf: float = 0.3, final_leaf: float = 0.3):

@@ -8,6 +8,9 @@
 //   System::SaveMap            (src/slam/system.cpp:310-329)  -> SaveMap
 //   System::VisualizeGlobalMap (src/slam/system.cpp:864-893)  -> GlobalMap::Round
 //   LoopClosure::GetSubMap     (src/slam/loop_closure.cpp:188-230) -> GetSubMap
+// and adds place recognition by Scan Context (fls_keyframes_detect_loop / _place_query):
+//   LoopClosure::DetectByFeature (src/slam/loop_closure.cpp:120-122, a stub upstream) -> DetectLoopByFeature
+//   the keyframe a scan was taken near, for Localization::Init without a clicked pose     -> PlaceQuery
 // Each takes the keyframes (for their current pose_) under the caller's mutex_keyframes_, as upstream does.  The store serializes
 // calls from the three threads itself.  Poses relative to a reference keyframe are computed here with the caller's Eigen
 // (loop_closure.cpp:210-215), so the library receives final poses.
@@ -83,6 +86,40 @@ public:
         std::vector<float> map;
         Run(ids, poses, 0.2f, 0.f, nullptr, 0, &map, nullptr, 0);
         return ToCloud(map);
+    }
+
+    // Scan Context result: the candidate keyframe, its descriptor distance and the yaw that turns the query into its frame
+    // (keyframe pose * Rz(yaw) is the query's coarse pose).  candidate_id stays invalid when there is none.
+    struct PlaceMatch {
+        KeyFrame::ID candidate_id = -1;  // KeyFrame::kInvalidID (include/common/keyframe.h:17)
+        double distance = 1.0;
+        double yaw = 0.0;
+    };
+
+    // LoopClosure::DetectByFeature: the best keyframe with curr_id - id > skip_near_keyframe_threshold (the span rule of
+    // CheckCandidateKeyFrames, loop_closure.cpp:171).  The caller compares distance against its threshold and then takes the
+    // GetSubMap path with std::make_pair(curr_id, candidate_id).
+    PlaceMatch DetectLoopByFeature(KeyFrame::ID curr_id, KeyFrame::ID skip_near_keyframe_threshold) {
+        fls_place_match m{};
+        size_t n = 0;
+        PlaceMatch r;
+        if (Ok(fls_keyframes_detect_loop(store_, &sc_cfg_, curr_id, skip_near_keyframe_threshold, 1, &m, &n, nullptr), "fls_keyframes_detect_loop") &&
+            n == 1)
+            r = PlaceMatch{static_cast<KeyFrame::ID>(m.id), m.distance, m.yaw};
+        return r;
+    }
+
+    // the stored keyframe nearest to a scan (its ordered cloud, sensor frame)
+    PlaceMatch PlaceQuery(const PCLPointCloudXYZI& cloud) {
+        fls_place_match m{};
+        size_t n = 0;
+        PlaceMatch r;
+        if (Ok(fls_keyframes_place_query(store_, &sc_cfg_, cloud.points.data(), cloud.points.size(), sizeof(PCLPointXYZI), 1, &m, &n, nullptr,
+                                         nullptr),
+               "fls_keyframes_place_query") &&
+            n == 1)
+            r = PlaceMatch{static_cast<KeyFrame::ID>(m.id), m.distance, m.yaw};
+        return r;
     }
 
     // System::VisualizeGlobalMap's state (global_map, last_frame_id; system.cpp:851-852) with global_map kept on the device in two
@@ -184,6 +221,7 @@ private:
 
     fls_keyframes* store_ = nullptr;
     std::vector<size_t> sizes_;  // records per keyframe id
+    fls_sc_cfg sc_cfg_{20, 60, 80.f, 2.f};  // the paper's descriptor
 };
 
 #endif  // FUNNY_LIDAR_SLAM_B200_KEYFRAME_MAP_H

@@ -31,6 +31,8 @@
  *                                 searching an x-y-yaw grid around the given pose
  *   fls_relocalize_wide /      <- the same over a whole local map (up to 2^31 hypotheses), by exact branch and bound
  *   _wide_device
+ *   fls_keyframes_detect_loop  <- LoopClosure::DetectByFeature (src/slam/loop_closure.cpp:62-64, a stub upstream), by Scan Context
+ *   fls_keyframes_place_query  <- the keyframe a scan was taken near, and its yaw: the guess of fls_relocalize without a clicked pose
  *
  * Conventions
  *   * Points are read from caller memory as {float x, y, z, <pad>, intensity ...} records `stride_bytes`
@@ -610,6 +612,60 @@ int fls_keyframes_count(fls_keyframes* s, size_t* n_keyframes, size_t* n_points)
  * holds more than 2^31 - 1 records. */
 int fls_keyframes_assemble(fls_keyframes* s, const int64_t* ids, size_t n_ids, const double* T_colmajor, float leaf, float final_leaf,
                            const void* d_base, size_t n_base, float* out, float* d_out, size_t capacity, size_t* n_out, fls_match_stats* stats);
+
+/* ---- Place recognition on the keyframe store: Scan Context (G. Kim, A. Kim, IROS 2018), DESIGN.md §3.12 ----
+ *
+ * Descriptor of a cloud (packed x, y, z, intensity in the sensor frame, z up): an n_rings x n_sectors fp32 matrix, row-major.  Each
+ * point with finite x, y and z, every operation rounded on its own (no FMA):
+ *   r = sqrt(x*x + y*y) in fp64 (x, y widened from float); kept only if r < R (R = max_radius)
+ *   ring = min(n_rings - 1, floor((r * n_rings) / R)) in fp64
+ *   th = (double)atan2f(y, x) (the pinned atan2f of fls_atan.cuh), plus 2*pi when th < 0
+ *   sector = min(n_sectors - 1, floor((th * n_sectors) / (2*pi)))
+ *   cell = max over its points of (float)(z + z_offset) (-0.0 < +0.0); 0 for a cell without a point.
+ * Distance of query Q to candidate C: column norms are fp64 sums over rings in ring order, then sqrt.  For each shift s in
+ * [0, n_sectors), over the columns j (ascending) where both |Q_j| and |C_(j+s) mod n_sectors| are non-zero, E_s of them:
+ *   cos_j = dot_j / (|Q_j| * |C_(j+s)|), dot_j an fp64 sum over rings in ring order;  d_s = 1 - (sum_j cos_j) / E_s  (1 when E_s = 0)
+ * D = min_s d_s, ties to the smallest s; yaw = s * (2*pi / n_sectors), minus 2*pi when above pi.  A query taken where the candidate
+ * was, with the sensor turned by +psi about z, has its best shift near psi / (2*pi / n_sectors): Rz(yaw) maps query-frame points into
+ * the candidate frame, and T_candidate * Rz(yaw) is the query's coarse pose.  Results are ordered by (D, id) ascending, the same bits
+ * from call to call. */
+typedef struct {
+    int32_t n_rings;   /* 1..64, 20 in the paper */
+    int32_t n_sectors; /* 1..360, 60 in the paper; n_rings * n_sectors <= 4096 */
+    float max_radius;  /* finite, > 0: 80 m in the paper */
+    float z_offset;    /* finite: added to z before the maximum (2 m: the sensor height, so ground cells are near zero) */
+} fls_sc_cfg;
+
+typedef struct {
+    int64_t id;       /* keyframe id */
+    double distance;  /* D */
+    double yaw;       /* rad, in (-pi, pi] */
+    int32_t shift;    /* the best shift s */
+    int32_t reserved;
+} fls_place_match;
+
+/* The descriptors of keyframes ids[0 .. n_ids) (below the count), n_rings * n_sectors floats each, one after another. */
+int fls_keyframes_scan_context(fls_keyframes* s, const fls_sc_cfg* cfg, const int64_t* ids, size_t n_ids, float* desc);
+/* LoopClosure::DetectByFeature: the query is stored keyframe query_id, the candidates the ids with query_id - id > min_span (the span
+ * rule of CheckCandidateKeyFrames, src/slam/loop_closure.cpp:171, min_span = skip_near_keyframe_threshold).  FLS_ERR_INVALID_ARG when
+ * query_id is not below the keyframe count or min_span < 0.  *n_found = min(k, candidates), possibly 0; out has room for k records.
+ * The library applies no distance threshold: the caller does. */
+int fls_keyframes_detect_loop(fls_keyframes* s, const fls_sc_cfg* cfg, int64_t query_id, int64_t min_span, size_t k, fls_place_match* out,
+                              size_t* n_found, fls_match_stats* stats);
+/* The query is a scan (host records stride_bytes apart, FLS_LAYOUT_*; _device: n packed float4 on the store's device, complete when
+ * the call is made), the candidates every stored keyframe.  query_desc (optional, n_rings * n_sectors floats) receives its descriptor. */
+int fls_keyframes_place_query(fls_keyframes* s, const fls_sc_cfg* cfg, const void* pts, size_t n, size_t stride_bytes, size_t k,
+                              fls_place_match* out, size_t* n_found, float* query_desc, fls_match_stats* stats);
+int fls_keyframes_place_query_device(fls_keyframes* s, const fls_sc_cfg* cfg, const void* d_pts, size_t n, size_t k, fls_place_match* out,
+                                     size_t* n_found, float* query_desc, fls_match_stats* stats);
+/* Common to the three: k >= 1; a bad cfg, k or pointer returns FLS_ERR_INVALID_ARG before any device work.  The store keeps one
+ * descriptor per keyframe for the cfg of the last call; each call first describes the keyframes added since (all of them after a cfg
+ * change) in one segmented pass.  Launches: that pass (a memset, a binning kernel when it reads a point, a finalize; nothing when
+ * there is nothing to describe), the host query's repack when its stride is not 16, and the search, sort and pick (none without a
+ * candidate).  One host wait (stream synchronisation); a call that grows the descriptor cache also frees its old buffers, and that
+ * cudaFree waits for the device (the cache doubles, so this happens a logarithmic number of times).  None of this depends on the
+ * keyframe count.  stats (optional): gpu_ms, gpu_launches, h2d_bytes,
+ * d2h_bytes, n_source = points the pass read, n_valid = candidates, iterations = the host waits of the call. */
 
 const char* fls_strerror(int status);
 const char* fls_last_error(void); /* thread-local text of the last CUDA failure */
