@@ -21,6 +21,7 @@ EXPORTS = [
     "fls_preprocess_device", "fls_keyframes_create", "fls_keyframes_destroy", "fls_keyframes_add", "fls_keyframes_add_device",
     "fls_keyframes_count", "fls_keyframes_assemble", "fls_get_ndt_voxels", "fls_gn_step_probe",
     "fls_relocalize", "fls_relocalize_device", "fls_relocalize_wide", "fls_relocalize_wide_device", "fls_relocalize_wide_levels",
+    "fls_relocalize_multi", "fls_relocalize_multi_device",
     "fls_keyframes_scan_context", "fls_keyframes_detect_loop", "fls_keyframes_place_query", "fls_keyframes_place_query_device",
 ]
 
@@ -81,6 +82,9 @@ def lib():
     L.fls_relocalize_wide.argtypes = [vp, vp, sz, sz] + wide_outs
     L.fls_relocalize_wide_device.argtypes = [vp, vp, sz] + wide_outs
     L.fls_relocalize_wide_levels.argtypes = [vp, vp, C.c_int]
+    multi_outs = [C.POINTER(FlsRelocCfg), vp, C.c_int32] + wide_outs[1:]
+    L.fls_relocalize_multi.argtypes = [vp, vp, sz, sz] + multi_outs
+    L.fls_relocalize_multi_device.argtypes = [vp, vp, sz] + multi_outs
     L.fls_get_iter_log.argtypes = [vp, C.POINTER(FlsIterLog), C.c_int]
     L.fls_get_iter_log_scan.argtypes = [vp, C.c_int, C.POINTER(FlsIterLog), C.c_int]
     L.fls_get_map_info.argtypes = [vp, C.POINTER(FlsMapInfo)]

@@ -598,24 +598,26 @@ int fls_fitness(fls_handle* hh, float max_range, float* score) {
     FLS_CATCH
 }
 
-// fls_relocalize (wide: fls_relocalize_wide) of a host scan of `host_stride` bytes per record or (0) a device scan: the checks that need
-// no device first, then the plug-ins and modes without a batch Match in localization mode, which answer with no side effect
-static int relocalize(fls_handle* hh, bool wide, const void* scan, size_t n, size_t host_stride, const fls_reloc_cfg* cfg, double* T,
-                      fls_reloc_result* out, double* refined_T, int32_t* refined_converged, float* refined_fitness, int64_t* refined_index,
-                      double* coarse_scores, size_t coarse_cap, int64_t* evaluations) {
+// fls_relocalize (wide: fls_relocalize_wide) of a host scan of `host_stride` bytes per record or (0) a device scan, or with guesses
+// (G of them, checked by guesses_ok) fls_relocalize_multi: the checks that need no device first, then the plug-ins and modes without a batch Match in
+// localization mode, which answer with no side effect
+static int relocalize(fls_handle* hh, bool wide, const void* scan, size_t n, size_t host_stride, const fls_reloc_cfg* cfg, const double* guesses,
+                      int G, double* T, fls_reloc_result* out, double* refined_T, int32_t* refined_converged, float* refined_fitness,
+                      int64_t* refined_index, double* coarse_scores, size_t coarse_cap, int64_t* evaluations) {
     Handle* h = reinterpret_cast<Handle*>(hh);
     if (!h || !cfg || !T || !out || (!scan && n) || (coarse_cap && !coarse_scores) || n > 0x3fffffffull) return FLS_ERR_INVALID_ARG;
     fls::RelocGrid g;
     const int v = fls::reloc_grid(*cfg, &g, wide);
     if (v != FLS_OK) return v;
+    if (g.P > fls::kRelocWideMaxHypotheses / G) return FLS_ERR_INVALID_ARG;  // G * P > 2^31
     if (!h->cfg.localization_mode || (h->cfg.method != FLS_P2PLANE_IVOX && h->cfg.method != FLS_NDT)) return FLS_ERR_UNSUPPORTED;
     if (h->plugin->batch_pending()) return FLS_ERR_INVALID_ARG;  // one batch in flight per handle (fls_match_batch_begin)
     if (h->fit_cloud_n == 0) return FLS_ERR_NO_MAP;
     FLS_TRY
     h->begin_call();
     const float4* d = host_stride ? h->upload(scan, n, host_stride, h->src) : static_cast<const float4*>(scan);
-    return h->relocalize(d, n, *cfg, g, wide, T, out, refined_T, refined_converged, refined_fitness, refined_index, coarse_scores, coarse_cap,
-                         evaluations);
+    return h->relocalize(d, n, *cfg, g, wide, guesses, G, T, out, refined_T, refined_converged, refined_fitness, refined_index, coarse_scores,
+                         coarse_cap, evaluations);
     FLS_CATCH
 }
 
@@ -623,26 +625,51 @@ int fls_relocalize(fls_handle* hh, const void* scan, size_t n, size_t stride, co
                    double* refined_T, int32_t* refined_converged, float* refined_fitness, int64_t* refined_index, double* coarse_scores,
                    size_t coarse_cap) {
     if (!stride_ok(stride)) return FLS_ERR_INVALID_ARG;
-    return relocalize(hh, false, scan, n, stride, cfg, T, out, refined_T, refined_converged, refined_fitness, refined_index, coarse_scores, coarse_cap,
-                      nullptr);
+    return relocalize(hh, false, scan, n, stride, cfg, T, 1, T, out, refined_T, refined_converged, refined_fitness, refined_index, coarse_scores,
+                      coarse_cap, nullptr);
 }
 
 int fls_relocalize_device(fls_handle* hh, const void* d_scan, size_t n, const fls_reloc_cfg* cfg, double T[16], fls_reloc_result* out,
                           double* refined_T, int32_t* refined_converged, float* refined_fitness, int64_t* refined_index, double* coarse_scores,
                           size_t coarse_cap) {
-    return relocalize(hh, false, d_scan, n, 0, cfg, T, out, refined_T, refined_converged, refined_fitness, refined_index, coarse_scores, coarse_cap,
-                      nullptr);
+    return relocalize(hh, false, d_scan, n, 0, cfg, T, 1, T, out, refined_T, refined_converged, refined_fitness, refined_index, coarse_scores,
+                      coarse_cap, nullptr);
 }
 
 int fls_relocalize_wide(fls_handle* hh, const void* scan, size_t n, size_t stride, const fls_reloc_cfg* cfg, double T[16], fls_reloc_result* out,
                         double* refined_T, int32_t* refined_converged, float* refined_fitness, int64_t* refined_index, int64_t* evaluations) {
     if (!stride_ok(stride)) return FLS_ERR_INVALID_ARG;
-    return relocalize(hh, true, scan, n, stride, cfg, T, out, refined_T, refined_converged, refined_fitness, refined_index, nullptr, 0, evaluations);
+    return relocalize(hh, true, scan, n, stride, cfg, T, 1, T, out, refined_T, refined_converged, refined_fitness, refined_index, nullptr, 0,
+                      evaluations);
 }
 
 int fls_relocalize_wide_device(fls_handle* hh, const void* d_scan, size_t n, const fls_reloc_cfg* cfg, double T[16], fls_reloc_result* out,
                                double* refined_T, int32_t* refined_converged, float* refined_fitness, int64_t* refined_index, int64_t* evaluations) {
-    return relocalize(hh, true, d_scan, n, 0, cfg, T, out, refined_T, refined_converged, refined_fitness, refined_index, nullptr, 0, evaluations);
+    return relocalize(hh, true, d_scan, n, 0, cfg, T, 1, T, out, refined_T, refined_converged, refined_fitness, refined_index, nullptr, 0, evaluations);
+}
+
+// fls_relocalize_multi's own checks: 1..64 guesses, every entry finite
+static bool guesses_ok(const double* guesses, int G) {
+    if (!guesses || G < 1 || G > fls::kRelocMaxGuesses) return false;
+    for (int k = 0; k < 16 * G; ++k)
+        if (!std::isfinite(guesses[k])) return false;
+    return true;
+}
+
+int fls_relocalize_multi(fls_handle* hh, const void* scan, size_t n, size_t stride, const fls_reloc_cfg* cfg, const double* guesses, int32_t n_guesses,
+                         double T[16], fls_reloc_result* out, double* refined_T, int32_t* refined_converged, float* refined_fitness,
+                         int64_t* refined_index, int64_t* evaluations) {
+    if (!stride_ok(stride) || !guesses_ok(guesses, n_guesses)) return FLS_ERR_INVALID_ARG;
+    return relocalize(hh, true, scan, n, stride, cfg, guesses, n_guesses, T, out, refined_T, refined_converged, refined_fitness, refined_index, nullptr, 0,
+                      evaluations);
+}
+
+int fls_relocalize_multi_device(fls_handle* hh, const void* d_scan, size_t n, const fls_reloc_cfg* cfg, const double* guesses, int32_t n_guesses,
+                                double T[16], fls_reloc_result* out, double* refined_T, int32_t* refined_converged, float* refined_fitness,
+                                int64_t* refined_index, int64_t* evaluations) {
+    if (!guesses_ok(guesses, n_guesses)) return FLS_ERR_INVALID_ARG;
+    return relocalize(hh, true, d_scan, n, 0, cfg, guesses, n_guesses, T, out, refined_T, refined_converged, refined_fitness, refined_index, nullptr, 0,
+                      evaluations);
 }
 
 int fls_relocalize_wide_levels(const fls_handle* hh, int64_t* nodes, int capacity) {

@@ -65,7 +65,8 @@ struct KeyFrameGate {
 
 // the hypothesis grid of fls_relocalize (fls_b200.h): offsets -I..I in x and y, yaw offsets k0..K (n_yaw of them), P hypotheses
 static constexpr long long kRelocMaxHypotheses = 1LL << 20;
-static constexpr long long kRelocWideMaxHypotheses = 1LL << 31;  // and I <= 32767: fls_relocalize_wide
+static constexpr long long kRelocWideMaxHypotheses = 1LL << 31;  // and I <= 32767: fls_relocalize_wide, and G * P for fls_relocalize_multi
+static constexpr int kRelocMaxGuesses = 64;                       // fls_relocalize_multi
 struct RelocGrid {
     int I = 0, K = 0, k0 = 0;
     long long n_yaw = 1, P = 1;  // n_yaw reaches 2^31 on the full circle of the wide cap
@@ -254,11 +255,13 @@ struct Handle {
     int fitness(float max_range, float* score);
     int fit_grid_for(float max_range, int* waits);  // (re)builds fit_grid for max_range when needed; counts its wait
     void fitness_enqueue(const float4* d_src, size_t n, int P, float max_range);  // P poses of fit_pose -> fit_out / fit_cnt
-    // fls_relocalize, or fls_relocalize_wide when wide, on a device scan (the call has begun; g from reloc_grid(c, &g, wide)); coarse_scores
-    // and coarse_cap are fls_relocalize's, evaluations fls_relocalize_wide's
-    int relocalize(const float4* d_scan, size_t n, const fls_reloc_cfg& c, const RelocGrid& g, bool wide, double* T, fls_reloc_result* out, double* refined_T,
-                   int32_t* refined_converged, float* refined_fitness, int64_t* refined_index, double* coarse_scores, size_t coarse_cap,
-                   int64_t* evaluations);
+    // fls_relocalize, or fls_relocalize_wide / fls_relocalize_multi when wide, on a device scan (the call has begun; g from
+    // reloc_grid(c, &g, wide)) over the grids of G column-major guesses (G = 1 and guesses == T for the single-guess entries; T
+    // receives the chosen pose, or guess 0 after an empty coarse cloud); coarse_scores and coarse_cap are fls_relocalize's,
+    // evaluations those of the wide entries
+    int relocalize(const float4* d_scan, size_t n, const fls_reloc_cfg& c, const RelocGrid& g, bool wide, const double* guesses, int G, double* T,
+                   fls_reloc_result* out, double* refined_T, int32_t* refined_converged, float* refined_fitness, int64_t* refined_index,
+                   double* coarse_scores, size_t coarse_cap, int64_t* evaluations);
     int relocalize_levels(int64_t* nodes, int capacity) const;  // fls_relocalize_wide_levels (0 levels before a wide call)
 
     // localization-mode map path (fls_localmap.cu): resident global map, +-100 m crop around the pose when needed

@@ -167,28 +167,32 @@ __global__ void pose_score_reduce_kernel(const double* __restrict__ part_sum, co
     if (ids) ids[p] = (unsigned long long)(nodes ? nodes[p] : base + p);
 }
 
-// the hypothesis grid of fls_relocalize (fls_b200.h): pose p in fp64, row-major R | t
+// the hypothesis grids of fls_relocalize (fls_b200.h) around G guesses: leaf g * P + p is pose p of guess g's grid, in fp64, row-major
+// R | t.  The guesses live in a device table, not in this struct: BoundTerm carries it by value into every sweep's kernel argument.
 struct RelocGridArgs {
-    double R[9], t[3];  // the guess
+    const double* __restrict__ guess;  // [G][12]: row-major R, then t
     double xy_step, yaw_step;
     int I, K, k0;  // yaw offsets k0 .. K
-    long long n_yaw, P;
+    long long n_yaw, P;  // P: hypotheses per guess
 };
-// hypothesis p of the grid: the one formula of both searches, so that a leaf has the same bits in each
-__device__ __forceinline__ void reloc_leaf_pose(const RelocGridArgs& g, long long p, double* o) {
+// leaf `leaf` of the grids: the one formula of every search, so that a hypothesis has the same bits in each
+__device__ __forceinline__ void reloc_leaf_pose(const RelocGridArgs& g, long long leaf, double* o) {
+    const long long gi = leaf / g.P, p = leaf - gi * g.P;
+    const double* R = g.guess + gi * 12;
+    const double* t = R + 9;
     const long long nx = 2LL * g.I + 1;
     const long long ky = p % g.n_yaw, ix = (p / g.n_yaw) % nx, jy = p / (g.n_yaw * nx);
     const double psi = __dmul_rn((double)(g.k0 + ky), g.yaw_step);
     const double c = cos(psi), s = sin(psi);
     for (int j = 0; j < 3; ++j) {
-        const double a = g.R[j], b = g.R[3 + j];
+        const double a = __ldg(R + j), b = __ldg(R + 3 + j);
         o[j] = __dsub_rn(__dmul_rn(c, a), __dmul_rn(s, b));
         o[3 + j] = __dadd_rn(__dmul_rn(s, a), __dmul_rn(c, b));
-        o[6 + j] = g.R[6 + j];
+        o[6 + j] = __ldg(R + 6 + j);
     }
-    o[9] = __dadd_rn(g.t[0], __dmul_rn((double)(ix - g.I), g.xy_step));
-    o[10] = __dadd_rn(g.t[1], __dmul_rn((double)(jy - g.I), g.xy_step));
-    o[11] = g.t[2];
+    o[9] = __dadd_rn(__ldg(t), __dmul_rn((double)(ix - g.I), g.xy_step));
+    o[10] = __dadd_rn(__ldg(t + 1), __dmul_rn((double)(jy - g.I), g.xy_step));
+    o[11] = __ldg(t + 2);
 }
 // the selected hypotheses: {index, coarse score, pose} records, read back in one copy
 struct RelocPick {
@@ -377,6 +381,7 @@ namespace {
 // A node of level l is an aligned block of 2^l x 2^l x 2^l leaves (hypotheses) in (x, y, yaw) index space, clipped at the grid's
 // edges; its id orders the blocks as the leaves are ordered (yaw fastest, then x, then y), so a level-0 node is a leaf.  A node is
 // evaluated at one representative leaf: the one 2^(l-1) past its low corner in each index, or the last one where the block is clipped.
+// With G guesses a node never spans two grids: node g * N_l + b is block b of guess g's grid, N_l the blocks of one grid at level l.
 //
 // The bound.  Let q_i be scan point p_i moved by the representative as the score kernel moves it (the fp64 pose cast to float,
 // xform_row_f), and b_i a lower bound on the distance from q_i to the fit cloud (the lattice below).  A leaf of the node moves p_i to
@@ -395,9 +400,11 @@ namespace {
 //   LB = sum_i min(max(0, b_i - delta_i)^2, max_range)        (in fp64).
 // Both sums are fp64 sums of up to 2^30 non-negative terms in different orders: their rounding is below m 2^-53 < 1.2e-7 of the
 // sum, so a node is pruned only when LB / m > U (1 + kPruneMargin).
+// Over G guesses the bound takes w_i = max_g |(R_g p_i)_xy| and tau over every guess's leaves: both only make delta_i larger than
+// the one guess g of the node needs, so LB stays a lower bound of every leaf of every grid (for G = 1 both are the values above).
 //
 // U is the n-th smallest exact score among the distinct leaves scored so far: the representatives of the start level (the lowest
-// level with at most 2^20 nodes) are all scored exactly, and no later level scores any (those reps would repeat leaves already
+// level with at most 2^20 nodes over all guesses) are all scored exactly, and no later level scores any (those reps would repeat leaves already
 // scored or be scored again at level 0; the start level's U already comes from up to 2^20 leaves spread over the whole grid).  A
 // node is kept iff LB / m <= U (1 + margin): every leaf scoring <= U keeps all its ancestors, so the n best leaves of the whole grid,
 // and every tie at the n-th score, reach level 0, where all survivors are scored exactly and sorted on (score bits, leaf index).
@@ -426,16 +433,24 @@ __device__ inline long long block_rep(long long b, int l, long long n, int& h) {
     return r;
 }
 
+// node id -> (guess, block of that guess's grid at level l in yaw, x, y)
+struct NodeIdx {
+    long long g, bk, bx, by;
+};
+__device__ inline NodeIdx node_idx(long long id, int l, long long nx, long long nk) {
+    const long long nbk = level_blocks(nk, l), nbx = level_blocks(nx, l), b = id % (nbk * nbx * nbx);
+    return {id / (nbk * nbx * nbx), b % nbk, (b / nbk) % nbx, b / (nbk * nbx)};
+}
+
 struct NodeRep {
     long long leaf;
     int hx, hy, hk;
 };
 __device__ inline NodeRep node_rep(long long id, int l, long long nx, long long nk) {
-    const long long nbk = level_blocks(nk, l), nbx = level_blocks(nx, l);
-    const long long bk = id % nbk, bx = (id / nbk) % nbx, by = id / (nbk * nbx);
+    const NodeIdx d = node_idx(id, l, nx, nk);
     NodeRep r;
-    const long long rk = block_rep(bk, l, nk, r.hk), rx = block_rep(bx, l, nx, r.hx), ry = block_rep(by, l, nx, r.hy);
-    r.leaf = (ry * nx + rx) * nk + rk;
+    const long long rk = block_rep(d.bk, l, nk, r.hk), rx = block_rep(d.bx, l, nx, r.hx), ry = block_rep(d.by, l, nx, r.hy);
+    r.leaf = (d.g * nx + ry) * nx * nk + rx * nk + rk;
     return r;
 }
 
@@ -452,7 +467,7 @@ __global__ void reloc_rep_poses_kernel(RelocGridArgs g, const long long* __restr
 }
 
 // pose_score_kernel's term of LB (derived at the head of this section): the pose of a node's representative, and per point
-// min(max(0, b_i - delta_i)^2, max_range).  The points are the coarse cloud with w = |(R_guess p)_xy| rounded up
+// min(max(0, b_i - delta_i)^2, max_range).  The points are the coarse cloud with w = max over the guesses of |(R_g p)_xy| rounded up
 // (reloc_slack_points_kernel).
 struct BoundTerm {
     static constexpr bool kCounts = false;
@@ -507,26 +522,24 @@ __global__ void reloc_keep_kernel(const double* __restrict__ part, int N, int n_
     const double U = __longlong_as_double((long long)*u_key);
     int k = 0;
     if (lb / (double)m <= U * (1.0 + kPruneMargin)) {
-        const long long id = nodes[i], nbk = level_blocks(nk, l), nbx = level_blocks(nx, l);
-        const long long bk = id % nbk, bx = (id / nbk) % nbx, by = id / (nbk * nbx);
+        const NodeIdx d = node_idx(nodes[i], l, nx, nk);
         const long long ck = level_blocks(nk, l - 1), cx = level_blocks(nx, l - 1);
-        k = (int)((min(2 * bk + 2, ck) - 2 * bk) * (min(2 * bx + 2, cx) - 2 * bx) * (min(2 * by + 2, cx) - 2 * by));
+        k = (int)((min(2 * d.bk + 2, ck) - 2 * d.bk) * (min(2 * d.bx + 2, cx) - 2 * d.bx) * (min(2 * d.by + 2, cx) - 2 * d.by));
     }
     n_children[i] = k;
 }
 
-// the children of the kept nodes of level l, at their offsets in the level l - 1 list
+// the children of the kept nodes of level l, at their offsets in the level l - 1 list (in the same guess)
 __global__ void reloc_children_kernel(const long long* __restrict__ nodes, const int* __restrict__ n_children, const int* __restrict__ offset, int N,
                                       int l, long long nx, long long nk, long long* __restrict__ out) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= N || n_children[i] == 0) return;
-    const long long id = nodes[i], nbk = level_blocks(nk, l), nbx = level_blocks(nx, l);
-    const long long bk = id % nbk, bx = (id / nbk) % nbx, by = id / (nbk * nbx);
+    const NodeIdx d = node_idx(nodes[i], l, nx, nk);
     const long long ck = level_blocks(nk, l - 1), cx = level_blocks(nx, l - 1);
     long long* o = out + offset[i];
-    for (long long y = 2 * by; y < min(2 * by + 2, cx); ++y)
-        for (long long x = 2 * bx; x < min(2 * bx + 2, cx); ++x)
-            for (long long k = 2 * bk; k < min(2 * bk + 2, ck); ++k) *o++ = (y * cx + x) * ck + k;
+    for (long long y = 2 * d.by; y < min(2 * d.by + 2, cx); ++y)
+        for (long long x = 2 * d.bx; x < min(2 * d.bx + 2, cx); ++x)
+            for (long long k = 2 * d.bk; k < min(2 * d.bk + 2, ck); ++k) *o++ = ((d.g * cx + y) * cx + x) * ck + k;
 }
 
 // ---- the lower-bound distance lattice -------------------------------------------------------------------------------------------
@@ -630,23 +643,29 @@ __global__ void lattice_store_kernel(const unsigned* __restrict__ d, int nx, int
     v[i] = (unsigned short)fmin(floor(b / q), 65535.0);
 }
 
-// per scan point: its coordinates and |(R_guess p)_xy| rounded up, the node-independent part of the slack
-__global__ void reloc_slack_points_kernel(const float4* __restrict__ src, int n, RelocGridArgs g, float4* __restrict__ out) {
+// per scan point: its coordinates and max over the G guesses of |(R_g p)_xy| rounded up, the node-independent part of the slack
+__global__ void reloc_slack_points_kernel(const float4* __restrict__ src, int n, const double* __restrict__ guess, int G, float4* __restrict__ out) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const float4 p = src[i];
-    const double vx = g.R[0] * p.x + g.R[1] * p.y + g.R[2] * p.z, vy = g.R[3] * p.x + g.R[4] * p.y + g.R[5] * p.z;
-    out[i] = make_float4(p.x, p.y, p.z, __double2float_ru(sqrt(vx * vx + vy * vy)));
+    double w = 0.0;
+    for (int g = 0; g < G; ++g) {
+        const double* R = guess + 12 * g;
+        const double vx = R[0] * p.x + R[1] * p.y + R[2] * p.z, vy = R[3] * p.x + R[4] * p.y + R[5] * p.z;
+        const double v = sqrt(vx * vx + vy * vy);
+        w = g ? fmax(w, v) : v;
+    }
+    out[i] = make_float4(p.x, p.y, p.z, __double2float_ru(w));
 }
 
 }  // namespace
 
-// Relocalization's state on a handle, made by its first call: the coarse cloud and its copy with each point's slack term, a launch's
-// poses and partials, sort keys and leaf ids (an unsorted and a sorted half each), the node lists of a level and the next with their
+// Relocalization's state on a handle, made by its first call: the guess table, the coarse cloud and its copy with each point's slack
+// term, a launch's poses and partials, sort keys and leaf ids (an unsorted and a sorted half each), the node lists of a level and the next with their
 // child counts and offsets, U's sort key, the picks, the lower-bound lattice of the fit cloud, and the levels of the last wide search.
 struct Reloc {
     DevBuf<float4> coarse, slack_pts;
-    DevBuf<double> poses, part_sum;
+    DevBuf<double> guess, poses, part_sum;
     DevBuf<unsigned> part_cnt;
     DevBuf<unsigned long long> key, leaf, u;
     DevBuf<long long> nodes, next;
@@ -709,9 +728,9 @@ int Reloc::lattice_for(Handle& hd, float max_range, int* waits) {
     return FLS_OK;
 }
 
-int Handle::relocalize(const float4* d_scan, size_t n, const fls_reloc_cfg& c, const RelocGrid& gr, bool wide, double* T, fls_reloc_result* out,
-                       double* refined_T, int32_t* refined_converged, float* refined_fitness, int64_t* refined_index, double* coarse_scores,
-                       size_t coarse_cap, int64_t* evaluations) {
+int Handle::relocalize(const float4* d_scan, size_t n, const fls_reloc_cfg& c, const RelocGrid& gr, bool wide, const double* guesses, int G, double* T,
+                       fls_reloc_result* out, double* refined_T, int32_t* refined_converged, float* refined_fitness, int64_t* refined_index,
+                       double* coarse_scores, size_t coarse_cap, int64_t* evaluations) {
     if (!reloc) reloc.reset(new Reloc);
     Reloc& s = *reloc;
     int L = 0, W = 0;  // launches and waits of the whole call
@@ -719,7 +738,8 @@ int Handle::relocalize(const float4* d_scan, size_t n, const fls_reloc_cfg& c, c
     if (evaluations) *evaluations = 0;
     if (wide) s.levels.clear();
     std::memset(out, 0, sizeof(*out));
-    out->n_hypotheses = gr.P;
+    const long long P = (long long)G * gr.P, nx = 2LL * gr.I + 1, nk = gr.n_yaw;  // every grid's hypotheses; one grid's axes
+    out->n_hypotheses = P;
     out->best_hypothesis = -1;
     out->fitness = FLT_MAX;
     out->coarse_score = FLT_MAX;
@@ -728,6 +748,7 @@ int Handle::relocalize(const float4* d_scan, size_t n, const fls_reloc_cfg& c, c
     s.coarse.reserve(n + 1);
     const size_t m = voxel_grid_device(d_scan, n, c.coarse_leaf, s.coarse.p, scratch, stream, &launches, &W);
     if (m == 0) {
+        if (T != guesses) std::memcpy(T, guesses, 16 * sizeof(double));
         last_src = d_scan;
         last_src_n = 0;
         out->gpu_launches = launches;
@@ -736,9 +757,12 @@ int Handle::relocalize(const float4* d_scan, size_t n, const fls_reloc_cfg& c, c
     }
     int rc = fit_grid_for(c.max_range, &W);
     if (rc != FLS_OK) return rc;
+    double rows[kMaxBatch * 12];
+    for (int g = 0; g < G; ++g) pose_rows(guesses + 16 * g, rows + 12 * g);
+    s.guess.reserve((size_t)G * 12);
+    FLS_CUDA(cudaMemcpyAsync(s.guess.p, rows, sizeof(double) * 12 * (size_t)G, cudaMemcpyHostToDevice, stream));
     RelocGridArgs ga;
-    pose_rows(T, ga.R);
-    for (int k = 0; k < 3; ++k) ga.t[k] = T[12 + k];
+    ga.guess = s.guess.p;
     ga.xy_step = gr.I ? c.xy_step : 0.0;  // an unused step may be anything
     ga.yaw_step = gr.K ? c.yaw_step : 0.0;
     ga.I = gr.I;
@@ -746,12 +770,12 @@ int Handle::relocalize(const float4* d_scan, size_t n, const fls_reloc_cfg& c, c
     ga.k0 = gr.k0;
     ga.n_yaw = gr.n_yaw;
     ga.P = gr.P;
-    // ---- the start level: the lowest with at most 2^20 nodes (level 0 on every grid fls_relocalize accepts) -----------------------
-    const long long P = gr.P, nx = 2LL * gr.I + 1, nk = gr.n_yaw;
+    // ---- the start level: the lowest with at most 2^20 nodes over all guesses (level 0 on every grid fls_relocalize accepts) -------
     const int nr = P < c.n_refine ? (int)P : c.n_refine;
+    auto level_nodes = [&](int l) { return G * level_blocks(nx, l) * level_blocks(nx, l) * level_blocks(nk, l); };
     int ls = 0;
-    while (level_blocks(nx, ls) * level_blocks(nx, ls) * level_blocks(nk, ls) > kWideChunk) ++ls;
-    long long N = level_blocks(nx, ls) * level_blocks(nx, ls) * level_blocks(nk, ls);
+    while (level_nodes(ls) > kWideChunk) ++ls;
+    long long N = level_nodes(ls);
     const size_t tiles = (m + kCoarseTile - 1) / kCoarseTile;
     auto reserve_chunk = [&](size_t k) {  // a launch's poses and partials
         s.poses.reserve(k * 12);
@@ -790,10 +814,15 @@ int Handle::relocalize(const float4* d_scan, size_t n, const fls_reloc_cfg& c, c
         ++L;
         s.u.reserve(1);
         FLS_CUDA(cudaMemcpyAsync(s.u.p, s.key.p + N + nr - 1, sizeof(unsigned long long), cudaMemcpyDeviceToDevice, stream));
-        // the slack's float terms (derivation above): tau, the largest translation coordinate of any leaf
-        const double tau = std::fmax(std::fmax(std::fabs(ga.t[0]), std::fabs(ga.t[1])) + gr.I * ga.xy_step, std::fabs(ga.t[2]));
+        // the slack's float terms (derivation above): tau, the largest translation coordinate of any leaf of any guess
+        double tau = 0.0;
+        for (int g = 0; g < G; ++g) {
+            const double* t = rows + 12 * g + 9;
+            const double tg = std::fmax(std::fmax(std::fabs(t[0]), std::fabs(t[1])) + gr.I * ga.xy_step, std::fabs(t[2]));
+            tau = g ? std::fmax(tau, tg) : tg;
+        }
         s.slack_pts.reserve(m);
-        reloc_slack_points_kernel<<<grid_for(m, 256), 256, 0, stream>>>(s.coarse.p, (int)m, ga, s.slack_pts.p);
+        reloc_slack_points_kernel<<<grid_for(m, 256), 256, 0, stream>>>(s.coarse.p, (int)m, s.guess.p, G, s.slack_pts.p);
         ++L;
         BoundTerm bound{s.lat, ga, nullptr, 0, 32.0 * kU * tau + 8.0 * kU * std::sqrt((double)c.max_range), 32.0 * kU, c.max_range};
         for (int l = ls; l >= 1; --l) {
@@ -820,7 +849,8 @@ int Handle::relocalize(const float4* d_scan, size_t n, const fls_reloc_cfg& c, c
             ++L;
             const long long next = (long long)last[0] + last[1];
             if (next > kWideCap) {
-                set_last_error("fls_relocalize_wide: " + std::to_string(next) + " nodes survive at level " + std::to_string(l - 1));
+                set_last_error(std::string(G > 1 ? "fls_relocalize_multi: " : "fls_relocalize_wide: ") + std::to_string(next) +
+                               " nodes survive at level " + std::to_string(l - 1));
                 out->gpu_launches = L + launches;
                 out->host_waits = W;
                 return FLS_ERR_CAPACITY;
@@ -833,7 +863,7 @@ int Handle::relocalize(const float4* d_scan, size_t n, const fls_reloc_cfg& c, c
             N = next;
         }
     }
-    // ---- level 0: every leaf left scored exactly, a stable sort on (score bits, leaf index), the n best -----------------------------
+    // ---- level 0: every leaf left scored exactly, a stable sort on (score bits, leaf index g * P + p), the n best ---------------------
     // A descent's survivors are scored into the upper halves and first sorted into leaf order; a grid scored whole is in leaf order.
     s.key.reserve((size_t)N * 2);
     s.leaf.reserve((size_t)N * 2);

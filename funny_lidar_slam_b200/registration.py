@@ -73,6 +73,13 @@ def reloc_cfg(xy_radius=10.0, xy_step=1.0, yaw_range=np.pi, yaw_step=np.deg2rad(
     return c
 
 
+def _guesses(Ts):
+    """The guesses of a multi-guess call, column-major per pose, and the start value of its output pose (guess 0, which the call
+    overwrites; the identity when there is none)."""
+    Ts = np.asarray(Ts, np.float64).reshape(-1, 4, 4)
+    return _batch_poses(Ts), (Ts[0] if len(Ts) else np.eye(4))
+
+
 def _batch_poses(Ts):
     return np.ascontiguousarray(np.transpose(np.asarray(Ts, np.float64), (0, 2, 1))).copy()  # Eigen column-major per pose
 
@@ -226,7 +233,7 @@ class Registration:
         return bool(conv.value)
 
     # -- relocalization from a coarse pose (Localization::Init upstream) -----------------------------------
-    def _relocalize(self, call, T_guess, coarse_scores, cfg, wide=False):
+    def _relocalize(self, call, T_guess, coarse_scores, cfg, wide=False, name=None):
         c = cfg if isinstance(cfg, _abi.FlsRelocCfg) else reloc_cfg(**cfg)
         k = max(1, int(c.n_refine))
         Tc = np.ascontiguousarray(np.asarray(T_guess, np.float64).T).copy()
@@ -239,7 +246,8 @@ class Registration:
         vp = lambda a: a.ctypes.data_as(C.c_void_p)
         evals = C.c_int64(-1)
         if wide:
-            check(call(C.byref(c), vp(Tc), C.byref(res), vp(rT), vp(rconv), vp(rfit), vp(ridx), C.byref(evals)), "fls_relocalize_wide")
+            check(call(C.byref(c), vp(Tc), C.byref(res), vp(rT), vp(rconv), vp(rfit), vp(ridx), C.byref(evals)),
+                  name or "fls_relocalize_wide")
         else:
             check(call(C.byref(c), vp(Tc), C.byref(res), vp(rT), vp(rconv), vp(rfit), vp(ridx), vp(cs) if coarse_scores else None, int(coarse_scores)),
                   "fls_relocalize")
@@ -281,6 +289,25 @@ class Registration:
         """relocalize_wide with a device-resident packed float4 scan (it must stay valid until the next Match)."""
         return self._relocalize(lambda *a: lib().fls_relocalize_wide_device(self._h, C.c_void_p(int(d_ptr)) if d_ptr else None, int(n), *a), T_guess, 0,
                                 cfg if cfg is not None else kw, wide=True)
+
+    def relocalize_multi(self, cloud_or_cluster, guesses, cfg=None, **kw):
+        """fls_relocalize_multi: relocalize_wide over the grids of every guess in `guesses` ((G,4,4), 1..64 poses, e.g. place_pose of
+        each place_query candidate) as one search; hypothesis g * P + p is hypothesis p of guess g's grid.  Returns (RelocResult
+        without coarse_scores, the number of pose evaluations the search ran)."""
+        c = cloud_or_cluster
+        if isinstance(c, PointcloudCluster):
+            c = c.ordered_cloud if self.cfg.method == _abi.FLS_NDT else c.planar_cloud
+        p, n, s, keep = _cloud(c)
+        G, T0 = _guesses(guesses)
+        return self._relocalize(lambda cp, *a: lib().fls_relocalize_multi(self._h, p, n, s, cp, G.ctypes.data_as(C.c_void_p), len(G), *a), T0, 0,
+                                cfg if cfg is not None else kw, wide=True, name="fls_relocalize_multi")
+
+    def relocalize_multi_device(self, d_ptr: int, n: int, guesses, cfg=None, **kw):
+        """relocalize_multi with a device-resident packed float4 scan (it must stay valid until the next Match)."""
+        G, T0 = _guesses(guesses)
+        d = C.c_void_p(int(d_ptr)) if d_ptr else None
+        return self._relocalize(lambda cp, *a: lib().fls_relocalize_multi_device(self._h, d, int(n), cp, G.ctypes.data_as(C.c_void_p), len(G), *a), T0,
+                                0, cfg if cfg is not None else kw, wide=True, name="fls_relocalize_multi_device")
 
     def relocalize_wide_levels(self) -> list:
         """fls_relocalize_wide_levels: the nodes the last relocalize_wide reached per level, from its start level down to 0."""

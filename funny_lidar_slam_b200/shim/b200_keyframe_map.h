@@ -122,6 +122,18 @@ public:
         return r;
     }
 
+    // the k stored keyframes nearest to a scan, best first (fewer when the store holds fewer): the guesses of a RelocalizeMulti
+    std::vector<PlaceMatch> PlaceQuery(const PCLPointCloudXYZI& cloud, int k) {
+        std::vector<fls_place_match> m(k > 0 ? (size_t)k : 0);
+        size_t n = 0;
+        std::vector<PlaceMatch> r;
+        if (k > 0 && Ok(fls_keyframes_place_query(store_, &sc_cfg_, cloud.points.data(), cloud.points.size(), sizeof(PCLPointXYZI), (size_t)k, m.data(), &n,
+                                                  nullptr, nullptr),
+                        "fls_keyframes_place_query"))
+            for (size_t i = 0; i < n; ++i) r.push_back(PlaceMatch{static_cast<KeyFrame::ID>(m[i].id), m[i].distance, m[i].yaw});
+        return r;
+    }
+
     // System::VisualizeGlobalMap's state (global_map, last_frame_id; system.cpp:851-852) with global_map kept on the device in two
     // buffers used in turn: one is the base of a round, the other receives its result.
     class GlobalMap {

@@ -16,6 +16,7 @@
 
 #include <glog/logging.h>
 
+#include <algorithm>
 #include <limits>
 #include <memory>
 #include <string>
@@ -111,6 +112,28 @@ public:
             return false;
         }
         DLOG(INFO) << "B200 RelocalizeWide hypotheses=" << res.n_hypotheses << " evaluations=" << evaluations << " fitness=" << res.fitness;
+        return res.accepted != 0;
+    }
+
+    // Relocalize from several coarse poses in one search (fls_relocalize_multi): the grids of up to 64 guesses, e.g. place_pose of each
+    // of KeyFrameMap::PlaceQuery's top-k candidates, ranked together and the best refined by one batch Match.  T receives the chosen
+    // pose (also when false is returned); guesses are not modified.
+    bool RelocalizeMulti(const PointcloudClusterPtr& source_cloud_cluster, const std::vector<Mat4d>& guesses, Mat4d& T, const fls_reloc_cfg& cfg,
+                         float* fitness) {
+        const auto& cloud = method_ == FLS_NDT ? source_cloud_cluster->ordered_cloud_.points : source_cloud_cluster->planar_cloud_.points;
+        std::vector<double> g(16 * guesses.size());
+        for (size_t k = 0; k < guesses.size(); ++k) std::copy(guesses[k].data(), guesses[k].data() + 16, g.data() + 16 * k);
+        fls_reloc_result res;
+        int64_t evaluations = 0;
+        const int rc = fls_relocalize_multi(handle_, cloud.data(), cloud.size(), sizeof(PCLPointXYZI), &cfg, g.data(), (int32_t)guesses.size(), T.data(),
+                                            &res, nullptr, nullptr, nullptr, nullptr, &evaluations);
+        if (fitness) *fitness = rc == FLS_OK ? res.fitness : FloatNaN;
+        if (rc != FLS_OK) {
+            LOG(WARNING) << "fls_relocalize_multi: " << fls_strerror(rc) << " " << fls_last_error();
+            return false;
+        }
+        DLOG(INFO) << "B200 RelocalizeMulti guesses=" << guesses.size() << " hypotheses=" << res.n_hypotheses << " evaluations=" << evaluations
+                   << " fitness=" << res.fitness;
         return res.accepted != 0;
     }
 

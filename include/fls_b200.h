@@ -31,6 +31,8 @@
  *                                 searching an x-y-yaw grid around the given pose
  *   fls_relocalize_wide /      <- the same over a whole local map (up to 2^31 hypotheses), by exact branch and bound
  *   _wide_device
+ *   fls_relocalize_multi /     <- the same around up to 64 guesses at once (the top-k candidates of fls_keyframes_place_query),
+ *   _multi_device                 ranked together in one search and refined by one batch Match
  *   fls_keyframes_detect_loop  <- LoopClosure::DetectByFeature (src/slam/loop_closure.cpp:62-64, a stub upstream), by Scan Context
  *   fls_keyframes_place_query  <- the keyframe a scan was taken near, and its yaw: the guess of fls_relocalize without a clicked pose
  *
@@ -316,6 +318,30 @@ int fls_relocalize_wide_device(fls_handle* h, const void* d_scan, size_t n, cons
  * level: all its blocks; below: the children of the blocks kept one level up; 0 levels after an empty scan or a failed call before
  * the search).  Writes min(capacity, levels) values and returns the number of levels, or FLS_ERR_INVALID_ARG. */
 int fls_relocalize_wide_levels(const fls_handle* h, int64_t* nodes, int capacity);
+
+/* Relocalization from several coarse poses in one search: the grids that fls_relocalize defines for cfg around each of G = n_guesses
+ * guesses (1..64; guess g is the column-major pose at guesses_colmajor + 16 g), searched as one grid of G * P hypotheses.  Hypothesis
+ * g * P + p is hypothesis p of guess g's grid (P: the hypotheses of one grid), with the coarse score fls_relocalize gives it on guess
+ * g, bit for bit; out->n_hypotheses = G * P, and best_hypothesis and refined_index use this index (the guess is index / P).  The
+ * selection (the n_refine smallest scores of all grids, ties to the lower index), the one batch Match of the picks, the fitness and
+ * the choice are fls_relocalize's.  The search is fls_relocalize_wide's exact branch and bound over all grids together: one
+ * pruning threshold, the n_refine-th best score of any guess, and a lower bound that holds for every guess's hypotheses; a block
+ * never spans two guesses.  When G * P <= 2^20 it scores every hypothesis.  *evaluations and fls_relocalize_wide_levels report the
+ * search as for fls_relocalize_wide, and launches and waits are those of fls_relocalize_wide with the same node counts: on at most
+ * 2^20 hypotheses in all they do not depend on G.
+ *
+ * T is output only: it receives the chosen pose, or guess 0 after an empty scan or an empty coarse cloud.  Grids are not merged
+ * where they overlap (identical guesses tie, and the lower index wins); a grid off the map scores max_range and is not picked.
+ * Caps: G * P <= 2^31 and floor(xy_radius / xy_step) <= 32767.  FLS_ERR_INVALID_ARG, in addition to fls_relocalize_wide's cases,
+ * for a NULL guesses_colmajor, n_guesses outside 1..64, a non-finite entry of any guess, or G * P > 2^31.  FLS_ERR_CAPACITY,
+ * plug-ins, modes, FLS_ERR_NO_MAP, the batch-in-flight refusal, the empty scan and the state left for fls_fitness and Match are
+ * fls_relocalize_wide's; a refused call leaves T and the handle as they were. */
+int fls_relocalize_multi(fls_handle* h, const void* scan, size_t n, size_t stride_bytes, const fls_reloc_cfg* cfg, const double* guesses_colmajor,
+                         int32_t n_guesses, double T_colmajor[16], fls_reloc_result* out, double* refined_T, int32_t* refined_converged,
+                         float* refined_fitness, int64_t* refined_index, int64_t* evaluations);
+int fls_relocalize_multi_device(fls_handle* h, const void* d_scan, size_t n, const fls_reloc_cfg* cfg, const double* guesses_colmajor,
+                                int32_t n_guesses, double T_colmajor[16], fls_reloc_result* out, double* refined_T, int32_t* refined_converged,
+                                float* refined_fitness, int64_t* refined_index, int64_t* evaluations);
 
 /* Device-side results for a consumer that lives on the GPU (the per-batch NCCL all-gather of poses, SURVEY.md §8e): once set,
  * every Match additionally writes, for scan s of the call, 18 doubles at d_results + 18*s — the column-major Mat4d pose
