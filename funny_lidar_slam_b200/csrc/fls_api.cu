@@ -35,9 +35,6 @@ Handle::Handle(const fls_config& c) : cfg(c) {
 }
 
 void Handle::release() {
-    if (h_state) cudaFreeHost(h_state);
-    h_state = nullptr;
-    h_batch.release();
     for (auto& e : prof_ev) {
         if (e) cudaEventDestroy(e);
         e = nullptr;
@@ -54,9 +51,7 @@ void Handle::init() {
     FLS_CUDA(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
     FLS_CUDA(cudaEventCreate(&ev0));
     FLS_CUDA(cudaEventCreate(&ev1));
-    FLS_CUDA(cudaMallocHost(&h_state, sizeof(GnState) * kMaxBatch + 64));
-    h_abort = reinterpret_cast<unsigned*>(h_state + kMaxBatch);  // pinned: a copy into pageable memory would make the enqueue wait for the kernel
-    *h_abort = 0;
+    h_state.reserve(kMaxBatch);
     state.reserve(kMaxBatch);
     switch (cfg.method) {
         case FLS_P2PLANE_IVOX: plugin = make_ivox_plugin(*this); break;
@@ -163,21 +158,11 @@ unsigned Handle::next_ll_epoch(size_t n_records) {
     return match_epoch << 8;
 }
 
-unsigned char* Handle::batch_table(size_t bytes) {
-    d_batch.reserve(bytes);
-    return h_batch.reserve(bytes);
-}
-
-void Handle::send_batch_table(size_t bytes) {
-    FLS_CUDA(cudaMemcpyAsync(d_batch.p, h_batch.p, bytes, cudaMemcpyHostToDevice, stream));
-    h2d_bytes += (long long)bytes;
-}
-
 void Handle::read_back(int B) {
     // h_log is about to hold this call's logs: until unpack records their sizes, no scan has one (a Match that fails after
     // its launch, e.g. through the v9 watchdog, leaves no log rather than a mix of two calls)
     log_n.assign(1, 0);
-    FLS_CUDA(cudaMemcpyAsync(h_state, state.p, sizeof(GnState) * (size_t)B, cudaMemcpyDeviceToHost, stream));
+    FLS_CUDA(cudaMemcpyAsync(h_state.p, state.p, sizeof(GnState) * (size_t)B, cudaMemcpyDeviceToHost, stream));
     d2h_bytes += (long long)(sizeof(GnState) * (size_t)B);
     if (log_cap) {
         const size_t bytes = sizeof(fls_iter_log) * (size_t)log_cap * (size_t)B;
@@ -190,14 +175,8 @@ void Handle::unpack(int B, const size_t* n, double* T, int* converged, fls_match
     float kernel_ms = 0.f;
     if (profile) FLS_CUDA(cudaEventElapsedTime(&kernel_ms, prof_ev[0], prof_ev[1]));
     for (int s = 0; s < B; ++s) {
-        const GnState& gs = h_state[s];
-        double* Ts = T + 16 * s;
-        for (int r = 0; r < 3; ++r) {
-            for (int c = 0; c < 3; ++c) Ts[c * 4 + r] = gs.R[r * 3 + c];
-            Ts[12 + r] = gs.t[r];
-        }
-        Ts[3] = Ts[7] = Ts[11] = 0.0;
-        Ts[15] = 1.0;
+        const GnState& gs = h_state.p[s];
+        gn_pose_T(gs.R, gs.t, T + 16 * s);
         if (converged) converged[s] = gs.converged;
         if (st) {
             fls_match_stats& o = st[s];
@@ -217,7 +196,7 @@ void Handle::unpack(int B, const size_t* n, double* T, int* converged, fls_match
     }
     std::memcpy(T_final, T, sizeof(T_final));
     log_n.resize(B);
-    for (int s = 0; s < B; ++s) log_n[s] = h_state[s].iter < log_cap ? h_state[s].iter : log_cap;
+    for (int s = 0; s < B; ++s) log_n[s] = h_state.p[s].iter < log_cap ? h_state.p[s].iter : log_cap;
 }
 
 int Handle::filter_batch(int B, const float4* const* d, const size_t* n, float leaf, DevBuf<float4>& dst, size_t* off, size_t* ns) {
@@ -257,19 +236,14 @@ int Handle::inserted(int rc, fls_match_stats* st) {
 }
 
 // IsNeedAddCloud of the ICP and kd-tree LOAM plug-ins
-static void mat3_from_T(const double* T, double* R) {
-    for (int r = 0; r < 3; ++r)
-        for (int c = 0; c < 3; ++c) R[r * 3 + c] = T[c * 4 + r];
-}
-
 bool KeyFrameGate::need(const double* T, double dist_thre, double rot_thre) {
     if (!have_last) {
         std::memcpy(last_T, T, 16 * sizeof(double));
         have_last = true;
     }
-    double Rl[9], Rc[9], Rli[9], Rd[9];
-    mat3_from_T(last_T, Rl);
-    mat3_from_T(T, Rc);
+    const GnPose last = gn_pose(last_T), cur = gn_pose(T);
+    const double* Rl = last.R;
+    double Rli[9], Rd[9];
     {  // 3x3 inverse by cofactors
         const double c00 = Rl[4] * Rl[8] - Rl[5] * Rl[7], c01 = Rl[5] * Rl[6] - Rl[3] * Rl[8], c02 = Rl[3] * Rl[7] - Rl[4] * Rl[6];
         const double id = 1.0 / (Rl[0] * c00 + Rl[1] * c01 + Rl[2] * c02);
@@ -277,7 +251,7 @@ bool KeyFrameGate::need(const double* T, double dist_thre, double rot_thre) {
         Rli[3] = c01 * id; Rli[4] = (Rl[0] * Rl[8] - Rl[2] * Rl[6]) * id; Rli[5] = (Rl[2] * Rl[3] - Rl[0] * Rl[5]) * id;
         Rli[6] = c02 * id; Rli[7] = (Rl[1] * Rl[6] - Rl[0] * Rl[7]) * id; Rli[8] = (Rl[0] * Rl[4] - Rl[1] * Rl[3]) * id;
     }
-    mat3_mul(Rli, Rc, Rd);
+    mat3_mul(Rli, cur.R, Rd);
     const double roll = std::atan2(Rd[7], Rd[8]), pitch = std::asin(-Rd[6]), yaw = std::atan2(Rd[3], Rd[0]);
     const double dt[3] = {T[12] - last_T[12], T[13] - last_T[13], T[14] - last_T[14]};
     if (norm3(dt) > dist_thre || std::fabs(roll) > rot_thre || std::fabs(pitch) > rot_thre || std::fabs(yaw) > rot_thre) {

@@ -1,6 +1,6 @@
-// fls_gn.cu — state initialisation of a single NDT or ICP Match's Gauss-Newton loop (a sub-grid launch starts each scan with
-// gn_start_kernel, the LOAM-iVox path in its batch prep kernel), and the per-device kernel attributes that size and prepare every
-// persistent launch.  The solve / update / stop rule itself (K6) is device code in fls_gn.cuh: gn_step_pre, which every persistent
+// fls_gn.cu — state initialisation of a single NDT or ICP Match's Gauss-Newton loop (every loop starts from gn_state_init, fls_gn.cuh:
+// here, in a sub-grid launch's gn_start_kernel and in the LOAM-iVox batch prep kernel), and the per-device kernel attributes that size
+// and prepare every persistent launch.  The solve / update / stop rule itself (K6) is device code in fls_gn.cuh: gn_step_pre, which every persistent
 // kernel runs, and the single-level fold around it (gn_handover / gn_handover_rows), which every one but the LOAM-iVox batch kernel
 // uses.
 // fls_gn_step_probe runs gn_step_pre alone on constructed cases, for the tests that hold the step to a reference.

@@ -43,10 +43,11 @@ struct __align__(16) GnBatchItem {
     int pad[2];
 };
 
-// the pose a loop starts from
+// the pose a loop starts from; also the 12-double record of the pose tables the scoring kernels read (fls_reloc.cu)
 struct GnPose {
     double R[9], t[3];  // row-major R
 };
+static_assert(sizeof(GnPose) == 12 * sizeof(double), "GnPose is a packed row-major R | t record");
 inline GnPose gn_pose(const double* T_colmajor) {
     GnPose p;
     for (int r = 0; r < 3; ++r) {
@@ -54,6 +55,15 @@ inline GnPose gn_pose(const double* T_colmajor) {
         p.t[r] = T_colmajor[12 + r];
     }
     return p;
+}
+// and back: row-major R and t into a column-major 4x4
+inline void gn_pose_T(const double* R, const double* t, double* T_colmajor) {
+    for (int r = 0; r < 3; ++r) {
+        for (int c = 0; c < 3; ++c) T_colmajor[c * 4 + r] = R[r * 3 + c];
+        T_colmajor[12 + r] = t[r];
+    }
+    T_colmajor[3] = T_colmajor[7] = T_colmajor[11] = 0.0;
+    T_colmajor[15] = 1.0;
 }
 
 void launch_gn_init(GnState* d_state, const double* T_colmajor, cudaStream_t st);  // the state alone (single NDT / ICP Match)

@@ -1,5 +1,5 @@
 // fls_handle.h — the object behind `fls_handle*`: configuration, stream, what every plug-in's Match shares, and the one
-// registration plug-in that cfg.method names, which owns its map.
+// registration plug-in that cfg.method names, which owns its map and the buffers only it uses.
 #pragma once
 #include <memory>
 #include <vector>
@@ -96,10 +96,9 @@ struct Handle {
     // Gauss-Newton state shared by the plug-ins
     DevBuf<uint4> ll_rows;      // LL hand-over records of the persistent kernels: [grid][32] rows + pose records
     unsigned match_epoch = 0;   // tag prefix of those records
-    PinnedBuf<unsigned char> h_batch;  // staging of the LOAM-iVox per-batch tables (poses, offsets, scan descriptors, CTA map, pointers)
-    DevBuf<unsigned char> d_batch;     // their device copy, or the items of a match_subgrids launch
+    DevBuf<unsigned char> subgrid_items;  // the items of a match_subgrids launch (GnBatchItem<Args>[B])
     DevBuf<GnState> state;
-    GnState* h_state = nullptr;  // pinned
+    PinnedBuf<GnState> h_state;  // the states of the last Match, read back (room for kMaxBatch)
     DevBuf<fls_iter_log> log;
     std::vector<fls_iter_log> h_log;  // FLS_FLAG_ITER_LOG: log_cap entries per scan of the last Match
     int log_cap = 0;
@@ -109,7 +108,6 @@ struct Handle {
     bool profile = false;
     long long per_point_iter_bytes = 0;  // fixed part of the algorithmic bytes per point-iteration (set by gn_launch)
     long long per_cand_bytes = 0;        // bytes per scanned map record
-    unsigned* h_abort = nullptr;  // watchdog word of the last LOAM-iVox batch launch (pinned, behind h_state; read back with the states)
     BuildScratch scratch;                // voxel-grid passes of Match and the local-map crop
 
     // optional caller-owned device buffer that receives {pose, converged, iterations} per scan (fls_set_result_buffer_device)
@@ -157,8 +155,20 @@ struct Handle {
     unsigned next_ll_epoch(size_t n_records);  // LL records for the next launch; returns its tag base
     fls_iter_log* scan_log(int s) { return log_cap ? log.p + (size_t)s * log_cap : nullptr; }
     double* scan_result(int s) { return (result_buf && (size_t)s < result_cap) ? result_buf + (size_t)s * kResultLen : nullptr; }
-    unsigned char* batch_table(size_t bytes);  // pinned staging of a per-batch table ...
-    void send_batch_table(size_t bytes);       // ... and its copy to d_batch
+    // the control block of scan s's loop in a launch of tag base `tag_base`: its state, LL rows and pose record, the plug-in's
+    // parameters, its iteration log and its result record
+    GnLoopCtl loop_ctl(int s, int method, int min_effective, unsigned tag_base, uint4* rows, uint4* pose) {
+        GnLoopCtl c;
+        c.state = state.p + s;
+        c.ll_rows = rows;
+        c.ll_pose = pose;
+        c.tag_base = tag_base;
+        c.gp = gn_params(method, min_effective);
+        c.log = scan_log(s);
+        c.log_cap = log_cap;
+        c.result = scan_result(s);
+        return c;
+    }
     // the fused Gauss-Newton launch: roofline byte rates, profile events around `launch`, the launch counter and the source
     // cloud GetFitnessScore reads afterwards
     template <class F>
@@ -180,15 +190,8 @@ struct Handle {
     template <class F>
     void match_single(int method, int min_effective, int grid, long long point_iter_bytes, long long cand_bytes, const float4* src, size_t src_n,
                       size_t n_source, double* T, int* converged, fls_match_stats* st, F&& launch) {
-        GnLoopCtl ctl;
-        ctl.tag_base = next_ll_epoch((size_t)grid * 32 + kLlPoseLen);
-        ctl.state = state.p;
-        ctl.ll_rows = ll_rows.p;
-        ctl.ll_pose = ll_rows.p + (size_t)grid * 32;
-        ctl.gp = gn_params(method, min_effective);
-        ctl.log = scan_log(0);
-        ctl.log_cap = log_cap;
-        ctl.result = scan_result(0);
+        const unsigned tag_base = next_ll_epoch((size_t)grid * 32 + kLlPoseLen);  // may move ll_rows
+        const GnLoopCtl ctl = loop_ctl(0, method, min_effective, tag_base, ll_rows.p, ll_rows.p + (size_t)grid * 32);
         launch_gn_init(state.p, T, stream);
         launches++;
         gn_launch(point_iter_bytes, cand_bytes, src, src_n, [&] { launch(ctl); });
@@ -203,7 +206,7 @@ struct Handle {
     // The Gauss-Newton half of such a Match; a single kd-tree LOAM Match is B = 1, whose sub-grid is the whole grid.  Scan s (ns[s]
     // points, also its n_source) gets one CTA per `per_cta` points, all scaled down together when the `cap` co-resident CTAs of the
     // kernel cannot hold them (more scans than CTAs: FLS_ERR_INVALID_ARG).  Then, per scan: its control block and its item, whose arguments
-    // fill(s, item.a) sets, and one launch that starts its state from T and writes the item to d_batch; the gn_launch of
+    // fill(s, item.a) sets, and one launch that starts its state from T and writes the item to subgrid_items; the gn_launch of
     // launch(d_items, grid), the wait, and T / converged / stats of every scan.  fit_src / fit_n: the cloud GetFitnessScore reads
     // afterwards.
     template <class Args, class Fill, class Launch>
@@ -222,21 +225,14 @@ struct Handle {
             grid += ncta[s];
         }
         const unsigned tag_base = next_ll_epoch((size_t)grid * 32 + (size_t)B * kLlPoseLen);
-        GnBatchItem<Args>* d_items = reinterpret_cast<GnBatchItem<Args>*>(d_batch.reserve(sizeof(GnBatchItem<Args>) * (size_t)B));
+        GnBatchItem<Args>* d_items = reinterpret_cast<GnBatchItem<Args>*>(subgrid_items.reserve(sizeof(GnBatchItem<Args>) * (size_t)B));
         uint4* pose_base = ll_rows.p + (size_t)grid * 32;
         int cta0 = 0;
         for (int s = 0; s < B; ++s) {
             GnBatchItem<Args> it;
             std::memset(&it, 0, sizeof(it));
             fill(s, it.a);
-            it.ctl.state = state.p + s;
-            it.ctl.ll_rows = ll_rows.p + (size_t)cta0 * 32;
-            it.ctl.ll_pose = pose_base + (size_t)s * kLlPoseLen;
-            it.ctl.tag_base = tag_base;
-            it.ctl.gp = gn_params(method, min_effective);
-            it.ctl.log = scan_log(s);
-            it.ctl.log_cap = log_cap;
-            it.ctl.result = scan_result(s);
+            it.ctl = loop_ctl(s, method, min_effective, tag_base, ll_rows.p + (size_t)cta0 * 32, pose_base + (size_t)s * kLlPoseLen);
             it.cta0 = cta0;
             it.ncta = ncta[s];
             cta0 += ncta[s];

@@ -200,7 +200,7 @@ class IcpPlugin final : public Plugin {
         h.match_single(FLS_ICP_P2P, 0, grid, 16 + 16LL * 27, 16, scan.p, n, n, T, converged, st,
                        [&](const GnLoopCtl& ctl) { launch_icp_loop(a, ctl, grid, h.stream); });
         // IsNeedAddCloud (:218-236): key-frame gating on translation / RPY deltas against a persistent last_T
-        if (h.h_state->converged && !cfg.localization_mode && gate.need(T, cfg.dist_thre_add_cloud, cfg.rot_thre_add_cloud)) {
+        if (h.h_state.p->converged && !cfg.localization_mode && gate.need(T, cfg.dist_thre_add_cloud, cfg.rot_thre_add_cloud)) {
             ins.reserve(n);
             launch_transform_f(scan.p, n, T, ins.p, h.stream);  // :156 TransformPointCloud(source, final) in float
             h.launches++;

@@ -359,7 +359,7 @@ class KdPlugin final : public Plugin {
         const int rc = match_scans(1, &d_planar, &n_planar, &d_corner, &n_corner, T, converged, st);
         if (rc != FLS_OK) return rc;
         // key-frame insertion: loam_point_to_plane_kdtree.h:146-150 (gate evaluated before the mode test), loam_full_kdtree.h:178-186
-        if (h.h_state->converged && gate.need(T, cfg.dist_thre_add_cloud, cfg.rot_thre_add_cloud) && (full || !cfg.localization_mode)) {
+        if (h.h_state.p->converged && gate.need(T, cfg.dist_thre_add_cloud, cfg.rot_thre_add_cloud) && (full || !cfg.localization_mode)) {
             int rc2;
             if (full) {
                 ins.reserve(n_planar);

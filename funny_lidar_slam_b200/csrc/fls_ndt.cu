@@ -644,7 +644,7 @@ class NdtPlugin final : public Plugin {
         // 80 B voxel record per estimated voxel hit; the 6x6 sums are fused (no per-point output).
         h.match_single(FLS_NDT, cfg.ndt_min_effective_pts, grid, 16 + 16LL * 7, 80, scan.p, n, n, T, converged, st,
                        [&](const GnLoopCtl& ctl) { launch_ndt_loop(a, ctl, grid, h.stream); });
-        if (!h.h_state->failed && !cfg.localization_mode) {
+        if (!h.h_state.p->failed && !cfg.localization_mode) {
             // :326-330 — the scan enters the map transformed by the INPUT guess T, not the optimised pose  [quirk 6]
             ins.reserve(n);
             launch_transform_f(scan.p, n, T_in, ins.p, h.stream);

@@ -1,8 +1,9 @@
 // fls_p2plane.cu — K1 (+ fused K6), generation 8: the whole LoamPointToPlaneIVOX Gauss-Newton loop of ONE scan as one persistent
 // kernel with a CTA barrier per iteration.  It serves the single Match (fls_match / fls_match_device); batches run on generation 9
 // (fls_p2plane_v9.cu), which shares the per-point arithmetic (fls_knn.cuh, fls_plane.cuh).  This file also holds the per-batch query
-// preparation (one kernel: state init + tile-local locality sort), the Match-internal insertion rule of mapping mode, the k-NN test entry
-// and the plug-in's host half (IvoxPlugin: its iVox map, AddCloudToLocalMap, and the single and batch Match on v8 / v9).
+// preparation (one kernel: every scan's gn_state_init + tile-local locality sort), the Match-internal insertion rule of mapping mode, the
+// k-NN test entry and the plug-in's host half (IvoxPlugin: its iVox map, its per-batch table and watchdog word, AddCloudToLocalMap, and
+// the single and batch Match on v8 / v9 over the shared host half of a Match in Handle).
 //
 // Per source point and iteration it fuses what LoamPointToPlaneIVOX::PlanerMatch / ::SumCoefficient do
 // (include/registration/loam_point_to_plane_ivox.h:256-340 upstream): transform with the current pose, bounded
@@ -29,6 +30,8 @@
 //     a 32-byte record {J[6], |d|} per valid point (two float4 arrays) + a flag byte, re-read only on the stale path.
 #include <cooperative_groups.h>
 
+#include <algorithm>
+
 #include <cub/cub.cuh>
 
 #include "fls_gn.cuh"
@@ -40,11 +43,6 @@
 namespace fls {
 
 static constexpr int kP2PlaneBlock = 768;  // shape of the single-scan kernel: one 24-warp CTA per SM
-
-struct PoseArg {
-    double R[9];  // row-major
-    double t[3];
-};
 
 // whole-loop arguments of the single-scan kernel (generation 8)
 struct P2PlaneArgs {
@@ -264,7 +262,7 @@ __device__ __forceinline__ unsigned spread_bits3(unsigned v) {  // up to 10 bits
 constexpr int kOrdThreads = 512, kOrdItems = kOrderTile / kOrdThreads;
 
 __global__ void __launch_bounds__(kOrdThreads) p2plane_prep_kernel(const float4* const* __restrict__ scan_ptrs, const int* __restrict__ offsets,
-                                                                   const int* __restrict__ tile_off, int n_scans, const PoseArg* __restrict__ poses,
+                                                                   const int* __restrict__ tile_off, int n_scans, const GnPose* __restrict__ poses,
                                                                    float inv_res, unsigned* __restrict__ zero, int n_zero,
                                                                    unsigned char* __restrict__ flags, GnState* __restrict__ states,
                                                                    float4* __restrict__ dst, const HashSlot* __restrict__ ctab, unsigned cmask,
@@ -272,20 +270,7 @@ __global__ void __launch_bounds__(kOrdThreads) p2plane_prep_kernel(const float4*
     using Sort = cub::BlockRadixSort<unsigned, kOrdThreads, kOrdItems, unsigned>;
     __shared__ typename Sort::TempStorage s_sort;
     if (blockIdx.x == 0) {
-        if ((int)threadIdx.x < n_scans) {
-            GnState* s = states + threadIdx.x;
-            const PoseArg& pose = poses[threadIdx.x];
-            for (int k = 0; k < 9; ++k) s->R[k] = s->R0[k] = s->Rprev[k] = pose.R[k];
-            for (int k = 0; k < 3; ++k) s->t[k] = s->t0[k] = s->tprev[k] = pose.t[k];
-            s->last_rot = s->last_pos = 0.0;
-            s->sum_res = 0;
-            s->cand_total = s->hits_total = 0;
-            s->n_valid = 0;
-            s->iter = 0;
-            s->done = 0;
-            s->converged = 0;
-            s->failed = 0;
-        }
+        if ((int)threadIdx.x < n_scans) gn_state_init(states + threadIdx.x, poses[threadIdx.x]);
         for (int k = threadIdx.x; k < n_zero; k += blockDim.x) zero[k] = 0;
     }
     const int tile = (int)blockIdx.x;
@@ -303,7 +288,7 @@ __global__ void __launch_bounds__(kOrdThreads) p2plane_prep_kernel(const float4*
     const int first = __ldg(offsets + sid) + (tile - __ldg(tile_off + sid)) * kOrderTile;  // batch position of the tile
     const int n_here = min(kOrderTile, __ldg(offsets + sid + 1) - first);
     const float4* __restrict__ src = scan_ptrs[sid] + (first - __ldg(offsets + sid));
-    const PoseArg& pose = poses[sid];
+    const GnPose& pose = poses[sid];
     unsigned key[kOrdItems], pos[kOrdItems];
 #pragma unroll
     for (int k = 0; k < kOrdItems; ++k) {  // striped: item k of thread t is point k * kOrdThreads + t of the tile (coalesced)
@@ -371,7 +356,7 @@ __global__ void ivox_knn_test_kernel(IvoxView map, const float4* __restrict__ q,
 // last PlanerMatch found (those were searched at the pose BEFORE the last update — GnState::Rprev/tprev) and at the
 // centre of the 0.5 m cell it falls into:  class 2 ("no need to down-sample": nearest neighbour outside the cell in all
 // three axes), class 1 (no cached neighbour closer to the cell centre than the point itself), class 0 (dropped)  [quirk 8].
-__global__ void ivox_insert_rule_kernel(IvoxView map, const float4* __restrict__ src, int n, PoseArg prev, PoseArg fin, double filter,
+__global__ void ivox_insert_rule_kernel(IvoxView map, const float4* __restrict__ src, int n, GnPose prev, GnPose fin, double filter,
                                         unsigned char* __restrict__ cls, float4* __restrict__ world) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
@@ -449,33 +434,29 @@ static void launch_p2plane_loop(const P2PlaneArgs& a, const GnLoopCtl& ctl, int 
     launch_cooperative(p2plane_gn_kernel<kP2PlaneBlock, kMinB>, grid, kP2PlaneBlock, p2plane_smem(), st, a, ctl);
 }
 
+// The per-batch table of a LOAM-iVox Match, staged in pinned memory and sent with one copy
+struct IvoxBatchTable {
+    GnPose pose[kMaxBatch];        // the pose each scan starts from
+    int off[kMaxBatch + 4];        // [n_scans + 1]: the scans' positions in the batch
+    int tile_off[kMaxBatch + 4];   // [n_scans + 1]: prefix sums of order_tiles(n) over the scans
+    P2PlaneScan desc[kMaxBatch];   // the v9 kernel's scan descriptors
+    const float4* ptr[kMaxBatch];  // device pointers of the scans
+};
+
 // Per-batch preparation: state init, flag and ticket reset and the locality order of every scan, in one launch of one block per
-// tile (one block for an empty batch).  d_scan_ptrs[n_scans]: device pointers of the scans; d_offsets[n_scans + 1]: their positions
-// in the batch; d_tile_off[n_scans + 1]: prefix sums of order_tiles(n) over the scans; d_zero[n_zero]: words zeroed on the way (v9
-// tickets).
-static void prepare_queries(const float4* const* d_scan_ptrs, const int* d_offsets, const int* d_tile_off, int n_tiles, int n_scans,
-                            const PoseArg* d_poses, GnState* d_states, const IvoxView& map, unsigned char* d_flags, float4* d_sorted,
-                            unsigned* d_zero, int n_zero, cudaStream_t st, int* launches) {
-    p2plane_prep_kernel<<<n_tiles > 0 ? n_tiles : 1, kOrdThreads, 0, st>>>(d_scan_ptrs, d_offsets, d_tile_off, n_scans, d_poses, map.inv_res, d_zero,
-                                                                          n_zero, d_flags, d_states, d_sorted, map.ctab, map.cmask, map.lists);
+// tile (one block for an empty batch).  d_tbl: the batch's table on the device; d_zero[n_zero]: words zeroed on the way (v9 tickets).
+static void prepare_queries(const IvoxBatchTable* d_tbl, int n_tiles, int n_scans, GnState* d_states, const IvoxView& map, unsigned char* d_flags,
+                            float4* d_sorted, unsigned* d_zero, int n_zero, cudaStream_t st, int* launches) {
+    p2plane_prep_kernel<<<n_tiles > 0 ? n_tiles : 1, kOrdThreads, 0, st>>>(d_tbl->ptr, d_tbl->off, d_tbl->tile_off, n_scans, d_tbl->pose, map.inv_res,
+                                                                          d_zero, n_zero, d_flags, d_states, d_sorted, map.ctab, map.cmask, map.lists);
     if (launches) *launches += 1;
 }
 
 // The Match-internal AddCloudToLocalMap of mapping mode: classifies and compacts the points that enter the map (d_world, d_out: n
 // records).  Returns the number of points selected for insertion (class 1 then class 2, input order) in d_out; synchronises the stream.
-static size_t select_ivox_inserts(const IvoxView& map, const float4* d_src, int n, const double* R_prev, const double* t_prev, const double* R_fin,
-                                  const double* t_fin, double filter, float4* d_world, float4* d_out, BuildScratch& sc, cudaStream_t st,
-                                  int* launches) {
+static size_t select_ivox_inserts(const IvoxView& map, const float4* d_src, int n, const GnPose& prev, const GnPose& fin, double filter, float4* d_world,
+                                  float4* d_out, BuildScratch& sc, cudaStream_t st, int* launches) {
     if (n <= 0) return 0;
-    PoseArg prev, fin;
-    for (int k = 0; k < 9; ++k) {
-        prev.R[k] = R_prev[k];
-        fin.R[k] = R_fin[k];
-    }
-    for (int k = 0; k < 3; ++k) {
-        prev.t[k] = t_prev[k];
-        fin.t[k] = t_fin[k];
-    }
     sc.minmax.reserve((size_t)n / 4 + 16);  // class bytes
     unsigned char* cls = reinterpret_cast<unsigned char*>(sc.minmax.p);
     sc.keys.reserve((size_t)n + 1);
@@ -502,6 +483,11 @@ class IvoxPlugin final : public Plugin {
     DevBuf<unsigned char> flags;
     DevBuf<unsigned> tickets;   // chunk ticket counters of the v9 kernel (dynamic work distribution)
     DevBuf<float4> ins_world, ins;  // Match-internal insert: the scan at its final pose, the points that enter the map
+    PinnedBuf<unsigned char> h_tbl;  // the per-batch table (IvoxBatchTable), staged ...
+    DevBuf<unsigned char> d_tbl;     // ... and its device copy
+    // watchdog word of the last batch launch, read back with the states (pinned: a copy into pageable memory would make the enqueue
+    // wait for the kernel)
+    PinnedBuf<unsigned> h_abort;
     std::vector<size_t> pend_n;     // scans of the batch in flight (empty: none)
     bool pend_v9 = false;
 
@@ -540,49 +526,38 @@ class IvoxPlugin final : public Plugin {
         queries.reserve(nt + 1);
         // one LL row per CTA + one LL pose record per scan (+ the group rows of v9)
         const unsigned tag_base = h.next_ll_epoch((size_t)B * grid * 32 + (size_t)B * kLlPoseLen + (size_t)B * 16 * 32);
-        // ---- per-batch tables, staged in one pinned block and sent with one copy -------------------------------------------
-        const size_t o_pose = 0, o_off = o_pose + sizeof(PoseArg) * kMaxBatch, o_toff = o_off + sizeof(int) * (kMaxBatch + 4),
-                     o_desc = o_toff + sizeof(int) * (kMaxBatch + 4), o_ptr = o_desc + sizeof(P2PlaneScan) * kMaxBatch;
-        const size_t tbl_bytes = o_ptr + sizeof(void*) * kMaxBatch;
-        unsigned char* const tbl = h.batch_table(tbl_bytes);
-        PoseArg* hp = reinterpret_cast<PoseArg*>(tbl + o_pose);
-        int* ho = reinterpret_cast<int*>(tbl + o_off);
-        int* ht = reinterpret_cast<int*>(tbl + o_toff);
-        ht[0] = 0;
-        P2PlaneScan* hd = reinterpret_cast<P2PlaneScan*>(tbl + o_desc);
-        const float4** hq = reinterpret_cast<const float4**>(tbl + o_ptr);
+        // ---- the per-batch table -------------------------------------------------------------------------------------------
+        IvoxBatchTable& t = *reinterpret_cast<IvoxBatchTable*>(h_tbl.reserve(sizeof(IvoxBatchTable)));
+        const IvoxBatchTable* d_t = reinterpret_cast<const IvoxBatchTable*>(d_tbl.reserve(sizeof(IvoxBatchTable)));
+        // scan s's control block: its rows of grid x 32 LL records, then its LL pose record after every scan's rows
         uint4* pose_base = h.ll_rows.p + (size_t)B * grid * 32;
+        auto ctl = [&](int s) {
+            return h.loop_ctl(s, FLS_P2PLANE_IVOX, 50, tag_base, h.ll_rows.p + (size_t)s * grid * 32, pose_base + (size_t)s * kLlPoseLen);
+        };
+        t.tile_off[0] = 0;
         for (int s = 0; s < B; ++s) {
-            const double* Ts = T + 16 * s;
-            for (int r = 0; r < 3; ++r) {
-                for (int c = 0; c < 3; ++c) hp[s].R[r * 3 + c] = Ts[c * 4 + r];
-                hp[s].t[r] = Ts[12 + r];
-            }
-            ho[s] = off[s];
-            ht[s + 1] = ht[s] + order_tiles((int)n[s]);
-            hq[s] = d_scans[s];
-            P2PlaneScan& d = hd[s];
+            t.pose[s] = gn_pose(T + 16 * s);
+            t.off[s] = off[s];
+            t.tile_off[s + 1] = t.tile_off[s] + order_tiles((int)n[s]);
+            t.ptr[s] = d_scans[s];
+            const GnLoopCtl c = ctl(s);
+            P2PlaneScan& d = t.desc[s];
             d.src = queries.p + off[s];
             d.n = (int)n[s];
-            d.tag_base = tag_base;
-            d.state = h.state.p + s;
+            d.tag_base = c.tag_base;
+            d.state = c.state;
             d.rec0 = rec0.p + off[s];
             d.rec1 = rec1.p + off[s];
             d.flags = flags.p + off[s];
-            d.rows = h.ll_rows.p + (size_t)s * grid * 32;
-            d.ll_pose = pose_base + (size_t)s * kLlPoseLen;
-            d.log = h.scan_log(s);
-            d.result = h.scan_result(s);
+            d.rows = c.ll_rows;
+            d.ll_pose = c.ll_pose;
+            d.log = c.log;
+            d.result = c.result;
             d.grows = pose_base + (size_t)B * kLlPoseLen + (size_t)s * 16 * 32;
         }
-        ho[B] = off[B];
-        h.send_batch_table(tbl_bytes);
-        const unsigned char* d_batch = h.d_batch.p;
-        const PoseArg* d_poses = reinterpret_cast<const PoseArg*>(d_batch + o_pose);
-        const int* d_off = reinterpret_cast<const int*>(d_batch + o_off);
-        const int* d_toff = reinterpret_cast<const int*>(d_batch + o_toff);
-        const P2PlaneScan* d_desc = reinterpret_cast<const P2PlaneScan*>(d_batch + o_desc);
-        const float4* const* d_ptrs = reinterpret_cast<const float4* const*>(d_batch + o_ptr);
+        t.off[B] = off[B];
+        FLS_CUDA(cudaMemcpyAsync(d_tbl.p, &t, sizeof(t), cudaMemcpyHostToDevice, stream));
+        h.h2d_bytes += (long long)sizeof(t);
         // chunk tickets of v9's dynamic work distribution: one counter per (scan, iteration) + the watchdog's abort word, zeroed by
         // the prep kernel
         const int ticket_stride = h.cfg.max_iterations + 2;
@@ -591,14 +566,13 @@ class IvoxPlugin final : public Plugin {
         // ONE prep kernel for the whole batch (state init, flag and ticket reset): every tile of a scan ends up in Morton order of the
         // voxel its points fall into at the initial pose (locality only: the sums are order-free up to fp64 rounding, and the
         // persistent per-point records live in the same order for the whole Match)
-        prepare_queries(d_ptrs, d_off, d_toff, ht[B], B, d_poses, h.state.p, view(), flags.p, queries.p, use_v9 ? tickets.p : nullptr, n_tickets,
-                        stream, &h.launches);
+        prepare_queries(d_t, t.tile_off[B], B, h.state.p, view(), flags.p, queries.p, use_v9 ? tickets.p : nullptr, n_tickets, stream, &h.launches);
         P2PlaneLoopArgs a;
         a.map = view();
         a.plane_thres = h.cfg.point_to_planar_thres;
         a.gp = h.gn_params(FLS_P2PLANE_IVOX, 50);
         a.log_cap = h.log_cap;
-        a.scans = d_desc;
+        a.scans = d_t->desc;
         a.n_scans = B;
         a.tickets = nullptr;
         a.ticket_stride = 0;
@@ -613,22 +587,13 @@ class IvoxPlugin final : public Plugin {
                 launch_p2plane_v9(a, grid, stream);
             } else {  // the single scan: the same buffers as scan 0's descriptor above
                 const P2PlaneArgs one{a.map, a.plane_thres, queries.p, (int)n[0], rec0.p, rec1.p, flags.p};
-                GnLoopCtl ctl;
-                ctl.state = h.state.p;
-                ctl.ll_rows = h.ll_rows.p;
-                ctl.ll_pose = pose_base;
-                ctl.tag_base = tag_base;
-                ctl.gp = a.gp;
-                ctl.log = h.scan_log(0);
-                ctl.log_cap = h.log_cap;
-                ctl.result = h.scan_result(0);
-                launch_p2plane_loop(one, ctl, grid, stream);
+                launch_p2plane_loop(one, ctl(0), grid, stream);
             }
         });
         // ---- read back: every scan's state (+ its iteration log) ----------------------------------------------------------
         h.read_back(B);
-        *h.h_abort = 0;
-        if (use_v9) FLS_CUDA(cudaMemcpyAsync(h.h_abort, a.abort_word, sizeof(unsigned), cudaMemcpyDeviceToHost, stream));
+        *h_abort.p = 0;
+        if (use_v9) FLS_CUDA(cudaMemcpyAsync(h_abort.p, a.abort_word, sizeof(unsigned), cudaMemcpyDeviceToHost, stream));
         pend_n.assign(n, n + B);
         pend_v9 = use_v9;
         return FLS_OK;
@@ -639,7 +604,7 @@ class IvoxPlugin final : public Plugin {
         const int B = (int)pend_n.size();
         if (B < 1) return FLS_ERR_INVALID_ARG;
         h.end_call(st);
-        if (pend_v9 && *h.h_abort) {
+        if (pend_v9 && *h_abort.p) {
             pend_n.clear();
             set_last_error("p2plane_v9_kernel: watchdog — a wait loop gave up after 4 s (hand-over protocol error)");
             return FLS_ERR_CUDA;
@@ -662,6 +627,7 @@ class IvoxPlugin final : public Plugin {
         map.set_resolution(h.cfg.ivox_resolution);
         map.incremental = !h.cfg.localization_mode;  // mapping mode: the map grows by small inserts
         map.n_stencil = counts[h.cfg.ivox_nearby];
+        h_abort.reserve(1);
     }
 
     // external non-first insert in mapping mode: relies on Match-internal caches upstream
@@ -683,13 +649,16 @@ class IvoxPlugin final : public Plugin {
         const int rc = run(1, scans, ns, T, &conv, st);
         if (rc != FLS_OK) return rc;
         if (converged) *converged = conv;
-        const GnState& s = *h.h_state;
+        const GnState& s = h.h_state.p[0];
         if (s.converged && !h.cfg.localization_mode) {
-            // :205-206 — the scan enters the map through the cached-5-NN rule (body-frame points, final pose)  [quirk 8]
+            // :205-206 — the scan enters the map through the cached-5-NN rule (body-frame points, final pose T)  [quirk 8]
+            GnPose prev;
+            std::copy(s.Rprev, s.Rprev + 9, prev.R);
+            std::copy(s.tprev, s.tprev + 3, prev.t);
             ins.reserve(n + 1);
             ins_world.reserve(n + 1);
-            const size_t n_add = select_ivox_inserts(view(), d_src, (int)n, s.Rprev, s.tprev, s.R, s.t, 0.5 /* filter_size_map_min_ (:351) */,
-                                                     ins_world.p, ins.p, h.scratch, h.stream, &h.launches);
+            const size_t n_add = select_ivox_inserts(view(), d_src, (int)n, prev, gn_pose(T), 0.5 /* filter_size_map_min_ (:351) */, ins_world.p,
+                                                     ins.p, h.scratch, h.stream, &h.launches);
             return h.inserted(append(ins.p, n_add), st);
         }
         return FLS_OK;

@@ -253,13 +253,6 @@ void Handle::fitness_enqueue(const float4* d_src, size_t n, int P, float max_ran
     launches += 2;
 }
 
-static void pose_rows(const double* T, double* o) {  // column-major Mat4d -> row-major R | t
-    for (int r = 0; r < 3; ++r) {
-        for (int c = 0; c < 3; ++c) o[r * 3 + c] = T[c * 4 + r];
-        o[9 + r] = T[12 + r];
-    }
-}
-
 static float fitness_of(double sum, unsigned cnt) { return cnt > 0 ? (float)(sum / (double)cnt) : FLT_MAX; }
 
 int Handle::fitness(float max_range, float* score) {
@@ -269,10 +262,9 @@ int Handle::fitness(float max_range, float* score) {
     begin_call();
     const int rc = fit_grid_for(max_range, nullptr);
     if (rc != FLS_OK) return rc;
-    double pose[12];
-    pose_rows(T_final, pose);
+    const GnPose pose = gn_pose(T_final);
     fit_pose.reserve(12);
-    FLS_CUDA(cudaMemcpyAsync(fit_pose.p, pose, sizeof(pose), cudaMemcpyHostToDevice, stream));
+    FLS_CUDA(cudaMemcpyAsync(fit_pose.p, &pose, sizeof(pose), cudaMemcpyHostToDevice, stream));
     fitness_enqueue(last_src, last_src_n, 1, max_range);
     double sum = 0;
     unsigned cnt = 0;
@@ -317,13 +309,7 @@ static int reloc_refine(Handle& h, const float4* d_scan, size_t n, const fls_rel
     const void* scans[kMaxBatch];
     size_t ns[kMaxBatch];
     for (int r = 0; r < nr; ++r) {
-        double* Ts = Tr + 16 * r;
-        for (int i = 0; i < 3; ++i) {
-            for (int j = 0; j < 3; ++j) Ts[j * 4 + i] = pick[r].pose[i * 3 + j];
-            Ts[12 + i] = pick[r].pose[9 + i];
-        }
-        Ts[3] = Ts[7] = Ts[11] = 0.0;
-        Ts[15] = 1.0;
+        gn_pose_T(pick[r].pose, pick[r].pose + 9, Tr + 16 * r);
         scans[r] = d_scan;
         ns[r] = n;
     }
@@ -334,10 +320,10 @@ static int reloc_refine(Handle& h, const float4* d_scan, size_t n, const fls_rel
     h.launches = 0;
     if (rc != FLS_OK) return rc;
     // ---- fitness of every refined pose on the cloud fls_fitness reads after that Match, in one launch -------------------------------
-    double rows[kMaxBatch * 12];
-    for (int r = 0; r < nr; ++r) pose_rows(Tr + 16 * r, rows + 12 * r);
+    GnPose rows[kMaxBatch];
+    for (int r = 0; r < nr; ++r) rows[r] = gn_pose(Tr + 16 * r);
     h.fit_pose.reserve((size_t)nr * 12);
-    FLS_CUDA(cudaMemcpyAsync(h.fit_pose.p, rows, sizeof(double) * 12 * (size_t)nr, cudaMemcpyHostToDevice, h.stream));
+    FLS_CUDA(cudaMemcpyAsync(h.fit_pose.p, rows, sizeof(GnPose) * (size_t)nr, cudaMemcpyHostToDevice, h.stream));
     float fit[kMaxBatch];
     for (int r = 0; r < nr; ++r) fit[r] = FLT_MAX;
     if (h.last_src && h.last_src_n) {
@@ -757,10 +743,10 @@ int Handle::relocalize(const float4* d_scan, size_t n, const fls_reloc_cfg& c, c
     }
     int rc = fit_grid_for(c.max_range, &W);
     if (rc != FLS_OK) return rc;
-    double rows[kMaxBatch * 12];
-    for (int g = 0; g < G; ++g) pose_rows(guesses + 16 * g, rows + 12 * g);
+    GnPose rows[kMaxBatch];
+    for (int g = 0; g < G; ++g) rows[g] = gn_pose(guesses + 16 * g);
     s.guess.reserve((size_t)G * 12);
-    FLS_CUDA(cudaMemcpyAsync(s.guess.p, rows, sizeof(double) * 12 * (size_t)G, cudaMemcpyHostToDevice, stream));
+    FLS_CUDA(cudaMemcpyAsync(s.guess.p, rows, sizeof(GnPose) * (size_t)G, cudaMemcpyHostToDevice, stream));
     RelocGridArgs ga;
     ga.guess = s.guess.p;
     ga.xy_step = gr.I ? c.xy_step : 0.0;  // an unused step may be anything
@@ -817,7 +803,7 @@ int Handle::relocalize(const float4* d_scan, size_t n, const fls_reloc_cfg& c, c
         // the slack's float terms (derivation above): tau, the largest translation coordinate of any leaf of any guess
         double tau = 0.0;
         for (int g = 0; g < G; ++g) {
-            const double* t = rows + 12 * g + 9;
+            const double* t = rows[g].t;
             const double tg = std::fmax(std::fmax(std::fabs(t[0]), std::fabs(t[1])) + gr.I * ga.xy_step, std::fabs(t[2]));
             tau = g ? std::fmax(tau, tg) : tg;
         }
