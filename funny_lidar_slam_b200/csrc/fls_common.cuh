@@ -197,7 +197,7 @@ int with_workspace(int device, F&& body) {
 // ---- voxel keys / hash table ---------------------------------------------------------------------------
 // Hash slot = one 16-byte record so a probe is a single LDG.128:
 //   {u64 packed key (21 bits per axis, two's complement), u32 start, u32 count}
-// start/count address the voxel's points inside the voxel-contiguous point array.
+// start/count address the voxel's points inside the voxel-contiguous point array (NdtMap: voxel index and estimated flag).
 struct __align__(16) HashSlot {
     unsigned long long key;
     unsigned int start;
@@ -252,6 +252,20 @@ __device__ __forceinline__ bool table_find(const HashSlot* __restrict__ tab, uns
             return true;
         }
         if (k == kEmptyKey) return false;
+        h = (h + 1) & mask;
+    }
+}
+
+// Claims key's slot in a table being filled (VoxelTable, fls_maps.h): returns the slot and sets `created` when this thread inserted
+// the key.  Only the key is written; start and count are the caller's.
+__device__ __forceinline__ unsigned table_claim(HashSlot* tab, unsigned mask, unsigned long long key, bool& created) {
+    unsigned h = hash_key(key) & mask;
+    for (;;) {
+        const unsigned long long prev = atomicCAS(&tab[h].key, kEmptyKey, key);
+        if (prev == kEmptyKey || prev == key) {
+            created = prev == kEmptyKey;
+            return h;
+        }
         h = (h + 1) & mask;
     }
 }

@@ -244,7 +244,7 @@ class IcpPlugin final : public Plugin {
         const SearchGrid& g = window.grid;
         out->n_points = (long long)g.n_pts;
         out->n_voxels = (long long)g.n_vox;
-        out->table_slots = g.n_pts ? (long long)g.mask + 1 : 0;
+        out->table_slots = g.n_pts ? (long long)g.table.slots : 0;
         out->bytes = (long long)g.bytes();
     }
 };

@@ -262,7 +262,7 @@ static void launch_loam(const GnBatchItem<LoamArgs>* d_items, int n_scans, unsig
 static void window_info(const WindowMap& w, fls_map_info* out) {
     out->n_points += (long long)w.n;
     out->n_voxels += (long long)w.grid.n_vox;
-    out->table_slots += w.n ? (long long)w.grid.mask + 1 : 0;
+    out->table_slots += w.n ? (long long)w.grid.table.slots : 0;
     out->bytes += (long long)(w.grid.bytes() + w.cloud.bytes());
 }
 

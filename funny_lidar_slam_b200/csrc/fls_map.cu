@@ -7,10 +7,13 @@
 // The stable sort keeps insertion order inside a voxel, so the k-NN tie order matches a sequential insert.
 // LRU eviction (capacity_, ivox_map.cpp:133-136) is emulated exactly: every point carries its insertion stamp, the stamp of a
 // voxel's last point is its position in upstream's list, and the sequential insert of a call is simulated on the host against
-// the candidates (IvoxMap::evict_lru, lru_simulate).  window_add keeps the sliding-window local map of the ICP and kd-tree LOAM
-// plug-ins on top of a SearchGrid.
+// the candidates (IvoxMap::evict_lru).  window_add keeps the sliding-window local map of the ICP and kd-tree LOAM plug-ins on top
+// of a SearchGrid.
+// Shared with the NDT map (fls_ndt.cu): VoxelTable, the open-addressing table of every map, and LruEviction, the exact-LRU
+// eviction pass around lru_simulate.
 #include <cub/cub.cuh>
 
+#include <algorithm>
 #include <cstdlib>
 #include <functional>
 #include <queue>
@@ -50,6 +53,34 @@ size_t lru_candidate_bound(size_t n_vox, int n_new, int n_touched, long long cap
     const long long e0 = (long long)n_vox + n_new - (capacity - 1);
     const size_t K = (size_t)(e0 > 0 ? e0 : 0) + 2 * (size_t)n_touched + 64;
     return K < n_cand ? K : n_cand;
+}
+
+int LruEviction::run(int n_cand, const unsigned* d_create, int n_create, int n_touched, size_t size0, long long capacity,
+                     DevBuf<unsigned char>& cub_tmp, cudaStream_t st, int* launches,
+                     const std::function<void(const unsigned*, int, unsigned*)>& write_first) {
+    stamps_sorted.reserve((size_t)n_cand + 1);
+    ids_sorted.reserve((size_t)n_cand + 1);
+    cub_pass(cub_tmp, [&](void* tmp, size_t& bytes) {
+        return cub::DeviceRadixSort::SortPairs(tmp, bytes, stamps.p, stamps_sorted.p, ids.p, ids_sorted.p, n_cand, 0, 64, st);
+    });
+    const size_t K = lru_candidate_bound(size0, n_create, n_touched, capacity, (size_t)n_cand);
+    first_touch.reserve(K + 1);
+    write_first(ids_sorted.p, (int)K, first_touch.p);
+    *launches += 3;  // the sort counts two
+    h_first.resize(K);
+    h_create.resize((size_t)n_create);
+    FLS_CUDA(cudaMemcpyAsync(h_first.data(), first_touch.p, sizeof(unsigned) * K, cudaMemcpyDeviceToHost, st));
+    if (n_create) FLS_CUDA(cudaMemcpyAsync(h_create.data(), d_create, sizeof(unsigned) * (size_t)n_create, cudaMemcpyDeviceToHost, st));
+    FLS_CUDA(cudaStreamSynchronize(st));
+    if (!lru_simulate(size0, (size_t)capacity, h_first, h_create, h_victims, h_recreated)) return FLS_ERR_CAPACITY;
+    n_victims = h_victims.size();
+    n_recreated = (size_t)std::count(h_recreated.begin(), h_recreated.end(), 1);
+    if (n_victims == 0) return FLS_OK;
+    victims.reserve(n_victims + 1);
+    recreated.reserve(n_victims + 1);
+    FLS_CUDA(cudaMemcpyAsync(victims.p, h_victims.data(), sizeof(unsigned) * n_victims, cudaMemcpyHostToDevice, st));
+    FLS_CUDA(cudaMemcpyAsync(recreated.p, h_recreated.data(), n_victims, cudaMemcpyHostToDevice, st));
+    return FLS_OK;
 }
 
 BuildScratch::BuildScratch() {
@@ -157,16 +188,10 @@ __global__ void table_clear_kernel(HashSlot* tab, size_t slots) {
 }
 
 __device__ __forceinline__ void table_insert(HashSlot* tab, unsigned mask, unsigned long long key, unsigned start, unsigned count) {
-    unsigned h = hash_key(key) & mask;
-    for (;;) {
-        const unsigned long long prev = atomicCAS(&tab[h].key, kEmptyKey, key);
-        if (prev == kEmptyKey || prev == key) {
-            tab[h].start = start;
-            tab[h].count = count;
-            return;
-        }
-        h = (h + 1) & mask;
-    }
+    bool created;
+    HashSlot& slot = tab[table_claim(tab, mask, key, created)];
+    slot.start = start;
+    slot.count = count;
 }
 
 // one thread per occupied voxel (run of equal Morton codes)
@@ -408,15 +433,26 @@ static int sorted_runs(const float4* pts, size_t n, float inv_res, float4* dst, 
     return runs;
 }
 
-// the table of `slots` (a power of two) slots over the runs of sorted_runs; returns its mask
-static unsigned fill_table(DevBuf<HashSlot>& table, size_t slots, int runs, const BuildScratch& sc, cudaStream_t st, int* launches) {
-    const unsigned mask = (unsigned)(slots - 1);
-    table.reserve(slots);
-    table_clear_kernel<<<grid_for(slots, 256), 256, 0, st>>>(table.p, slots);
-    ivox_insert_kernel<<<grid_for(runs, 256), 256, 0, st>>>(sc.uniq.p, sc.starts.p, sc.counts.p, runs, table.p, mask);
+void VoxelTable::size_for(size_t n, size_t factor, bool grow_only) {
+    size_t want = 1024;
+    while (want < factor * n) want <<= 1;
+    if (!grow_only || want > slots) slots = want;
+    buf.reserve(slots);
+    mask = (unsigned)(slots - 1);
+}
+
+void VoxelTable::clear(cudaStream_t st, int* launches) {
+    table_clear_kernel<<<grid_for(slots, 256), 256, 0, st>>>(buf.p, slots);
     FLS_CUDA(cudaGetLastError());
-    *launches += 2;
-    return mask;
+    ++*launches;
+}
+
+// the table (sized) over the runs of sorted_runs
+static void fill_table(VoxelTable& table, int runs, const BuildScratch& sc, cudaStream_t st, int* launches) {
+    table.clear(st, launches);
+    ivox_insert_kernel<<<grid_for(runs, 256), 256, 0, st>>>(sc.uniq.p, sc.starts.p, sc.counts.p, runs, table.buf.p, table.mask);
+    FLS_CUDA(cudaGetLastError());
+    *launches += 1;
 }
 
 int SearchGrid::build(const float4* d_cloud, size_t n, BuildScratch& sc, cudaStream_t st, int* launches) {
@@ -425,9 +461,8 @@ int SearchGrid::build(const float4* d_cloud, size_t n, BuildScratch& sc, cudaStr
     if (n > 0xfffffff0ull) return FLS_ERR_INVALID_ARG;
     pts_sorted.reserve(n);
     const int runs = sorted_runs<true>(d_cloud, n, 1.0f / res, pts_sorted.p, sc, st, launches);
-    size_t slots = 1024;
-    while (slots < 2 * (size_t)runs) slots <<= 1;
-    mask = fill_table(table, slots, runs, sc, st, launches);
+    table.size_for((size_t)runs, 2);
+    fill_table(table, runs, sc, st, launches);
     n_pts = n;
     n_vox = (size_t)runs;
     return FLS_OK;
@@ -456,10 +491,10 @@ int IvoxMap::append_incremental(const float4* d_new, size_t n_new, long long cap
     inc_old_count.reserve((size_t)T + 1);
     inc_new_count.reserve((size_t)T + 1);
     inc_new_off.reserve((size_t)T + 1);
-    lru_cnt.reserve(8);
-    FLS_CUDA(cudaMemsetAsync(lru_cnt.p, 0, 8 * sizeof(int), st));
-    inc_plan_kernel<<<grid_for((size_t)T, 256), 256, 0, st>>>(sc.uniq.p, sc.counts.p, T, table.p, mask, inc_old_start.p, inc_old_count.p, inc_new_count.p,
-                                                            lru_cnt.p);
+    inc_cnt.reserve(8);
+    FLS_CUDA(cudaMemsetAsync(inc_cnt.p, 0, 8 * sizeof(int), st));
+    inc_plan_kernel<<<grid_for((size_t)T, 256), 256, 0, st>>>(sc.uniq.p, sc.counts.p, T, table.buf.p, table.mask, inc_old_start.p, inc_old_count.p,
+                                                            inc_new_count.p, inc_cnt.p);
     // sized by sort_pairs: the same scan over n_new >= T items
     cub_run(sc.cub_tmp, [&](void* tmp, size_t& bytes) { return cub::DeviceScan::ExclusiveSum(tmp, bytes, inc_new_count.p, inc_new_off.p, T, st); });
     // affected centres: every centre whose stencil contains a touched voxel
@@ -478,7 +513,7 @@ int IvoxMap::append_incremental(const float4* d_new, size_t n_new, long long cap
     int hc[8];
     unsigned last_off = 0, last_cnt = 0;
     int n_aff = 0;
-    FLS_CUDA(cudaMemcpyAsync(hc, lru_cnt.p, 8 * sizeof(int), cudaMemcpyDeviceToHost, st));
+    FLS_CUDA(cudaMemcpyAsync(hc, inc_cnt.p, 8 * sizeof(int), cudaMemcpyDeviceToHost, st));
     FLS_CUDA(cudaMemcpyAsync(&last_off, inc_new_off.p + (T - 1), sizeof(unsigned), cudaMemcpyDeviceToHost, st));
     FLS_CUDA(cudaMemcpyAsync(&last_cnt, inc_new_count.p + (T - 1), sizeof(unsigned), cudaMemcpyDeviceToHost, st));
     FLS_CUDA(cudaMemcpyAsync(&n_aff, sc.num_runs.p + 1, sizeof(int), cudaMemcpyDeviceToHost, st));
@@ -489,19 +524,19 @@ int IvoxMap::append_incremental(const float4* d_new, size_t n_new, long long cap
     // has to take the full path: eviction, no room, table load
     if (capacity > 0 && (long long)n_vox + n_created >= capacity) return 1;
     if (pts_end + moved > pts_sorted.cap) return 1;
-    if (2 * (n_vox + (size_t)n_created) > (size_t)mask + 1) return 1;
+    if (2 * (n_vox + (size_t)n_created) > table.slots) return 1;
     // voxels first (the centre runs are gathered from their new locations)
     inc_move_kernel<<<grid_for((size_t)T * 32, 256), 256, 0, st>>>(sc.uniq.p, T, inc_old_start.p, inc_old_count.p, sc.starts.p, sc.counts.p, inc_new_off.p,
-                                                                 (unsigned)pts_end, sc.idx_sorted.p, d_new, pts_sorted.p, table.p, mask);
+                                                                 (unsigned)pts_end, sc.idx_sorted.p, d_new, pts_sorted.p, table.buf.p, table.mask);
     // centre runs
     ccount.reserve((size_t)n_aff + 1);
     cstart.reserve((size_t)n_aff + 1);
-    list_count_kernel<<<grid_for((size_t)n_aff, 128), 128, 0, st>>>(cuniq.p, n_aff, n_stencil, table.p, mask, ccount.p);
-    FLS_CUDA(cudaMemsetAsync(lru_cnt.p, 0, 8 * sizeof(int), st));
-    inc_new_centres_kernel<<<grid_for((size_t)n_aff, 256), 256, 0, st>>>(cuniq.p, n_aff, ctab.p, cmask, ccount.p, lru_cnt.p);
+    list_count_kernel<<<grid_for((size_t)n_aff, 128), 128, 0, st>>>(cuniq.p, n_aff, n_stencil, table.buf.p, table.mask, ccount.p);
+    FLS_CUDA(cudaMemsetAsync(inc_cnt.p, 0, 8 * sizeof(int), st));
+    inc_new_centres_kernel<<<grid_for((size_t)n_aff, 256), 256, 0, st>>>(cuniq.p, n_aff, ctab.buf.p, ctab.mask, ccount.p, inc_cnt.p);
     cub_pass(sc.cub_tmp, [&](void* tmp, size_t& bytes) { return cub::DeviceScan::ExclusiveSum(tmp, bytes, ccount.p, cstart.p, n_aff, st); });
     unsigned l_off = 0, l_cnt = 0;
-    FLS_CUDA(cudaMemcpyAsync(hc, lru_cnt.p, 8 * sizeof(int), cudaMemcpyDeviceToHost, st));
+    FLS_CUDA(cudaMemcpyAsync(hc, inc_cnt.p, 8 * sizeof(int), cudaMemcpyDeviceToHost, st));
     FLS_CUDA(cudaMemcpyAsync(&l_off, cstart.p + (n_aff - 1), sizeof(unsigned), cudaMemcpyDeviceToHost, st));
     FLS_CUDA(cudaMemcpyAsync(&l_cnt, ccount.p + (n_aff - 1), sizeof(unsigned), cudaMemcpyDeviceToHost, st));
     FLS_CUDA(cudaStreamSynchronize(st));
@@ -513,10 +548,10 @@ int IvoxMap::append_incremental(const float4* d_new, size_t n_new, long long cap
     // From here on the point array and the occupied table are already updated; if the lists do not fit, the caller's full build
     // regenerates everything from pts_all (which it extends itself), so nothing is lost.
     if (lists_end + run_total > lists.cap || lists_end + run_total > 0xfffffff0ull) return 1;
-    if (4 * (n_centers + (size_t)n_new_centres) > (size_t)cmask + 1) return 1;
+    if (4 * (n_centers + (size_t)n_new_centres) > ctab.slots) return 1;
     add_base_kernel<<<grid_for((size_t)n_aff, 256), 256, 0, st>>>(cstart.p, n_aff, (unsigned)lists_end);
-    list_fill_kernel<<<grid_for((size_t)n_aff * 32, 256), 256, 0, st>>>(cuniq.p, n_aff, n_stencil, table.p, mask, pts_sorted.p, cstart.p, ccount.p, lists.p,
-                                                                       ctab.p, cmask);
+    list_fill_kernel<<<grid_for((size_t)n_aff * 32, 256), 256, 0, st>>>(cuniq.p, n_aff, n_stencil, table.buf.p, table.mask, pts_sorted.p, cstart.p, ccount.p,
+                                                                       lists.p, ctab.buf.p, ctab.mask);
     FLS_CUDA(cudaGetLastError());
     *launches += 2;
     // bookkeeping
@@ -599,10 +634,8 @@ int IvoxMap::build_full(size_t n_old, size_t n_in, long long capacity, cudaStrea
         n = n_after;
         runs = sorted_runs<false>(pts_all.p, n, inv_res, pts_sorted.p, scratch, st, launches);  // n only shrank: pts_sorted has room
     }
-    size_t slots = 1024;
-    while (slots < (incremental ? 4 : 2) * (size_t)runs) slots <<= 1;  // mapping mode: room for the voxels to come
-    if (incremental && slots <= (size_t)mask + 1 && table.cap >= (size_t)mask + 1 && (size_t)mask + 1 >= 2 * (size_t)runs) slots = (size_t)mask + 1;  // keep the table while it is big enough
-    mask = fill_table(table, slots, runs, scratch, st, launches);
+    table.size_for((size_t)runs, incremental ? 4 : 2, incremental);  // mapping mode: room for the voxels to come
+    fill_table(table, runs, scratch, st, launches);
     n_pts = n;
     n_vox = (size_t)runs;
     pts_end = n;
@@ -617,45 +650,31 @@ int IvoxMap::build_full(size_t n_old, size_t n_in, long long capacity, cudaStrea
 int IvoxMap::evict_lru(size_t n_old, size_t n, int runs, long long capacity, cudaStream_t st, size_t* n_after, int* launches) {
     BuildScratch& sc = scratch;
     if (n_vox == 0) return FLS_ERR_CAPACITY;  // the first cloud alone overflows the capacity
-    lru_old.reserve((size_t)runs + 1);
     lru_first.reserve((size_t)runs + 1);
     lru_nold.reserve((size_t)runs + 1);
-    lru_keys.reserve((size_t)runs + 1);
-    lru_keys_sorted.reserve((size_t)runs + 1);
-    lru_vals.reserve((size_t)runs + 1);
-    lru_vals_sorted.reserve((size_t)runs + 1);
     lru_cnt.reserve(4);
     FLS_CUDA(cudaMemsetAsync(lru_cnt.p, 0, 4 * sizeof(int), st));
     ivox_run_info_kernel<<<grid_for(runs, 256), 256, 0, st>>>(runs, sc.starts.p, sc.counts.p, sc.idx_sorted.p, stamp_all.p, (unsigned)n_old, lru_nold.p,
-                                                            lru_first.p, lru_keys.p, lru_vals.p, sc.k32b.reserve(n + 1), lru_cnt.p);
+                                                            lru_first.p, eviction.stamps.reserve((size_t)runs + 1),
+                                                            eviction.ids.reserve((size_t)runs + 1), sc.k32b.reserve(n + 1), lru_cnt.p);
+    ++*launches;
     int hc[4] = {0, 0, 0, 0};
     FLS_CUDA(cudaMemcpyAsync(hc, lru_cnt.p, 4 * sizeof(int), cudaMemcpyDeviceToHost, st));
     FLS_CUDA(cudaStreamSynchronize(st));
     const int n_cand = hc[0], n_create = hc[1], n_touched = hc[2];
     if (n_cand == 0) return FLS_ERR_CAPACITY;
-    cub_pass(sc.cub_tmp, [&](void* tmp, size_t& bytes) {
-        return cub::DeviceRadixSort::SortPairs(tmp, bytes, lru_keys.p, lru_keys_sorted.p, lru_vals.p, lru_vals_sorted.p, n_cand, 0, 64, st);
-    });
-    const size_t K = lru_candidate_bound(n_vox, n_create, n_touched, capacity, (size_t)n_cand);
-    sc.k32a.reserve(K + 1);
-    ivox_cand_kernel<<<grid_for(K, 256), 256, 0, st>>>(lru_vals_sorted.p, (int)K, lru_first.p, sc.k32a.p);
-    std::vector<unsigned> cand(K), creat((size_t)n_create);
-    FLS_CUDA(cudaMemcpyAsync(cand.data(), sc.k32a.p, sizeof(unsigned) * K, cudaMemcpyDeviceToHost, st));
-    if (n_create) FLS_CUDA(cudaMemcpyAsync(creat.data(), sc.k32b.p, sizeof(unsigned) * (size_t)n_create, cudaMemcpyDeviceToHost, st));
-    FLS_CUDA(cudaStreamSynchronize(st));
-    std::vector<unsigned> victims;
-    std::vector<unsigned char> recreated;
-    if (!lru_simulate(n_vox, (size_t)capacity, cand, creat, victims, recreated)) return FLS_ERR_CAPACITY;
-    *launches += 4;
+    const int rc = eviction.run(n_cand, sc.k32b.p, n_create, n_touched, n_vox, capacity, sc.cub_tmp, st, launches,
+                                [&](const unsigned* runs_sorted, int K, unsigned* out) {
+                                    ivox_cand_kernel<<<grid_for(K, 256), 256, 0, st>>>(runs_sorted, K, lru_first.p, out);
+                                });
+    if (rc != FLS_OK) return rc;
     *n_after = n;
-    if (victims.empty()) return FLS_OK;
+    if (eviction.n_victims == 0) return FLS_OK;
     // flags: 1 = keep; the victims' points from before this call go
     lru_flags.reserve(n + 1);
     FLS_CUDA(cudaMemsetAsync(lru_flags.p, 1, n, st));
-    sc.k32a.reserve(victims.size() + 1);
-    FLS_CUDA(cudaMemcpyAsync(sc.k32a.p, victims.data(), sizeof(unsigned) * victims.size(), cudaMemcpyHostToDevice, st));
-    ivox_kill_kernel<<<grid_for(victims.size() * 32, 256), 256, 0, st>>>(sc.k32a.p, (int)victims.size(), lru_vals_sorted.p, sc.starts.p, lru_nold.p,
-                                                                        sc.idx_sorted.p, lru_flags.p);
+    ivox_kill_kernel<<<grid_for(eviction.n_victims * 32, 256), 256, 0, st>>>(eviction.victims.p, (int)eviction.n_victims, eviction.ids_sorted.p, sc.starts.p,
+                                                                            lru_nold.p, sc.idx_sorted.p, lru_flags.p);
     // stable compaction of the points and their stamps (pts_sorted / keys are rebuilt by the second sort anyway: use them as targets)
     sc.keys.reserve(n + 1);
     auto keep_pts = [&](void* tmp, size_t& bytes) {
@@ -668,7 +687,7 @@ int IvoxMap::evict_lru(size_t n_old, size_t n, int runs, long long capacity, cud
     cub_run(sc.cub_tmp, keep_pts);
     cub_run(sc.cub_tmp, keep_stamps);
     FLS_CUDA(cudaMemcpyAsync(sc.h_num_runs, sc.num_runs.p, sizeof(int), cudaMemcpyDeviceToHost, st));
-    FLS_CUDA(cudaStreamSynchronize(st));  // also: the host vectors above are read by the copies
+    FLS_CUDA(cudaStreamSynchronize(st));
     const size_t kept = (size_t)*sc.h_num_runs;
     FLS_CUDA(cudaMemcpyAsync(pts_all.p, pts_sorted.p, kept * sizeof(float4), cudaMemcpyDeviceToDevice, st));
     FLS_CUDA(cudaMemcpyAsync(stamp_all.p, sc.keys.p, kept * sizeof(unsigned long long), cudaMemcpyDeviceToDevice, st));
@@ -680,11 +699,10 @@ int IvoxMap::evict_lru(size_t n_old, size_t n, int runs, long long capacity, cud
 size_t IvoxMap::dump_keys(unsigned long long* h_out, size_t cap, cudaStream_t st) {
     // packed keys of the occupied voxels, from the table (tests)
     if (n_vox == 0) return 0;
-    const size_t slots = (size_t)mask + 1;
     scratch.keys.reserve(n_vox + 1);
     scratch.num_runs.reserve(2);
     FLS_CUDA(cudaMemsetAsync(scratch.num_runs.p, 0, sizeof(int), st));
-    table_dump_kernel<<<grid_for(slots, 256), 256, 0, st>>>(table.p, slots, scratch.keys.p, scratch.num_runs.p);
+    table_dump_kernel<<<grid_for(table.slots, 256), 256, 0, st>>>(table.buf.p, table.slots, scratch.keys.p, scratch.num_runs.p);
     int n = 0;
     FLS_CUDA(cudaMemcpyAsync(&n, scratch.num_runs.p, sizeof(int), cudaMemcpyDeviceToHost, st));
     FLS_CUDA(cudaStreamSynchronize(st));
@@ -715,29 +733,25 @@ int IvoxMap::build_stencil_lists(cudaStream_t st, int* launches) {
     const int nc = *sc.h_num_runs;
     ccount.reserve((size_t)nc);
     cstart.reserve((size_t)nc);
-    list_count_kernel<<<grid_for((size_t)nc, 128), 128, 0, st>>>(cuniq.p, nc, n_stencil, table.p, mask, ccount.p);
+    list_count_kernel<<<grid_for((size_t)nc, 128), 128, 0, st>>>(cuniq.p, nc, n_stencil, table.buf.p, table.mask, ccount.p);
     cub_pass(sc.cub_tmp, [&](void* tmp, size_t& bytes) { return cub::DeviceScan::ExclusiveSum(tmp, bytes, ccount.p, cstart.p, nc, st); });
     // load factor <= 0.25: the centre table is probed once per point-iteration and a long linear-probing chain stalls
     // a whole warp, so it is kept sparser than the occupied table
-    size_t slots = 1024;
-    while (slots < (incremental ? 8 : 4) * (size_t)nc) slots <<= 1;
-    if (incremental && slots <= (size_t)cmask + 1 && ctab.cap >= (size_t)cmask + 1 && (size_t)cmask + 1 >= 4 * (size_t)nc) slots = (size_t)cmask + 1;
-    ctab.reserve(slots);
-    cmask = (unsigned)(slots - 1);
+    ctab.size_for((size_t)nc, incremental ? 8 : 4, incremental);
     if (incremental) {  // mapping mode: room for the runs the incremental inserts append, geometric growth
         if (2 * total + 1048576 > lists.cap) lists.reserve(4 * total + 1048576);
     } else {
         lists.reserve(total);
     }
-    table_clear_kernel<<<grid_for(slots, 256), 256, 0, st>>>(ctab.p, slots);
-    list_fill_kernel<<<grid_for((size_t)nc * 32, 256), 256, 0, st>>>(cuniq.p, nc, n_stencil, table.p, mask, pts_sorted.p, cstart.p, ccount.p, lists.p,
-                                                                     ctab.p, cmask);
+    ctab.clear(st, launches);
+    list_fill_kernel<<<grid_for((size_t)nc * 32, 256), 256, 0, st>>>(cuniq.p, nc, n_stencil, table.buf.p, table.mask, pts_sorted.p, cstart.p, ccount.p,
+                                                                     lists.p, ctab.buf.p, ctab.mask);
     FLS_CUDA(cudaGetLastError());
     n_centers = (size_t)nc;
     n_list = total;
     lists_end = total;
     lists_garbage = 0;
-    *launches += 7;
+    *launches += 6;
     // the transient key arrays are the largest buffers of the build; give them back
     if (!incremental) {
         ckeys.release();

@@ -7,8 +7,8 @@
 //   * cold   : sigma, counters and a carry buffer of <= min_points_in_voxel pending points per voxel, touched only
 //              by AddCloudToLocalMap / UpdateVoxel (:130-227)
 // LRU eviction at `capacity` (:203-206) is emulated exactly: stamps per voxel + a host simulation of the sequential insert
-// (NdtMap::evict_lru, lru_simulate in fls_map.cu).  NdtPlugin at the end is the plug-in's host half: its map, AddCloudToLocalMap and
-// the single and batch Match.
+// (NdtMap::evict_lru).  The table and the eviction pass are the ones the iVox map uses: VoxelTable and LruEviction in fls_map.cu.
+// NdtPlugin at the end is the plug-in's host half: its map, AddCloudToLocalMap and the single and batch Match.
 #include <cub/cub.cuh>
 
 #include <cstring>
@@ -43,16 +43,6 @@ __global__ void ndt_keys_kernel(const float4* __restrict__ pts, size_t n, double
     idx[i] = (unsigned)i;
 }
 
-__global__ void ndt_table_clear_kernel(HashSlot* tab, size_t slots, int* counter) {
-    const size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
-    if (i < slots) {
-        tab[i].key = kEmptyKey;
-        tab[i].start = 0xffffffffu;
-        tab[i].count = 0;
-    }
-    if (i == 0) *counter = 0;
-}
-
 __device__ __forceinline__ void inv3_sym_reg(const double* S, double* Ai) {
     // cofactor inverse of a general 3x3 (Eigen's fixed-size inverse, incremental_ndt.h:134,151 upstream)
     const double c00 = S[4] * S[8] - S[5] * S[7], c01 = S[5] * S[6] - S[3] * S[8], c02 = S[3] * S[7] - S[4] * S[6];
@@ -75,7 +65,7 @@ struct NdtUpdateArgs {
     NdtHot* hot;
     NdtCold* cold;
     double* carry;
-    int* counter;  // [0] high-water mark of voxel indices, [1] overflow flag, [2] free-list cursor
+    int* counter;  // NdtMap::counter
     const int* free_list;
     int n_free;
     unsigned long long call_hi;  // call number << 32
@@ -130,29 +120,20 @@ __global__ void ndt_update_kernel(NdtUpdateArgs a, int* overflow) {
     if (r >= a.runs) return;
     const unsigned long long key = a.run_keys[r];
     const unsigned s = a.starts[r], c = a.counts[r];
-    // find or insert
-    unsigned h = hash_key(key) & a.mask;
+    bool created;
+    const unsigned h = table_claim(a.tab, a.mask, key, created);
     unsigned vi;
-    bool created = false;
-    for (;;) {
-        const unsigned long long prev = atomicCAS(&a.tab[h].key, kEmptyKey, key);
-        if (prev == kEmptyKey) {
-            // indices of evicted voxels first (the LRU tail was evicted before this kernel: NdtMap::evict_lru), then fresh ones
-            int id;
-            const int k = atomicAdd(a.counter + 2, 1);
-            if (k < a.n_free) id = a.free_list[a.n_free - 1 - k];  // the list is a stack
-            else id = atomicAdd(a.counter, 1);
-            if ((long long)id >= a.capacity) atomicExch(overflow, 1);  // cannot happen once the eviction ran
-            vi = (unsigned)id;
-            a.tab[h].start = vi;
-            created = true;
-            break;
-        }
-        if (prev == key) {
-            vi = a.tab[h].start;
-            break;
-        }
-        h = (h + 1) & a.mask;
+    if (created) {
+        // indices of evicted voxels first (the LRU tail was evicted before this kernel: NdtMap::evict_lru), then fresh ones
+        int id;
+        const int k = atomicAdd(a.counter + NdtMap::kFreeCursor, 1);
+        if (k < a.n_free) id = a.free_list[a.n_free - 1 - k];  // the list is a stack
+        else id = atomicAdd(a.counter + NdtMap::kHiWater, 1);
+        if ((long long)id >= a.capacity) atomicExch(overflow, 1);  // cannot happen once the eviction ran
+        vi = (unsigned)id;
+        a.tab[h].start = vi;
+    } else {
+        vi = a.tab[h].start;
     }
     if ((long long)vi >= a.capacity) return;
     NdtCold& cd = a.cold[vi];
@@ -232,7 +213,7 @@ __global__ void ndt_update_kernel(NdtUpdateArgs a, int* overflow) {
 }
 
 // ---- LRU bookkeeping (incremental_ndt.h:193-214) -------------------------------------------------------------------------------
-// which touched voxels exist already; counters[3] = to be created, counters[4] = existing and touched
+// which touched voxels exist already: how many are to be created, how many existing ones are touched
 __global__ void ndt_lookup_kernel(int runs, const unsigned long long* __restrict__ run_keys, const HashSlot* __restrict__ tab, unsigned mask,
                                   int* __restrict__ run_vi, int* __restrict__ touch_run, int* counters) {
     const int r = blockIdx.x * blockDim.x + threadIdx.x;
@@ -241,17 +222,17 @@ __global__ void ndt_lookup_kernel(int runs, const unsigned long long* __restrict
     if (table_find(tab, mask, run_keys[r], vi, est)) {
         run_vi[r] = (int)vi;
         touch_run[vi] = r;
-        atomicAdd(counters + 4, 1);
+        atomicAdd(counters + NdtMap::kTouched, 1);
     } else {
         run_vi[r] = -1;
-        atomicAdd(counters + 3, 1);
+        atomicAdd(counters + NdtMap::kCreations, 1);
     }
 }
 __global__ void ndt_live_kernel(const NdtCold* __restrict__ cold, int hi_water, unsigned long long* __restrict__ stamps, unsigned* __restrict__ vis,
-                                int* counters) {
+                                int* cursor) {
     const int vi = blockIdx.x * blockDim.x + threadIdx.x;
     if (vi >= hi_water || !cold[vi].alive) return;
-    const int pos = atomicAdd(counters + 5, 1);
+    const int pos = atomicAdd(cursor, 1);
     stamps[pos] = cold[vi].stamp;
     vis[pos] = (unsigned)vi;
 }
@@ -282,25 +263,10 @@ __global__ void ndt_evict_kernel(const unsigned* __restrict__ victim_pos, const 
 __global__ void ndt_table_rebuild_kernel(const NdtCold* __restrict__ cold, int hi_water, HashSlot* tab, unsigned mask) {
     const int vi = blockIdx.x * blockDim.x + threadIdx.x;
     if (vi >= hi_water || !cold[vi].alive) return;
-    const unsigned long long key = cold[vi].key;
-    unsigned h = hash_key(key) & mask;
-    for (;;) {
-        const unsigned long long prev = atomicCAS(&tab[h].key, kEmptyKey, key);
-        if (prev == kEmptyKey) {
-            tab[h].start = (unsigned)vi;
-            tab[h].count = cold[vi].estimated ? 1u : 0u;
-            return;
-        }
-        h = (h + 1) & mask;
-    }
-}
-__global__ void ndt_table_clear_only_kernel(HashSlot* tab, size_t slots) {
-    const size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
-    if (i < slots) {
-        tab[i].key = kEmptyKey;
-        tab[i].start = 0xffffffffu;
-        tab[i].count = 0;
-    }
+    bool created;  // the live keys are distinct
+    HashSlot& slot = tab[table_claim(tab, mask, cold[vi].key, created)];
+    slot.start = (unsigned)vi;
+    slot.count = cold[vi].estimated ? 1u : 0u;
 }
 __global__ void ndt_dump_keys_kernel(const NdtCold* __restrict__ cold, int hi_water, unsigned long long* __restrict__ out, int* cursor) {
     const int vi = blockIdx.x * blockDim.x + threadIdx.x;
@@ -452,18 +418,14 @@ int NdtMap::add_cloud(const float4* d_cloud, size_t n, float leaf, bool first_sc
     filtered.reserve(n);
     const size_t nf = voxel_grid_device(d_cloud, n, leaf, filtered.p, scratch, st, launches);  // :186
     if (nf == 0) return FLS_OK;
-    if (slots == 0) {  // first use: size everything by the configured capacity
-        size_t want = 1024;
-        while (want < 2 * (size_t)capacity) want <<= 1;
-        slots = want;
-        mask = (unsigned)(slots - 1);
-        table.reserve(slots);
+    if (table.slots == 0) {  // first use: size everything by the configured capacity
+        table.size_for((size_t)capacity, 2);
         hot.reserve((size_t)capacity);
         cold.reserve((size_t)capacity);
         carry.reserve((size_t)capacity * (size_t)(min_pts > 0 ? min_pts : 1) * 3);
-        counter.reserve(8);
-        ndt_table_clear_kernel<<<grid_for(slots, 256), 256, 0, st>>>(table.p, slots, counter.p);
-        ++*launches;
+        counter.reserve(kCounters);
+        FLS_CUDA(cudaMemsetAsync(counter.p, 0, kCounters * sizeof(int), st));
+        table.clear(st, launches);
     }
     BuildScratch& sc = scratch;
     sc.reserve_runs<unsigned long long>(nf);
@@ -476,19 +438,18 @@ int NdtMap::add_cloud(const float4* d_cloud, size_t n, float leaf, bool first_sc
     run_vi.reserve((size_t)runs + 1);
     touch_run.reserve((size_t)capacity + 1);
     free_list.reserve((size_t)capacity + 1);
-    FLS_CUDA(cudaMemsetAsync(counter.p + 1, 0, 7 * sizeof(int), st));
+    FLS_CUDA(cudaMemsetAsync(counter.p + kOverflow, 0, (kCounters - kOverflow) * sizeof(int), st));
     if (hi_water0 > 0) FLS_CUDA(cudaMemsetAsync(touch_run.p, 0xff, sizeof(int) * (size_t)hi_water0, st));
-    ndt_lookup_kernel<<<grid_for(runs, 256), 256, 0, st>>>(runs, sc.uniq.p, table.p, mask, run_vi.p, touch_run.p, counter.p);
-    int hc[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-    FLS_CUDA(cudaMemcpyAsync(hc, counter.p, 8 * sizeof(int), cudaMemcpyDeviceToHost, st));
+    ndt_lookup_kernel<<<grid_for(runs, 256), 256, 0, st>>>(runs, sc.uniq.p, table.buf.p, table.mask, run_vi.p, touch_run.p, counter.p);
+    int hc[kCounters] = {};
+    FLS_CUDA(cudaMemcpyAsync(hc, counter.p, sizeof(hc), cudaMemcpyDeviceToHost, st));
     FLS_CUDA(cudaStreamSynchronize(st));
     *launches += 1;
-    const int n_new = hc[3], n_touched = hc[4];
+    const int n_new = hc[kCreations], n_touched = hc[kTouched];
     ++call_no;
-    int n_victims = 0, n_recreated = 0;
     // upstream: after every creation `if (data_.size() >= capacity_) pop_back()` (:203-206) — the list never holds `capacity` voxels
     if ((long long)n_vox + n_new >= capacity) {
-        const int rc = evict_lru(runs, n_new, n_touched, st, &n_victims, &n_recreated, launches);
+        const int rc = evict_lru(runs, n_new, n_touched, st, launches);
         if (rc != FLS_OK) return rc;
     }
     NdtUpdateArgs ua;
@@ -498,8 +459,8 @@ int NdtMap::add_cloud(const float4* d_cloud, size_t n, float leaf, bool first_sc
     ua.starts = sc.starts.p;
     ua.counts = sc.counts.p;
     ua.runs = runs;
-    ua.tab = table.p;
-    ua.mask = mask;
+    ua.tab = table.buf.p;
+    ua.mask = table.mask;
     ua.hot = hot.p;
     ua.cold = cold.p;
     ua.carry = carry.p;
@@ -511,78 +472,59 @@ int NdtMap::add_cloud(const float4* d_cloud, size_t n, float leaf, bool first_sc
     ua.min_pts = min_pts;
     ua.max_pts = max_pts;
     ua.first_scan = first_scan ? 1 : 0;
-    int* overflow = counter.p + 1;
-    FLS_CUDA(cudaMemsetAsync(counter.p + 1, 0, 2 * sizeof(int), st));  // overflow flag, free-list cursor
-    ndt_update_kernel<<<grid_for(runs, 128), 128, 0, st>>>(ua, overflow);
-    int h[3] = {0, 0, 0};
+    FLS_CUDA(cudaMemsetAsync(counter.p + kOverflow, 0, 2 * sizeof(int), st));  // overflow flag, free-stack cursor
+    ndt_update_kernel<<<grid_for(runs, 128), 128, 0, st>>>(ua, counter.p + kOverflow);
+    int h[3] = {0, 0, 0};  // up to the free-stack cursor
     FLS_CUDA(cudaMemcpyAsync(h, counter.p, 3 * sizeof(int), cudaMemcpyDeviceToHost, st));
     FLS_CUDA(cudaStreamSynchronize(st));
     *launches += 6;
-    hi_water = h[0];
-    n_free -= h[2] < n_free ? h[2] : n_free;  // the creations popped that many indices off the free stack
-    n_vox = n_vox + (size_t)n_new + (size_t)n_recreated - (size_t)n_victims;
-    if (h[1]) return FLS_ERR_CAPACITY;
+    hi_water = h[kHiWater];
+    n_free -= h[kFreeCursor] < n_free ? h[kFreeCursor] : n_free;  // the creations popped that many indices off the free stack
+    n_vox += (size_t)n_new;
+    if (h[kOverflow]) return FLS_ERR_CAPACITY;
     return FLS_OK;
 }
 
 // Evicts what upstream's sequential insert would evict during this call (exact, including a victim that is touched again later in
 // the call): candidates = live voxels by ascending stamp, simulated on the host against the creation times of the new voxels.
-int NdtMap::evict_lru(int runs, int n_new, int n_touched, cudaStream_t st, int* n_victims, int* n_recreated, int* launches) {
+int NdtMap::evict_lru(int runs, int n_new, int n_touched, cudaStream_t st, int* launches) {
     BuildScratch& sc = scratch;
     const int hw = hi_water;
     const size_t n_live = n_vox;
     if (n_live == 0) return FLS_ERR_CAPACITY;  // the first cloud alone overflows the capacity: upstream dereferences an erased voxel (:216-220)
-    lru_keys.reserve(n_live + 1);
-    lru_keys_sorted.reserve(n_live + 1);
-    lru_vals.reserve(n_live + 1);
-    lru_vals_sorted.reserve(n_live + 1);
-    ndt_live_kernel<<<grid_for(hw, 256), 256, 0, st>>>(cold.p, hw, lru_keys.p, lru_vals.p, counter.p);
-    cub_pass(sc.cub_tmp, [&](void* tmp, size_t& bytes) {
-        return cub::DeviceRadixSort::SortPairs(tmp, bytes, lru_keys.p, lru_keys_sorted.p, lru_vals.p, lru_vals_sorted.p, (int)n_live, 0, 64, st);
-    });
-    const size_t K = lru_candidate_bound(n_live, n_new, n_touched, capacity, n_live);
-    sc.k32a.reserve(K + 1);
-    sc.k32b.reserve((size_t)n_new + 1);
-    ndt_cand_kernel<<<grid_for(K, 256), 256, 0, st>>>(lru_vals_sorted.p, (int)K, touch_run.p, sc.starts.p, sc.idx_sorted.p, sc.k32a.p);
-    FLS_CUDA(cudaMemsetAsync(counter.p + 6, 0, sizeof(int), st));
-    ndt_create_times_kernel<<<grid_for(runs, 256), 256, 0, st>>>(runs, run_vi.p, sc.starts.p, sc.idx_sorted.p, sc.k32b.p, counter.p + 6);
-    std::vector<unsigned> cand(K), creat((size_t)n_new);
-    FLS_CUDA(cudaMemcpyAsync(cand.data(), sc.k32a.p, sizeof(unsigned) * K, cudaMemcpyDeviceToHost, st));
-    if (n_new) FLS_CUDA(cudaMemcpyAsync(creat.data(), sc.k32b.p, sizeof(unsigned) * (size_t)n_new, cudaMemcpyDeviceToHost, st));
-    FLS_CUDA(cudaStreamSynchronize(st));
-    *launches += 5;
-    std::vector<unsigned> victims;
-    std::vector<unsigned char> recreated;
-    if (!lru_simulate(n_live, (size_t)capacity, cand, creat, victims, recreated)) return FLS_ERR_CAPACITY;
-    *n_victims = (int)victims.size();
-    *n_recreated = 0;
-    for (unsigned char r : recreated) *n_recreated += r ? 1 : 0;
-    if (victims.empty()) return FLS_OK;
+    ndt_live_kernel<<<grid_for(hw, 256), 256, 0, st>>>(cold.p, hw, eviction.stamps.reserve(n_live + 1), eviction.ids.reserve(n_live + 1),
+                                                       counter.p + kLiveCursor);
+    ndt_create_times_kernel<<<grid_for(runs, 256), 256, 0, st>>>(runs, run_vi.p, sc.starts.p, sc.idx_sorted.p, sc.k32b.reserve((size_t)n_new + 1),
+                                                                counter.p + kCreateCursor);
+    *launches += 2;
+    const int rc = eviction.run((int)n_live, sc.k32b.p, n_new, n_touched, n_live, capacity, sc.cub_tmp, st, launches,
+                                [&](const unsigned* vis_sorted, int K, unsigned* out) {
+                                    ndt_cand_kernel<<<grid_for(K, 256), 256, 0, st>>>(vis_sorted, K, touch_run.p, sc.starts.p, sc.idx_sorted.p, out);
+                                });
+    if (rc != FLS_OK) return rc;
+    const int n_victims = (int)eviction.n_victims;
+    n_vox = n_vox + eviction.n_recreated - eviction.n_victims;
+    if (n_victims == 0) return FLS_OK;
     // victims -> free list, their keys out of the table (rebuild: open addressing has no cheap delete)
-    sc.k32a.reserve(victims.size() + 1);
-    sc.minmax.reserve(victims.size() / 4 + 16);
-    FLS_CUDA(cudaMemcpyAsync(sc.k32a.p, victims.data(), sizeof(unsigned) * victims.size(), cudaMemcpyHostToDevice, st));
-    FLS_CUDA(cudaMemcpyAsync(sc.minmax.p, recreated.data(), victims.size(), cudaMemcpyHostToDevice, st));
-    ndt_evict_kernel<<<grid_for(victims.size(), 128), 128, 0, st>>>(sc.k32a.p, reinterpret_cast<const unsigned char*>(sc.minmax.p), (int)victims.size(),
-                                                                   lru_vals_sorted.p, cold.p, free_list.p, n_free, touch_run.p, run_vi.p);
-    n_free += (int)victims.size();
-    ndt_table_clear_only_kernel<<<grid_for(slots, 256), 256, 0, st>>>(table.p, slots);
-    ndt_table_rebuild_kernel<<<grid_for(hw, 256), 256, 0, st>>>(cold.p, hw, table.p, mask);
-    FLS_CUDA(cudaStreamSynchronize(st));  // the host vectors above are read by the copies
-    *launches += 3;
+    ndt_evict_kernel<<<grid_for(n_victims, 128), 128, 0, st>>>(eviction.victims.p, eviction.recreated.p, n_victims, eviction.ids_sorted.p, cold.p,
+                                                              free_list.p, n_free, touch_run.p, run_vi.p);
+    n_free += n_victims;
+    table.clear(st, launches);
+    ndt_table_rebuild_kernel<<<grid_for(hw, 256), 256, 0, st>>>(cold.p, hw, table.buf.p, table.mask);
+    *launches += 2;
     return FLS_OK;
 }
 
 size_t NdtMap::dump_keys(unsigned long long* h_out, size_t cap, cudaStream_t st) {
     if (n_vox == 0 || hi_water == 0) return 0;
-    lru_keys.reserve(n_vox + 1);
-    FLS_CUDA(cudaMemsetAsync(counter.p + 7, 0, sizeof(int), st));
-    ndt_dump_keys_kernel<<<grid_for(hi_water, 256), 256, 0, st>>>(cold.p, hi_water, lru_keys.p, counter.p + 7);
+    scratch.keys.reserve(n_vox + 1);
+    FLS_CUDA(cudaMemsetAsync(counter.p + kDumpCursor, 0, sizeof(int), st));
+    ndt_dump_keys_kernel<<<grid_for(hi_water, 256), 256, 0, st>>>(cold.p, hi_water, scratch.keys.p, counter.p + kDumpCursor);
     int n = 0;
-    FLS_CUDA(cudaMemcpyAsync(&n, counter.p + 7, sizeof(int), cudaMemcpyDeviceToHost, st));
+    FLS_CUDA(cudaMemcpyAsync(&n, counter.p + kDumpCursor, sizeof(int), cudaMemcpyDeviceToHost, st));
     FLS_CUDA(cudaStreamSynchronize(st));
     const size_t m = (size_t)n < cap ? (size_t)n : cap;
-    FLS_CUDA(cudaMemcpy(h_out, lru_keys.p, sizeof(unsigned long long) * m, cudaMemcpyDeviceToHost));
+    FLS_CUDA(cudaMemcpy(h_out, scratch.keys.p, sizeof(unsigned long long) * m, cudaMemcpyDeviceToHost));
     return m;
 }
 
@@ -591,10 +533,10 @@ void NdtMap::dump_voxels(std::vector<fls_ndt_voxel>& out, cudaStream_t st) {
     if (n_vox == 0 || hi_water == 0) return;
     DevBuf<fls_ndt_voxel> d;
     d.reserve(n_vox + 1);
-    FLS_CUDA(cudaMemsetAsync(counter.p + 7, 0, sizeof(int), st));
-    ndt_dump_voxels_kernel<<<grid_for(hi_water, 256), 256, 0, st>>>(cold.p, hot.p, hi_water, d.p, counter.p + 7);
+    FLS_CUDA(cudaMemsetAsync(counter.p + kDumpCursor, 0, sizeof(int), st));
+    ndt_dump_voxels_kernel<<<grid_for(hi_water, 256), 256, 0, st>>>(cold.p, hot.p, hi_water, d.p, counter.p + kDumpCursor);
     int n = 0;
-    FLS_CUDA(cudaMemcpyAsync(&n, counter.p + 7, sizeof(int), cudaMemcpyDeviceToHost, st));
+    FLS_CUDA(cudaMemcpyAsync(&n, counter.p + kDumpCursor, sizeof(int), cudaMemcpyDeviceToHost, st));
     FLS_CUDA(cudaStreamSynchronize(st));
     out.resize((size_t)n);
     if (n) FLS_CUDA(cudaMemcpy(out.data(), d.p, sizeof(fls_ndt_voxel) * (size_t)n, cudaMemcpyDeviceToHost));
@@ -684,7 +626,7 @@ class NdtPlugin final : public Plugin {
 
     void map_info(fls_map_info* out) const override {
         out->n_voxels = (long long)map.n_vox;
-        out->table_slots = (long long)map.slots;
+        out->table_slots = (long long)map.table.slots;
         out->bytes = (long long)map.bytes();
     }
 

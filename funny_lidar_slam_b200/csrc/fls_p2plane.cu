@@ -496,7 +496,8 @@ class IvoxPlugin final : public Plugin {
         // a query and a candidate of its stencil differ by at most 2*res per axis with a non-zero offset and res otherwise:
         // d^2 <= 12 res^2 for the full 26-neighbourhood
         const unsigned fast_knn = 12.0 * 1.01 * (double)map.res * (double)map.res < (double)max_range2 ? 1u : 0u;
-        return {map.pts_sorted.p, map.table.p, map.mask, map.inv_res, max_range2, map.n_stencil, map.lists.p, map.ctab.p, map.cmask, fast_knn};
+        return {map.pts_sorted.p, map.table.buf.p, map.table.mask, map.inv_res, max_range2, map.n_stencil, map.lists.p, map.ctab.buf.p, map.ctab.mask,
+                fast_knn};
     }
     int append(const float4* d, size_t n) { return map.append_and_build(d, n, h.cfg.ivox_capacity, h.stream, &h.launches); }
 
@@ -684,7 +685,7 @@ class IvoxPlugin final : public Plugin {
     void map_info(fls_map_info* out) const override {
         out->n_points = (long long)map.n_pts;
         out->n_voxels = (long long)map.n_vox;
-        out->table_slots = map.n_pts ? (long long)map.mask + 1 : 0;
+        out->table_slots = map.n_pts ? (long long)map.table.slots : 0;
         out->bytes = (long long)map.bytes();
         out->incremental_inserts = (long long)map.n_incremental;
         out->full_builds = (long long)map.n_full;
