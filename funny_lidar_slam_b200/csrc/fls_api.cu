@@ -39,18 +39,18 @@ void Handle::release() {
         if (e) cudaEventDestroy(e);
         e = nullptr;
     }
-    if (ev0) cudaEventDestroy(ev0);
-    if (ev1) cudaEventDestroy(ev1);
-    ev0 = ev1 = nullptr;
-    if (stream) cudaStreamDestroy(stream);
-    stream = nullptr;
+    if (call.e0) cudaEventDestroy(call.e0);
+    if (call.e1) cudaEventDestroy(call.e1);
+    call.e0 = call.e1 = nullptr;
+    if (call.stream) cudaStreamDestroy(call.stream);
+    call.stream = nullptr;
 }
 
 void Handle::init() {
     FLS_CUDA(cudaSetDevice(cfg.device));
-    FLS_CUDA(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
-    FLS_CUDA(cudaEventCreate(&ev0));
-    FLS_CUDA(cudaEventCreate(&ev1));
+    FLS_CUDA(cudaStreamCreateWithFlags(&call.stream, cudaStreamNonBlocking));
+    FLS_CUDA(cudaEventCreate(&call.e0));
+    FLS_CUDA(cudaEventCreate(&call.e1));
     h_state.reserve(kMaxBatch);
     state.reserve(kMaxBatch);
     switch (cfg.method) {
@@ -71,13 +71,13 @@ void Handle::init() {
 
 Handle::~Handle() {
     cudaSetDevice(cfg.device);
-    if (stream) cudaStreamSynchronize(stream);
+    if (call.stream) cudaStreamSynchronize(call.stream);
     release();
 }
 
 // Copy a caller cloud (host memory, `stride` bytes per record) into packed float4 device memory.
 void Handle::upload_into(const void* pts, size_t n, size_t stride, float4* dst) {
-    upload_records(pts, n, stride, dst, raw, stream, &h2d_bytes, &launches);
+    upload_records(pts, n, stride, dst, raw, call);
 }
 
 const float4* Handle::upload(const void* pts, size_t n, size_t stride, DevBuf<float4>& dst) {
@@ -112,21 +112,12 @@ int Handle::begin_batch(int B, const void* const* scans, const size_t* n, size_t
 
 void Handle::begin_call() {
     FLS_CUDA(cudaSetDevice(cfg.device));
-    launches = waits = 0;
-    h2d_bytes = d2h_bytes = 0;
-    FLS_CUDA(cudaEventRecord(ev0, stream));
-}
-
-void Handle::end_call(fls_match_stats* st) {
-    FLS_CUDA(cudaEventRecord(ev1, stream));
-    FLS_CUDA(cudaStreamSynchronize(stream));
-    ++waits;
-    fill_call_stats(st, ev0, ev1, launches, h2d_bytes, d2h_bytes);
+    call.begin();
 }
 
 void Handle::set_fit_cloud(const float4* d, size_t n) {
     fit_cloud.reserve(n);
-    if (n) FLS_CUDA(cudaMemcpyAsync(fit_cloud.p, d, n * sizeof(float4), cudaMemcpyDeviceToDevice, stream));
+    if (n) FLS_CUDA(cudaMemcpyAsync(fit_cloud.p, d, n * sizeof(float4), cudaMemcpyDeviceToDevice, call.stream));
     set_fit_view(fit_cloud.p, n);
 }
 
@@ -152,7 +143,7 @@ GnParams Handle::gn_params(int method, int min_effective) const {
 unsigned Handle::next_ll_epoch(size_t n_records) {
     const size_t cap0 = ll_rows.cap;
     ll_rows.reserve(n_records);
-    if (ll_rows.cap != cap0) FLS_CUDA(cudaMemsetAsync(ll_rows.p, 0, ll_rows.cap * sizeof(uint4), stream));
+    if (ll_rows.cap != cap0) FLS_CUDA(cudaMemsetAsync(ll_rows.p, 0, ll_rows.cap * sizeof(uint4), call.stream));
     match_epoch = (match_epoch + 1) & 0xffffffu;
     if (match_epoch == 0) match_epoch = 1;
     return match_epoch << 8;
@@ -162,12 +153,12 @@ void Handle::read_back(int B) {
     // h_log is about to hold this call's logs: until unpack records their sizes, no scan has one (a Match that fails after
     // its launch, e.g. through the v9 watchdog, leaves no log rather than a mix of two calls)
     log_n.assign(1, 0);
-    FLS_CUDA(cudaMemcpyAsync(h_state.p, state.p, sizeof(GnState) * (size_t)B, cudaMemcpyDeviceToHost, stream));
-    d2h_bytes += (long long)(sizeof(GnState) * (size_t)B);
+    FLS_CUDA(cudaMemcpyAsync(h_state.p, state.p, sizeof(GnState) * (size_t)B, cudaMemcpyDeviceToHost, call.stream));
+    call.d2h += (long long)(sizeof(GnState) * (size_t)B);
     if (log_cap) {
         const size_t bytes = sizeof(fls_iter_log) * (size_t)log_cap * (size_t)B;
-        FLS_CUDA(cudaMemcpyAsync(h_log.data(), log.p, bytes, cudaMemcpyDeviceToHost, stream));
-        d2h_bytes += (long long)bytes;
+        FLS_CUDA(cudaMemcpyAsync(h_log.data(), log.p, bytes, cudaMemcpyDeviceToHost, call.stream));
+        call.d2h += (long long)bytes;
     }
 }
 
@@ -219,7 +210,7 @@ int Handle::filter_batch(int B, const float4* const* d, const size_t* n, float l
             ns[s] = ns[first];
             continue;
         }
-        const size_t nf = voxel_grid_device(d[s], n[s], leaf, dst.p + end, scratch, stream, &launches, &waits);
+        const size_t nf = voxel_grid_device(d[s], n[s], leaf, dst.p + end, scratch, call);
         if (nf > 0x3fffffffull) return FLS_ERR_INVALID_ARG;
         off[s] = end;
         ns[s] = nf;
@@ -229,9 +220,8 @@ int Handle::filter_batch(int B, const float4* const* d, const size_t* n, float l
 }
 
 int Handle::inserted(int rc, fls_match_stats* st) {
-    FLS_CUDA(cudaStreamSynchronize(stream));
-    ++waits;
-    if (st) st->gpu_launches = launches;
+    call.sync();
+    if (st) st->gpu_launches = call.launches;
     return rc;
 }
 
@@ -464,7 +454,7 @@ int fls_add_cloud(fls_handle* hh, int n_clouds, const void* const* pts, const si
         const float4* dc = two ? h->upload(pts[1], n[1], stride, h->up_corner) : nullptr;
         rc = h->plugin->add_cloud(d, n[0], dc, two ? n[1] : 0);
     }
-    h->end_call(nullptr);
+    h->call.end(nullptr);
     return rc;
     FLS_CATCH
 }
@@ -677,7 +667,7 @@ int fls_set_global_map(fls_handle* hh, const void* pts, size_t n, size_t stride)
     FLS_TRY
     h->begin_call();
     const int rc = h->set_global_map(pts, n, stride);
-    h->end_call(nullptr);
+    h->call.end(nullptr);
     return rc;
     FLS_CATCH
 }
@@ -688,7 +678,7 @@ int fls_update_local_map(fls_handle* hh, const double* T, int* updated, size_t* 
     FLS_TRY
     h->begin_call();
     const int rc = h->update_local_map(T, updated, n_local);
-    h->end_call(nullptr);
+    h->call.end(nullptr);
     return rc;
     FLS_CATCH
 }
@@ -794,14 +784,14 @@ int fls_voxel_grid(int device, const void* pts, size_t n, size_t stride, float l
     *n_out = 0;
     if (n == 0) return FLS_OK;
     return fls::with_workspace<VoxelWorkspace>(device, [&](VoxelWorkspace& w) -> int {
-        long long h2d = 0;
-        int launches = 0;
+        fls::Call& c = w.call;
+        c.begin();
         w.in.reserve(n);
         w.out.reserve(n);
-        fls::upload_records(pts, n, stride, w.in.p, w.raw, w.st, &h2d, &launches);
-        const size_t m = fls::voxel_grid_device(w.in.p, n, leaf, w.out.p, w.sc, w.st, &launches);
-        FLS_CUDA(cudaMemcpyAsync(out, w.out.p, m * 16, cudaMemcpyDeviceToHost, w.st));
-        FLS_CUDA(cudaStreamSynchronize(w.st));
+        fls::upload_records(pts, n, stride, w.in.p, w.raw, c);
+        const size_t m = fls::voxel_grid_device(w.in.p, n, leaf, w.out.p, w.sc, c);
+        FLS_CUDA(cudaMemcpyAsync(out, w.out.p, m * 16, cudaMemcpyDeviceToHost, c.stream));
+        c.sync();
         *n_out = m;
         return FLS_OK;
     });

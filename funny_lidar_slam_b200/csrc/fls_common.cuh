@@ -72,15 +72,39 @@ void launch_cooperative(void (*fn)(P...), int grid, int block, size_t smem, cuda
 // caller record layouts: packed float4, or x y z at 0 / 4 / 8 and the intensity at 16 of a larger record
 inline bool stride_ok(size_t stride) { return stride == 16 || (stride >= 20 && stride % 4 == 0); }
 
-// clears *st (when given) and fills the call-level figures: device time from e0 to e1 (both complete), launches and copies
-inline void fill_call_stats(fls_match_stats* st, cudaEvent_t e0, cudaEvent_t e1, int launches, long long h2d, long long d2h) {
-    if (!st) return;
-    std::memset(st, 0, sizeof(*st));
-    FLS_CUDA(cudaEventElapsedTime(&st->gpu_ms, e0, e1));
-    st->gpu_launches = launches;
-    st->h2d_bytes = h2d;
-    st->d2h_bytes = d2h;
-}
+// ---- one call: its stream, the events that time it and what it reports ----------------------------------------------------
+// launches and the bytes copied each way (h2d / d2h) are counted where they are enqueued, waits (stream synchronisations) by
+// sync().  Its owner (Handle, Workspace, KeyframeStore) creates the stream and the events; every helper of the call takes the
+// Call and counts into it.
+struct Call {
+    cudaStream_t stream = nullptr;
+    cudaEvent_t e0 = nullptr, e1 = nullptr;
+    int launches = 0, waits = 0;
+    long long h2d = 0, d2h = 0;
+
+    // zeroes the counts and records e0
+    void begin() {
+        launches = waits = 0;
+        h2d = d2h = 0;
+        FLS_CUDA(cudaEventRecord(e0, stream));
+    }
+    void sync() {
+        FLS_CUDA(cudaStreamSynchronize(stream));
+        ++waits;
+    }
+    // records e1 and waits for it, then clears *st (when given) and fills the call-level figures: device time from e0 to e1,
+    // launches and copies
+    void end(fls_match_stats* st) {
+        FLS_CUDA(cudaEventRecord(e1, stream));
+        sync();
+        if (!st) return;
+        std::memset(st, 0, sizeof(*st));
+        FLS_CUDA(cudaEventElapsedTime(&st->gpu_ms, e0, e1));
+        st->gpu_launches = launches;
+        st->h2d_bytes = h2d;
+        st->d2h_bytes = d2h;
+    }
+};
 
 // ---- device buffer (grow-only) ------------------------------------------------------------------------
 template <typename T>
@@ -174,8 +198,7 @@ struct PinnedBuf {
 struct Workspace {
     std::mutex mu;
     bool ready = false;
-    cudaStream_t st = nullptr;  // created on first use
-    cudaEvent_t e0 = nullptr, e1 = nullptr;
+    Call call;  // stream and events created on first use
 };
 
 // Runs body(W&) on `device` (checked by check_device) under the workspace's lock.
@@ -186,9 +209,9 @@ int with_workspace(int device, F&& body) {
     std::lock_guard<std::mutex> lock(w.mu);
     FLS_CUDA(cudaSetDevice(device));
     if (!w.ready) {
-        FLS_CUDA(cudaStreamCreateWithFlags(&w.st, cudaStreamNonBlocking));
-        FLS_CUDA(cudaEventCreate(&w.e0));
-        FLS_CUDA(cudaEventCreate(&w.e1));
+        FLS_CUDA(cudaStreamCreateWithFlags(&w.call.stream, cudaStreamNonBlocking));
+        FLS_CUDA(cudaEventCreate(&w.call.e0));
+        FLS_CUDA(cudaEventCreate(&w.call.e1));
         w.ready = true;
     }
     return body(w);

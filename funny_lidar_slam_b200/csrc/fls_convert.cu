@@ -364,19 +364,18 @@ int convert_cloud_device(const fls_convert_cfg& c, const fls_pointcloud2& m, flo
     if (n == 0) return FLS_OK;  // upstream reads points.back() of the empty cloud here (DESIGN.md §8)
 
     return with_workspace<ConvWorkspace>(c.device, [&](ConvWorkspace& w) -> int {
-        cudaStream_t st = w.st;
+        Call& call = w.call;
+        const cudaStream_t st = call.stream;
         fls_convert_result* const h_res = w.h_res.reserve(1);
         int* const h_count = w.h_count.reserve(1);
-        long long h2d = 0, d2h = 0;
-        int launches = 0;
-        FLS_CUDA(cudaEventRecord(w.e0, st));
+        call.begin();
         const size_t bytes = (size_t)m.height * m.row_step;
         if (m.data_on_device) {
             p.data = static_cast<const unsigned char*>(m.data);
         } else {
             w.staging.reserve(bytes + 1);
             FLS_CUDA(cudaMemcpyAsync(w.staging.p, m.data, bytes, cudaMemcpyHostToDevice, st));
-            h2d += (long long)bytes;
+            call.h2d += (long long)bytes;
             p.data = w.staging.p;
         }
         float4* ox = d_xyzi ? reinterpret_cast<float4*>(d_xyzi) : w.xyzi.reserve(n);
@@ -413,7 +412,7 @@ int convert_cloud_device(const fls_convert_cfg& c, const fls_pointcloud2& m, flo
         }
         cub_run(w.cub_tmp, positions);
         conv_emit_kernel<<<g, 256, 0, st>>>(p, w.flag.p, w.pos.p, d_first_kept, ox, orr, ot, d_count);
-        launches += 3;
+        call.launches += 3;
         if (offsets) {  // ComputePointOffsetTime(cloud, 10.0): the kernels run, the last one writes only when the condition holds
             OffsetParams q;
             q.omega = 2.0 * M_PI * 10.0;  // :518
@@ -425,10 +424,10 @@ int convert_cloud_device(const fls_convert_cfg& c, const fls_pointcloud2& m, flo
             off_map_kernel<<<g, 256, 0, st>>>(q, w.key_sorted.p, w.idx_sorted.p, w.yaw.p, d_first, (int)n, w.map.p);
             cub_run(w.cub_tmp, compose);
             off_write_kernel<<<g, 256, 0, st>>>(q, w.key_sorted.p, w.idx_sorted.p, w.yaw.p, d_first, w.state.p, d_go, (int)n, ot);
-            launches += 6;
+            call.launches += 6;
         }
         conv_window_kernel<<<1, kWinThreads, 0, st>>>(p, m.stamp_us, ot, d_count, d_first_kept, offsets ? d_go : nullptr, w.res.p);
-        ++launches;
+        ++call.launches;
         FLS_CUDA(cudaGetLastError());
         // the host copies cover the capacity, so that the call waits once
         if (xyzi) FLS_CUDA(cudaMemcpyAsync(xyzi, ox, n * sizeof(float4), cudaMemcpyDeviceToHost, st));
@@ -436,14 +435,12 @@ int convert_cloud_device(const fls_convert_cfg& c, const fls_pointcloud2& m, flo
         if (time) FLS_CUDA(cudaMemcpyAsync(time, ot, n * sizeof(float), cudaMemcpyDeviceToHost, st));
         FLS_CUDA(cudaMemcpyAsync(h_count, d_count, sizeof(int), cudaMemcpyDeviceToHost, st));
         FLS_CUDA(cudaMemcpyAsync(h_res, w.res.p, sizeof(fls_convert_result), cudaMemcpyDeviceToHost, st));
-        d2h += (long long)(n * ((xyzi ? 16 : 0) + (ring ? 4 : 0) + (time ? 4 : 0)) + sizeof(int) + sizeof(fls_convert_result));
-        FLS_CUDA(cudaEventRecord(w.e1, st));
-        FLS_CUDA(cudaStreamSynchronize(st));  // the only wait
+        call.d2h += (long long)(n * ((xyzi ? 16 : 0) + (ring ? 4 : 0) + (time ? 4 : 0)) + sizeof(int) + sizeof(fls_convert_result));
+        call.end(stats);  // the only wait
         const size_t cnt = (size_t)*h_count;
         *n_out = cnt;
         *res = *h_res;
         if (stats) {
-            fill_call_stats(stats, w.e0, w.e1, launches, h2d, d2h);
             stats->n_source = (long long)n;
             // the message read once, the outputs written once; the offsets read xyzi + ring and rewrite the times
             stats->algo_bytes = (long long)(n * m.point_step + cnt * 24 + (res->recomputed ? cnt * 24 : 0));

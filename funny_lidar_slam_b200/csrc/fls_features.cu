@@ -500,34 +500,36 @@ int extract_features_device(int device, const float* depth, const int* col, size
             FLS_CUDA(cudaEventCreate(&w.k0));
             FLS_CUDA(cudaEventCreate(&w.k1));
         }
-        cudaStream_t st = w.st;
+        Call& c = w.call;
+        const cudaStream_t st = c.stream;
         const size_t idx_cap = (size_t)n_rows * 120 + p.planar_cap;
         w.d_depth.reserve(n);
         w.d_col.reserve(n);
         w.d_rows.reserve((size_t)n_rows * 2);
         w.d_idx.reserve(idx_cap);
         int* const h_out = w.h_out.reserve(idx_cap + 2);
-        FLS_CUDA(cudaEventRecord(w.e0, st));
+        c.begin();
         FLS_CUDA(cudaMemcpyAsync(w.d_depth.p, depth, n * 4, cudaMemcpyHostToDevice, st));
         FLS_CUDA(cudaMemcpyAsync(w.d_col.p, col, n * 4, cudaMemcpyHostToDevice, st));
         FLS_CUDA(cudaMemcpyAsync(w.d_rows.p, row_start, n_rows * 4, cudaMemcpyHostToDevice, st));
         FLS_CUDA(cudaMemcpyAsync(w.d_rows.p + n_rows, row_end, n_rows * 4, cudaMemcpyHostToDevice, st));
+        c.h2d += (long long)(n * 8 + (size_t)n_rows * 8);
         FLS_CUDA(cudaEventRecord(w.k0, st));
         const int* d_tot = enqueue_features(w.s, p, device, w.d_depth.p, w.d_col.p, w.d_rows.p, corner_thr, planar_thr, nullptr, w.d_idx.p, nullptr,
                                             nullptr, st);
+        c.launches += kFeatLaunches;
         FLS_CUDA(cudaEventRecord(w.k1, st));
         FLS_CUDA(cudaMemcpyAsync(h_out, d_tot, 2 * sizeof(int), cudaMemcpyDeviceToHost, st));
-        FLS_CUDA(cudaStreamSynchronize(st));  // the two counts size the read-back
+        c.sync();  // the two counts size the read-back
         const size_t nc = (size_t)h_out[0], np = (size_t)h_out[1];
         if (nc + np) FLS_CUDA(cudaMemcpyAsync(h_out + 2, w.d_idx.p, (nc + np) * 4, cudaMemcpyDeviceToHost, st));
-        FLS_CUDA(cudaEventRecord(w.e1, st));
-        FLS_CUDA(cudaStreamSynchronize(st));
+        c.d2h += (long long)(2 + nc + np) * 4;
+        c.end(stats);
         std::memcpy(corner_idx, h_out + 2, nc * 4);
         std::memcpy(planar_idx, h_out + 2 + nc, np * 4);
         *n_corner = nc;
         *n_planar = np;
         if (stats) {
-            fill_call_stats(stats, w.e0, w.e1, kFeatLaunches, (long long)(n * 8 + (size_t)n_rows * 8), (long long)(2 + nc + np) * 4);
             FLS_CUDA(cudaEventElapsedTime(&stats->kernel_ms, w.k0, w.k1));
             stats->kernel_launches = kFeatLaunches;
             stats->n_source = (long long)n;

@@ -20,12 +20,12 @@ struct ProjStage {
 };
 
 // Uploads the raw records (+ ring, and time and the IMU samples when de-skewing) and enqueues PointcloudProjector::Project on
-// `st`: s.ordered / s.depth / s.col (V*H entries, the first *s.total meaningful), s.rows, s.total.  A reference time outside the
-// IMU buffer accepts no point.  Adds the bytes it copies to *h2d and the kernels it launches to *launches; nothing waits.
+// c.stream: s.ordered / s.depth / s.col (V*H entries, the first *s.total meaningful), s.rows, s.total.  A reference time outside the
+// IMU buffer accepts no point.  Counts the bytes it copies and the kernels it launches; nothing waits.
 // src_on_device: raw (packed float4, stride 16), ring and time are device arrays on the stream's device and only the IMU samples
 // are uploaded; the kernels are the same.
 int enqueue_project(ProjStage& s, const void* raw, const int* ring, const float* time, const fls_imu_buffer* imu, size_t n, size_t stride, int V,
-                    int H, float h_res, float min_d, float max_d, cudaStream_t st, long long* h2d, int* launches, bool src_on_device);
+                    int H, float h_res, float min_d, float max_d, Call& c, bool src_on_device);
 
 // launch shape of the feature kernels, from the host copy of the row bounds
 struct FeatPlan {

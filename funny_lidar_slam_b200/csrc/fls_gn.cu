@@ -146,13 +146,13 @@ extern "C" int fls_gn_step_probe(fls_handle* hh, const fls_gn_step_case* cases, 
     uint4* d_ll = reinterpret_cast<uint4*>(d + in_b + out_b + st_b);
     double* d_res = reinterpret_cast<double*>(d + in_b + out_b + st_b + ll_b);
     const std::vector<double> nan_fill(n * kResultLen, __builtin_nan(""));
-    FLS_CUDA(cudaMemcpyAsync(d_in, cases, in_b, cudaMemcpyHostToDevice, h->stream));
-    FLS_CUDA(cudaMemsetAsync(d_ll, 0, ll_b, h->stream));  // tag 0: no iteration's record
-    FLS_CUDA(cudaMemcpyAsync(d_res, nan_fill.data(), res_b, cudaMemcpyHostToDevice, h->stream));
-    gn_step_probe_kernel<<<(unsigned)((n + 127) / 128), 128, 0, h->stream>>>(d_in, d_out, d_st, d_ll, d_res, (int)n);
+    FLS_CUDA(cudaMemcpyAsync(d_in, cases, in_b, cudaMemcpyHostToDevice, h->call.stream));
+    FLS_CUDA(cudaMemsetAsync(d_ll, 0, ll_b, h->call.stream));  // tag 0: no iteration's record
+    FLS_CUDA(cudaMemcpyAsync(d_res, nan_fill.data(), res_b, cudaMemcpyHostToDevice, h->call.stream));
+    gn_step_probe_kernel<<<(unsigned)((n + 127) / 128), 128, 0, h->call.stream>>>(d_in, d_out, d_st, d_ll, d_res, (int)n);
     FLS_CUDA(cudaGetLastError());
-    FLS_CUDA(cudaMemcpyAsync(out, d_out, out_b, cudaMemcpyDeviceToHost, h->stream));
-    h->end_call(nullptr);
+    FLS_CUDA(cudaMemcpyAsync(out, d_out, out_b, cudaMemcpyDeviceToHost, h->call.stream));
+    h->call.end(nullptr);
     return FLS_OK;
     FLS_CATCH
 }

@@ -1,4 +1,4 @@
-// fls_handle.h — the object behind `fls_handle*`: configuration, stream, what every plug-in's Match shares, and the one
+// fls_handle.h — the object behind `fls_handle*`: configuration, the Call its entries run on, what every plug-in's Match shares, and the one
 // registration plug-in that cfg.method names, which owns its map and the buffers only it uses.
 #pragma once
 #include <memory>
@@ -81,12 +81,7 @@ struct RelocFree {
 
 struct Handle {
     fls_config cfg;
-    cudaStream_t stream = nullptr;
-    cudaEvent_t ev0 = nullptr, ev1 = nullptr;
-
-    // per-call accounting (fls_match_stats; waits: stream synchronisations of end_call / inserted and of the filters that count them)
-    int launches = 0, waits = 0;
-    long long h2d_bytes = 0, d2h_bytes = 0;
+    Call call;  // the stream of every entry, its timing events and the accounting of the current call
 
     // upload staging
     DevBuf<unsigned char> raw;  // strided caller records before repacking
@@ -140,8 +135,7 @@ struct Handle {
     Handle(const Handle&) = delete;
     Handle& operator=(const Handle&) = delete;
 
-    void begin_call();
-    void end_call(fls_match_stats* st);
+    void begin_call();  // makes cfg.device current and begins the call
     const float4* upload(const void* pts, size_t n, size_t stride, DevBuf<float4>& dst);
     void upload_into(const void* pts, size_t n, size_t stride, float4* dst);  // dst: room for n records
     // begin_call of a batch Match (clearing st[n_scans] when given) and its scans as device pointers: host records of `host_stride`
@@ -175,15 +169,15 @@ struct Handle {
     void gn_launch(long long point_iter_bytes, long long cand_bytes, const float4* src, size_t src_n, F&& launch) {
         per_point_iter_bytes = point_iter_bytes;
         per_cand_bytes = cand_bytes;
-        if (profile) FLS_CUDA(cudaEventRecord(prof_ev[0], stream));
+        if (profile) FLS_CUDA(cudaEventRecord(prof_ev[0], call.stream));
         launch();
-        if (profile) FLS_CUDA(cudaEventRecord(prof_ev[1], stream));
-        launches++;
+        if (profile) FLS_CUDA(cudaEventRecord(prof_ev[1], call.stream));
+        call.launches++;
         last_src = src;
         last_src_n = src_n;
     }
     void read_back(int n_scans);  // enqueues the copy of the states and of every scan's iteration log
-    // after end_call: T / converged / stats and log_n of every scan (call-level figures on stats[0]), T_final from scan 0
+    // after call.end: T / converged / stats and log_n of every scan (call-level figures on stats[0]), T_final from scan 0
     void unpack(int n_scans, const size_t* n_source, double* T, int* converged, fls_match_stats* st);
     // A single-scan Match on a persistent kernel of `grid` CTAs (NDT, ICP, kd-tree LOAM): control block, state from T, the
     // gn_launch of launch(ctl), then the wait and T / converged / stats of a scan of n_source points
@@ -192,11 +186,11 @@ struct Handle {
                       size_t n_source, double* T, int* converged, fls_match_stats* st, F&& launch) {
         const unsigned tag_base = next_ll_epoch((size_t)grid * 32 + kLlPoseLen);  // may move ll_rows
         const GnLoopCtl ctl = loop_ctl(0, method, min_effective, tag_base, ll_rows.p, ll_rows.p + (size_t)grid * 32);
-        launch_gn_init(state.p, T, stream);
-        launches++;
+        launch_gn_init(state.p, T, call.stream);
+        call.launches++;
         gn_launch(point_iter_bytes, cand_bytes, src, src_n, [&] { launch(ctl); });
         read_back(1);
-        end_call(st);
+        call.end(st);
         unpack(1, &n_source, T, converged, st);
     }
     // ---- a Match of one or more scans on sub-grids of one cooperative launch (NDT, ICP and kd-tree LOAM batches, kd-tree LOAM Match) ----
@@ -236,12 +230,12 @@ struct Handle {
             it.cta0 = cta0;
             it.ncta = ncta[s];
             cta0 += ncta[s];
-            launch_gn_start(it, d_items + s, T + 16 * s, stream);
-            launches++;
+            launch_gn_start(it, d_items + s, T + 16 * s, call.stream);
+            call.launches++;
         }
         gn_launch(point_iter_bytes, cand_bytes, fit_src, fit_n, [&] { launch(d_items, grid); });
         read_back(B);
-        end_call(st);
+        call.end(st);
         unpack(B, ns, T, converged, st);
         return FLS_OK;
     }
@@ -249,7 +243,7 @@ struct Handle {
     int inserted(int rc, fls_match_stats* st);
 
     int fitness(float max_range, float* score);
-    int fit_grid_for(float max_range, int* waits);  // (re)builds fit_grid for max_range when needed; counts its wait
+    int fit_grid_for(float max_range);  // (re)builds fit_grid for max_range when needed
     void fitness_enqueue(const float4* d_src, size_t n, int P, float max_range);  // P poses of fit_pose -> fit_out / fit_cnt
     // fls_relocalize, or fls_relocalize_wide / fls_relocalize_multi when wide, on a device scan (the call has begun; g from
     // reloc_grid(c, &g, wide)) over the grids of G column-major guesses (G = 1 and guesses == T for the single-guess entries; T

@@ -177,7 +177,7 @@ class IcpPlugin final : public Plugin {
         // icp_optimized.h:173-187: mapping mode slides a window of the last local_map_size clouds, localization mode replaces
         // the map; both end in local_map_ptr_ = VoxelGridCloud(local_map_ptr_, map_cloud_filter_size_)
         const int rc = window_add(window, d_cloud, n, (size_t)h.cfg.local_map_size, h.cfg.map_cloud_filter_size, true, h.cfg.localization_mode != 0,
-                                  h.scratch, h.stream, &h.launches);
+                                  h.scratch, h.call);
         h.set_fit_view(window.cloud.p, window.n);  // GetFitnessScore searches the same cloud
         return rc;
     }
@@ -187,7 +187,7 @@ class IcpPlugin final : public Plugin {
         if (n_in <= 10) return FLS_ERR_TOO_FEW_POINTS;  // CHECK_GT(ordered_cloud_.size(), 10u)  (:55)
         if (window.grid.n_pts == 0) return FLS_ERR_NO_MAP;
         scan.reserve(n_in);
-        const size_t n = voxel_grid_device(d_in, n_in, cfg.source_cloud_filter_size, scan.p, h.scratch, h.stream, &h.launches);  // :57
+        const size_t n = voxel_grid_device(d_in, n_in, cfg.source_cloud_filter_size, scan.p, h.scratch, h.call);  // :57
         const int ni = (int)n;
         const int grid = icp_grid_blocks(ni, cfg.device);
         IcpArgs a;
@@ -198,12 +198,12 @@ class IcpPlugin final : public Plugin {
         a.state = h.state.p;
         // roofline accounting (SURVEY.md §8d, K3): 16 B source point + 27 x 16 B slot probes, 16 B per scanned map record
         h.match_single(FLS_ICP_P2P, 0, grid, 16 + 16LL * 27, 16, scan.p, n, n, T, converged, st,
-                       [&](const GnLoopCtl& ctl) { launch_icp_loop(a, ctl, grid, h.stream); });
+                       [&](const GnLoopCtl& ctl) { launch_icp_loop(a, ctl, grid, h.call.stream); });
         // IsNeedAddCloud (:218-236): key-frame gating on translation / RPY deltas against a persistent last_T
         if (h.h_state.p->converged && !cfg.localization_mode && gate.need(T, cfg.dist_thre_add_cloud, cfg.rot_thre_add_cloud)) {
             ins.reserve(n);
-            launch_transform_f(scan.p, n, T, ins.p, h.stream);  // :156 TransformPointCloud(source, final) in float
-            h.launches++;
+            launch_transform_f(scan.p, n, T, ins.p, h.call.stream);  // :156 TransformPointCloud(source, final) in float
+            h.call.launches++;
             return h.inserted(add_cloud(ins.p, n, nullptr, 0), st);
         }
         return FLS_OK;
@@ -237,7 +237,7 @@ class IcpPlugin final : public Plugin {
                                              a.max_corr = cfg.icp_max_correspond_distance;
                                              a.state = h.state.p + s;
                                          },
-                                         [&](const GnBatchItem<IcpArgs>* d_items, int grid) { launch_icp_batch(d_items, B, grid, h.stream); });
+                                         [&](const GnBatchItem<IcpArgs>* d_items, int grid) { launch_icp_batch(d_items, B, grid, h.call.stream); });
     }
 
     void map_info(fls_map_info* out) const override {

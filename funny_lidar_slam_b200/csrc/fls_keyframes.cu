@@ -116,8 +116,7 @@ struct KeyframeStore {
     int device = 0;
     size_t capacity = 0, used = 0;
     std::mutex mu;
-    cudaStream_t stream = nullptr;
-    cudaEvent_t ev0 = nullptr, ev1 = nullptr;
+    Call call;
     float4* arena = nullptr;
     std::vector<unsigned long long> begin;  // per keyframe id: first arena record
     std::vector<unsigned> count;            // per keyframe id: records
@@ -134,9 +133,9 @@ struct KeyframeStore {
     KeyframeStore(int dev, size_t cap) : device(dev), capacity(cap) {
         try {
             FLS_CUDA(cudaSetDevice(device));
-            FLS_CUDA(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
-            FLS_CUDA(cudaEventCreate(&ev0));
-            FLS_CUDA(cudaEventCreate(&ev1));
+            FLS_CUDA(cudaStreamCreateWithFlags(&call.stream, cudaStreamNonBlocking));
+            FLS_CUDA(cudaEventCreate(&call.e0));
+            FLS_CUDA(cudaEventCreate(&call.e1));
             FLS_CUDA(cudaMalloc(&arena, capacity * sizeof(float4)));
         } catch (...) {
             release();
@@ -148,12 +147,12 @@ struct KeyframeStore {
         h_table.release();
         h_out.release();
         if (arena) cudaFree(arena);
-        if (ev0) cudaEventDestroy(ev0);
-        if (ev1) cudaEventDestroy(ev1);
-        if (stream) cudaStreamDestroy(stream);
+        if (call.e0) cudaEventDestroy(call.e0);
+        if (call.e1) cudaEventDestroy(call.e1);
+        if (call.stream) cudaStreamDestroy(call.stream);
         arena = nullptr;
-        ev0 = ev1 = nullptr;
-        stream = nullptr;
+        call.e0 = call.e1 = nullptr;
+        call.stream = nullptr;
     }
 
     int add(long long id, const void* pts, size_t n, size_t stride, bool on_device) {
@@ -162,15 +161,14 @@ struct KeyframeStore {
         if (n > capacity - used) return FLS_ERR_CAPACITY;
         if (n) {
             FLS_CUDA(cudaSetDevice(device));
+            call.begin();
             float4* dst = arena + used;
             if (on_device) {
-                FLS_CUDA(cudaMemcpyAsync(dst, pts, n * sizeof(float4), cudaMemcpyDeviceToDevice, stream));
+                FLS_CUDA(cudaMemcpyAsync(dst, pts, n * sizeof(float4), cudaMemcpyDeviceToDevice, call.stream));
             } else {
-                long long h2d = 0;  // the store reports no figures for an add
-                int launches = 0;
-                upload_records(pts, n, stride, dst, raw, stream, &h2d, &launches);
+                upload_records(pts, n, stride, dst, raw, call);
             }
-            FLS_CUDA(cudaStreamSynchronize(stream));
+            call.sync();
         }
         begin.push_back(used);
         count.push_back((unsigned)n);
@@ -193,11 +191,10 @@ struct KeyframeStore {
             return FLS_ERR_CAPACITY;
         }
         FLS_CUDA(cudaSetDevice(device));
-        int launches = 0, waits = 0;
-        long long h2d = 0, d2h = 0;
+        const cudaStream_t stream = call.stream;
         const float inv = 1.0f / leaf;
         const bool final_pass = final_leaf > 0.f;
-        FLS_CUDA(cudaEventRecord(ev0, stream));
+        call.begin();
         size_t runs = 0;
         const KfSeg* d_segs = nullptr;
         const MinMaxOrd* d_mm = nullptr;
@@ -230,7 +227,7 @@ struct KeyframeStore {
             }
             table.reserve(bytes);
             FLS_CUDA(cudaMemcpyAsync(table.p, h, bytes, cudaMemcpyHostToDevice, stream));
-            h2d += (long long)bytes;
+            call.h2d += (long long)bytes;
             d_segs = reinterpret_cast<const KfSeg*>(table.p);
             MinMaxOrd* mm = reinterpret_cast<MinMaxOrd*>(table.p + off_mm);
             d_mm = mm;
@@ -242,11 +239,10 @@ struct KeyframeStore {
             FLS_CUDA(cudaGetLastError());
             // the cell id takes the low 32 bits, the segment the next 16 (all 32 beyond 65536 keyframes): a fixed bit range keeps the
             // sort's passes, and so the launches, the same for every selection size
-            sc.sort_pairs<unsigned long long>(N, K <= 65536 ? 48 : 64, stream);
-            runs = (size_t)sc.encode_runs<unsigned long long>(N, stream);
-            d2h += (long long)sizeof(int);
-            launches += 4;
-            ++waits;
+            sc.sort_pairs<unsigned long long>(N, K <= 65536 ? 48 : 64, call);
+            runs = (size_t)sc.encode_runs<unsigned long long>(N, call);
+            call.d2h += (long long)sizeof(int);
+            call.launches += 4;
         }
         const size_t R = n_base + runs;
         if (!final_pass && R > capacity_out) {
@@ -257,17 +253,17 @@ struct KeyframeStore {
         float4* catp = (!final_pass && d_out) ? d_out : cat.reserve(std::max<size_t>(R, 1));
         if (n_base) FLS_CUDA(cudaMemcpyAsync(catp, d_base, n_base * sizeof(float4), cudaMemcpyDeviceToDevice, stream));
         if (runs) {
-            sc.run_starts((int)runs, stream);
+            sc.run_starts((int)runs, call);
             kf_centroid_kernel<<<grid_for(runs, 128), 128, 0, stream>>>(arena, d_segs, d_mm, inv, sc.uniq.p, sc.idx_sorted.p, sc.starts.p,
                                                                         sc.counts.p, (int)runs, catp + n_base);
             FLS_CUDA(cudaGetLastError());
-            launches += 2;
+            call.launches += 2;
         }
         size_t m = R;
         const float4* res = catp;
         if (final_pass && R) {
             fin.reserve(R);
-            m = voxel_grid_device(catp, R, final_leaf, fin.p, vg, stream, &launches, &waits);
+            m = voxel_grid_device(catp, R, final_leaf, fin.p, vg, call);
             res = fin.p;
         }
         if (m > capacity_out) {
@@ -277,15 +273,12 @@ struct KeyframeStore {
         if (m && d_out && res != d_out) FLS_CUDA(cudaMemcpyAsync(d_out, res, m * sizeof(float4), cudaMemcpyDeviceToDevice, stream));
         if (m && out) {
             FLS_CUDA(cudaMemcpyAsync(out, res, m * sizeof(float4), cudaMemcpyDeviceToHost, stream));
-            d2h += (long long)(m * sizeof(float4));
+            call.d2h += (long long)(m * sizeof(float4));
         }
-        FLS_CUDA(cudaEventRecord(ev1, stream));
-        FLS_CUDA(cudaStreamSynchronize(stream));
-        ++waits;
+        call.end(stats);
         *n_out = m;
         if (stats) {
-            fill_call_stats(stats, ev0, ev1, launches, h2d, d2h);
-            stats->iterations = waits;
+            stats->iterations = call.waits;
             stats->n_source = (int64_t)N;
             stats->n_valid = (int64_t)runs;
         }
@@ -298,14 +291,13 @@ struct KeyframeStore {
         for (size_t k = 0; k < n_ids; ++k)
             if (ids[k] < 0 || ids[k] >= (int64_t)count.size()) return FLS_ERR_INVALID_ARG;
         FLS_CUDA(cudaSetDevice(device));
-        int launches = 0;
-        long long h2d = 0;
-        place.describe(cfg, arena, begin, count, nullptr, 0, false, stream, &launches, &h2d);
+        call.begin();
+        place.describe(cfg, arena, begin, count, nullptr, 0, false, call);
         const size_t nc = place.n_cells();
         float* h = reinterpret_cast<float*>(h_out.reserve(std::max<size_t>(n_ids * nc * sizeof(float), 1)));
         for (size_t k = 0; k < n_ids; ++k)
-            FLS_CUDA(cudaMemcpyAsync(h + k * nc, place.desc((size_t)ids[k]), nc * sizeof(float), cudaMemcpyDeviceToHost, stream));
-        FLS_CUDA(cudaStreamSynchronize(stream));
+            FLS_CUDA(cudaMemcpyAsync(h + k * nc, place.desc((size_t)ids[k]), nc * sizeof(float), cudaMemcpyDeviceToHost, call.stream));
+        call.sync();
         if (n_ids) std::memcpy(desc, h, n_ids * nc * sizeof(float));
         return FLS_OK;
     }
@@ -320,39 +312,35 @@ struct KeyframeStore {
         const size_t n_cand = scan ? K : (size_t)std::max<int64_t>(0, query_id - min_span);  // ids with query_id - id > min_span
         const size_t n_out = std::min(k, n_cand);
         FLS_CUDA(cudaSetDevice(device));
-        int launches = 0;
-        long long h2d = 0, d2h = 0;
-        FLS_CUDA(cudaEventRecord(ev0, stream));
+        call.begin();
         const float4* d_query = nullptr;
         if (scan && n) {
             if (on_device) {
                 d_query = reinterpret_cast<const float4*>(pts);
             } else {
                 query.reserve(n);
-                upload_records(pts, n, stride, query.p, raw, stream, &h2d, &launches);
+                upload_records(pts, n, stride, query.p, raw, call);
                 d_query = query.p;
             }
         }
-        const size_t n_read = place.describe(cfg, arena, begin, count, d_query, n, scan, stream, &launches, &h2d);
+        const size_t n_read = place.describe(cfg, arena, begin, count, d_query, n, scan, call);
         const size_t q = scan ? K : (size_t)query_id, nc = place.n_cells();
         const size_t off_desc = (n_out * sizeof(fls_place_match) + 15) & ~size_t(15);
         unsigned char* h = h_out.reserve(off_desc + nc * sizeof(float));
         if (n_cand) {
-            place.search(q, n_cand, n_out, reinterpret_cast<fls_place_match*>(h), stream, device, &launches);
-            d2h += (long long)(n_out * sizeof(fls_place_match));
+            place.search(q, n_cand, n_out, reinterpret_cast<fls_place_match*>(h), call, device);
+            call.d2h += (long long)(n_out * sizeof(fls_place_match));
         }
         if (query_desc) {
-            FLS_CUDA(cudaMemcpyAsync(h + off_desc, place.desc(q), nc * sizeof(float), cudaMemcpyDeviceToHost, stream));
-            d2h += (long long)(nc * sizeof(float));
+            FLS_CUDA(cudaMemcpyAsync(h + off_desc, place.desc(q), nc * sizeof(float), cudaMemcpyDeviceToHost, call.stream));
+            call.d2h += (long long)(nc * sizeof(float));
         }
-        FLS_CUDA(cudaEventRecord(ev1, stream));
-        FLS_CUDA(cudaStreamSynchronize(stream));
+        call.end(stats);
         if (n_out) std::memcpy(out, h, n_out * sizeof(fls_place_match));
         if (query_desc) std::memcpy(query_desc, h + off_desc, nc * sizeof(float));
         *n_found = n_out;
         if (stats) {
-            fill_call_stats(stats, ev0, ev1, launches, h2d, d2h);
-            stats->iterations = 1;
+            stats->iterations = call.waits;
             stats->n_source = (int64_t)n_read;
             stats->n_valid = (int64_t)n_cand;
         }

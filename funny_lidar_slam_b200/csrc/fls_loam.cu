@@ -314,8 +314,8 @@ class KdPlugin final : public Plugin {
                                               a.flags = flags.p + off[s];
                                           },
                                           [&](const GnBatchItem<LoamArgs>* d_items, int grid) {
-                                              launch_loam(d_items, B, flags.p, total, grid, h.stream);
-                                              if (total > 0) h.launches++;  // the flag reset in front of the loop
+                                              launch_loam(d_items, B, flags.p, total, grid, h.call.stream);
+                                              if (total > 0) h.call.launches++;  // the flag reset in front of the loop
                                           });
     }
 
@@ -341,16 +341,14 @@ class KdPlugin final : public Plugin {
             // loam_point_to_plane_kdtree.h:56-80: localization mode replaces the map, mapping mode slides a window; both
             // end in VoxelGridCloud(local_map, map_cloud_filter_size) + kd-tree
             const int rc = window_add(planar, d_planar, n_planar, (size_t)cfg.local_map_size, cfg.map_cloud_filter_size, true, cfg.localization_mode != 0,
-                                      h.scratch, h.stream, &h.launches);
+                                      h.scratch, h.call);
             if (rc == FLS_OK) h.set_fit_cloud(planar.cloud.p, planar.n);  // GetFitnessScore searches the same tree (:159-183)
             return rc;
         }
         // loam_full_kdtree.h:66-104: {planar, corner}, both windows slide, filters only beyond 5 clouds
-        const int rc = window_add(planar, d_planar, n_planar, (size_t)cfg.local_map_size, cfg.map_cloud_filter_size, false, false, h.scratch, h.stream,
-                                  &h.launches);
+        const int rc = window_add(planar, d_planar, n_planar, (size_t)cfg.local_map_size, cfg.map_cloud_filter_size, false, false, h.scratch, h.call);
         if (rc != FLS_OK) return rc;
-        return window_add(*corner, d_corner, n_corner, (size_t)cfg.corner_local_map_size, cfg.corner_map_filter_size, false, false, h.scratch, h.stream,
-                          &h.launches);
+        return window_add(*corner, d_corner, n_corner, (size_t)cfg.corner_local_map_size, cfg.corner_map_filter_size, false, false, h.scratch, h.call);
     }
 
     int match(const float4* d_planar, size_t n_planar, const float4* d_corner, size_t n_corner, double* T, int* converged,
@@ -364,14 +362,14 @@ class KdPlugin final : public Plugin {
             if (full) {
                 ins.reserve(n_planar);
                 ins_corner.reserve(n_corner);
-                launch_transform_d(d_planar, n_planar, T, ins.p, h.stream);  // pcl::transformPointCloud(cloud, out, T_) with the double matrix
-                launch_transform_d(d_corner, n_corner, T, ins_corner.p, h.stream);
-                h.launches += 2;
+                launch_transform_d(d_planar, n_planar, T, ins.p, h.call.stream);  // pcl::transformPointCloud(cloud, out, T_) with the double matrix
+                launch_transform_d(d_corner, n_corner, T, ins_corner.p, h.call.stream);
+                h.call.launches += 2;
                 rc2 = add_cloud(ins.p, n_planar, ins_corner.p, n_corner);
             } else {
                 ins.reserve(n_planar);
-                launch_transform_f(d_planar, n_planar, T, ins.p, h.stream);  // TransformPointCloud(source, final): fp32 with R, t cast to float
-                h.launches++;
+                launch_transform_f(d_planar, n_planar, T, ins.p, h.call.stream);  // TransformPointCloud(source, final): fp32 with R, t cast to float
+                h.call.launches++;
                 rc2 = add_cloud(ins.p, n_planar, nullptr, 0);
             }
             return h.inserted(rc2, st);

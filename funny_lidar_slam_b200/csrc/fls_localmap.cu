@@ -35,7 +35,7 @@ __global__ void crop_flags_kernel(const float4* __restrict__ p, size_t n, float 
 int Handle::set_global_map(const void* pts, size_t n, size_t stride) {
     const float4* d = upload(pts, n, stride, up_cloud);
     global_map.reserve(n + 1);
-    if (n) FLS_CUDA(cudaMemcpyAsync(global_map.p, d, n * sizeof(float4), cudaMemcpyDeviceToDevice, stream));
+    if (n) FLS_CUDA(cudaMemcpyAsync(global_map.p, d, n * sizeof(float4), cudaMemcpyDeviceToDevice, call.stream));
     global_n = n;
     have_edge = false;  // `first || !has_init_`: local_map_edge_.clear() (:369-373)
     return FLS_OK;
@@ -62,16 +62,16 @@ int Handle::update_local_map(const double* T, int* updated, size_t* n_local) {
     crop_keep.reserve(global_n + 1);
     local_map.reserve(global_n + 1);
     scratch.num_runs.reserve(2);
-    crop_flags_kernel<<<(unsigned)((global_n + 255) / 256), 256, 0, stream>>>(global_map.p, global_n, (float)local_edge[0], (float)local_edge[1],
-                                                                            (float)local_edge[2], (float)local_edge[3], (float)local_edge[4],
-                                                                            (float)local_edge[5], crop_keep.p);  // :401-402 .cast<float>()
+    crop_flags_kernel<<<(unsigned)((global_n + 255) / 256), 256, 0, call.stream>>>(global_map.p, global_n, (float)local_edge[0], (float)local_edge[1],
+                                                                                 (float)local_edge[2], (float)local_edge[3], (float)local_edge[4],
+                                                                                 (float)local_edge[5], crop_keep.p);  // :401-402 .cast<float>()
     cub_pass(scratch.cub_tmp, [&](void* tmp, size_t& bytes) {
-        return cub::DeviceSelect::Flagged(tmp, bytes, global_map.p, crop_keep.p, local_map.p, scratch.num_runs.p, (int)global_n, stream);
+        return cub::DeviceSelect::Flagged(tmp, bytes, global_map.p, crop_keep.p, local_map.p, scratch.num_runs.p, (int)global_n, call.stream);
     });
-    FLS_CUDA(cudaMemcpyAsync(scratch.h_num_runs, scratch.num_runs.p, sizeof(int), cudaMemcpyDeviceToHost, stream));
-    FLS_CUDA(cudaStreamSynchronize(stream));
+    FLS_CUDA(cudaMemcpyAsync(scratch.h_num_runs, scratch.num_runs.p, sizeof(int), cudaMemcpyDeviceToHost, call.stream));
+    call.sync();
     const size_t m = (size_t)*scratch.h_num_runs;
-    launches += 2;
+    call.launches += 2;
     if (n_local) *n_local = m;
     if (updated) *updated = 1;
     if (m == 0) return FLS_OK;  // `local_map->empty()`: the caller gives up (:129-131); the matcher keeps its map

@@ -56,8 +56,8 @@ size_t lru_candidate_bound(size_t n_vox, int n_new, int n_touched, long long cap
 }
 
 int LruEviction::run(int n_cand, const unsigned* d_create, int n_create, int n_touched, size_t size0, long long capacity,
-                     DevBuf<unsigned char>& cub_tmp, cudaStream_t st, int* launches,
-                     const std::function<void(const unsigned*, int, unsigned*)>& write_first) {
+                     DevBuf<unsigned char>& cub_tmp, Call& c, const std::function<void(const unsigned*, int, unsigned*)>& write_first) {
+    const cudaStream_t st = c.stream;
     stamps_sorted.reserve((size_t)n_cand + 1);
     ids_sorted.reserve((size_t)n_cand + 1);
     cub_pass(cub_tmp, [&](void* tmp, size_t& bytes) {
@@ -66,12 +66,12 @@ int LruEviction::run(int n_cand, const unsigned* d_create, int n_create, int n_t
     const size_t K = lru_candidate_bound(size0, n_create, n_touched, capacity, (size_t)n_cand);
     first_touch.reserve(K + 1);
     write_first(ids_sorted.p, (int)K, first_touch.p);
-    *launches += 3;  // the sort counts two
+    c.launches += 3;  // the sort counts two
     h_first.resize(K);
     h_create.resize((size_t)n_create);
     FLS_CUDA(cudaMemcpyAsync(h_first.data(), first_touch.p, sizeof(unsigned) * K, cudaMemcpyDeviceToHost, st));
     if (n_create) FLS_CUDA(cudaMemcpyAsync(h_create.data(), d_create, sizeof(unsigned) * (size_t)n_create, cudaMemcpyDeviceToHost, st));
-    FLS_CUDA(cudaStreamSynchronize(st));
+    c.sync();
     if (!lru_simulate(size0, (size_t)capacity, h_first, h_create, h_victims, h_recreated)) return FLS_ERR_CAPACITY;
     n_victims = h_victims.size();
     n_recreated = (size_t)std::count(h_recreated.begin(), h_recreated.end(), 1);
@@ -133,7 +133,8 @@ void BuildScratch::reserve_runs(size_t n) {
 }
 
 template <class K>
-void BuildScratch::sort_pairs(size_t n, int end_bit, cudaStream_t st) {
+void BuildScratch::sort_pairs(size_t n, int end_bit, Call& c) {
+    const cudaStream_t st = c.stream;
     const RunKeys<K> k = run_keys(*this, K());
     auto sort = [&](void* tmp, size_t& bytes) {
         return cub::DeviceRadixSort::SortPairs(tmp, bytes, k.in.p, k.sorted.p, idx.p, idx_sorted.p, (int)n, 0, end_bit, st);
@@ -143,21 +144,21 @@ void BuildScratch::sort_pairs(size_t n, int end_bit, cudaStream_t st) {
 }
 
 template <class K>
-int BuildScratch::encode_runs(size_t n, cudaStream_t st) {
-    cub_run(cub_tmp, encode_pass<K>(*this, (int)n, st));
-    FLS_CUDA(cudaMemcpyAsync(h_num_runs, num_runs.p, sizeof(int), cudaMemcpyDeviceToHost, st));
-    FLS_CUDA(cudaStreamSynchronize(st));
+int BuildScratch::encode_runs(size_t n, Call& c) {
+    cub_run(cub_tmp, encode_pass<K>(*this, (int)n, c.stream));
+    FLS_CUDA(cudaMemcpyAsync(h_num_runs, num_runs.p, sizeof(int), cudaMemcpyDeviceToHost, c.stream));
+    c.sync();
     return *h_num_runs;
 }
 
-void BuildScratch::run_starts(int runs, cudaStream_t st) { cub_run(cub_tmp, starts_pass(*this, runs, st)); }
+void BuildScratch::run_starts(int runs, Call& c) { cub_run(cub_tmp, starts_pass(*this, runs, c.stream)); }
 
 template void BuildScratch::reserve_runs<unsigned long long>(size_t);
 template void BuildScratch::reserve_runs<unsigned>(size_t);
-template void BuildScratch::sort_pairs<unsigned long long>(size_t, int, cudaStream_t);
-template void BuildScratch::sort_pairs<unsigned>(size_t, int, cudaStream_t);
-template int BuildScratch::encode_runs<unsigned long long>(size_t, cudaStream_t);
-template int BuildScratch::encode_runs<unsigned>(size_t, cudaStream_t);
+template void BuildScratch::sort_pairs<unsigned long long>(size_t, int, Call&);
+template void BuildScratch::sort_pairs<unsigned>(size_t, int, Call&);
+template int BuildScratch::encode_runs<unsigned long long>(size_t, Call&);
+template int BuildScratch::encode_runs<unsigned>(size_t, Call&);
 
 namespace {
 
@@ -397,9 +398,9 @@ static void launch_repack(const unsigned char* d_raw, size_t n, size_t stride, f
     repack_kernel<<<grid_for(n, 256), 256, 0, st>>>(d_raw, n, stride, d_out);
 }
 
-void upload_records(const void* pts, size_t n, size_t stride, float4* dst, DevBuf<unsigned char>& staging, cudaStream_t st, long long* h2d,
-                    int* launches) {
+void upload_records(const void* pts, size_t n, size_t stride, float4* dst, DevBuf<unsigned char>& staging, Call& c) {
     if (n == 0) return;
+    const cudaStream_t st = c.stream;
     if (stride == FLS_LAYOUT_PACKED) {
         FLS_CUDA(cudaMemcpyAsync(dst, pts, n * 16, cudaMemcpyHostToDevice, st));
     } else {
@@ -407,9 +408,9 @@ void upload_records(const void* pts, size_t n, size_t stride, float4* dst, DevBu
         FLS_CUDA(cudaMemcpyAsync(staging.p, pts, n * stride, cudaMemcpyHostToDevice, st));
         launch_repack(staging.p, n, stride, dst, st);
         FLS_CUDA(cudaGetLastError());
-        ++*launches;
+        ++c.launches;
     }
-    *h2d += (long long)(n * stride);
+    c.h2d += (long long)(n * stride);
 }
 
 void launch_transform_f(const float4* d_in, size_t n, const double* T, float4* d_out, cudaStream_t st) {
@@ -422,14 +423,14 @@ void launch_transform_f(const float4* d_in, size_t n, const double* T, float4* d
 // The build steps IvoxMap and SearchGrid share.  keys -> stable sort -> gather into dst (room for n) -> run-length encode ->
 // starts: the n points at pts in voxel-contiguous order; returns the voxel count.
 template <bool kFloor>
-static int sorted_runs(const float4* pts, size_t n, float inv_res, float4* dst, BuildScratch& sc, cudaStream_t st, int* launches) {
+static int sorted_runs(const float4* pts, size_t n, float inv_res, float4* dst, BuildScratch& sc, Call& c) {
     sc.reserve_runs<unsigned long long>(n);
-    voxel_keys_kernel<kFloor><<<grid_for(n, 256), 256, 0, st>>>(pts, n, inv_res, sc.keys.p, sc.idx.p);
-    sc.sort_pairs<unsigned long long>(n, 63, st);
-    gather_kernel<<<grid_for(n, 256), 256, 0, st>>>(pts, sc.idx_sorted.p, n, dst);
-    const int runs = sc.encode_runs<unsigned long long>(n, st);
-    sc.run_starts(runs, st);
-    *launches += 6;
+    voxel_keys_kernel<kFloor><<<grid_for(n, 256), 256, 0, c.stream>>>(pts, n, inv_res, sc.keys.p, sc.idx.p);
+    sc.sort_pairs<unsigned long long>(n, 63, c);
+    gather_kernel<<<grid_for(n, 256), 256, 0, c.stream>>>(pts, sc.idx_sorted.p, n, dst);
+    const int runs = sc.encode_runs<unsigned long long>(n, c);
+    sc.run_starts(runs, c);
+    c.launches += 6;
     return runs;
 }
 
@@ -441,28 +442,28 @@ void VoxelTable::size_for(size_t n, size_t factor, bool grow_only) {
     mask = (unsigned)(slots - 1);
 }
 
-void VoxelTable::clear(cudaStream_t st, int* launches) {
-    table_clear_kernel<<<grid_for(slots, 256), 256, 0, st>>>(buf.p, slots);
+void VoxelTable::clear(Call& c) {
+    table_clear_kernel<<<grid_for(slots, 256), 256, 0, c.stream>>>(buf.p, slots);
     FLS_CUDA(cudaGetLastError());
-    ++*launches;
+    ++c.launches;
 }
 
 // the table (sized) over the runs of sorted_runs
-static void fill_table(VoxelTable& table, int runs, const BuildScratch& sc, cudaStream_t st, int* launches) {
-    table.clear(st, launches);
-    ivox_insert_kernel<<<grid_for(runs, 256), 256, 0, st>>>(sc.uniq.p, sc.starts.p, sc.counts.p, runs, table.buf.p, table.mask);
+static void fill_table(VoxelTable& table, int runs, const BuildScratch& sc, Call& c) {
+    table.clear(c);
+    ivox_insert_kernel<<<grid_for(runs, 256), 256, 0, c.stream>>>(sc.uniq.p, sc.starts.p, sc.counts.p, runs, table.buf.p, table.mask);
     FLS_CUDA(cudaGetLastError());
-    *launches += 1;
+    c.launches += 1;
 }
 
-int SearchGrid::build(const float4* d_cloud, size_t n, BuildScratch& sc, cudaStream_t st, int* launches) {
+int SearchGrid::build(const float4* d_cloud, size_t n, BuildScratch& sc, Call& c) {
     n_pts = n_vox = 0;
     if (n == 0) return FLS_OK;
     if (n > 0xfffffff0ull) return FLS_ERR_INVALID_ARG;
     pts_sorted.reserve(n);
-    const int runs = sorted_runs<true>(d_cloud, n, 1.0f / res, pts_sorted.p, sc, st, launches);
+    const int runs = sorted_runs<true>(d_cloud, n, 1.0f / res, pts_sorted.p, sc, c);
     table.size_for((size_t)runs, 2);
-    fill_table(table, runs, sc, st, launches);
+    fill_table(table, runs, sc, c);
     n_pts = n;
     n_vox = (size_t)runs;
     return FLS_OK;
@@ -475,17 +476,18 @@ int SearchGrid::build(const float4* d_cloud, size_t n, BuildScratch& sc, cudaStr
 // redirected.  The space left behind is garbage until the next full build, which happens when the slack runs out, when a table
 // would exceed its load factor, when the garbage outweighs the live data, or when the LRU has to evict.
 // Returns 1 when the caller has to take the full path instead.
-int IvoxMap::append_incremental(const float4* d_new, size_t n_new, long long capacity, cudaStream_t st, int* launches) {
+int IvoxMap::append_incremental(const float4* d_new, size_t n_new, long long capacity, Call& c) {
     if (!incremental || n_pts == 0 || n_new == 0) return 1;
+    const cudaStream_t st = c.stream;
     BuildScratch& sc = scratch;
     const size_t S = (size_t)n_stencil;
     // new points -> voxel runs (stable: input order inside a voxel)
     sc.reserve_runs<unsigned long long>(n_new);
     sc.num_runs.reserve(4);
     voxel_keys_kernel<false><<<grid_for(n_new, 256), 256, 0, st>>>(d_new, n_new, inv_res, sc.keys.p, sc.idx.p);
-    sc.sort_pairs<unsigned long long>(n_new, 63, st);
-    const int T = sc.encode_runs<unsigned long long>(n_new, st);  // touched voxels
-    sc.run_starts(T, st);
+    sc.sort_pairs<unsigned long long>(n_new, 63, c);
+    const int T = sc.encode_runs<unsigned long long>(n_new, c);  // touched voxels
+    sc.run_starts(T, c);
     // plan: old location / length of every touched voxel, how many are created
     inc_old_start.reserve((size_t)T + 1);
     inc_old_count.reserve((size_t)T + 1);
@@ -517,8 +519,8 @@ int IvoxMap::append_incremental(const float4* d_new, size_t n_new, long long cap
     FLS_CUDA(cudaMemcpyAsync(&last_off, inc_new_off.p + (T - 1), sizeof(unsigned), cudaMemcpyDeviceToHost, st));
     FLS_CUDA(cudaMemcpyAsync(&last_cnt, inc_new_count.p + (T - 1), sizeof(unsigned), cudaMemcpyDeviceToHost, st));
     FLS_CUDA(cudaMemcpyAsync(&n_aff, sc.num_runs.p + 1, sizeof(int), cudaMemcpyDeviceToHost, st));
-    FLS_CUDA(cudaStreamSynchronize(st));
-    *launches += 9;
+    c.sync();
+    c.launches += 9;
     const int n_created = hc[0];
     const size_t moved = (size_t)last_off + last_cnt;  // points of the rewritten voxels
     // has to take the full path: eviction, no room, table load
@@ -539,12 +541,12 @@ int IvoxMap::append_incremental(const float4* d_new, size_t n_new, long long cap
     FLS_CUDA(cudaMemcpyAsync(hc, inc_cnt.p, 8 * sizeof(int), cudaMemcpyDeviceToHost, st));
     FLS_CUDA(cudaMemcpyAsync(&l_off, cstart.p + (n_aff - 1), sizeof(unsigned), cudaMemcpyDeviceToHost, st));
     FLS_CUDA(cudaMemcpyAsync(&l_cnt, ccount.p + (n_aff - 1), sizeof(unsigned), cudaMemcpyDeviceToHost, st));
-    FLS_CUDA(cudaStreamSynchronize(st));
+    c.sync();
     const size_t run_total = (size_t)l_off + l_cnt;
     const int n_new_centres = hc[0];
     unsigned long long old_records = 0;
     std::memcpy(&old_records, hc + 2, sizeof(old_records));
-    *launches += 5;
+    c.launches += 5;
     // From here on the point array and the occupied table are already updated; if the lists do not fit, the caller's full build
     // regenerates everything from pts_all (which it extends itself), so nothing is lost.
     if (lists_end + run_total > lists.cap || lists_end + run_total > 0xfffffff0ull) return 1;
@@ -553,7 +555,7 @@ int IvoxMap::append_incremental(const float4* d_new, size_t n_new, long long cap
     list_fill_kernel<<<grid_for((size_t)n_aff * 32, 256), 256, 0, st>>>(cuniq.p, n_aff, n_stencil, table.buf.p, table.mask, pts_sorted.p, cstart.p, ccount.p,
                                                                        lists.p, ctab.buf.p, ctab.mask);
     FLS_CUDA(cudaGetLastError());
-    *launches += 2;
+    c.launches += 2;
     // bookkeeping
     pts_end += moved;
     pts_garbage += moved - n_new;  // the old copies of the rewritten voxels
@@ -567,31 +569,31 @@ int IvoxMap::append_incremental(const float4* d_new, size_t n_new, long long cap
     return FLS_OK;
 }
 
-int IvoxMap::append_and_build(const float4* d_new, size_t n_new, long long capacity, cudaStream_t st, int* launches) {
+int IvoxMap::append_and_build(const float4* d_new, size_t n_new, long long capacity, Call& c) {
     // mapping mode: append without touching the rest of the map whenever that is possible
     if (incremental && n_pts > 0 && n_new > 0 && (lists_garbage < n_list + (n_list >> 1)) && (pts_garbage < 2 * n_pts)) {
         // pts_all / stamp_all first (the full path and the LRU read them)
         const size_t n_old0 = n_pts, n0 = n_old0 + n_new;
         if (n0 <= pts_all.cap && (capacity <= 0 || n0 <= stamp_all.cap)) {
-            FLS_CUDA(cudaMemcpyAsync(pts_all.p + n_old0, d_new, n_new * sizeof(float4), cudaMemcpyDeviceToDevice, st));
+            FLS_CUDA(cudaMemcpyAsync(pts_all.p + n_old0, d_new, n_new * sizeof(float4), cudaMemcpyDeviceToDevice, c.stream));
             if (capacity > 0) {
                 ++call_no;
-                ivox_stamp_kernel<<<grid_for(n_new, 256), 256, 0, st>>>(stamp_all.p + n_old0, n_new, call_no << 32);
+                ivox_stamp_kernel<<<grid_for(n_new, 256), 256, 0, c.stream>>>(stamp_all.p + n_old0, n_new, call_no << 32);
             }
-            const int rc = append_incremental(d_new, n_new, capacity, st, launches);
+            const int rc = append_incremental(d_new, n_new, capacity, c);
             if (rc == FLS_OK) return FLS_OK;
             if (rc < 0) return rc;
             // full path below: pts_all / stamp_all already hold the new points
-            return build_full(n_old0, n0, capacity, st, launches, /*appended=*/true);
+            return build_full(n_old0, n0, capacity, c, /*appended=*/true);
         }
     }
-    return build_full(n_pts, n_pts + n_new, capacity, st, launches, false, d_new, n_new);
+    return build_full(n_pts, n_pts + n_new, capacity, c, false, d_new, n_new);
 }
 
-int IvoxMap::build_full(size_t n_old, size_t n_in, long long capacity, cudaStream_t st, int* launches, bool appended, const float4* d_new,
-                        size_t n_new) {
+int IvoxMap::build_full(size_t n_old, size_t n_in, long long capacity, Call& c, bool appended, const float4* d_new, size_t n_new) {
     size_t n = n_in;
     if (n == 0) return FLS_OK;
+    const cudaStream_t st = c.stream;
     if (n > 0xfffffff0ull) return FLS_ERR_INVALID_ARG;
     const bool lru = capacity > 0;
     // grow pts_all (and the insertion stamps) preserving the old contents
@@ -599,7 +601,7 @@ int IvoxMap::build_full(size_t n_old, size_t n_in, long long capacity, cudaStrea
         DevBuf<float4> bigger;
         bigger.reserve(incremental ? 3 * n : n + n / 2);
         if (n_old) FLS_CUDA(cudaMemcpyAsync(bigger.p, pts_all.p, n_old * sizeof(float4), cudaMemcpyDeviceToDevice, st));
-        FLS_CUDA(cudaStreamSynchronize(st));
+        c.sync();
         std::swap(bigger.p, pts_all.p);
         std::swap(bigger.cap, pts_all.cap);
     }
@@ -607,7 +609,7 @@ int IvoxMap::build_full(size_t n_old, size_t n_in, long long capacity, cudaStrea
         DevBuf<unsigned long long> bigger;
         bigger.reserve(incremental ? 3 * n : n + n / 2);
         if (n_old) FLS_CUDA(cudaMemcpyAsync(bigger.p, stamp_all.p, n_old * sizeof(unsigned long long), cudaMemcpyDeviceToDevice, st));
-        FLS_CUDA(cudaStreamSynchronize(st));
+        c.sync();
         std::swap(bigger.p, stamp_all.p);
         std::swap(bigger.cap, stamp_all.cap);
     }
@@ -625,29 +627,30 @@ int IvoxMap::build_full(size_t n_old, size_t n_in, long long capacity, cudaStrea
     } else {
         pts_sorted.reserve(n);
     }
-    int runs = sorted_runs<false>(pts_all.p, n, inv_res, pts_sorted.p, scratch, st, launches);
+    int runs = sorted_runs<false>(pts_all.p, n, inv_res, pts_sorted.p, scratch, c);
     if (lru && (long long)runs >= capacity) {
         // IVoxMap::AddPoints would have evicted the LRU tail while inserting (ivox_map.cpp:133-136): drop those voxels' old points
         size_t n_after = n;
-        const int rc = evict_lru(n_old, n, runs, capacity, st, &n_after, launches);
+        const int rc = evict_lru(n_old, n, runs, capacity, c, &n_after);
         if (rc != FLS_OK) return rc;
         n = n_after;
-        runs = sorted_runs<false>(pts_all.p, n, inv_res, pts_sorted.p, scratch, st, launches);  // n only shrank: pts_sorted has room
+        runs = sorted_runs<false>(pts_all.p, n, inv_res, pts_sorted.p, scratch, c);  // n only shrank: pts_sorted has room
     }
     table.size_for((size_t)runs, incremental ? 4 : 2, incremental);  // mapping mode: room for the voxels to come
-    fill_table(table, runs, scratch, st, launches);
+    fill_table(table, runs, scratch, c);
     n_pts = n;
     n_vox = (size_t)runs;
     pts_end = n;
     pts_garbage = 0;
     ++n_full;
-    return build_stencil_lists(st, launches);
+    return build_stencil_lists(c);
 }
 
 // Exact LRU of IVoxMap::AddPoints for this call (see lru_simulate): a voxel's position in upstream's list is the insertion time of
 // its last point, so the stamps of the points are all the state there is.  Victims lose every point they held before the call;
 // one that is touched again later in the call keeps this call's points (it is created anew).  Compacts pts_all / stamp_all.
-int IvoxMap::evict_lru(size_t n_old, size_t n, int runs, long long capacity, cudaStream_t st, size_t* n_after, int* launches) {
+int IvoxMap::evict_lru(size_t n_old, size_t n, int runs, long long capacity, Call& c, size_t* n_after) {
+    const cudaStream_t st = c.stream;
     BuildScratch& sc = scratch;
     if (n_vox == 0) return FLS_ERR_CAPACITY;  // the first cloud alone overflows the capacity
     lru_first.reserve((size_t)runs + 1);
@@ -657,13 +660,13 @@ int IvoxMap::evict_lru(size_t n_old, size_t n, int runs, long long capacity, cud
     ivox_run_info_kernel<<<grid_for(runs, 256), 256, 0, st>>>(runs, sc.starts.p, sc.counts.p, sc.idx_sorted.p, stamp_all.p, (unsigned)n_old, lru_nold.p,
                                                             lru_first.p, eviction.stamps.reserve((size_t)runs + 1),
                                                             eviction.ids.reserve((size_t)runs + 1), sc.k32b.reserve(n + 1), lru_cnt.p);
-    ++*launches;
+    ++c.launches;
     int hc[4] = {0, 0, 0, 0};
     FLS_CUDA(cudaMemcpyAsync(hc, lru_cnt.p, 4 * sizeof(int), cudaMemcpyDeviceToHost, st));
-    FLS_CUDA(cudaStreamSynchronize(st));
+    c.sync();
     const int n_cand = hc[0], n_create = hc[1], n_touched = hc[2];
     if (n_cand == 0) return FLS_ERR_CAPACITY;
-    const int rc = eviction.run(n_cand, sc.k32b.p, n_create, n_touched, n_vox, capacity, sc.cub_tmp, st, launches,
+    const int rc = eviction.run(n_cand, sc.k32b.p, n_create, n_touched, n_vox, capacity, sc.cub_tmp, c,
                                 [&](const unsigned* runs_sorted, int K, unsigned* out) {
                                     ivox_cand_kernel<<<grid_for(K, 256), 256, 0, st>>>(runs_sorted, K, lru_first.p, out);
                                 });
@@ -687,11 +690,11 @@ int IvoxMap::evict_lru(size_t n_old, size_t n, int runs, long long capacity, cud
     cub_run(sc.cub_tmp, keep_pts);
     cub_run(sc.cub_tmp, keep_stamps);
     FLS_CUDA(cudaMemcpyAsync(sc.h_num_runs, sc.num_runs.p, sizeof(int), cudaMemcpyDeviceToHost, st));
-    FLS_CUDA(cudaStreamSynchronize(st));
+    c.sync();
     const size_t kept = (size_t)*sc.h_num_runs;
     FLS_CUDA(cudaMemcpyAsync(pts_all.p, pts_sorted.p, kept * sizeof(float4), cudaMemcpyDeviceToDevice, st));
     FLS_CUDA(cudaMemcpyAsync(stamp_all.p, sc.keys.p, kept * sizeof(unsigned long long), cudaMemcpyDeviceToDevice, st));
-    *launches += 4;
+    c.launches += 4;
     *n_after = kept;
     return FLS_OK;
 }
@@ -711,7 +714,8 @@ size_t IvoxMap::dump_keys(unsigned long long* h_out, size_t cap, cudaStream_t st
     return m;
 }
 
-int IvoxMap::build_stencil_lists(cudaStream_t st, int* launches) {
+int IvoxMap::build_stencil_lists(Call& c) {
+    const cudaStream_t st = c.stream;
     BuildScratch& sc = scratch;
     const size_t S = (size_t)n_stencil;
     const size_t n_keys = n_vox * S;
@@ -729,7 +733,7 @@ int IvoxMap::build_stencil_lists(cudaStream_t st, int* launches) {
     cub_run(sc.cub_tmp, sort);
     cub_run(sc.cub_tmp, unique);
     FLS_CUDA(cudaMemcpyAsync(sc.h_num_runs, sc.num_runs.p, sizeof(int), cudaMemcpyDeviceToHost, st));
-    FLS_CUDA(cudaStreamSynchronize(st));
+    c.sync();
     const int nc = *sc.h_num_runs;
     ccount.reserve((size_t)nc);
     cstart.reserve((size_t)nc);
@@ -743,7 +747,7 @@ int IvoxMap::build_stencil_lists(cudaStream_t st, int* launches) {
     } else {
         lists.reserve(total);
     }
-    ctab.clear(st, launches);
+    ctab.clear(c);
     list_fill_kernel<<<grid_for((size_t)nc * 32, 256), 256, 0, st>>>(cuniq.p, nc, n_stencil, table.buf.p, table.mask, pts_sorted.p, cstart.p, ccount.p,
                                                                      lists.p, ctab.buf.p, ctab.mask);
     FLS_CUDA(cudaGetLastError());
@@ -751,7 +755,7 @@ int IvoxMap::build_stencil_lists(cudaStream_t st, int* launches) {
     n_list = total;
     lists_end = total;
     lists_garbage = 0;
-    *launches += 6;
+    c.launches += 6;
     // the transient key arrays are the largest buffers of the build; give them back
     if (!incremental) {
         ckeys.release();
@@ -761,7 +765,8 @@ int IvoxMap::build_stencil_lists(cudaStream_t st, int* launches) {
 }
 
 int window_add(WindowMap& w, const float4* d_cloud, size_t n, size_t window, float leaf, bool filter_always, bool replace, BuildScratch& sc,
-               cudaStream_t st, int* launches) {
+               Call& call) {
+    const cudaStream_t st = call.stream;
     const float4* merged = d_cloud;
     size_t n_merged = n;
     size_t depth = 1;
@@ -772,7 +777,7 @@ int window_add(WindowMap& w, const float4* d_cloud, size_t n, size_t window, flo
         c->n = n;
         w.deque.push_back(std::move(c));
         if (w.deque.size() > window) {
-            FLS_CUDA(cudaStreamSynchronize(st));  // the evicted buffer may still feed a copy in flight
+            call.sync();  // the evicted buffer may still feed a copy in flight
             w.deque.pop_front();
         }
         n_merged = 0;
@@ -788,12 +793,12 @@ int window_add(WindowMap& w, const float4* d_cloud, size_t n, size_t window, flo
     }
     w.cloud.reserve(n_merged);
     if (filter_always || depth > 5) {
-        w.n = voxel_grid_device(merged, n_merged, leaf, w.cloud.p, sc, st, launches);
+        w.n = voxel_grid_device(merged, n_merged, leaf, w.cloud.p, sc, call);
     } else {
         if (n_merged) FLS_CUDA(cudaMemcpyAsync(w.cloud.p, merged, n_merged * sizeof(float4), cudaMemcpyDeviceToDevice, st));
         w.n = n_merged;
     }
-    return w.grid.build(w.cloud.p, w.n, sc, st, launches);
+    return w.grid.build(w.cloud.p, w.n, sc, call);
 }
 
 }  // namespace fls

@@ -1,5 +1,5 @@
-// fls_maps.h — host-side owners of the device-resident map structures (SearchGrid, IvoxMap, NdtMap, WindowMap).  Every builder adds
-// the kernels it launches to `*launches`.
+// fls_maps.h — host-side owners of the device-resident map structures (SearchGrid, IvoxMap, NdtMap, WindowMap).  Every builder runs
+// on the stream of the Call it is given and counts its launches and waits into it.
 #pragma once
 #include <deque>
 #include <functional>
@@ -39,9 +39,9 @@ struct LruEviction {
     size_t n_victims = 0, n_recreated = 0;
     std::vector<unsigned> h_first, h_create, h_victims;
     std::vector<unsigned char> h_recreated;
-    // write_first(ids_sorted, K, out) enqueues one kernel on st that writes the first touch of candidates 0..K-1 to out[0..K-1]
+    // write_first(ids_sorted, K, out) enqueues one kernel on c.stream that writes the first touch of candidates 0..K-1 to out[0..K-1]
     int run(int n_cand, const unsigned* d_create, int n_create, int n_touched, size_t size0, long long capacity, DevBuf<unsigned char>& cub_tmp,
-            cudaStream_t st, int* launches, const std::function<void(const unsigned*, int, unsigned*)>& write_first);
+            Call& c, const std::function<void(const unsigned*, int, unsigned*)>& write_first);
 };
 
 // Scratch shared by the sort / run-length passes of every map build and of the voxel-grid filter.
@@ -51,7 +51,7 @@ struct LruEviction {
 // sort idx -> idx_sorted and write counts and starts.  It is split in steps so that a caller can work between them:
 //   reserve_runs<K>(n)          the arrays, before the caller's key kernel fills the keys and idx
 //   sort_pairs<K>(n, end_bit)   sizes cub_tmp once for sort, encode and sum over n, then sorts
-//   encode_runs<K>(n)           encodes and returns the run count, read through h_num_runs after one stream wait
+//   encode_runs<K>(n)           encodes and returns the run count, read through h_num_runs after one wait
 //   run_starts(runs)            the exclusive sum of the run lengths
 struct BuildScratch {
     DevBuf<unsigned long long> keys, keys_sorted, uniq;
@@ -66,16 +66,14 @@ struct BuildScratch {
     template <class K>
     void reserve_runs(size_t n);
     template <class K>
-    void sort_pairs(size_t n, int end_bit, cudaStream_t st);
+    void sort_pairs(size_t n, int end_bit, Call& c);
     template <class K>
-    int encode_runs(size_t n, cudaStream_t st);
-    void run_starts(int runs, cudaStream_t st);
+    int encode_runs(size_t n, Call& c);
+    void run_starts(int runs, Call& c);
 };
 
-// K7: VoxelGridCloud on the device.  d_out must hold n records; returns the output count.  `waits` (optional) counts the
-// stream synchronisations the call made.
-size_t voxel_grid_device(const float4* d_pts, size_t n, float leaf, float4* d_out, BuildScratch& sc, cudaStream_t st, int* launches,
-                         int* waits = nullptr);
+// K7: VoxelGridCloud on the device.  d_out must hold n records; returns the output count.
+size_t voxel_grid_device(const float4* d_pts, size_t n, float leaf, float4* d_out, BuildScratch& sc, Call& c);
 
 // Open-addressing table of HashSlot {key, start, count}, linear probing: table_find reads it, table_claim inserts (fls_common.cuh).
 // A power of two of at least 1024 slots.
@@ -85,7 +83,7 @@ struct VoxelTable {
     size_t slots = 0;
     // room for n keys at `factor` slots per key; grow_only (mapping mode) keeps a larger table as it is, for the keys to come
     void size_for(size_t n, size_t factor, bool grow_only = false);
-    void clear(cudaStream_t st, int* launches);  // every slot empty; one kernel
+    void clear(Call& c);  // every slot empty; one kernel
 };
 
 // Uniform search grid over a cloud for the exact 1-NN of IcpOptimized / GetFitnessScore and the exact 5-NN of the kd-tree LOAM
@@ -103,7 +101,7 @@ struct SearchGrid {
     DevBuf<float4> pts_sorted;
     VoxelTable table;
     // rebuilds the grid over the n points at d_cloud (an empty cloud leaves it empty and launches nothing); returns fls_status
-    int build(const float4* d_cloud, size_t n, BuildScratch& sc, cudaStream_t st, int* launches);
+    int build(const float4* d_cloud, size_t n, BuildScratch& sc, Call& c);
     GridView view() const { return {pts_sorted.p, table.buf.p, table.mask, 1.0f / res, res, (unsigned)n_pts}; }
     size_t bytes() const { return pts_sorted.bytes() + table.buf.bytes(); }
 };
@@ -142,13 +140,12 @@ struct IvoxMap {
         inv_res = 1.0f / r;
     }
     void clear() { n_pts = n_vox = n_centers = n_list = 0; }
-    int evict_lru(size_t n_old, size_t n, int runs, long long capacity, cudaStream_t st, size_t* n_after, int* launches);
+    int evict_lru(size_t n_old, size_t n, int runs, long long capacity, Call& c, size_t* n_after);
     size_t dump_keys(unsigned long long* h_out, size_t cap, cudaStream_t st);  // packed keys of the occupied voxels (tests)
     // append n points that are already on the device (packed float4) and rebuild; returns fls_status
-    int append_and_build(const float4* d_new, size_t n_new, long long capacity, cudaStream_t st, int* launches);
-    int build_full(size_t n_old, size_t n_in, long long capacity, cudaStream_t st, int* launches, bool appended, const float4* d_new = nullptr,
-                   size_t n_new = 0);
-    int append_incremental(const float4* d_new, size_t n_new, long long capacity, cudaStream_t st, int* launches);
+    int append_and_build(const float4* d_new, size_t n_new, long long capacity, Call& c);
+    int build_full(size_t n_old, size_t n_in, long long capacity, Call& c, bool appended, const float4* d_new = nullptr, size_t n_new = 0);
+    int append_incremental(const float4* d_new, size_t n_new, long long capacity, Call& c);
     // log-structured state of the incremental path (mapping mode)
     bool incremental = false;          // set by the owner: the map grows by small inserts (mapping mode)
     size_t pts_end = 0, pts_garbage = 0;      // used part of pts_sorted, dead records in it
@@ -156,7 +153,7 @@ struct IvoxMap {
     size_t n_incremental = 0, n_full = 0;     // how many inserts took which path
     DevBuf<unsigned> inc_old_start, inc_old_count, inc_new_count, inc_new_off;
     DevBuf<int> inc_cnt;  // created voxels, then new centres and (u64 at [2]) the records of the centre runs they replace
-    int build_stencil_lists(cudaStream_t st, int* launches);
+    int build_stencil_lists(Call& c);
     size_t bytes() const { return pts_all.bytes() + pts_sorted.bytes() + table.buf.bytes() + lists.bytes() + ctab.buf.bytes(); }
 };
 
@@ -210,13 +207,13 @@ struct NdtMap {
 
     void configure(double voxel_size, int min_points, int max_points, long long cap);
     // evict the LRU tail exactly as upstream's sequential insert would (incremental_ndt.h:203-206), n_vox net of it; called by add_cloud
-    int evict_lru(int runs, int n_new, int n_touched, cudaStream_t st, int* launches);
+    int evict_lru(int runs, int n_new, int n_touched, Call& c);
     // packed voxel keys of the live voxels (tests); returns how many
     size_t dump_keys(unsigned long long* h_out, size_t cap, cudaStream_t st);
     // every live voxel with its mean, information and counters, in device order (tests)
     void dump_voxels(std::vector<fls_ndt_voxel>& out, cudaStream_t st);
     // VoxelGridCloud(cloud, leaf) then insert/update voxels; `first_scan` = flag_first_scan_ upstream
-    int add_cloud(const float4* d_cloud, size_t n, float leaf, bool first_scan, cudaStream_t st, int* launches);
+    int add_cloud(const float4* d_cloud, size_t n, float leaf, bool first_scan, Call& c);
     NdtView view() const {
         NdtView v;
         v.tab = table.buf.p;
@@ -244,7 +241,7 @@ struct WindowMap {
 // Adds a device cloud to w (replace: the window is that cloud alone) and rebuilds it.  filter_always false: VoxelGrid(leaf) only
 // once the window holds more than 5 clouds (loam_full_kdtree.h:91-99).
 int window_add(WindowMap& w, const float4* d_cloud, size_t n, size_t window, float leaf, bool filter_always, bool replace, BuildScratch& sc,
-               cudaStream_t st, int* launches);
+               Call& call);
 
 // K4: LOAM feature extraction on the projector's arrays (host in / host out); see fls_features.cu
 int extract_features_device(int device, const float* depth, const int* col, size_t n, const int* row_start, const int* row_end, int n_rows,
@@ -262,10 +259,9 @@ int project_device(int device, const void* raw, const int* ring, const float* ti
 // PreProcessing::Run, non-feature branch (preprocessing.cpp:181-225): raw x,y,z,intensity,time records -> ordered + planar clouds (host)
 int preprocess_device(int device, const float* raw_xyzit, size_t n, const fls_imu_buffer* imu, float min_d, float max_d, int jump_span, float leaf,
                       float* ordered_out, size_t* n_ordered, float* planar_out, size_t* n_planar);
-// Copies n host records of `stride` bytes (stride_ok) to packed float4 at dst on st: one copy when they are packed already, else a
-// copy to `staging` and one repack kernel.  Adds the bytes copied to *h2d and the kernel to *launches.
-void upload_records(const void* pts, size_t n, size_t stride, float4* dst, DevBuf<unsigned char>& staging, cudaStream_t st, long long* h2d,
-                    int* launches);
+// Copies n host records of `stride` bytes (stride_ok) to packed float4 at dst on c.stream: one copy when they are packed already, else
+// a copy to `staging` and one repack kernel.  Counts the bytes copied and the kernel.
+void upload_records(const void* pts, size_t n, size_t stride, float4* dst, DevBuf<unsigned char>& staging, Call& c);
 // TransformPointCloud(cloud, Mat4d) with R, t cast to float first (pointcloud_utility.h:141-158 upstream); T column-major
 void launch_transform_f(const float4* d_in, size_t n, const double* T_colmajor, float4* d_out, cudaStream_t st);
 void launch_transform_d(const float4* d_in, size_t n, const double* T_colmajor, float4* d_out, cudaStream_t st);

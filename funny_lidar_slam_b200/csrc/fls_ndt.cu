@@ -413,10 +413,11 @@ void NdtMap::configure(double voxel_size, int min_points, int max_points, long l
     capacity = cap;
 }
 
-int NdtMap::add_cloud(const float4* d_cloud, size_t n, float leaf, bool first_scan, cudaStream_t st, int* launches) {
+int NdtMap::add_cloud(const float4* d_cloud, size_t n, float leaf, bool first_scan, Call& c) {
     if (n == 0) return FLS_OK;
+    const cudaStream_t st = c.stream;
     filtered.reserve(n);
-    const size_t nf = voxel_grid_device(d_cloud, n, leaf, filtered.p, scratch, st, launches);  // :186
+    const size_t nf = voxel_grid_device(d_cloud, n, leaf, filtered.p, scratch, c);  // :186
     if (nf == 0) return FLS_OK;
     if (table.slots == 0) {  // first use: size everything by the configured capacity
         table.size_for((size_t)capacity, 2);
@@ -425,14 +426,14 @@ int NdtMap::add_cloud(const float4* d_cloud, size_t n, float leaf, bool first_sc
         carry.reserve((size_t)capacity * (size_t)(min_pts > 0 ? min_pts : 1) * 3);
         counter.reserve(kCounters);
         FLS_CUDA(cudaMemsetAsync(counter.p, 0, kCounters * sizeof(int), st));
-        table.clear(st, launches);
+        table.clear(c);
     }
     BuildScratch& sc = scratch;
     sc.reserve_runs<unsigned long long>(nf);
     ndt_keys_kernel<<<grid_for(nf, 256), 256, 0, st>>>(filtered.p, nf, inv_voxel, sc.keys.p, sc.idx.p);
-    sc.sort_pairs<unsigned long long>(nf, 63, st);
-    const int runs = sc.encode_runs<unsigned long long>(nf, st);
-    sc.run_starts(runs, st);
+    sc.sort_pairs<unsigned long long>(nf, 63, c);
+    const int runs = sc.encode_runs<unsigned long long>(nf, c);
+    sc.run_starts(runs, c);
     // ---- LRU bookkeeping: which touched voxels exist, how many are created, who has to go first --------------------------------
     const int hi_water0 = hi_water;
     run_vi.reserve((size_t)runs + 1);
@@ -443,13 +444,13 @@ int NdtMap::add_cloud(const float4* d_cloud, size_t n, float leaf, bool first_sc
     ndt_lookup_kernel<<<grid_for(runs, 256), 256, 0, st>>>(runs, sc.uniq.p, table.buf.p, table.mask, run_vi.p, touch_run.p, counter.p);
     int hc[kCounters] = {};
     FLS_CUDA(cudaMemcpyAsync(hc, counter.p, sizeof(hc), cudaMemcpyDeviceToHost, st));
-    FLS_CUDA(cudaStreamSynchronize(st));
-    *launches += 1;
+    c.sync();
+    c.launches += 1;
     const int n_new = hc[kCreations], n_touched = hc[kTouched];
     ++call_no;
     // upstream: after every creation `if (data_.size() >= capacity_) pop_back()` (:203-206) — the list never holds `capacity` voxels
     if ((long long)n_vox + n_new >= capacity) {
-        const int rc = evict_lru(runs, n_new, n_touched, st, launches);
+        const int rc = evict_lru(runs, n_new, n_touched, c);
         if (rc != FLS_OK) return rc;
     }
     NdtUpdateArgs ua;
@@ -476,8 +477,8 @@ int NdtMap::add_cloud(const float4* d_cloud, size_t n, float leaf, bool first_sc
     ndt_update_kernel<<<grid_for(runs, 128), 128, 0, st>>>(ua, counter.p + kOverflow);
     int h[3] = {0, 0, 0};  // up to the free-stack cursor
     FLS_CUDA(cudaMemcpyAsync(h, counter.p, 3 * sizeof(int), cudaMemcpyDeviceToHost, st));
-    FLS_CUDA(cudaStreamSynchronize(st));
-    *launches += 6;
+    c.sync();
+    c.launches += 6;
     hi_water = h[kHiWater];
     n_free -= h[kFreeCursor] < n_free ? h[kFreeCursor] : n_free;  // the creations popped that many indices off the free stack
     n_vox += (size_t)n_new;
@@ -487,7 +488,8 @@ int NdtMap::add_cloud(const float4* d_cloud, size_t n, float leaf, bool first_sc
 
 // Evicts what upstream's sequential insert would evict during this call (exact, including a victim that is touched again later in
 // the call): candidates = live voxels by ascending stamp, simulated on the host against the creation times of the new voxels.
-int NdtMap::evict_lru(int runs, int n_new, int n_touched, cudaStream_t st, int* launches) {
+int NdtMap::evict_lru(int runs, int n_new, int n_touched, Call& c) {
+    const cudaStream_t st = c.stream;
     BuildScratch& sc = scratch;
     const int hw = hi_water;
     const size_t n_live = n_vox;
@@ -496,8 +498,8 @@ int NdtMap::evict_lru(int runs, int n_new, int n_touched, cudaStream_t st, int* 
                                                        counter.p + kLiveCursor);
     ndt_create_times_kernel<<<grid_for(runs, 256), 256, 0, st>>>(runs, run_vi.p, sc.starts.p, sc.idx_sorted.p, sc.k32b.reserve((size_t)n_new + 1),
                                                                 counter.p + kCreateCursor);
-    *launches += 2;
-    const int rc = eviction.run((int)n_live, sc.k32b.p, n_new, n_touched, n_live, capacity, sc.cub_tmp, st, launches,
+    c.launches += 2;
+    const int rc = eviction.run((int)n_live, sc.k32b.p, n_new, n_touched, n_live, capacity, sc.cub_tmp, c,
                                 [&](const unsigned* vis_sorted, int K, unsigned* out) {
                                     ndt_cand_kernel<<<grid_for(K, 256), 256, 0, st>>>(vis_sorted, K, touch_run.p, sc.starts.p, sc.idx_sorted.p, out);
                                 });
@@ -509,9 +511,9 @@ int NdtMap::evict_lru(int runs, int n_new, int n_touched, cudaStream_t st, int* 
     ndt_evict_kernel<<<grid_for(n_victims, 128), 128, 0, st>>>(eviction.victims.p, eviction.recreated.p, n_victims, eviction.ids_sorted.p, cold.p,
                                                               free_list.p, n_free, touch_run.p, run_vi.p);
     n_free += n_victims;
-    table.clear(st, launches);
+    table.clear(c);
     ndt_table_rebuild_kernel<<<grid_for(hw, 256), 256, 0, st>>>(cold.p, hw, table.buf.p, table.mask);
-    *launches += 2;
+    c.launches += 2;
     return FLS_OK;
 }
 
@@ -557,10 +559,10 @@ class NdtPlugin final : public Plugin {
 
     int add_cloud(const float4* d_cloud, size_t n, const float4*, size_t) override {
         const fls_config& cfg = h.cfg;
-        const int rc = map.add_cloud(d_cloud, n, cfg.source_cloud_filter_size, first_scan, h.stream, &h.launches);
+        const int rc = map.add_cloud(d_cloud, n, cfg.source_cloud_filter_size, first_scan, h.call);
         if (cfg.localization_mode && rc == FLS_OK) {
             // kdtree_flann_.setInputCloud(cloud_world) — the voxel-filtered cloud (incremental_ndt.h:188-190)
-            const size_t nf = voxel_grid_device(d_cloud, n, cfg.source_cloud_filter_size, map.filtered.p, map.scratch, h.stream, &h.launches);
+            const size_t nf = voxel_grid_device(d_cloud, n, cfg.source_cloud_filter_size, map.filtered.p, map.scratch, h.call);
             h.set_fit_cloud(map.filtered.p, nf);
         }
         first_scan = cfg.localization_mode != 0;  // :222-226
@@ -571,7 +573,7 @@ class NdtPlugin final : public Plugin {
         const fls_config& cfg = h.cfg;
         if (map.n_vox == 0) return FLS_ERR_NO_MAP;  // CHECK(!grids_.empty())
         scan.reserve(n_in);
-        const size_t n = voxel_grid_device(d_in, n_in, cfg.source_cloud_filter_size, scan.p, h.scratch, h.stream, &h.launches, &h.waits);  // :232
+        const size_t n = voxel_grid_device(d_in, n_in, cfg.source_cloud_filter_size, scan.p, h.scratch, h.call);  // :232
         const int ni = (int)n;
         const int grid = ndt_grid(ni, cfg.device);
         double T_in[16];
@@ -585,12 +587,12 @@ class NdtPlugin final : public Plugin {
         // roofline accounting (SURVEY.md §8d, K2): 16 B source point + 7 x 16 B slot probes per point-iteration,
         // 80 B voxel record per estimated voxel hit; the 6x6 sums are fused (no per-point output).
         h.match_single(FLS_NDT, cfg.ndt_min_effective_pts, grid, 16 + 16LL * 7, 80, scan.p, n, n, T, converged, st,
-                       [&](const GnLoopCtl& ctl) { launch_ndt_loop(a, ctl, grid, h.stream); });
+                       [&](const GnLoopCtl& ctl) { launch_ndt_loop(a, ctl, grid, h.call.stream); });
         if (!h.h_state.p->failed && !cfg.localization_mode) {
             // :326-330 — the scan enters the map transformed by the INPUT guess T, not the optimised pose  [quirk 6]
             ins.reserve(n);
-            launch_transform_f(scan.p, n, T_in, ins.p, h.stream);
-            h.launches++;
+            launch_transform_f(scan.p, n, T_in, ins.p, h.call.stream);
+            h.call.launches++;
             return h.inserted(add_cloud(ins.p, n, nullptr, 0), st);
         }
         return FLS_OK;
@@ -621,7 +623,7 @@ class NdtPlugin final : public Plugin {
                                              a.outlier_thres = cfg.ndt_outlier_thres;
                                              a.state = h.state.p + s;
                                          },
-                                         [&](const GnBatchItem<NdtArgs>* d_items, int grid) { launch_ndt_batch(d_items, B, grid, h.stream); });
+                                         [&](const GnBatchItem<NdtArgs>* d_items, int grid) { launch_ndt_batch(d_items, B, grid, h.call.stream); });
     }
 
     void map_info(fls_map_info* out) const override {
@@ -633,14 +635,14 @@ class NdtPlugin final : public Plugin {
     int voxel_keys(std::vector<unsigned long long>& packed, size_t cap, size_t* n) override {
         FLS_CUDA(cudaSetDevice(h.cfg.device));
         packed.resize(cap + 1);
-        packed.resize(map.dump_keys(packed.data(), cap, h.stream));
+        packed.resize(map.dump_keys(packed.data(), cap, h.call.stream));
         *n = map.n_vox;
         return FLS_OK;
     }
 
     int ndt_voxels(std::vector<fls_ndt_voxel>& out) override {
         FLS_CUDA(cudaSetDevice(h.cfg.device));
-        map.dump_voxels(out, h.stream);
+        map.dump_voxels(out, h.call.stream);
         return FLS_OK;
     }
 };

@@ -446,17 +446,19 @@ struct IvoxBatchTable {
 // Per-batch preparation: state init, flag and ticket reset and the locality order of every scan, in one launch of one block per
 // tile (one block for an empty batch).  d_tbl: the batch's table on the device; d_zero[n_zero]: words zeroed on the way (v9 tickets).
 static void prepare_queries(const IvoxBatchTable* d_tbl, int n_tiles, int n_scans, GnState* d_states, const IvoxView& map, unsigned char* d_flags,
-                            float4* d_sorted, unsigned* d_zero, int n_zero, cudaStream_t st, int* launches) {
-    p2plane_prep_kernel<<<n_tiles > 0 ? n_tiles : 1, kOrdThreads, 0, st>>>(d_tbl->ptr, d_tbl->off, d_tbl->tile_off, n_scans, d_tbl->pose, map.inv_res,
-                                                                          d_zero, n_zero, d_flags, d_states, d_sorted, map.ctab, map.cmask, map.lists);
-    if (launches) *launches += 1;
+                            float4* d_sorted, unsigned* d_zero, int n_zero, Call& c) {
+    p2plane_prep_kernel<<<n_tiles > 0 ? n_tiles : 1, kOrdThreads, 0, c.stream>>>(d_tbl->ptr, d_tbl->off, d_tbl->tile_off, n_scans, d_tbl->pose,
+                                                                                map.inv_res, d_zero, n_zero, d_flags, d_states, d_sorted, map.ctab,
+                                                                                map.cmask, map.lists);
+    c.launches += 1;
 }
 
 // The Match-internal AddCloudToLocalMap of mapping mode: classifies and compacts the points that enter the map (d_world, d_out: n
-// records).  Returns the number of points selected for insertion (class 1 then class 2, input order) in d_out; synchronises the stream.
+// records).  Returns the number of points selected for insertion (class 1 then class 2, input order) in d_out; waits once.
 static size_t select_ivox_inserts(const IvoxView& map, const float4* d_src, int n, const GnPose& prev, const GnPose& fin, double filter, float4* d_world,
-                                  float4* d_out, BuildScratch& sc, cudaStream_t st, int* launches) {
+                                  float4* d_out, BuildScratch& sc, Call& c) {
     if (n <= 0) return 0;
+    const cudaStream_t st = c.stream;
     sc.minmax.reserve((size_t)n / 4 + 16);  // class bytes
     unsigned char* cls = reinterpret_cast<unsigned char*>(sc.minmax.p);
     sc.keys.reserve((size_t)n + 1);
@@ -469,8 +471,8 @@ static size_t select_ivox_inserts(const IvoxView& map, const float4* d_src, int 
     ivox_insert_scatter_kernel<<<(n + 255) / 256, 256, 0, st>>>(cls, sc.keys_sorted.p, n, d_world, d_out, d_total);
     unsigned long long total = 0;
     FLS_CUDA(cudaMemcpyAsync(&total, d_total, sizeof(total), cudaMemcpyDeviceToHost, st));
-    FLS_CUDA(cudaStreamSynchronize(st));
-    if (launches) *launches += 4;
+    c.sync();
+    c.launches += 4;
     return (size_t)(total & 0xffffffffull) + (size_t)(total >> 32);
 }
 
@@ -499,13 +501,13 @@ class IvoxPlugin final : public Plugin {
         return {map.pts_sorted.p, map.table.buf.p, map.table.mask, map.inv_res, max_range2, map.n_stencil, map.lists.p, map.ctab.buf.p, map.ctab.mask,
                 fast_knn};
     }
-    int append(const float4* d, size_t n) { return map.append_and_build(d, n, h.cfg.ivox_capacity, h.stream, &h.launches); }
+    int append(const float4* d, size_t n) { return map.append_and_build(d, n, h.cfg.ivox_capacity, h.call); }
 
     // everything of a batch up to the asynchronous read-back of the states: nothing here waits for the device
     int enqueue(int B, const float4* const* d_scans, const size_t* n, const double* T) {
         if (map.n_pts == 0) return FLS_ERR_NO_MAP;
         const int device = h.cfg.device;
-        cudaStream_t stream = h.stream;
+        cudaStream_t stream = h.call.stream;
         int off[kMaxBatch + 1];
         off[0] = 0;
         int grid = 1;
@@ -558,7 +560,7 @@ class IvoxPlugin final : public Plugin {
         }
         t.off[B] = off[B];
         FLS_CUDA(cudaMemcpyAsync(d_tbl.p, &t, sizeof(t), cudaMemcpyHostToDevice, stream));
-        h.h2d_bytes += (long long)sizeof(t);
+        h.call.h2d += (long long)sizeof(t);
         // chunk tickets of v9's dynamic work distribution: one counter per (scan, iteration) + the watchdog's abort word, zeroed by
         // the prep kernel
         const int ticket_stride = h.cfg.max_iterations + 2;
@@ -567,7 +569,7 @@ class IvoxPlugin final : public Plugin {
         // ONE prep kernel for the whole batch (state init, flag and ticket reset): every tile of a scan ends up in Morton order of the
         // voxel its points fall into at the initial pose (locality only: the sums are order-free up to fp64 rounding, and the
         // persistent per-point records live in the same order for the whole Match)
-        prepare_queries(d_t, t.tile_off[B], B, h.state.p, view(), flags.p, queries.p, use_v9 ? tickets.p : nullptr, n_tickets, stream, &h.launches);
+        prepare_queries(d_t, t.tile_off[B], B, h.state.p, view(), flags.p, queries.p, use_v9 ? tickets.p : nullptr, n_tickets, h.call);
         P2PlaneLoopArgs a;
         a.map = view();
         a.plane_thres = h.cfg.point_to_planar_thres;
@@ -604,7 +606,7 @@ class IvoxPlugin final : public Plugin {
     int finish(double* T, int* converged, fls_match_stats* st) {
         const int B = (int)pend_n.size();
         if (B < 1) return FLS_ERR_INVALID_ARG;
-        h.end_call(st);
+        h.call.end(st);
         if (pend_v9 && *h_abort.p) {
             pend_n.clear();
             set_last_error("p2plane_v9_kernel: watchdog — a wait loop gave up after 4 s (hand-over protocol error)");
@@ -659,7 +661,7 @@ class IvoxPlugin final : public Plugin {
             ins.reserve(n + 1);
             ins_world.reserve(n + 1);
             const size_t n_add = select_ivox_inserts(view(), d_src, (int)n, prev, gn_pose(T), 0.5 /* filter_size_map_min_ (:351) */, ins_world.p,
-                                                     ins.p, h.scratch, h.stream, &h.launches);
+                                                     ins.p, h.scratch, h.call);
             return h.inserted(append(ins.p, n_add), st);
         }
         return FLS_OK;
@@ -694,14 +696,14 @@ class IvoxPlugin final : public Plugin {
     int voxel_keys(std::vector<unsigned long long>& packed, size_t cap, size_t* n) override {
         FLS_CUDA(cudaSetDevice(h.cfg.device));
         packed.resize(cap + 1);
-        packed.resize(map.dump_keys(packed.data(), cap, h.stream));
+        packed.resize(map.dump_keys(packed.data(), cap, h.call.stream));
         *n = map.n_vox;
         return FLS_OK;
     }
 
     int map_points(float* xyzi, size_t cap, size_t* n) override {
         FLS_CUDA(cudaSetDevice(h.cfg.device));
-        FLS_CUDA(cudaStreamSynchronize(h.stream));
+        FLS_CUDA(cudaStreamSynchronize(h.call.stream));
         const size_t m = map.n_pts < cap ? map.n_pts : cap;
         if (m) FLS_CUDA(cudaMemcpy(xyzi, map.pts_all.p, m * sizeof(float4), cudaMemcpyDeviceToHost));
         *n = map.n_pts;
@@ -716,10 +718,10 @@ class IvoxPlugin final : public Plugin {
         DevBuf<int> d_found;
         d_out.reserve(n * 5);
         d_found.reserve(n);
-        if (n > 0) ivox_knn_test_kernel<<<(unsigned)((n + 127) / 128), 128, 0, h.stream>>>(view(), dq, (int)n, d_out.p, d_found.p);
-        FLS_CUDA(cudaMemcpyAsync(out_pts, d_out.p, n * 5 * sizeof(float4), cudaMemcpyDeviceToHost, h.stream));
-        FLS_CUDA(cudaMemcpyAsync(out_count, d_found.p, n * sizeof(int), cudaMemcpyDeviceToHost, h.stream));
-        h.end_call(nullptr);
+        if (n > 0) ivox_knn_test_kernel<<<(unsigned)((n + 127) / 128), 128, 0, h.call.stream>>>(view(), dq, (int)n, d_out.p, d_found.p);
+        FLS_CUDA(cudaMemcpyAsync(out_pts, d_out.p, n * 5 * sizeof(float4), cudaMemcpyDeviceToHost, h.call.stream));
+        FLS_CUDA(cudaMemcpyAsync(out_count, d_found.p, n * sizeof(int), cudaMemcpyDeviceToHost, h.call.stream));
+        h.call.end(nullptr);
         return FLS_OK;
     }
 
@@ -727,7 +729,7 @@ class IvoxPlugin final : public Plugin {
     int ivox_add_points(const void* pts, size_t n, size_t stride) override {
         h.begin_call();
         const int rc = append(h.upload(pts, n, stride, h.up_cloud), n);
-        h.end_call(nullptr);
+        h.call.end(nullptr);
         return rc;
     }
 };

@@ -190,13 +190,14 @@ bool sc_cfg_ok(const fls_sc_cfg& c) {
 }
 
 size_t PlaceIndex::describe(const fls_sc_cfg& c, const float4* arena, const std::vector<unsigned long long>& begin, const std::vector<unsigned>& count,
-                          const float4* d_query, size_t n_query, bool with_query, cudaStream_t st, int* launches, long long* h2d) {
+                          const float4* d_query, size_t n_query, bool with_query, Call& call) {
     if (std::memcmp(&c, &cfg, sizeof(c)) != 0) {  // bitwise: z_offset -0.0 and +0.0 give different cells for z = -0.0
         cfg = c;
         described = 0;
     }
     const size_t K = count.size(), first = described, last = K + (with_query ? 1 : 0);
     if (first == last) return 0;
+    const cudaStream_t st = call.stream;
     const size_t NC = n_cells(), S = (size_t)cfg.n_sectors;
     // descriptors the buffers hold at this cfg: they were sized for the cfg of their last growth, which may have had fewer cells
     const size_t held = std::min(cells.cap / NC, norms.cap / S);
@@ -216,7 +217,7 @@ size_t PlaceIndex::describe(const fls_sc_cfg& c, const float4* arena, const std:
     const size_t off_tiles = align16(n_segs * sizeof(ScSeg)), bytes = off_tiles + n_tiles * sizeof(ScTile);
     const ScGeom g = geom(cfg);
     FLS_CUDA(cudaMemsetAsync(cells.p + first * NC, 0, n_segs * NC * sizeof(unsigned), st));
-    ++*launches;
+    ++call.launches;
     if (n_tiles) {
         unsigned char* h = h_table.reserve(bytes);
         ScSeg* hs = reinterpret_cast<ScSeg*>(h);
@@ -230,20 +231,21 @@ size_t PlaceIndex::describe(const fls_sc_cfg& c, const float4* arena, const std:
         }
         table.reserve(bytes);
         FLS_CUDA(cudaMemcpyAsync(table.p, h, bytes, cudaMemcpyHostToDevice, st));
-        *h2d += (long long)bytes;
+        call.h2d += (long long)bytes;
         sc_bin_kernel<<<(unsigned)n_tiles, kThreads, 0, st>>>(reinterpret_cast<const ScSeg*>(table.p),
                                                                reinterpret_cast<const ScTile*>(table.p + off_tiles), g, cells.p);
         FLS_CUDA(cudaGetLastError());
-        ++*launches;
+        ++call.launches;
     }
     sc_finalize_kernel<<<grid_for(n_segs * S, 128), 128, 0, st>>>(cells.p, norms.p, first, n_segs, g);
     FLS_CUDA(cudaGetLastError());
-    ++*launches;
+    ++call.launches;
     described = K;
     return n_pts;
 }
 
-void PlaceIndex::search(size_t q, size_t n_cand, size_t n_out, fls_place_match* h_out, cudaStream_t st, int device, int* launches) {
+void PlaceIndex::search(size_t q, size_t n_cand, size_t n_out, fls_place_match* h_out, Call& call, int device) {
+    const cudaStream_t st = call.stream;
     const ScGeom g = geom(cfg);
     const size_t base = search_smem(0, g), per = search_smem(1, g) - base;
     const int tile = (int)std::min<size_t>(kMaxSearchTile, std::max<size_t>(1, (kSearchSmem - base) / per));
@@ -256,11 +258,11 @@ void PlaceIndex::search(size_t q, size_t n_cand, size_t n_out, fls_place_match* 
     sc_search_kernel<<<grid_for(n_cand, tile), kThreads, smem, st>>>(desc(0), norms.p, q, (unsigned)n_cand, tile, g, sc.keys.p, sc.idx.p, dist.p,
                                                                      shift.p);
     FLS_CUDA(cudaGetLastError());
-    sc.sort_pairs<unsigned long long>(n_cand, 64, st);
+    sc.sort_pairs<unsigned long long>(n_cand, 64, call);
     sc_pick_kernel<<<grid_for(n_out, 128), 128, 0, st>>>(sc.idx_sorted.p, dist.p, shift.p, (int)n_out, cfg.n_sectors, pick.p);
     FLS_CUDA(cudaGetLastError());
     FLS_CUDA(cudaMemcpyAsync(h_out, pick.p, n_out * sizeof(fls_place_match), cudaMemcpyDeviceToHost, st));
-    *launches += 3;
+    call.launches += 3;
 }
 
 }  // namespace fls

@@ -30,13 +30,13 @@ struct PlaceIndex {
     size_t n_cells() const { return (size_t)cfg.n_rings * cfg.n_sectors; }
     const float* desc(size_t slot) const { return reinterpret_cast<const float*>(cells.p) + slot * n_cells(); }
     // Describes what is not described for c yet: keyframes [described, K) of the arena and, when with_query, the n_query packed
-    // records at d_query into slot K.  Enqueued on st (no wait): a memset, the binning kernel when any point is read, the finalize.
-    // Returns the points read.
+    // records at d_query into slot K.  Enqueued on call.stream (no wait): a memset, the binning kernel when any point is read, the
+    // finalize.  Returns the points read.
     size_t describe(const fls_sc_cfg& c, const float4* arena, const std::vector<unsigned long long>& begin, const std::vector<unsigned>& count,
-                  const float4* d_query, size_t n_query, bool with_query, cudaStream_t st, int* launches, long long* h2d);
+                  const float4* d_query, size_t n_query, bool with_query, Call& call);
     // Ranks candidates [0, n_cand) against the descriptor in slot q by (D, id) and enqueues the copy of the first n_out records to
     // h_out (pinned).  n_cand > 0.  Three launches: the search, the sort, the pick.
-    void search(size_t q, size_t n_cand, size_t n_out, fls_place_match* h_out, cudaStream_t st, int device, int* launches);
+    void search(size_t q, size_t n_cand, size_t n_out, fls_place_match* h_out, Call& call, int device);
 };
 
 }  // namespace fls

@@ -126,7 +126,9 @@ int run_preprocess(int device, const float* xyzi, const float* time, bool src_on
     if (n > 0x7fffffffull || jump_span < 1 || !(leaf > 0.f)) return FLS_ERR_INVALID_ARG;
     if (n == 0) return FLS_OK;
     return with_workspace<PpWorkspace>(device, [&](PpWorkspace& w) -> int {
-        cudaStream_t st = w.st;
+        Call& c = w.call;
+        const cudaStream_t st = c.stream;
+        c.begin();
         DeskewView dv;
         bool ref_outside;
         const int rc = make_deskew_view(imu, w.imu_t, w.imu_q, st, dv, ref_outside);
@@ -163,13 +165,12 @@ int run_preprocess(int device, const float* xyzi, const float* time, bool src_on
         FLS_CUDA(cudaMemcpyAsync(&last[1], w.f_ord.p + (n - 1), sizeof(unsigned), cudaMemcpyDeviceToHost, st));
         FLS_CUDA(cudaMemcpyAsync(&last[2], w.e_pl.p + (n - 1), sizeof(unsigned), cudaMemcpyDeviceToHost, st));
         FLS_CUDA(cudaMemcpyAsync(&last[3], w.f_pl.p + (n - 1), sizeof(unsigned), cudaMemcpyDeviceToHost, st));
-        FLS_CUDA(cudaStreamSynchronize(st));
+        c.sync();
         const size_t no = (size_t)last[0] + last[1], npl = (size_t)last[2] + last[3];
-        int l = 0;
-        const size_t nf = npl ? voxel_grid_device(w.planar.p, npl, leaf, filtered, w.scratch, st, &l) : 0;  // :224-225
+        const size_t nf = npl ? voxel_grid_device(w.planar.p, npl, leaf, filtered, w.scratch, c) : 0;  // :224-225
         if (no && ordered_out) FLS_CUDA(cudaMemcpyAsync(ordered_out, ord, no * sizeof(float4), cudaMemcpyDeviceToHost, st));
         if (nf && planar_out) FLS_CUDA(cudaMemcpyAsync(planar_out, filtered, nf * sizeof(float4), cudaMemcpyDeviceToHost, st));
-        FLS_CUDA(cudaStreamSynchronize(st));
+        c.sync();
         *n_ordered = no;
         *n_planar = nf;
         return FLS_OK;

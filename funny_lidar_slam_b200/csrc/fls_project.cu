@@ -84,14 +84,15 @@ int make_deskew_view(const fls_imu_buffer* imu, DevBuf<unsigned long long>& d_t,
                      bool& ref_outside);
 
 int enqueue_project(ProjStage& w, const void* raw, const int* ring, const float* time, const fls_imu_buffer* imu, size_t n, size_t stride, int V, int H,
-                    float h_res, float min_d, float max_d, cudaStream_t st, long long* h2d, int* launches, bool src_on_device) {
+                    float h_res, float min_d, float max_d, Call& c, bool src_on_device) {
+    const cudaStream_t st = c.stream;
     const size_t cells = (size_t)V * H;
     DeskewView dv;
     const bool use_imu = imu && imu->n_imu && time;
     bool ref_outside;
     const int rc = make_deskew_view(use_imu ? imu : nullptr, w.imu_t, w.imu_q, st, dv, ref_outside);
     if (rc != FLS_OK) return rc;
-    if (dv.m > 0) *h2d += (long long)(imu->n_imu * (sizeof(unsigned long long) + 4 * sizeof(double)));
+    if (dv.m > 0) c.h2d += (long long)(imu->n_imu * (sizeof(unsigned long long) + 4 * sizeof(double)));
     if (ref_outside) n = 0;  // SetRefTime failed: no point is accepted
     w.raw.reserve(n + 1);
     w.ring.reserve(n + 1);
@@ -102,7 +103,7 @@ int enqueue_project(ProjStage& w, const void* raw, const int* ring, const float*
     const float* d_time = src_on_device && use_imu ? time : w.time.p;
     if (n && use_imu && !src_on_device) {
         FLS_CUDA(cudaMemcpyAsync(w.time.p, time, n * sizeof(float), cudaMemcpyHostToDevice, st));
-        *h2d += (long long)(n * sizeof(float));
+        c.h2d += (long long)(n * sizeof(float));
     }
     w.winner.reserve(cells);
     w.flag.reserve(cells);
@@ -113,9 +114,9 @@ int enqueue_project(ProjStage& w, const void* raw, const int* ring, const float*
     w.col.reserve(cells);
     w.rows.reserve((size_t)V * 2);
     if (n && !src_on_device) {
-        upload_records(raw, n, stride, w.raw.p, w.staging, st, h2d, launches);
+        upload_records(raw, n, stride, w.raw.p, w.staging, c);
         FLS_CUDA(cudaMemcpyAsync(w.ring.p, ring, n * sizeof(int), cudaMemcpyHostToDevice, st));
-        *h2d += (long long)(n * sizeof(int));
+        c.h2d += (long long)(n * sizeof(int));
     }
     const unsigned gc = (unsigned)((cells + 255) / 256);
     proj_clear_kernel<<<gc, 256, 0, st>>>(w.winner.p, cells);
@@ -127,7 +128,7 @@ int enqueue_project(ProjStage& w, const void* raw, const int* ring, const float*
     FLS_CUDA(cudaMemsetAsync(w.col.p, 0, cells * sizeof(int), st));
     proj_emit_kernel<<<gc, 256, 0, st>>>(d_raw, d_time, dv, w.winner.p, w.excl.p, V, H, w.ordered.p, w.depth.p, w.col.p, w.rows.p, w.rows.p + V, w.total.p);
     FLS_CUDA(cudaGetLastError());
-    *launches += n ? 5 : 4;
+    c.launches += n ? 5 : 4;
     return FLS_OK;
 }
 
@@ -140,11 +141,11 @@ int project_device(int device, const void* raw, const int* ring, const float* ti
     const size_t cells = (size_t)V * H;
     if (cells > 0x7fffffffull) return FLS_ERR_INVALID_ARG;
     return with_workspace<ProjWorkspace>(device, [&](ProjWorkspace& ws) -> int {
-        cudaStream_t st = ws.st;
+        Call& c = ws.call;
+        const cudaStream_t st = c.stream;
         ProjStage& w = ws.s;
-        long long h2d = 0;
-        int launches = 0;
-        const int rc = enqueue_project(w, raw, ring, time, imu, n, stride, V, H, h_res, min_d, max_d, st, &h2d, &launches, false);
+        c.begin();
+        const int rc = enqueue_project(w, raw, ring, time, imu, n, stride, V, H, h_res, min_d, max_d, c, false);
         if (rc != FLS_OK) return rc;
         unsigned total = 0;
         FLS_CUDA(cudaMemcpyAsync(&total, w.total.p, sizeof(total), cudaMemcpyDeviceToHost, st));
@@ -152,7 +153,7 @@ int project_device(int device, const void* raw, const int* ring, const float* ti
         FLS_CUDA(cudaMemcpyAsync(col_out, w.col.p, cells * sizeof(int), cudaMemcpyDeviceToHost, st));
         FLS_CUDA(cudaMemcpyAsync(row_start, w.rows.p, (size_t)V * sizeof(int), cudaMemcpyDeviceToHost, st));
         FLS_CUDA(cudaMemcpyAsync(row_end, w.rows.p + V, (size_t)V * sizeof(int), cudaMemcpyDeviceToHost, st));
-        FLS_CUDA(cudaStreamSynchronize(st));
+        c.sync();
         if (total) FLS_CUDA(cudaMemcpy(ordered_out, w.ordered.p, (size_t)total * sizeof(float4), cudaMemcpyDeviceToHost));
         *n_out = total;
         return FLS_OK;

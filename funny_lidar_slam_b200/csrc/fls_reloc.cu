@@ -228,12 +228,11 @@ void pose_score_launch(const Term& t, const float4* d_src, int n, int P, double*
 // ---- GetFitnessScore ---------------------------------------------------------------------------------------------------------
 // The fit grid is the search grid over the fit cloud with cells of sqrt(max_range): every point within the gate lies in the 27 cells
 // around a query.  Rebuilt when the cloud or max_range changed (one wait).
-int Handle::fit_grid_for(float max_range, int* waits) {
+int Handle::fit_grid_for(float max_range) {
     if (fit_grid_version == fit_cloud_version && fit_grid_range == max_range) return FLS_OK;
     fit_grid.res = std::sqrt(max_range) * 1.001f;
-    const int rc = fit_grid.build(fit_pts, fit_cloud_n, scratch, stream, &launches);
+    const int rc = fit_grid.build(fit_pts, fit_cloud_n, scratch, call);
     if (rc != FLS_OK) return rc;
-    if (waits) ++*waits;
     fit_grid_version = fit_cloud_version;
     fit_grid_range = max_range;
     return FLS_OK;
@@ -247,10 +246,10 @@ void Handle::fitness_enqueue(const float4* d_src, size_t n, int P, float max_ran
     fit_part_cnt.reserve((size_t)P * tiles + 1);
     fit_out.reserve((size_t)P);
     fit_cnt.reserve((size_t)P);
-    pose_score_launch<false>(FitTerm{fit_grid.view(), fit_pose.p, max_range}, d_src, (int)n, P, fit_part_sum.p, fit_part_cnt.p, stream);
-    pose_score_reduce_kernel<<<grid_for((size_t)P, 64), 64, 0, stream>>>(fit_part_sum.p, fit_part_cnt.p, P, (int)tiles, 0, max_range, fit_out.p, fit_cnt.p,
-                                                                         nullptr, nullptr, 0, nullptr);
-    launches += 2;
+    pose_score_launch<false>(FitTerm{fit_grid.view(), fit_pose.p, max_range}, d_src, (int)n, P, fit_part_sum.p, fit_part_cnt.p, call.stream);
+    pose_score_reduce_kernel<<<grid_for((size_t)P, 64), 64, 0, call.stream>>>(fit_part_sum.p, fit_part_cnt.p, P, (int)tiles, 0, max_range, fit_out.p,
+                                                                              fit_cnt.p, nullptr, nullptr, 0, nullptr);
+    call.launches += 2;
 }
 
 static float fitness_of(double sum, unsigned cnt) { return cnt > 0 ? (float)(sum / (double)cnt) : FLT_MAX; }
@@ -260,17 +259,17 @@ int Handle::fitness(float max_range, float* score) {
     // no cloud to search: LoamFull (loam_full_kdtree.h:206-208), NDT / iVox outside localization mode, or no map yet
     if (fit_cloud_n == 0 || last_src == nullptr || last_src_n == 0 || !(max_range > 0.f)) return FLS_OK;
     begin_call();
-    const int rc = fit_grid_for(max_range, nullptr);
+    const int rc = fit_grid_for(max_range);
     if (rc != FLS_OK) return rc;
     const GnPose pose = gn_pose(T_final);
     fit_pose.reserve(12);
-    FLS_CUDA(cudaMemcpyAsync(fit_pose.p, &pose, sizeof(pose), cudaMemcpyHostToDevice, stream));
+    FLS_CUDA(cudaMemcpyAsync(fit_pose.p, &pose, sizeof(pose), cudaMemcpyHostToDevice, call.stream));
     fitness_enqueue(last_src, last_src_n, 1, max_range);
     double sum = 0;
     unsigned cnt = 0;
-    FLS_CUDA(cudaMemcpyAsync(&sum, fit_out.p, sizeof(sum), cudaMemcpyDeviceToHost, stream));
-    FLS_CUDA(cudaMemcpyAsync(&cnt, fit_cnt.p, sizeof(cnt), cudaMemcpyDeviceToHost, stream));
-    end_call(nullptr);
+    FLS_CUDA(cudaMemcpyAsync(&sum, fit_out.p, sizeof(sum), cudaMemcpyDeviceToHost, call.stream));
+    FLS_CUDA(cudaMemcpyAsync(&cnt, fit_cnt.p, sizeof(cnt), cudaMemcpyDeviceToHost, call.stream));
+    call.end(nullptr);
     *score = fitness_of(sum, cnt);
     return FLS_OK;
 }
@@ -300,8 +299,8 @@ int reloc_grid(const fls_reloc_cfg& c, RelocGrid* g, bool wide) {
 }
 
 // The tail of the search: the plug-in's batch Match of the nr picks, GetFitnessScore of every refined pose and Init's choice rule.
-// L and W are the launches and waits of the call so far; out has its defaults.
-static int reloc_refine(Handle& h, const float4* d_scan, size_t n, const fls_reloc_cfg& c, const RelocPick* pick, int nr, int L, int W, double* T,
+// out has its defaults.
+static int reloc_refine(Handle& h, const float4* d_scan, size_t n, const fls_reloc_cfg& c, const RelocPick* pick, int nr, double* T,
                         fls_reloc_result* out, double* refined_T, int32_t* refined_converged, float* refined_fitness, int64_t* refined_index) {
     // ---- refinement: the plug-in's batch Match of the picks, the same scan nr times ------------------------------------------------
     double Tr[kMaxBatch * 16];
@@ -313,27 +312,27 @@ static int reloc_refine(Handle& h, const float4* d_scan, size_t n, const fls_rel
         scans[r] = d_scan;
         ns[r] = n;
     }
-    L += h.launches;
-    const int rc = h.plugin->match_batch(nr, scans, ns, 0, Tr, conv, nullptr);  // begins its own call
-    L += h.launches;
-    W += h.waits;
-    h.launches = 0;
+    const Call before = h.call;  // the Match begins a call of its own: this call's counts go on after it
+    const int rc = h.plugin->match_batch(nr, scans, ns, 0, Tr, conv, nullptr);
+    h.call.launches += before.launches;
+    h.call.waits += before.waits;
+    h.call.h2d += before.h2d;
+    h.call.d2h += before.d2h;
     if (rc != FLS_OK) return rc;
     // ---- fitness of every refined pose on the cloud fls_fitness reads after that Match, in one launch -------------------------------
     GnPose rows[kMaxBatch];
     for (int r = 0; r < nr; ++r) rows[r] = gn_pose(Tr + 16 * r);
     h.fit_pose.reserve((size_t)nr * 12);
-    FLS_CUDA(cudaMemcpyAsync(h.fit_pose.p, rows, sizeof(GnPose) * (size_t)nr, cudaMemcpyHostToDevice, h.stream));
+    FLS_CUDA(cudaMemcpyAsync(h.fit_pose.p, rows, sizeof(GnPose) * (size_t)nr, cudaMemcpyHostToDevice, h.call.stream));
     float fit[kMaxBatch];
     for (int r = 0; r < nr; ++r) fit[r] = FLT_MAX;
     if (h.last_src && h.last_src_n) {
         h.fitness_enqueue(h.last_src, h.last_src_n, nr, c.max_range);
         double sums[kMaxBatch];
         unsigned cnts[kMaxBatch];
-        FLS_CUDA(cudaMemcpyAsync(sums, h.fit_out.p, sizeof(double) * (size_t)nr, cudaMemcpyDeviceToHost, h.stream));
-        FLS_CUDA(cudaMemcpyAsync(cnts, h.fit_cnt.p, sizeof(unsigned) * (size_t)nr, cudaMemcpyDeviceToHost, h.stream));
-        FLS_CUDA(cudaStreamSynchronize(h.stream));
-        ++W;
+        FLS_CUDA(cudaMemcpyAsync(sums, h.fit_out.p, sizeof(double) * (size_t)nr, cudaMemcpyDeviceToHost, h.call.stream));
+        FLS_CUDA(cudaMemcpyAsync(cnts, h.fit_cnt.p, sizeof(unsigned) * (size_t)nr, cudaMemcpyDeviceToHost, h.call.stream));
+        h.call.sync();
         for (int r = 0; r < nr; ++r) fit[r] = fitness_of(sums[r], cnts[r]);
     }
     // ---- choice: the converged pose of lowest fitness (ties: rank), else the lowest fitness -----------------------------------------
@@ -356,8 +355,8 @@ static int reloc_refine(Handle& h, const float4* d_scan, size_t n, const fls_rel
         if (refined_fitness) refined_fitness[r] = fit[r];
         if (refined_index) refined_index[r] = pick[r].index;
     }
-    out->gpu_launches = L + h.launches;  // h.launches: the fitness launches since the Match
-    out->host_waits = W;
+    out->gpu_launches = h.call.launches;
+    out->host_waits = h.call.waits;
     return FLS_OK;
 }
 
@@ -663,7 +662,7 @@ struct Reloc {
     float lat_range = -1.f;
     std::vector<long long> levels;  // nodes evaluated per level of the last fls_relocalize_wide call, from its start level down to 0
 
-    int lattice_for(Handle& hd, float max_range, int* waits);
+    int lattice_for(Handle& hd, float max_range);
 };
 
 void RelocFree::operator()(Reloc* r) const { delete r; }
@@ -676,16 +675,15 @@ int Handle::relocalize_levels(int64_t* out, int capacity) const {
 
 // The lattice of the current fit cloud and max_range, rebuilt like fit_grid (two waits when it is: the bounding box, and the end of
 // the build before its scratch is freed).
-int Reloc::lattice_for(Handle& hd, float max_range, int* waits) {
+int Reloc::lattice_for(Handle& hd, float max_range) {
     if (lat_version == hd.fit_cloud_version && lat_range == max_range) return FLS_OK;
-    const cudaStream_t stream = hd.stream;
+    const cudaStream_t stream = hd.call.stream;
     DevBuf<float> box;
     box.reserve(6);
     lattice_bbox_kernel<<<1, 256, 0, stream>>>(hd.fit_pts, hd.fit_cloud_n, box.p);
     float b[6];
     FLS_CUDA(cudaMemcpyAsync(b, box.p, sizeof(b), cudaMemcpyDeviceToHost, stream));
-    FLS_CUDA(cudaStreamSynchronize(stream));
-    if (waits) ++*waits;
+    hd.call.sync();
     double h = std::sqrt((double)max_range) / 4.0;
     long long n[3];
     for (;; h *= 2.0) {
@@ -706,9 +704,8 @@ int Reloc::lattice_for(Handle& hd, float max_range, int* waits) {
     lattice_edt_kernel<<<grid_for((size_t)lines[2], 128), 128, 0, stream>>>(d0.p, d1.p, s.p, t.p, lat.nx, lat.ny, lat.nz, 2);
     lattice_store_kernel<<<grid_for(cells, 256), 256, 0, stream>>>(d1.p, lat.nx, lat.ny, lat.nz, h, lat.q, lat_v.p);
     FLS_CUDA(cudaGetLastError());
-    FLS_CUDA(cudaStreamSynchronize(stream));  // the scratch above is freed on return
-    if (waits) ++*waits;
-    hd.launches += 6;
+    hd.call.sync();  // the scratch above is freed on return
+    hd.call.launches += 6;
     lat_version = hd.fit_cloud_version;
     lat_range = max_range;
     return FLS_OK;
@@ -719,7 +716,7 @@ int Handle::relocalize(const float4* d_scan, size_t n, const fls_reloc_cfg& c, c
                        double* coarse_scores, size_t coarse_cap, int64_t* evaluations) {
     if (!reloc) reloc.reset(new Reloc);
     Reloc& s = *reloc;
-    int L = 0, W = 0;  // launches and waits of the whole call
+    const cudaStream_t stream = call.stream;
     long long evals = 0;
     if (evaluations) *evaluations = 0;
     if (wide) s.levels.clear();
@@ -732,16 +729,16 @@ int Handle::relocalize(const float4* d_scan, size_t n, const fls_reloc_cfg& c, c
     // ---- coarse cloud and the fit grid; an empty coarse cloud ends the call: nothing to score or refine, and a later fls_fitness
     // scores the empty cloud --------------------------------------------------------------------------------------------------------
     s.coarse.reserve(n + 1);
-    const size_t m = voxel_grid_device(d_scan, n, c.coarse_leaf, s.coarse.p, scratch, stream, &launches, &W);
+    const size_t m = voxel_grid_device(d_scan, n, c.coarse_leaf, s.coarse.p, scratch, call);
     if (m == 0) {
         if (T != guesses) std::memcpy(T, guesses, 16 * sizeof(double));
         last_src = d_scan;
         last_src_n = 0;
-        out->gpu_launches = launches;
-        out->host_waits = W;
+        out->gpu_launches = call.launches;
+        out->host_waits = call.waits;
         return FLS_OK;
     }
-    int rc = fit_grid_for(c.max_range, &W);
+    int rc = fit_grid_for(c.max_range);
     if (rc != FLS_OK) return rc;
     GnPose rows[kMaxBatch];
     for (int g = 0; g < G; ++g) rows[g] = gn_pose(guesses + 16 * g);
@@ -780,24 +777,24 @@ int Handle::relocalize(const float4* d_scan, size_t n, const fls_reloc_cfg& c, c
             pose_score_launch<true>(FitTerm{fit_grid.view(), s.poses.p, c.max_range}, s.coarse.p, (int)m, k, s.part_sum.p, s.part_cnt.p, stream);
             pose_score_reduce_kernel<<<grid_for((size_t)k, 128), 128, 0, stream>>>(s.part_sum.p, s.part_cnt.p, k, (int)tiles, (int)m, c.max_range, nullptr,
                                                                                    nullptr, keys + o, chunk, o, ids ? ids + o : nullptr);
-            L += 3;
+            call.launches += 3;
         }
         evals += N_;
     };
     // ---- the descent from the start level to level 1 (fls_relocalize_wide past 2^20 hypotheses) ------------------------------------
     if (ls > 0) {
-        rc = s.lattice_for(*this, c.max_range, &W);
+        rc = s.lattice_for(*this, c.max_range);
         if (rc != FLS_OK) return rc;
         s.nodes.reserve((size_t)N);
         reloc_iota_kernel<<<grid_for((size_t)N, 256), 256, 0, stream>>>(s.nodes.p, N);
-        ++L;
+        ++call.launches;
         // U: the nr-th smallest score of the start level's representatives
         s.key.reserve((size_t)N * 2);
         exact(s.nodes.p, N, ls, s.key.p, nullptr);
         cub_pass(scratch.cub_tmp, [&](void* tmp, size_t& bytes) {
             return cub::DeviceRadixSort::SortKeys(tmp, bytes, s.key.p, s.key.p + N, (int)N, 0, 64, stream);
         });
-        ++L;
+        ++call.launches;
         s.u.reserve(1);
         FLS_CUDA(cudaMemcpyAsync(s.u.p, s.key.p + N + nr - 1, sizeof(unsigned long long), cudaMemcpyDeviceToDevice, stream));
         // the slack's float terms (derivation above): tau, the largest translation coordinate of any leaf of any guess
@@ -809,7 +806,7 @@ int Handle::relocalize(const float4* d_scan, size_t n, const fls_reloc_cfg& c, c
         }
         s.slack_pts.reserve(m);
         reloc_slack_points_kernel<<<grid_for(m, 256), 256, 0, stream>>>(s.coarse.p, (int)m, s.guess.p, G, s.slack_pts.p);
-        ++L;
+        ++call.launches;
         BoundTerm bound{s.lat, ga, nullptr, 0, 32.0 * kU * tau + 8.0 * kU * std::sqrt((double)c.max_range), 32.0 * kU, c.max_range};
         for (int l = ls; l >= 1; --l) {
             s.count.reserve((size_t)N * 2);
@@ -822,7 +819,7 @@ int Handle::relocalize(const float4* d_scan, size_t n, const fls_reloc_cfg& c, c
                 bound.level = l;
                 pose_score_launch<true>(bound, s.slack_pts.p, (int)m, k, s.part_sum.p, nullptr, stream);
                 reloc_keep_kernel<<<grid_for((size_t)k, 128), 128, 0, stream>>>(s.part_sum.p, k, (int)tiles, (int)m, s.u.p, s.nodes.p + o, l, nx, nk, cnt + o);
-                L += 2;
+                call.launches += 2;
             }
             evals += N;
             s.levels.push_back(N);
@@ -830,20 +827,19 @@ int Handle::relocalize(const float4* d_scan, size_t n, const fls_reloc_cfg& c, c
             int last[2];
             FLS_CUDA(cudaMemcpyAsync(last, cnt + N - 1, sizeof(int), cudaMemcpyDeviceToHost, stream));
             FLS_CUDA(cudaMemcpyAsync(last + 1, off + N - 1, sizeof(int), cudaMemcpyDeviceToHost, stream));
-            FLS_CUDA(cudaStreamSynchronize(stream));
-            ++W;
-            ++L;
+            call.sync();
+            ++call.launches;
             const long long next = (long long)last[0] + last[1];
             if (next > kWideCap) {
                 set_last_error(std::string(G > 1 ? "fls_relocalize_multi: " : "fls_relocalize_wide: ") + std::to_string(next) +
                                " nodes survive at level " + std::to_string(l - 1));
-                out->gpu_launches = L + launches;
-                out->host_waits = W;
+                out->gpu_launches = call.launches;
+                out->host_waits = call.waits;
                 return FLS_ERR_CAPACITY;
             }
             s.next.reserve((size_t)next);
             reloc_children_kernel<<<grid_for((size_t)N, 128), 128, 0, stream>>>(s.nodes.p, cnt, off, (int)N, l, nx, nk, s.next.p);
-            ++L;
+            ++call.launches;
             std::swap(s.nodes.p, s.next.p);
             std::swap(s.nodes.cap, s.next.cap);
             N = next;
@@ -863,23 +859,22 @@ int Handle::relocalize(const float4* d_scan, size_t n, const fls_reloc_cfg& c, c
     if (ls > 0) {
         cub_reserve(scratch.cub_tmp, by_leaf, by_key);
         cub_run(scratch.cub_tmp, by_leaf);
-        ++L;
+        ++call.launches;
     } else {
         cub_reserve(scratch.cub_tmp, by_key);
     }
     cub_run(scratch.cub_tmp, by_key);
     reloc_pick_kernel<<<1, kMaxBatch, 0, stream>>>(key2, leaf2, ga, nr, s.pick.p);
     FLS_CUDA(cudaGetLastError());
-    L += 2;
+    call.launches += 2;
     RelocPick pick[kMaxBatch];
     FLS_CUDA(cudaMemcpyAsync(pick, s.pick.p, sizeof(RelocPick) * (size_t)nr, cudaMemcpyDeviceToHost, stream));
     // fls_relocalize's coarse scores: the unsorted keys hold their bits
     const size_t n_cs = coarse_scores ? (coarse_cap < (size_t)P ? coarse_cap : (size_t)P) : 0;
     if (n_cs) FLS_CUDA(cudaMemcpyAsync(coarse_scores, key, sizeof(double) * n_cs, cudaMemcpyDeviceToHost, stream));
-    FLS_CUDA(cudaStreamSynchronize(stream));
-    ++W;
+    call.sync();
     if (evaluations) *evaluations = evals;
-    return reloc_refine(*this, d_scan, n, c, pick, nr, L, W, T, out, refined_T, refined_converged, refined_fitness, refined_index);
+    return reloc_refine(*this, d_scan, n, c, pick, nr, T, out, refined_T, refined_converged, refined_fitness, refined_index);
 }
 
 }  // namespace fls

@@ -60,10 +60,11 @@ __global__ void vg_centroid_kernel(const float4* __restrict__ pts, const unsigne
 
 }  // namespace
 
-// Returns the number of output points; d_out must hold n records.  Synchronises the stream twice
-// (bounding box, run count) — both values size the following launches.
-size_t voxel_grid_device(const float4* d_pts, size_t n, float leaf, float4* d_out, BuildScratch& sc, cudaStream_t st, int* launches, int* waits) {
+// Returns the number of output points; d_out must hold n records.  Waits twice (bounding box, run count) — both values size the
+// following launches.
+size_t voxel_grid_device(const float4* d_pts, size_t n, float leaf, float4* d_out, BuildScratch& sc, Call& c) {
     if (n == 0) return 0;
+    const cudaStream_t st = c.stream;
     const float inv = 1.0f / leaf;
     sc.minmax.reserve(16);
     MinMaxOrd* d_mm = reinterpret_cast<MinMaxOrd*>(sc.minmax.p);
@@ -72,9 +73,8 @@ size_t voxel_grid_device(const float4* d_pts, size_t n, float leaf, float4* d_ou
     minmax_kernel<<<nb, 256, 0, st>>>(d_pts, n, d_mm);
     MinMaxOrd ho;
     FLS_CUDA(cudaMemcpyAsync(&ho, d_mm, sizeof(ho), cudaMemcpyDeviceToHost, st));
-    FLS_CUDA(cudaStreamSynchronize(st));
-    if (launches) *launches += 2;
-    if (waits) *waits += 1;
+    c.sync();
+    c.launches += 2;
     const VgParams g = vg_params(ho, inv);
     if (g.overflow) {  // PCL: "Leaf size is too small" -> output = input
         FLS_CUDA(cudaMemcpyAsync(d_out, d_pts, n * sizeof(float4), cudaMemcpyDeviceToDevice, st));
@@ -87,13 +87,12 @@ size_t voxel_grid_device(const float4* d_pts, size_t n, float leaf, float4* d_ou
         const long long maxid = (long long)g.divb[0] * g.divb[1] * g.divb[2];
         while ((1LL << end_bit) < maxid && end_bit < 32) ++end_bit;
     }
-    sc.sort_pairs<unsigned>(n, end_bit, st);
-    const int runs = sc.encode_runs<unsigned>(n, st);
-    if (waits) *waits += 1;
-    sc.run_starts(runs, st);
+    sc.sort_pairs<unsigned>(n, end_bit, c);
+    const int runs = sc.encode_runs<unsigned>(n, c);
+    sc.run_starts(runs, c);
     vg_centroid_kernel<<<grid_for(runs, 128), 128, 0, st>>>(d_pts, sc.idx_sorted.p, sc.starts.p, sc.counts.p, runs, d_out);
     FLS_CUDA(cudaGetLastError());
-    if (launches) *launches += 6;
+    c.launches += 6;
     return (size_t)runs;
 }
 
