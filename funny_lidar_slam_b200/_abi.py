@@ -34,6 +34,7 @@ FLS_LAYOUT_PCL_XYZI = 32
 FLS_LAYOUT_PACKED = 16
 FLS_FLAG_ITER_LOG = 1
 FLS_FLAG_PROFILE = 2
+FLS_FLAG_INFORMATION = 4
 
 
 class FlsConfig(C.Structure):
@@ -64,6 +65,11 @@ class FlsMatchStats(C.Structure):
 class FlsIterLog(C.Structure):
     _fields_ = [("H", C.c_double * 36), ("g", C.c_double * 6), ("dx", C.c_double * 6), ("sum_residual", C.c_double),
                 ("n_valid", C.c_int64)]
+
+
+class FlsInformation(C.Structure):
+    _fields_ = [("H", C.c_double * 36), ("g", C.c_double * 6), ("sum_residual", C.c_double), ("n_valid", C.c_int64),
+                ("valid", C.c_int32), ("pad", C.c_int32)]
 
 
 class FlsMapInfo(C.Structure):

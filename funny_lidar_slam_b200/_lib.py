@@ -5,7 +5,7 @@ from __future__ import annotations
 import ctypes as C
 import os
 
-from ._abi import (FlsConfig, FlsConvertCfg, FlsConvertResult, FlsFeatureCfg, FlsIterLog, FlsLoamFrontendCfg, FlsMapInfo, FlsMatchStats,
+from ._abi import (FlsConfig, FlsConvertCfg, FlsConvertResult, FlsFeatureCfg, FlsInformation, FlsIterLog, FlsLoamFrontendCfg, FlsMapInfo, FlsMatchStats,
                    FlsPlaceMatch, FlsPointCloud2, FlsRelocCfg, FlsRelocResult, FlsScCfg)
 
 _PKG = os.path.dirname(os.path.abspath(__file__))
@@ -23,6 +23,7 @@ EXPORTS = [
     "fls_relocalize", "fls_relocalize_device", "fls_relocalize_wide", "fls_relocalize_wide_device", "fls_relocalize_wide_levels",
     "fls_relocalize_multi", "fls_relocalize_multi_device",
     "fls_keyframes_scan_context", "fls_keyframes_detect_loop", "fls_keyframes_place_query", "fls_keyframes_place_query_device",
+    "fls_get_information", "fls_get_information_scan",
 ]
 
 
@@ -87,6 +88,8 @@ def lib():
     L.fls_relocalize_multi_device.argtypes = [vp, vp, sz] + multi_outs
     L.fls_get_iter_log.argtypes = [vp, C.POINTER(FlsIterLog), C.c_int]
     L.fls_get_iter_log_scan.argtypes = [vp, C.c_int, C.POINTER(FlsIterLog), C.c_int]
+    L.fls_get_information.argtypes = [vp, C.POINTER(FlsInformation)]
+    L.fls_get_information_scan.argtypes = [vp, C.c_int, C.POINTER(FlsInformation)]
     L.fls_get_map_info.argtypes = [vp, C.POINTER(FlsMapInfo)]
     L.fls_get_voxel_keys.argtypes = [vp, vp, sz, C.POINTER(sz)]
     L.fls_get_map_points.argtypes = [vp, vp, sz, C.POINTER(sz)]

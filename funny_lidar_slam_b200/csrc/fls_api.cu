@@ -67,6 +67,11 @@ void Handle::init() {
         log.reserve((size_t)log_cap * kMaxBatch);
         h_log.resize((size_t)log_cap * kMaxBatch);
     }
+    if (cfg.flags & FLS_FLAG_INFORMATION) {
+        info_on = true;
+        info.reserve(kMaxBatch);
+        h_info.reserve(kMaxBatch);
+    }
 }
 
 Handle::~Handle() {
@@ -160,6 +165,12 @@ void Handle::read_back(int B) {
         FLS_CUDA(cudaMemcpyAsync(h_log.data(), log.p, bytes, cudaMemcpyDeviceToHost, call.stream));
         call.d2h += (long long)bytes;
     }
+    info_n = 0;
+    if (info_enqueued) {
+        const size_t bytes = sizeof(fls_information) * (size_t)B;
+        FLS_CUDA(cudaMemcpyAsync(h_info.p, info.p, bytes, cudaMemcpyDeviceToHost, call.stream));
+        call.d2h += (long long)bytes;
+    }
 }
 
 void Handle::unpack(int B, const size_t* n, double* T, int* converged, fls_match_stats* st) {
@@ -188,6 +199,8 @@ void Handle::unpack(int B, const size_t* n, double* T, int* converged, fls_match
     std::memcpy(T_final, T, sizeof(T_final));
     log_n.resize(B);
     for (int s = 0; s < B; ++s) log_n[s] = h_state.p[s].iter < log_cap ? h_state.p[s].iter : log_cap;
+    info_n = info_enqueued ? B : 0;
+    info_enqueued = false;
 }
 
 int Handle::filter_batch(int B, const float4* const* d, const size_t* n, float leaf, DevBuf<float4>& dst, size_t* off, size_t* ns) {
@@ -265,6 +278,17 @@ static bool loam_frontend_cfg_ok(const fls_loam_frontend_cfg& c) {
            c.planar_leaf > 0.f &&
            // the reference CHECK_NE()s both feature thresholds against FloatNaN (feature_extractor.cpp:19-20)
            c.corner_threshold < 3.0e38f && c.planar_threshold < 3.0e38f;
+}
+
+// Every Match entry runs through this: the call starts without an information record and leaves one only when it returns FLS_OK
+// (an argument check, a refusal or an error caught by FLS_CATCH all leave none).
+template <class F>
+static int info_scoped(fls_handle* hh, F&& call) {
+    Handle* h = reinterpret_cast<Handle*>(hh);
+    if (h) h->info_reset();
+    const int rc = call();
+    if (h && rc != FLS_OK) h->info_reset();
+    return rc;
 }
 
 // stage buffers of fls_voxel_grid
@@ -485,21 +509,27 @@ static int match_clouds(Handle* h, const void* ordered, size_t n_ordered, const 
 
 int fls_match(fls_handle* hh, const void* ordered, size_t n_ordered, const void* planar, size_t n_planar, const void* corner, size_t n_corner,
               size_t stride, double T[16], int* converged, fls_match_stats* st) {
-    if (!stride_ok(stride)) return FLS_ERR_INVALID_ARG;
-    return match_clouds(reinterpret_cast<Handle*>(hh), ordered, n_ordered, planar, n_planar, corner, n_corner, stride, T, converged, st);
+    return info_scoped(hh, [&] {
+        if (!stride_ok(stride)) return (int)FLS_ERR_INVALID_ARG;
+        return match_clouds(reinterpret_cast<Handle*>(hh), ordered, n_ordered, planar, n_planar, corner, n_corner, stride, T, converged, st);
+    });
 }
 
 int fls_match_device(fls_handle* hh, const void* d_points, size_t n, double T[16], int* converged, fls_match_stats* st) {
-    Handle* h = reinterpret_cast<Handle*>(hh);
-    // LoamFull reads two feature clouds: fls_match_cluster_device
-    if (h && T && h->plugin->reads == Plugin::kPlanarCorner) return !d_points && n ? FLS_ERR_INVALID_ARG : FLS_ERR_UNSUPPORTED;
-    // the one cloud is the ordered scan or the planar features, whichever the plug-in reads
-    return match_clouds(h, d_points, n, d_points, n, nullptr, 0, 0, T, converged, st);
+    return info_scoped(hh, [&] {
+        Handle* h = reinterpret_cast<Handle*>(hh);
+        // LoamFull reads two feature clouds: fls_match_cluster_device
+        if (h && T && h->plugin->reads == Plugin::kPlanarCorner) return (int)(!d_points && n ? FLS_ERR_INVALID_ARG : FLS_ERR_UNSUPPORTED);
+        // the one cloud is the ordered scan or the planar features, whichever the plug-in reads
+        return match_clouds(h, d_points, n, d_points, n, nullptr, 0, 0, T, converged, st);
+    });
 }
 
 int fls_match_cluster_device(fls_handle* hh, const void* d_ordered, size_t n_ordered, const void* d_planar, size_t n_planar, const void* d_corner,
                              size_t n_corner, double T[16], int* converged, fls_match_stats* st) {
-    return match_clouds(reinterpret_cast<Handle*>(hh), d_ordered, n_ordered, d_planar, n_planar, d_corner, n_corner, 0, T, converged, st);
+    return info_scoped(hh, [&] {
+        return match_clouds(reinterpret_cast<Handle*>(hh), d_ordered, n_ordered, d_planar, n_planar, d_corner, n_corner, 0, T, converged, st);
+    });
 }
 
 // A batch Match of host scans of `host_stride` bytes or (0) device scans.  Scans of one batch are matched against the same map state:
@@ -527,24 +557,23 @@ static int batch_begin(fls_handle* hh, int n_scans, const void* const* scans, co
 
 int fls_match_batch(fls_handle* hh, int n_scans, const void* const* planar, const size_t* n, size_t stride, double* T, int* converged,
                     fls_match_stats* st) {
-    return stride_ok(stride) ? match_batch(hh, n_scans, planar, n, stride, T, converged, st) : FLS_ERR_INVALID_ARG;
+    return info_scoped(hh, [&] { return stride_ok(stride) ? match_batch(hh, n_scans, planar, n, stride, T, converged, st) : (int)FLS_ERR_INVALID_ARG; });
 }
 
 int fls_match_batch_device(fls_handle* hh, int n_scans, const void* const* d_planar, const size_t* n, double* T, int* converged,
                            fls_match_stats* st) {
-    return match_batch(hh, n_scans, d_planar, n, 0, T, converged, st);
+    return info_scoped(hh, [&] { return match_batch(hh, n_scans, d_planar, n, 0, T, converged, st); });
 }
 
 int fls_match_batch_begin(fls_handle* hh, int n_scans, const void* const* planar, const size_t* n, size_t stride, const double* T) {
-    return stride_ok(stride) ? batch_begin(hh, n_scans, planar, n, stride, T) : FLS_ERR_INVALID_ARG;
+    return info_scoped(hh, [&] { return stride_ok(stride) ? batch_begin(hh, n_scans, planar, n, stride, T) : (int)FLS_ERR_INVALID_ARG; });
 }
 
 int fls_match_batch_begin_device(fls_handle* hh, int n_scans, const void* const* d_planar, const size_t* n, const double* T) {
-    return batch_begin(hh, n_scans, d_planar, n, 0, T);
+    return info_scoped(hh, [&] { return batch_begin(hh, n_scans, d_planar, n, 0, T); });
 }
 
-int fls_match_batch_end(fls_handle* hh, double* T, int* converged, fls_match_stats* st) {
-    Handle* h = reinterpret_cast<Handle*>(hh);
+static int batch_end(Handle* h, double* T, int* converged, fls_match_stats* st) {
     if (!h || !T) return FLS_ERR_INVALID_ARG;
     const int B = h->plugin->batch_pending();
     if (!B) return FLS_ERR_INVALID_ARG;
@@ -552,6 +581,14 @@ int fls_match_batch_end(fls_handle* hh, double* T, int* converged, fls_match_sta
     if (st) std::memset(st, 0, sizeof(*st) * (size_t)B);
     return h->plugin->batch_end(T, converged, st);
     FLS_CATCH
+}
+
+int fls_match_batch_end(fls_handle* hh, double* T, int* converged, fls_match_stats* st) {
+    // the records of the batch were enqueued by _begin (which left none readable): only an error clears them
+    Handle* h = reinterpret_cast<Handle*>(hh);
+    const int rc = batch_end(h, T, converged, st);
+    if (h && rc != FLS_OK) h->info_reset();
+    return rc;
 }
 
 int fls_fitness(fls_handle* hh, float max_range, float* score) {
@@ -569,6 +606,7 @@ static int relocalize(fls_handle* hh, bool wide, const void* scan, size_t n, siz
                       int G, double* T, fls_reloc_result* out, double* refined_T, int32_t* refined_converged, float* refined_fitness,
                       int64_t* refined_index, double* coarse_scores, size_t coarse_cap, int64_t* evaluations) {
     Handle* h = reinterpret_cast<Handle*>(hh);
+    if (h) h->info_reset();  // no record after any relocalization call
     if (!h || !cfg || !T || !out || (!scan && n) || (coarse_cap && !coarse_scores) || n > 0x3fffffffull) return FLS_ERR_INVALID_ARG;
     fls::RelocGrid g;
     const int v = fls::reloc_grid(*cfg, &g, wide);
@@ -577,6 +615,16 @@ static int relocalize(fls_handle* hh, bool wide, const void* scan, size_t n, siz
     if (!h->cfg.localization_mode || (h->cfg.method != FLS_P2PLANE_IVOX && h->cfg.method != FLS_NDT)) return FLS_ERR_UNSUPPORTED;
     if (h->plugin->batch_pending()) return FLS_ERR_INVALID_ARG;  // one batch in flight per handle (fls_match_batch_begin)
     if (h->fit_cloud_n == 0) return FLS_ERR_NO_MAP;
+    // the internal Matches of a relocalization do not evaluate their information
+    struct Suspend {
+        Handle* h;
+        bool on;
+        ~Suspend() {
+            h->info_on = on;
+            h->info_reset();
+        }
+    } suspend{h, h->info_on};
+    h->info_on = false;
     FLS_TRY
     h->begin_call();
     const float4* d = host_stride ? h->upload(scan, n, host_stride, h->src) : static_cast<const float4*>(scan);

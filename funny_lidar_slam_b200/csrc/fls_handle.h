@@ -55,6 +55,12 @@ std::unique_ptr<Plugin> make_ndt_plugin(Handle& h);   // IncrementalNDT (fls_ndt
 std::unique_ptr<Plugin> make_icp_plugin(Handle& h);   // IcpOptimized (fls_icp.cu)
 std::unique_ptr<Plugin> make_kd_plugin(Handle& h);    // LoamPointToPlaneKdtree and LoamFull (fls_loam.cu)
 
+// FLS_FLAG_INFORMATION: the evaluation of a Match's scans at their returned poses, enqueued before its read-back (fls_info.cuh), and
+// the launches it adds to the call
+template <class Args>
+void enqueue_information(Handle& h, const Args* a, int B);
+static constexpr int kInfoLaunches = 2;
+
 // IsNeedAddCloud (icp_optimized.h:218-236, loam_point_to_plane_kdtree.h:186-202, loam_full_kdtree.h:356-371): key-frame gating on
 // translation / RPY deltas against a persistent last_T that starts at the first pose it sees  [quirk 7]
 struct KeyFrameGate {
@@ -104,6 +110,19 @@ struct Handle {
     long long per_point_iter_bytes = 0;  // fixed part of the algorithmic bytes per point-iteration (set by gn_launch)
     long long per_cand_bytes = 0;        // bytes per scanned map record
     BuildScratch scratch;                // voxel-grid passes of Match and the local-map crop
+
+    // FLS_FLAG_INFORMATION (fls_info.cuh): each Match evaluates its scans' records after its loop (enqueue_information) and read_back
+    // copies them with the states; info_n of them belong to the last Match call (0: none)
+    bool info_on = false;        // the handle's flag, off while a relocalization runs its internal Matches
+    bool info_enqueued = false;  // the Match in progress has enqueued its evaluation
+    int info_n = 0;
+    DevBuf<fls_information> info;
+    PinnedBuf<fls_information> h_info;
+    DevBuf<double> info_part;  // per-CTA partial sums of the evaluation
+    void info_reset() {  // a Match call begins, or one ended without records
+        info_n = 0;
+        info_enqueued = false;
+    }
 
     // optional caller-owned device buffer that receives {pose, converged, iterations} per scan (fls_set_result_buffer_device)
     double* result_buf = nullptr;
@@ -179,16 +198,18 @@ struct Handle {
     void read_back(int n_scans);  // enqueues the copy of the states and of every scan's iteration log
     // after call.end: T / converged / stats and log_n of every scan (call-level figures on stats[0]), T_final from scan 0
     void unpack(int n_scans, const size_t* n_source, double* T, int* converged, fls_match_stats* st);
-    // A single-scan Match on a persistent kernel of `grid` CTAs (NDT, ICP, kd-tree LOAM): control block, state from T, the
-    // gn_launch of launch(ctl), then the wait and T / converged / stats of a scan of n_source points
-    template <class F>
+    // A single-scan Match on a persistent kernel of `grid` CTAs (NDT, ICP): control block, state from T, the gn_launch of
+    // launch(ctl), the information evaluation of the loop arguments `a` when the flag is on, then the wait and T / converged / stats
+    // of a scan of n_source points
+    template <class Args, class F>
     void match_single(int method, int min_effective, int grid, long long point_iter_bytes, long long cand_bytes, const float4* src, size_t src_n,
-                      size_t n_source, double* T, int* converged, fls_match_stats* st, F&& launch) {
+                      size_t n_source, double* T, int* converged, fls_match_stats* st, const Args& a, F&& launch) {
         const unsigned tag_base = next_ll_epoch((size_t)grid * 32 + kLlPoseLen);  // may move ll_rows
         const GnLoopCtl ctl = loop_ctl(0, method, min_effective, tag_base, ll_rows.p, ll_rows.p + (size_t)grid * 32);
         launch_gn_init(state.p, T, call.stream);
         call.launches++;
         gn_launch(point_iter_bytes, cand_bytes, src, src_n, [&] { launch(ctl); });
+        if (info_on) enqueue_information(*this, &a, 1);
         read_back(1);
         call.end(st);
         unpack(1, &n_source, T, converged, st);
@@ -201,8 +222,8 @@ struct Handle {
     // points, also its n_source) gets one CTA per `per_cta` points, all scaled down together when the `cap` co-resident CTAs of the
     // kernel cannot hold them (more scans than CTAs: FLS_ERR_INVALID_ARG).  Then, per scan: its control block and its item, whose arguments
     // fill(s, item.a) sets, and one launch that starts its state from T and writes the item to subgrid_items; the gn_launch of
-    // launch(d_items, grid), the wait, and T / converged / stats of every scan.  fit_src / fit_n: the cloud GetFitnessScore reads
-    // afterwards.
+    // launch(d_items, grid), the information evaluation of every scan's arguments when the flag is on, the wait, and T / converged /
+    // stats of every scan.  fit_src / fit_n: the cloud GetFitnessScore reads afterwards.
     template <class Args, class Fill, class Launch>
     int match_subgrids(int method, int min_effective, int B, const size_t* ns, int per_cta, int cap, long long point_iter_bytes, long long cand_bytes,
                        const float4* fit_src, size_t fit_n, double* T, int* converged, fls_match_stats* st, Fill&& fill, Launch&& launch) {
@@ -222,10 +243,12 @@ struct Handle {
         GnBatchItem<Args>* d_items = reinterpret_cast<GnBatchItem<Args>*>(subgrid_items.reserve(sizeof(GnBatchItem<Args>) * (size_t)B));
         uint4* pose_base = ll_rows.p + (size_t)grid * 32;
         int cta0 = 0;
+        Args args[kMaxBatch];  // what the information evaluation reads
         for (int s = 0; s < B; ++s) {
             GnBatchItem<Args> it;
             std::memset(&it, 0, sizeof(it));
             fill(s, it.a);
+            if (info_on) args[s] = it.a;
             it.ctl = loop_ctl(s, method, min_effective, tag_base, ll_rows.p + (size_t)cta0 * 32, pose_base + (size_t)s * kLlPoseLen);
             it.cta0 = cta0;
             it.ncta = ncta[s];
@@ -234,6 +257,7 @@ struct Handle {
             call.launches++;
         }
         gn_launch(point_iter_bytes, cand_bytes, fit_src, fit_n, [&] { launch(d_items, grid); });
+        if (info_on) enqueue_information(*this, args, B);
         read_back(B);
         call.end(st);
         unpack(B, ns, T, converged, st);

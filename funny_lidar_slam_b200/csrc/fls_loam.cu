@@ -24,6 +24,7 @@
 #include "fls_eig.cuh"
 #include "fls_gn.cuh"
 #include "fls_handle.h"
+#include "fls_info.cuh"
 #include "fls_plane.cuh"
 
 namespace fls {
@@ -174,6 +175,31 @@ __device__ __forceinline__ bool corner_term(const float4* __restrict__ P, const 
     return true;
 }
 
+// Feature point i's fresh term at the pose s_pose (row-major R, t): corner points [0, n_corner) then planar points, the exact 5-NN of
+// the point moved by the double pose, the point_search_thres gate and the line or plane fit -> J (6) and residual r in dx = [dθ, dt]
+// order; n_cand: the map records it scanned.  Called by all kLoamLanes lanes of the point's group; returns true on lane 0 when the
+// point has a term.  The Gauss-Newton loop and the information evaluation (fls_info.cuh) both call it.
+__device__ __forceinline__ bool loam_point(const LoamArgs& a, int i, const double* s_pose, int sub, unsigned group_mask, double (&J)[6], double& r,
+                                           unsigned& n_cand) {
+    const bool is_corner = i < a.n_corner;
+    const float4 sp = is_corner ? a.corner[i] : a.planar[i - a.n_corner];
+    // pcl::transformPoint with the double transform, stored back as fp32 (:219-220, :284-285, kdtree :211-212)
+    const float qx = xform_row_d(s_pose[0], s_pose[1], s_pose[2], s_pose[9], (double)sp.x, (double)sp.y, (double)sp.z);
+    const float qy = xform_row_d(s_pose[3], s_pose[4], s_pose[5], s_pose[10], (double)sp.x, (double)sp.y, (double)sp.z);
+    const float qz = xform_row_d(s_pose[6], s_pose[7], s_pose[8], s_pose[11], (double)sp.x, (double)sp.y, (double)sp.z);
+    const GridView& g = is_corner ? a.corner_map : a.planar_map;
+    Top5 nn;
+    grid_knn5(g, sub, group_mask, qx, qy, qz, a.gate, nn, n_cand);
+    bool use = false;
+    if (sub == 0 && nn.full() && !((double)nn.d4 > a.search_thres)) {  // :227 / :291 (search_thres = +inf for the kd-tree point-to-plane plug-in)
+        const unsigned js[5] = {nn.k0, nn.k1, nn.k2, nn.k3, nn.k4};
+        unsigned fb = 0;
+        use = is_corner ? corner_term(g.pts, js, sp, qx, qy, qz, s_pose, a.line_ratio, J, r)
+                        : plane_term(g.pts, js, sp, qx, qy, qz, s_pose, a.plane_thres, J, r, fb);
+    }
+    return use;
+}
+
 // One persistent launch runs every Gauss-Newton iteration of a Match, on the CTAs (cta, ncta) of the sub-grid that serves the scan.
 template <int BLOCK>
 __device__ __forceinline__ void loam_gn_loop(const LoamArgs& a, const GnLoopCtl& ctl, const int cta, const int ncta) {
@@ -190,24 +216,10 @@ __device__ __forceinline__ void loam_gn_loop(const LoamArgs& a, const GnLoopCtl&
         for (int k = 0; k < kNumAcc; ++k) acc[k] = 0.0;
         for (int i = (unsigned)cta * kPerBlock + threadIdx.x / kLoamLanes; i < n_total; i += (unsigned)ncta * kPerBlock) {
             const bool is_corner = i < a.n_corner;
-            const float4 sp = is_corner ? a.corner[i] : a.planar[i - a.n_corner];
-            // pcl::transformPoint with the double transform, stored back as fp32 (:219-220, :284-285, kdtree :211-212)
-            const float qx = xform_row_d(s_pose[0], s_pose[1], s_pose[2], s_pose[9], (double)sp.x, (double)sp.y, (double)sp.z);
-            const float qy = xform_row_d(s_pose[3], s_pose[4], s_pose[5], s_pose[10], (double)sp.x, (double)sp.y, (double)sp.z);
-            const float qz = xform_row_d(s_pose[6], s_pose[7], s_pose[8], s_pose[11], (double)sp.x, (double)sp.y, (double)sp.z);
-            const GridView& g = is_corner ? a.corner_map : a.planar_map;
-            Top5 nn;
-            unsigned n_cand;
-            grid_knn5(g, sub, group_mask, qx, qy, qz, a.gate, nn, n_cand);
-            acc[kAccCand] += (double)n_cand;
             double J[6], r = 0.0;
-            bool use = false;
-            if (sub == 0 && nn.full() && !((double)nn.d4 > a.search_thres)) {  // :227 / :291 (search_thres = +inf for the kd-tree point-to-plane plug-in)
-                const unsigned js[5] = {nn.k0, nn.k1, nn.k2, nn.k3, nn.k4};
-                unsigned fb = 0;
-                use = is_corner ? corner_term(g.pts, js, sp, qx, qy, qz, s_pose, a.line_ratio, J, r)
-                                : plane_term(g.pts, js, sp, qx, qy, qz, s_pose, a.plane_thres, J, r, fb);
-            }
+            unsigned n_cand;
+            bool use = loam_point(a, i, s_pose, sub, group_mask, J, r, n_cand);
+            acc[kAccCand] += (double)n_cand;
             if (sub != 0) continue;  // lane 0 of the group owns the point's record and sums
             double* rec = a.rec + (size_t)i * 8;
             if (use) {
@@ -243,12 +255,26 @@ __global__ void __launch_bounds__(BLOCK) loam_gn_kernel(const GnBatchItem<LoamAr
     gn_batch_loop<BLOCK>(items, n_scans, [](const LoamArgs& a, const GnLoopCtl& ctl, int cta, int ncta) { loam_gn_loop<BLOCK>(a, ctl, cta, ncta); });
 }
 
+
 __global__ void loam_clear_flags_kernel(unsigned char* flags, int n) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n) flags[i] = 0;
 }
 
 }  // namespace
+
+// FLS_FLAG_INFORMATION (fls_info.cuh): W = 1; LoamFull counts its corner and planar terms alike
+template <>
+struct InfoTerm<LoamArgs> {
+    static constexpr int kBlock = kLoamBlock, kLanes = kLoamLanes;
+    static __host__ __device__ int count(const LoamArgs& a) { return a.n_corner + a.n_planar; }
+    static __device__ __forceinline__ void point(const LoamArgs& a, int i, const double* pose, const float*, int sub, unsigned mask,
+                                                 double (&acc)[kNumAcc]) {
+        double J[6], r = 0.0;
+        unsigned n_cand;
+        if (loam_point(a, i, pose, sub, mask, J, r, n_cand)) info_add_J(J, r, acc);
+    }
+};
 
 static int loam_max_grid(int device) { return coresident_ctas((const void*)loam_gn_kernel<kLoamBlock>, kLoamBlock, 0, device); }
 // clears the flags of every scan of the Match (n of them in all) in one launch when there are any, then the loop kernel

@@ -36,6 +36,7 @@
 
 #include "fls_gn.cuh"
 #include "fls_handle.h"
+#include "fls_info.cuh"
 #include "fls_ivox.cuh"
 #include "fls_knn.cuh"
 #include "fls_plane.cuh"
@@ -422,6 +423,19 @@ size_t p2plane_smem() { return (size_t)(kP2PlaneBlock / 32) * 32 * kRecW * sizeo
 
 }  // namespace
 
+// FLS_FLAG_INFORMATION: the loops' per-point term (p2plane_point, fls_info.cuh), W = 1, over the scan in its locality order; the
+// evaluation reads map, plane_thres, src and n, never the persistent records
+template <>
+struct InfoTerm<P2PlaneArgs> {
+    static constexpr int kBlock = 256, kLanes = 1;
+    static __host__ __device__ int count(const P2PlaneArgs& a) { return a.n; }
+    static __device__ __forceinline__ void point(const P2PlaneArgs& a, int i, const double* pose, const float*, int, unsigned, double (&acc)[kNumAcc]) {
+        double J[6], ad = 0.0;
+        unsigned n_cand, n_fb;
+        if (p2plane_point(a.map, a.src[i], pose, a.plane_thres, J, ad, n_cand, n_fb)) info_add_J(J, ad, acc);
+    }
+};
+
 // CTAs that serve a scan of n points: its warp-sized (32-point) chunks / warps per CTA, + the folder, <= co-resident
 static int p2plane_grid(int n, int device) {
     const int W = kP2PlaneBlock / 32;
@@ -593,6 +607,11 @@ class IvoxPlugin final : public Plugin {
                 launch_p2plane_loop(one, ctl(0), grid, stream);
             }
         });
+        if (h.info_on) {
+            P2PlaneArgs info_args[kMaxBatch];
+            for (int s = 0; s < B; ++s) info_args[s] = {a.map, a.plane_thres, queries.p + off[s], (int)n[s], nullptr, nullptr, nullptr};
+            enqueue_information(h, info_args, B);
+        }
         // ---- read back: every scan's state (+ its iteration log) ----------------------------------------------------------
         h.read_back(B);
         *h_abort.p = 0;

@@ -14,7 +14,7 @@ from dataclasses import dataclass, field
 import numpy as np
 
 from . import _abi
-from ._abi import FlsConfig, FlsIterLog, FlsMapInfo, FlsMatchStats
+from ._abi import FlsConfig, FlsInformation, FlsIterLog, FlsMapInfo, FlsMatchStats
 from ._lib import check, lib
 
 
@@ -366,6 +366,15 @@ class Registration:
             check(n, "fls_get_iter_log_scan")
         return [dict(H=np.array(b.H).reshape(6, 6), g=np.array(b.g), dx=np.array(b.dx), sum_residual=b.sum_residual, n_valid=b.n_valid)
                 for b in buf[:n]]
+
+    def information(self, scan: int = 0):
+        """The information record of scan `scan` of the last Match (needs FLS_FLAG_INFORMATION): dict of H (6x6), g (6), n_valid and
+        sum_residual at the returned pose, in the order [dθ; dp] with R <- R·Exp(dθ), p <- p + dp; None when there is no record."""
+        rec = FlsInformation()
+        check(lib().fls_get_information_scan(self._h, int(scan), C.byref(rec)), "fls_get_information_scan")
+        if not rec.valid:
+            return None
+        return dict(H=np.array(rec.H).reshape(6, 6), g=np.array(rec.g), n_valid=int(rec.n_valid), sum_residual=float(rec.sum_residual))
 
     def gn_step_probe(self, cases):
         """One Gauss-Newton step (solve, pose update, stop rule) per case on the handle's device: fls_gn_step_probe.  A case is a dict

@@ -80,6 +80,23 @@ public:
         return score;
     }
 
+    // The information matrix of the last Match at the pose it returned (needs FLS_FLAG_INFORMATION in the config): H (a Mat6d) in the
+    // order [rotation; position] of lidar_pose_info_, for EdgeRotation's right perturbation R * Exp(dθ) and p + dp; g (a Vec6d),
+    // n_valid and sum_residual optional.  false when the last Match left no record.  Scaling H to a covariance is the integrator's
+    // choice.  A template so that the adapter needs no Eigen type until it is used.
+    template <class Mat6, class Vec6 = Mat6>
+    bool GetPoseInformation(Mat6& H, Vec6* g = nullptr, int64_t* n_valid = nullptr, double* sum_residual = nullptr) const {
+        fls_information rec;
+        if (fls_get_information(handle_, &rec) != FLS_OK || !rec.valid) return false;
+        for (int r = 0; r < 6; ++r)
+            for (int c = 0; c < 6; ++c) H(r, c) = rec.H[r * 6 + c];
+        if (g)
+            for (int r = 0; r < 6; ++r) (*g)(r) = rec.g[r];
+        if (n_valid) *n_valid = rec.n_valid;
+        if (sum_residual) *sum_residual = rec.sum_residual;
+        return true;
+    }
+
     // Localization::Init from the RViz "2D Pose Estimate" (localization.cpp:114-169): searches an x-y-yaw grid around T, refines the
     // best poses and picks one by Init's own rule.  T receives the chosen pose (also when false is returned, as upstream writes it);
     // *fitness its GetFitnessScore(cfg.max_range).  Returns whether it is accepted (converged and fitness < cfg.accept_fitness).

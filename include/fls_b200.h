@@ -135,6 +135,7 @@ typedef struct {
 
 #define FLS_FLAG_ITER_LOG 1u /* keep per-iteration H, g, dx, n_valid, sum_res for fls_get_iter_log */
 #define FLS_FLAG_PROFILE 2u  /* bracket the fused Gauss-Newton launch of a Match with CUDA events (fills kernel_ms / kernel_launches) */
+#define FLS_FLAG_INFORMATION 4u /* evaluate every Match's information matrix at its returned pose for fls_get_information */
 
 typedef struct {
     int32_t iterations;   /* GN iterations executed */
@@ -158,6 +159,22 @@ typedef struct {
     double sum_residual;
     int64_t n_valid;
 } fls_iter_log;
+
+/* FLS_FLAG_INFORMATION: how well a scan constrains the pose T_final its Match returned (DESIGN.md §3.13).  The terms are those the
+ * plug-in's Gauss-Newton iteration builds from a fresh correspondence search at T_final (same neighbour search, gates, residual
+ * and weight W; LoamFull: its planar and corner terms); a point without a correspondence adds nothing.  In the fusion
+ * parameterization: order [dtheta; dp], T_final perturbed as R <- R * Exp(dtheta), p <- p + dp (p in the world frame):
+ *   H = sum J_i^T W_i J_i,   g = sum J_i^T W_i r_i.
+ * Scaling H to a covariance is the caller's choice: NDT's residual is already Mahalanobis (W = the voxel information), the LOAM
+ * and ICP residuals are metres with W = 1. */
+typedef struct {
+    double H[36];         /* row-major 6x6, symmetric */
+    double g[6];
+    double sum_residual;  /* LOAM: sum |d|, NDT: sum of e^T W e, ICP: sum ||e|| over the contributing terms */
+    int64_t n_valid;      /* contributing terms: points (LOAM, ICP; LoamFull: planar + corner), point-voxel pairs (NDT) */
+    int32_t valid;        /* 1: the record belongs to the last Match call; 0: no record (see fls_get_information) */
+    int32_t pad;
+} fls_information;
 
 typedef struct {
     int64_t n_points;    /* map points resident on the device */
@@ -356,6 +373,13 @@ int fls_get_iter_log(const fls_handle* h, fls_iter_log* out, int capacity);
  * FLS_ICP_P2P and FLS_P2PLANE_KNN keep one log per scan);
  * FLS_ERR_INVALID_ARG when `scan` is not below that call's n_scans; a Match that fails after its launch leaves no log */
 int fls_get_iter_log_scan(const fls_handle* h, int scan, fls_iter_log* out, int capacity);
+
+/* the information record of scan `scan` of the last Match call (fls_information).  out->valid = 0 when the handle was created
+ * without FLS_FLAG_INFORMATION, before its first Match, after a Match call that returned an error, between
+ * fls_match_batch_begin and _end, and after any relocalization call (whose internal Matches do not evaluate).
+ * FLS_ERR_INVALID_ARG when `scan` is not below the n_scans of the call that left records (1 when there are none). */
+int fls_get_information_scan(const fls_handle* h, int scan, fls_information* out);
+int fls_get_information(const fls_handle* h, fls_information* out); /* scan 0 */
 
 int fls_get_map_info(const fls_handle* h, fls_map_info* out);
 /* Keys (x, y, z voxel coordinates, int32 triples) of the voxels the map currently holds, in no particular order: FLS_NDT
