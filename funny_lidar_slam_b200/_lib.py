@@ -24,6 +24,7 @@ EXPORTS = [
     "fls_relocalize_multi", "fls_relocalize_multi_device",
     "fls_keyframes_scan_context", "fls_keyframes_detect_loop", "fls_keyframes_place_query", "fls_keyframes_place_query_device",
     "fls_get_information", "fls_get_information_scan",
+    "fls_preprocess_motion", "fls_preprocess_device_motion", "fls_project_imu_motion", "fls_preprocess_loam_motion", "fls_preprocess_loam_device_motion",
 ]
 
 
@@ -63,6 +64,12 @@ def lib():
     L.fls_preprocess_loam_device.argtypes = [C.POINTER(FlsLoamFrontendCfg), vp, vp, vp, sz, vp, vp, vp, vp, vp, C.POINTER(sz), C.POINTER(sz),
                                              C.POINTER(FlsMatchStats)]
     L.fls_preprocess_device.argtypes = [C.c_int, vp, vp, sz, vp, f32, f32, i32, f32, vp, vp, C.POINTER(sz), vp, vp, C.POINTER(sz)]
+    # the *_motion siblings take the parent's arguments and the body velocity (3 doubles, or NULL) last
+    L.fls_preprocess_motion.argtypes = [C.c_int, vp, sz, vp, f32, f32, i32, f32, vp, C.POINTER(sz), vp, C.POINTER(sz), vp]
+    L.fls_preprocess_device_motion.argtypes = L.fls_preprocess_device.argtypes + [vp]
+    L.fls_project_imu_motion.argtypes = [C.c_int, vp, vp, vp, sz, sz, vp, i32, i32, f32, f32, f32, vp, vp, vp, vp, vp, C.POINTER(sz), vp]
+    L.fls_preprocess_loam_motion.argtypes = L.fls_preprocess_loam.argtypes + [vp]
+    L.fls_preprocess_loam_device_motion.argtypes = L.fls_preprocess_loam_device.argtypes + [vp]
     L.fls_convert_cloud.argtypes = [C.POINTER(FlsConvertCfg), C.POINTER(FlsPointCloud2), vp, vp, vp, vp, vp, vp, C.POINTER(sz),
                                     C.POINTER(FlsConvertResult), C.POINTER(FlsMatchStats)]
     L.fls_match_batch.argtypes = [vp, C.c_int, C.POINTER(vp), C.POINTER(sz), sz, vp, C.POINTER(C.c_int), C.POINTER(FlsMatchStats)]

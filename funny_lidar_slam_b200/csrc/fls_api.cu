@@ -280,6 +280,9 @@ static bool loam_frontend_cfg_ok(const fls_loam_frontend_cfg& c) {
            c.corner_threshold < 3.0e38f && c.planar_threshold < 3.0e38f;
 }
 
+// The body velocity of the *_motion entries: NULL (rotation only), or three finite components.  Checked before anything is written.
+static bool velocity_ok(const double* v) { return !v || (std::isfinite(v[0]) && std::isfinite(v[1]) && std::isfinite(v[2])); }
+
 // Every Match entry runs through this: the call starts without an information record and leaves one only when it returns FLS_OK
 // (an argument check, a refusal or an error caught by FLS_CATCH all leave none).
 template <class F>
@@ -317,7 +320,21 @@ int fls_project(int device, const void* raw, const int32_t* ring, size_t n, size
         return FLS_ERR_INVALID_ARG;
     if (check_device(device) != FLS_OK) return FLS_ERR_NO_DEVICE;
     FLS_TRY
-    return fls::project_device(device, raw, ring, nullptr, nullptr, n, stride, n_rows, n_cols, horizontal_resolution, min_distance, max_distance, ordered,
+    return fls::project_device(device, raw, ring, nullptr, nullptr, nullptr, n, stride, n_rows, n_cols, horizontal_resolution, min_distance, max_distance, ordered,
+                               depth, col, row_start, row_end, n_ordered);
+    FLS_CATCH
+}
+
+// fls_project_imu and fls_project_imu_motion (vel NULL: rotation only)
+static int project_imu_entry(int device, const void* raw, const int32_t* ring, const float* time, size_t n, size_t stride, const fls_imu_buffer* imu,
+                             const double* vel, int32_t n_rows, int32_t n_cols, float horizontal_resolution, float min_distance, float max_distance,
+                             float* ordered, float* depth, int32_t* col, int32_t* row_start, int32_t* row_end, size_t* n_ordered) {
+    if ((!raw && n) || (!ring && n) || !ordered || !depth || !col || !row_start || !row_end || !n_ordered || !stride_ok(stride))
+        return FLS_ERR_INVALID_ARG;
+    if (imu && imu->n_imu && !time && n) return FLS_ERR_INVALID_ARG;
+    if (check_device(device) != FLS_OK) return FLS_ERR_NO_DEVICE;
+    FLS_TRY
+    return fls::project_device(device, raw, ring, time, imu, vel, n, stride, n_rows, n_cols, horizontal_resolution, min_distance, max_distance, ordered,
                                depth, col, row_start, row_end, n_ordered);
     FLS_CATCH
 }
@@ -325,23 +342,39 @@ int fls_project(int device, const void* raw, const int32_t* ring, size_t n, size
 int fls_project_imu(int device, const void* raw, const int32_t* ring, const float* time, size_t n, size_t stride, const fls_imu_buffer* imu,
                     int32_t n_rows, int32_t n_cols, float horizontal_resolution, float min_distance, float max_distance, float* ordered, float* depth,
                     int32_t* col, int32_t* row_start, int32_t* row_end, size_t* n_ordered) {
-    if ((!raw && n) || (!ring && n) || !ordered || !depth || !col || !row_start || !row_end || !n_ordered || !stride_ok(stride))
-        return FLS_ERR_INVALID_ARG;
-    if (imu && imu->n_imu && !time && n) return FLS_ERR_INVALID_ARG;
+    return project_imu_entry(device, raw, ring, time, n, stride, imu, nullptr, n_rows, n_cols, horizontal_resolution, min_distance, max_distance, ordered,
+                             depth, col, row_start, row_end, n_ordered);
+}
+
+int fls_project_imu_motion(int device, const void* raw, const int32_t* ring, const float* time, size_t n, size_t stride, const fls_imu_buffer* imu,
+                           int32_t n_rows, int32_t n_cols, float horizontal_resolution, float min_distance, float max_distance, float* ordered,
+                           float* depth, int32_t* col, int32_t* row_start, int32_t* row_end, size_t* n_ordered, const double velocity_imu[3]) {
+    if (!velocity_ok(velocity_imu)) return FLS_ERR_INVALID_ARG;
+    return project_imu_entry(device, raw, ring, time, n, stride, imu, velocity_imu, n_rows, n_cols, horizontal_resolution, min_distance, max_distance,
+                             ordered, depth, col, row_start, row_end, n_ordered);
+}
+
+// fls_preprocess and fls_preprocess_motion
+static int preprocess_entry(int device, const float* raw_xyzit, size_t n, const fls_imu_buffer* imu, const double* vel, float min_distance,
+                            float max_distance, int32_t jump_span, float planar_leaf, float* ordered, size_t* n_ordered, float* planar, size_t* n_planar) {
+    if ((!raw_xyzit && n) || !ordered || !planar || !n_ordered || !n_planar || jump_span < 1 || !(planar_leaf > 0.f)) return FLS_ERR_INVALID_ARG;
     if (check_device(device) != FLS_OK) return FLS_ERR_NO_DEVICE;
     FLS_TRY
-    return fls::project_device(device, raw, ring, time, imu, n, stride, n_rows, n_cols, horizontal_resolution, min_distance, max_distance, ordered,
-                               depth, col, row_start, row_end, n_ordered);
+    return fls::preprocess_device(device, raw_xyzit, n, imu, vel, min_distance, max_distance, jump_span, planar_leaf, ordered, n_ordered, planar, n_planar);
     FLS_CATCH
 }
 
 int fls_preprocess(int device, const float* raw_xyzit, size_t n, const fls_imu_buffer* imu, float min_distance, float max_distance, int32_t jump_span,
                    float planar_leaf, float* ordered, size_t* n_ordered, float* planar, size_t* n_planar) {
-    if ((!raw_xyzit && n) || !ordered || !planar || !n_ordered || !n_planar || jump_span < 1 || !(planar_leaf > 0.f)) return FLS_ERR_INVALID_ARG;
-    if (check_device(device) != FLS_OK) return FLS_ERR_NO_DEVICE;
-    FLS_TRY
-    return fls::preprocess_device(device, raw_xyzit, n, imu, min_distance, max_distance, jump_span, planar_leaf, ordered, n_ordered, planar, n_planar);
-    FLS_CATCH
+    return preprocess_entry(device, raw_xyzit, n, imu, nullptr, min_distance, max_distance, jump_span, planar_leaf, ordered, n_ordered, planar, n_planar);
+}
+
+int fls_preprocess_motion(int device, const float* raw_xyzit, size_t n, const fls_imu_buffer* imu, float min_distance, float max_distance,
+                          int32_t jump_span, float planar_leaf, float* ordered, size_t* n_ordered, float* planar, size_t* n_planar,
+                          const double velocity_imu[3]) {
+    if (!velocity_ok(velocity_imu)) return FLS_ERR_INVALID_ARG;
+    return preprocess_entry(device, raw_xyzit, n, imu, velocity_imu, min_distance, max_distance, jump_span, planar_leaf, ordered, n_ordered, planar,
+                            n_planar);
 }
 
 const char* fls_strerror(int status) {
@@ -846,9 +879,10 @@ int fls_voxel_grid(int device, const void* pts, size_t n, size_t stride, float l
     FLS_CATCH
 }
 
-int fls_preprocess_loam(const fls_loam_frontend_cfg* cfg, const void* raw, const int32_t* ring, const float* time, size_t n, size_t stride,
-                        const fls_imu_buffer* imu, float* corner, float* planar, float* d_corner, float* d_planar, size_t* n_corner, size_t* n_planar,
-                        fls_match_stats* stats) {
+// fls_preprocess_loam and fls_preprocess_loam_motion
+static int preprocess_loam_entry(const fls_loam_frontend_cfg* cfg, const void* raw, const int32_t* ring, const float* time, size_t n, size_t stride,
+                                 const fls_imu_buffer* imu, const double* vel, float* corner, float* planar, float* d_corner, float* d_planar,
+                                 size_t* n_corner, size_t* n_planar, fls_match_stats* stats) {
     if (!cfg || !n_corner || !n_planar) return FLS_ERR_INVALID_ARG;
     *n_corner = *n_planar = 0;
     if ((!raw && n) || (!ring && n) || !stride_ok(stride) || n > 0x7fffffffull) return FLS_ERR_INVALID_ARG;
@@ -857,13 +891,27 @@ int fls_preprocess_loam(const fls_loam_frontend_cfg* cfg, const void* raw, const
     if (imu && imu->n_imu && !time && n) return FLS_ERR_INVALID_ARG;
     if (check_device(cfg->device) != FLS_OK) return FLS_ERR_NO_DEVICE;
     FLS_TRY
-    return fls::preprocess_loam_device(*cfg, raw, ring, time, n, stride, imu, corner, planar, d_corner, d_planar, n_corner, n_planar, stats, false);
+    return fls::preprocess_loam_device(*cfg, raw, ring, time, n, stride, imu, vel, corner, planar, d_corner, d_planar, n_corner, n_planar, stats, false);
     FLS_CATCH
 }
 
-int fls_preprocess_loam_device(const fls_loam_frontend_cfg* cfg, const float* d_xyzi, const int32_t* d_ring, const float* d_time, size_t n,
+int fls_preprocess_loam(const fls_loam_frontend_cfg* cfg, const void* raw, const int32_t* ring, const float* time, size_t n, size_t stride,
+                        const fls_imu_buffer* imu, float* corner, float* planar, float* d_corner, float* d_planar, size_t* n_corner, size_t* n_planar,
+                        fls_match_stats* stats) {
+    return preprocess_loam_entry(cfg, raw, ring, time, n, stride, imu, nullptr, corner, planar, d_corner, d_planar, n_corner, n_planar, stats);
+}
+
+int fls_preprocess_loam_motion(const fls_loam_frontend_cfg* cfg, const void* raw, const int32_t* ring, const float* time, size_t n, size_t stride,
                                const fls_imu_buffer* imu, float* corner, float* planar, float* d_corner, float* d_planar, size_t* n_corner,
-                               size_t* n_planar, fls_match_stats* stats) {
+                               size_t* n_planar, fls_match_stats* stats, const double velocity_imu[3]) {
+    if (!velocity_ok(velocity_imu)) return FLS_ERR_INVALID_ARG;
+    return preprocess_loam_entry(cfg, raw, ring, time, n, stride, imu, velocity_imu, corner, planar, d_corner, d_planar, n_corner, n_planar, stats);
+}
+
+// fls_preprocess_loam_device and fls_preprocess_loam_device_motion
+static int preprocess_loam_device_entry(const fls_loam_frontend_cfg* cfg, const float* d_xyzi, const int32_t* d_ring, const float* d_time, size_t n,
+                                        const fls_imu_buffer* imu, const double* vel, float* corner, float* planar, float* d_corner, float* d_planar,
+                                        size_t* n_corner, size_t* n_planar, fls_match_stats* stats) {
     if (!cfg || !n_corner || !n_planar) return FLS_ERR_INVALID_ARG;
     *n_corner = *n_planar = 0;
     if ((!d_xyzi && n) || (!d_ring && n) || n > 0x7fffffffull) return FLS_ERR_INVALID_ARG;
@@ -872,23 +920,52 @@ int fls_preprocess_loam_device(const fls_loam_frontend_cfg* cfg, const float* d_
     if (imu && imu->n_imu && !d_time && n) return FLS_ERR_INVALID_ARG;
     if (check_device(cfg->device) != FLS_OK) return FLS_ERR_NO_DEVICE;
     FLS_TRY
-    return fls::preprocess_loam_device(*cfg, d_xyzi, d_ring, d_time, n, FLS_LAYOUT_PACKED, imu, corner, planar, d_corner, d_planar, n_corner, n_planar,
-                                       stats, true);
+    return fls::preprocess_loam_device(*cfg, d_xyzi, d_ring, d_time, n, FLS_LAYOUT_PACKED, imu, vel, corner, planar, d_corner, d_planar, n_corner,
+                                       n_planar, stats, true);
     FLS_CATCH
 }
 
-int fls_preprocess_device(int device, const float* d_xyzi, const float* d_time, size_t n, const fls_imu_buffer* imu, float min_distance,
-                          float max_distance, int32_t jump_span, float planar_leaf, float* ordered, float* d_ordered, size_t* n_ordered, float* planar,
-                          float* d_planar, size_t* n_planar) {
+int fls_preprocess_loam_device(const fls_loam_frontend_cfg* cfg, const float* d_xyzi, const int32_t* d_ring, const float* d_time, size_t n,
+                               const fls_imu_buffer* imu, float* corner, float* planar, float* d_corner, float* d_planar, size_t* n_corner,
+                               size_t* n_planar, fls_match_stats* stats) {
+    return preprocess_loam_device_entry(cfg, d_xyzi, d_ring, d_time, n, imu, nullptr, corner, planar, d_corner, d_planar, n_corner, n_planar, stats);
+}
+
+int fls_preprocess_loam_device_motion(const fls_loam_frontend_cfg* cfg, const float* d_xyzi, const int32_t* d_ring, const float* d_time, size_t n,
+                                      const fls_imu_buffer* imu, float* corner, float* planar, float* d_corner, float* d_planar, size_t* n_corner,
+                                      size_t* n_planar, fls_match_stats* stats, const double velocity_imu[3]) {
+    if (!velocity_ok(velocity_imu)) return FLS_ERR_INVALID_ARG;
+    return preprocess_loam_device_entry(cfg, d_xyzi, d_ring, d_time, n, imu, velocity_imu, corner, planar, d_corner, d_planar, n_corner, n_planar, stats);
+}
+
+// fls_preprocess_device and fls_preprocess_device_motion
+static int preprocess_device_entry(int device, const float* d_xyzi, const float* d_time, size_t n, const fls_imu_buffer* imu, const double* vel,
+                                   float min_distance, float max_distance, int32_t jump_span, float planar_leaf, float* ordered, float* d_ordered,
+                                   size_t* n_ordered, float* planar, float* d_planar, size_t* n_planar) {
     if (!n_ordered || !n_planar) return FLS_ERR_INVALID_ARG;
     *n_ordered = *n_planar = 0;
     if ((!d_xyzi && n) || (!ordered && !d_ordered && !planar && !d_planar) || jump_span < 1 || !(planar_leaf > 0.f)) return FLS_ERR_INVALID_ARG;
     if (imu && imu->n_imu && !d_time && n) return FLS_ERR_INVALID_ARG;
     if (check_device(device) != FLS_OK) return FLS_ERR_NO_DEVICE;
     FLS_TRY
-    return fls::preprocess_device_input(device, d_xyzi, d_time, n, imu, min_distance, max_distance, jump_span, planar_leaf, ordered, d_ordered, n_ordered,
-                                        planar, d_planar, n_planar);
+    return fls::preprocess_device_input(device, d_xyzi, d_time, n, imu, vel, min_distance, max_distance, jump_span, planar_leaf, ordered, d_ordered,
+                                        n_ordered, planar, d_planar, n_planar);
     FLS_CATCH
+}
+
+int fls_preprocess_device(int device, const float* d_xyzi, const float* d_time, size_t n, const fls_imu_buffer* imu, float min_distance,
+                          float max_distance, int32_t jump_span, float planar_leaf, float* ordered, float* d_ordered, size_t* n_ordered, float* planar,
+                          float* d_planar, size_t* n_planar) {
+    return preprocess_device_entry(device, d_xyzi, d_time, n, imu, nullptr, min_distance, max_distance, jump_span, planar_leaf, ordered, d_ordered,
+                                   n_ordered, planar, d_planar, n_planar);
+}
+
+int fls_preprocess_device_motion(int device, const float* d_xyzi, const float* d_time, size_t n, const fls_imu_buffer* imu, float min_distance,
+                                 float max_distance, int32_t jump_span, float planar_leaf, float* ordered, float* d_ordered, size_t* n_ordered,
+                                 float* planar, float* d_planar, size_t* n_planar, const double velocity_imu[3]) {
+    if (!velocity_ok(velocity_imu)) return FLS_ERR_INVALID_ARG;
+    return preprocess_device_entry(device, d_xyzi, d_time, n, imu, velocity_imu, min_distance, max_distance, jump_span, planar_leaf, ordered, d_ordered,
+                                   n_ordered, planar, d_planar, n_planar);
 }
 
 int fls_convert_cloud(const fls_convert_cfg* cfg, const fls_pointcloud2* msg, float* xyzi, int32_t* ring, float* time, float* d_xyzi, int32_t* d_ring,

@@ -2,7 +2,8 @@
 // IMU orientation interpolated at the point's time (DataSearcher::SearchNearestTwoData, include/common/data_searcher.h:100-134;
 // MotionInterpolator::InterpolateQuaternionLerp, include/common/motion_interpolator.h:27-35), point moved lidar -> imu and rotated
 // by q_ref^-1 * q(t).  fp64 with explicit roundings in the evaluation order the oracle pins (oracle/orc_deskew.h), so the
-// corrected coordinates are bit-identical.
+// corrected coordinates are bit-identical.  With a body velocity (the *_motion entries, not upstream) the constant-velocity
+// translation v * dt is added in fp64 before the rounding to float (oracle_motion/orc_motion.h pins that order).
 #pragma once
 #include "fls_common.cuh"
 
@@ -12,14 +13,17 @@ struct DeskewView {
     const unsigned long long* __restrict__ t;  // IMU time stamps [us], ascending (device)
     const double* __restrict__ q;              // quaternions x, y, z, w (device)
     int m;                                     // 0: no de-skew (identity)
+    int move;                                  // 1: add v * dt (v has a non-zero component); 0: rotation only
     unsigned long long ref_time;
     double qri[4];   // q_ref^-1 (x, y, z, w) — SetRefTime (:19-34), computed on the host
     double T[16];    // lidar -> imu, column-major
+    double v[3];     // body velocity [m/s] in the IMU frame at ref_time (read when move)
 };
 
 #ifdef __CUDACC__
 __device__ __forceinline__ bool deskew_point(const DeskewView& d, float x, float y, float z, float rel_time, float& xo, float& yo, float& zo) {
-    const unsigned long long t = (unsigned long long)((long long)d.ref_time + trunc_i64(__dmul_rn((double)rel_time, 1.0e6)));
+    const long long dt_us = trunc_i64(__dmul_rn((double)rel_time, 1.0e6));
+    const unsigned long long t = (unsigned long long)((long long)d.ref_time + dt_us);
     const int m = d.m;
     if (m < 2 || d.t[0] > t || d.t[m - 1] < t) return false;
     int l;
@@ -66,9 +70,18 @@ __device__ __forceinline__ bool deskew_point(const DeskewView& d, float x, float
     double uy = __dsub_rn(__dmul_rn(pz, vx), __dmul_rn(px, vz));
     double uz = __dsub_rn(__dmul_rn(px, vy), __dmul_rn(py, vx));
     ux = __dadd_rn(ux, ux); uy = __dadd_rn(uy, uy); uz = __dadd_rn(uz, uz);
-    xo = (float)__dadd_rn(__dadd_rn(vx, __dmul_rn(pw, ux)), __dsub_rn(__dmul_rn(py, uz), __dmul_rn(pz, uy)));
-    yo = (float)__dadd_rn(__dadd_rn(vy, __dmul_rn(pw, uy)), __dsub_rn(__dmul_rn(pz, ux), __dmul_rn(px, uz)));
-    zo = (float)__dadd_rn(__dadd_rn(vz, __dmul_rn(pw, uz)), __dsub_rn(__dmul_rn(px, uy), __dmul_rn(py, ux)));
+    double ox = __dadd_rn(__dadd_rn(vx, __dmul_rn(pw, ux)), __dsub_rn(__dmul_rn(py, uz), __dmul_rn(pz, uy)));
+    double oy = __dadd_rn(__dadd_rn(vy, __dmul_rn(pw, uy)), __dsub_rn(__dmul_rn(pz, ux), __dmul_rn(px, uz)));
+    double oz = __dadd_rn(__dadd_rn(vz, __dmul_rn(pw, uz)), __dsub_rn(__dmul_rn(px, uy), __dmul_rn(py, ux)));
+    if (d.move) {  // + v * dt; skipped (not + 0.0) without motion, so a -0.0 stays -0.0
+        const double dt = __dmul_rn((double)dt_us, 1.0e-6);
+        ox = __dadd_rn(ox, __dmul_rn(d.v[0], dt));
+        oy = __dadd_rn(oy, __dmul_rn(d.v[1], dt));
+        oz = __dadd_rn(oz, __dmul_rn(d.v[2], dt));
+    }
+    xo = (float)ox;
+    yo = (float)oy;
+    zo = (float)oz;
     return true;
 }
 #endif

@@ -20,7 +20,7 @@ struct LoamWorkspace : Workspace {
 }  // namespace
 
 int preprocess_loam_device(const fls_loam_frontend_cfg& c, const void* raw, const int* ring, const float* time, size_t n, size_t stride,
-                           const fls_imu_buffer* imu, float* corner, float* planar, float* d_corner, float* d_planar, size_t* n_corner,
+                           const fls_imu_buffer* imu, const double* vel, float* corner, float* planar, float* d_corner, float* d_planar, size_t* n_corner,
                            size_t* n_planar, fls_match_stats* stats, bool src_on_device) {
     *n_corner = *n_planar = 0;
     const int V = c.n_rows, H = c.n_cols;
@@ -30,7 +30,7 @@ int preprocess_loam_device(const fls_loam_frontend_cfg& c, const void* raw, cons
         int* const h_small = w.h_small.reserve((size_t)2 * V + 1);
         call.begin();
         // ---- projector (+ de-skew) ----
-        int rc = enqueue_project(w.proj, raw, ring, time, imu, n, stride, V, H, c.horizontal_resolution, c.min_distance, c.max_distance, call, src_on_device);
+        int rc = enqueue_project(w.proj, raw, ring, time, imu, vel, n, stride, V, H, c.horizontal_resolution, c.min_distance, c.max_distance, call, src_on_device);
         if (rc != FLS_OK) return rc;
         // sync 1: n_ordered and the row bounds size the feature kernels (shared memory, planar capacity)
         FLS_CUDA(cudaMemcpyAsync(h_small, w.proj.total.p, sizeof(int), cudaMemcpyDeviceToHost, st));

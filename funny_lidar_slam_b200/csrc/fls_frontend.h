@@ -21,11 +21,12 @@ struct ProjStage {
 
 // Uploads the raw records (+ ring, and time and the IMU samples when de-skewing) and enqueues PointcloudProjector::Project on
 // c.stream: s.ordered / s.depth / s.col (V*H entries, the first *s.total meaningful), s.rows, s.total.  A reference time outside the
-// IMU buffer accepts no point.  Counts the bytes it copies and the kernels it launches; nothing waits.
+// IMU buffer accepts no point.  `vel` (NULL: rotation only) is the body velocity of the *_motion entries.  Counts the bytes it copies
+// and the kernels it launches; nothing waits.
 // src_on_device: raw (packed float4, stride 16), ring and time are device arrays on the stream's device and only the IMU samples
 // are uploaded; the kernels are the same.
-int enqueue_project(ProjStage& s, const void* raw, const int* ring, const float* time, const fls_imu_buffer* imu, size_t n, size_t stride, int V,
-                    int H, float h_res, float min_d, float max_d, Call& c, bool src_on_device);
+int enqueue_project(ProjStage& s, const void* raw, const int* ring, const float* time, const fls_imu_buffer* imu, const double* vel, size_t n,
+                    size_t stride, int V, int H, float h_res, float min_d, float max_d, Call& c, bool src_on_device);
 
 // launch shape of the feature kernels, from the host copy of the row bounds
 struct FeatPlan {
@@ -64,7 +65,7 @@ inline long long voxel_algo_bytes(size_t n_in, size_t n_out) { return (long long
 // fls_preprocess_loam (src_on_device false) and fls_preprocess_loam_device (true: raw / ring / time are device arrays, stride 16)
 // after their argument checks (fls_frontend.cu)
 int preprocess_loam_device(const fls_loam_frontend_cfg& c, const void* raw, const int* ring, const float* time, size_t n, size_t stride,
-                           const fls_imu_buffer* imu, float* corner, float* planar, float* d_corner, float* d_planar, size_t* n_corner,
+                           const fls_imu_buffer* imu, const double* vel, float* corner, float* planar, float* d_corner, float* d_planar, size_t* n_corner,
                            size_t* n_planar, fls_match_stats* stats, bool src_on_device);
 
 // fls_convert_cloud after its argument checks (fls_convert.cu)
@@ -73,8 +74,8 @@ int convert_cloud_device(const fls_convert_cfg& c, const fls_pointcloud2& m, flo
 
 // fls_preprocess_device (device float4 xyzi + float time) after its argument checks (fls_preprocess.cu; the host entry's driver is
 // preprocess_device, fls_maps.h)
-int preprocess_device_input(int device, const float* d_xyzi, const float* d_time, size_t n, const fls_imu_buffer* imu, float min_d, float max_d,
-                            int jump_span, float leaf, float* ordered_out, float* d_ordered, size_t* n_ordered, float* planar_out, float* d_planar,
-                            size_t* n_planar);
+int preprocess_device_input(int device, const float* d_xyzi, const float* d_time, size_t n, const fls_imu_buffer* imu, const double* vel, float min_d,
+                            float max_d, int jump_span, float leaf, float* ordered_out, float* d_ordered, size_t* n_ordered, float* planar_out,
+                            float* d_planar, size_t* n_planar);
 
 }  // namespace fls

@@ -253,12 +253,13 @@ int pcd_read(const char* path, std::vector<float>& xyzi, std::string& err);
 int pcd_write(const char* path, const float* xyzi, size_t n, std::string& err);
 
 // repack caller records (stride >= 20, intensity at byte 16) into packed float4 on the device
-int project_device(int device, const void* raw, const int* ring, const float* time, const fls_imu_buffer* imu, size_t n, size_t stride, int V, int H,
-                   float h_res, float min_d, float max_d, float* ordered_out, float* depth_out, int* col_out, int* row_start, int* row_end,
+int project_device(int device, const void* raw, const int* ring, const float* time, const fls_imu_buffer* imu, const double* vel, size_t n, size_t stride,
+                   int V, int H, float h_res, float min_d, float max_d, float* ordered_out, float* depth_out, int* col_out, int* row_start, int* row_end,
                    size_t* n_out);
 // PreProcessing::Run, non-feature branch (preprocessing.cpp:181-225): raw x,y,z,intensity,time records -> ordered + planar clouds (host)
-int preprocess_device(int device, const float* raw_xyzit, size_t n, const fls_imu_buffer* imu, float min_d, float max_d, int jump_span, float leaf,
-                      float* ordered_out, size_t* n_ordered, float* planar_out, size_t* n_planar);
+// `vel`: NULL, or the body velocity of fls_preprocess_motion (rotation only when all zero)
+int preprocess_device(int device, const float* raw_xyzit, size_t n, const fls_imu_buffer* imu, const double* vel, float min_d, float max_d, int jump_span,
+                      float leaf, float* ordered_out, size_t* n_ordered, float* planar_out, size_t* n_planar);
 // Copies n host records of `stride` bytes (stride_ok) to packed float4 at dst on c.stream: one copy when they are packed already, else
 // a copy to `staging` and one repack kernel.  Counts the bytes copied and the kernel.
 void upload_records(const void* pts, size_t n, size_t stride, float4* dst, DevBuf<unsigned char>& staging, Call& c);

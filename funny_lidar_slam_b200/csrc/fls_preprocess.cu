@@ -87,12 +87,13 @@ struct PpWorkspace : Workspace {
 
 }  // namespace
 
-// uploads the IMU samples and fills the view.  ref_outside: ref_time is outside the buffer (SetRefTime fails; the view stays the
+// uploads the IMU samples and fills the view; `vel` (NULL, or a finite body velocity checked by the entry) sets the translation
+// term, which an all-zero velocity leaves off.  ref_outside: ref_time is outside the buffer (SetRefTime fails; the view stays the
 // identity).  Returns FLS_ERR_INVALID_ARG for a null array, more than 2^31 - 1 samples, or a stamp followed by a smaller one:
 // deskew_point finds the interval by bisection, upstream by a downward scan (data_searcher.h:100-134), and the two pick the same
 // pair only on ascending stamps (equal ones allowed).
-int make_deskew_view(const fls_imu_buffer* imu, DevBuf<unsigned long long>& d_t, DevBuf<double>& d_q, cudaStream_t st, DeskewView& v,
-                     bool& ref_outside) {
+int make_deskew_view(const fls_imu_buffer* imu, const double* vel, DevBuf<unsigned long long>& d_t, DevBuf<double>& d_q, cudaStream_t st,
+                     DeskewView& v, bool& ref_outside) {
     std::memset(&v, 0, sizeof(v));
     ref_outside = false;
     if (!imu || imu->n_imu == 0) return FLS_OK;  // identity
@@ -112,6 +113,10 @@ int make_deskew_view(const fls_imu_buffer* imu, DevBuf<unsigned long long>& d_t,
     v.m = (int)imu->n_imu;
     v.ref_time = imu->ref_time_us;
     for (int k = 0; k < 16; ++k) v.T[k] = imu->T_lidar_to_imu[k];
+    if (vel && (vel[0] != 0.0 || vel[1] != 0.0 || vel[2] != 0.0)) {
+        v.move = 1;
+        for (int k = 0; k < 3; ++k) v.v[k] = vel[k];
+    }
     return FLS_OK;
 }
 
@@ -119,9 +124,9 @@ namespace {
 
 // The points are host records {x, y, z, intensity, time} (src_on_device false: uploaded first) or device arrays (float4 xyzi, float time).
 // ordered_cloud_ goes to ordered_out (host) and / or d_ordered, planar_cloud_ to planar_out and / or d_planar (NULL: not written).
-int run_preprocess(int device, const float* xyzi, const float* time, bool src_on_device, size_t n, const fls_imu_buffer* imu, float min_d, float max_d,
-                   int jump_span, float leaf, float* ordered_out, float* d_ordered, size_t* n_ordered, float* planar_out, float* d_planar,
-                   size_t* n_planar) {
+int run_preprocess(int device, const float* xyzi, const float* time, bool src_on_device, size_t n, const fls_imu_buffer* imu, const double* vel,
+                   float min_d, float max_d, int jump_span, float leaf, float* ordered_out, float* d_ordered, size_t* n_ordered, float* planar_out,
+                   float* d_planar, size_t* n_planar) {
     *n_ordered = *n_planar = 0;
     if (n > 0x7fffffffull || jump_span < 1 || !(leaf > 0.f)) return FLS_ERR_INVALID_ARG;
     if (n == 0) return FLS_OK;
@@ -131,7 +136,7 @@ int run_preprocess(int device, const float* xyzi, const float* time, bool src_on
         c.begin();
         DeskewView dv;
         bool ref_outside;
-        const int rc = make_deskew_view(imu, w.imu_t, w.imu_q, st, dv, ref_outside);
+        const int rc = make_deskew_view(imu, vel, w.imu_t, w.imu_q, st, dv, ref_outside);
         if (rc != FLS_OK) return rc;
         if (ref_outside) return FLS_OK;  // SetRefTime failed: upstream drops the scan (:178-183) -> empty clouds
         w.corrected.reserve(n);
@@ -179,16 +184,16 @@ int run_preprocess(int device, const float* xyzi, const float* time, bool src_on
 
 }  // namespace
 
-int preprocess_device(int device, const float* raw_xyzit, size_t n, const fls_imu_buffer* imu, float min_d, float max_d, int jump_span, float leaf,
-                      float* ordered_out, size_t* n_ordered, float* planar_out, size_t* n_planar) {
-    return run_preprocess(device, raw_xyzit, nullptr, false, n, imu, min_d, max_d, jump_span, leaf, ordered_out, nullptr, n_ordered, planar_out, nullptr,
+int preprocess_device(int device, const float* raw_xyzit, size_t n, const fls_imu_buffer* imu, const double* vel, float min_d, float max_d,
+                      int jump_span, float leaf, float* ordered_out, size_t* n_ordered, float* planar_out, size_t* n_planar) {
+    return run_preprocess(device, raw_xyzit, nullptr, false, n, imu, vel, min_d, max_d, jump_span, leaf, ordered_out, nullptr, n_ordered, planar_out, nullptr,
                           n_planar);
 }
 
-int preprocess_device_input(int device, const float* d_xyzi, const float* d_time, size_t n, const fls_imu_buffer* imu, float min_d, float max_d,
-                            int jump_span, float leaf, float* ordered_out, float* d_ordered, size_t* n_ordered, float* planar_out, float* d_planar,
-                            size_t* n_planar) {
-    return run_preprocess(device, d_xyzi, d_time, true, n, imu, min_d, max_d, jump_span, leaf, ordered_out, d_ordered, n_ordered, planar_out, d_planar,
+int preprocess_device_input(int device, const float* d_xyzi, const float* d_time, size_t n, const fls_imu_buffer* imu, const double* vel, float min_d,
+                            float max_d, int jump_span, float leaf, float* ordered_out, float* d_ordered, size_t* n_ordered, float* planar_out,
+                            float* d_planar, size_t* n_planar) {
+    return run_preprocess(device, d_xyzi, d_time, true, n, imu, vel, min_d, max_d, jump_span, leaf, ordered_out, d_ordered, n_ordered, planar_out, d_planar,
                           n_planar);
 }
 

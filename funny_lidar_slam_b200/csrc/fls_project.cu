@@ -80,17 +80,17 @@ struct ProjWorkspace : Workspace {
 
 }  // namespace
 
-int make_deskew_view(const fls_imu_buffer* imu, DevBuf<unsigned long long>& d_t, DevBuf<double>& d_q, cudaStream_t st, DeskewView& v,
-                     bool& ref_outside);
+int make_deskew_view(const fls_imu_buffer* imu, const double* vel, DevBuf<unsigned long long>& d_t, DevBuf<double>& d_q, cudaStream_t st,
+                     DeskewView& v, bool& ref_outside);
 
-int enqueue_project(ProjStage& w, const void* raw, const int* ring, const float* time, const fls_imu_buffer* imu, size_t n, size_t stride, int V, int H,
-                    float h_res, float min_d, float max_d, Call& c, bool src_on_device) {
+int enqueue_project(ProjStage& w, const void* raw, const int* ring, const float* time, const fls_imu_buffer* imu, const double* vel, size_t n,
+                    size_t stride, int V, int H, float h_res, float min_d, float max_d, Call& c, bool src_on_device) {
     const cudaStream_t st = c.stream;
     const size_t cells = (size_t)V * H;
     DeskewView dv;
     const bool use_imu = imu && imu->n_imu && time;
     bool ref_outside;
-    const int rc = make_deskew_view(use_imu ? imu : nullptr, w.imu_t, w.imu_q, st, dv, ref_outside);
+    const int rc = make_deskew_view(use_imu ? imu : nullptr, vel, w.imu_t, w.imu_q, st, dv, ref_outside);
     if (rc != FLS_OK) return rc;
     if (dv.m > 0) c.h2d += (long long)(imu->n_imu * (sizeof(unsigned long long) + 4 * sizeof(double)));
     if (ref_outside) n = 0;  // SetRefTime failed: no point is accepted
@@ -134,8 +134,9 @@ int enqueue_project(ProjStage& w, const void* raw, const int* ring, const float*
 
 // Host driver: raw cloud (host, `stride` bytes per record) + ring per point -> projector arrays (host).  depth_out / col_out hold V*H
 // entries (the first *n_out are meaningful, as upstream), ordered_out V*H packed float4 records.
-int project_device(int device, const void* raw, const int* ring, const float* time, const fls_imu_buffer* imu, size_t n, size_t stride, int V, int H,
-                   float h_res, float min_d, float max_d, float* ordered_out, float* depth_out, int* col_out, int* row_start, int* row_end, size_t* n_out) {
+int project_device(int device, const void* raw, const int* ring, const float* time, const fls_imu_buffer* imu, const double* vel, size_t n, size_t stride,
+                   int V, int H, float h_res, float min_d, float max_d, float* ordered_out, float* depth_out, int* col_out, int* row_start, int* row_end,
+                   size_t* n_out) {
     *n_out = 0;
     if (V <= 0 || H <= 0 || !(h_res > 0.f) || n > 0x7fffffffull) return FLS_ERR_INVALID_ARG;
     const size_t cells = (size_t)V * H;
@@ -145,7 +146,7 @@ int project_device(int device, const void* raw, const int* ring, const float* ti
         const cudaStream_t st = c.stream;
         ProjStage& w = ws.s;
         c.begin();
-        const int rc = enqueue_project(w, raw, ring, time, imu, n, stride, V, H, h_res, min_d, max_d, c, false);
+        const int rc = enqueue_project(w, raw, ring, time, imu, vel, n, stride, V, H, h_res, min_d, max_d, c, false);
         if (rc != FLS_OK) return rc;
         unsigned total = 0;
         FLS_CUDA(cudaMemcpyAsync(&total, w.total.p, sizeof(total), cudaMemcpyDeviceToHost, st));

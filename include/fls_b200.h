@@ -24,6 +24,8 @@
  *                                 (src/slam/preprocessing.cpp:262-571) and the scan's time window (:86-104)
  *   fls_preprocess_device /    <- fls_preprocess / fls_preprocess_loam reading a cloud already in device memory
  *   fls_preprocess_loam_device
+ *   fls_*_motion               <- the five de-skewing entries above with the sensor's translation over the sweep added (not
+ *                                 upstream: lidar_distortion_corrector.cpp:34 leaves it as a TODO)
  *   fls_keyframes_*            <- the keyframe-map loops of System::SaveMap (src/slam/system.cpp:299-341),
  *                                 System::VisualizeGlobalMap (src/slam/system.cpp:847-896) and
  *                                 LoopClosure::GetSubMap (src/slam/loop_closure.cpp:179-231)
@@ -620,6 +622,37 @@ int fls_preprocess_loam_device(const fls_loam_frontend_cfg* cfg, const float* d_
 int fls_preprocess_device(int device, const float* d_xyzi, const float* d_time, size_t n, const fls_imu_buffer* imu, float min_distance,
                           float max_distance, int32_t jump_span, float planar_leaf, float* ordered, float* d_ordered, size_t* n_ordered, float* planar,
                           float* d_planar, size_t* n_planar);
+
+/* ---- De-skew with the sensor's translation (not upstream: LidarDistortionCorrector de-skews rotation only,
+ *      src/lidar/lidar_distortion_corrector.cpp:34 "TODO: add translation") ----
+ *
+ * Each de-skewing entry has a _motion sibling with one more argument, velocity_imu: the body's velocity [m/s] expressed in the
+ * IMU frame at ref_time_us, taken as constant over the sweep.  A kept point becomes
+ *     p_corr = q_ref^-1 q(t) (R_li p + t_li) + v * dt
+ * where t = ref_time_us + trunc_i64(rel_time * 1e6) is the integer microsecond stamp the interpolation uses and dt_us = t - ref_time_us
+ * as a signed count.  Rounding, pinned: each coordinate is (float)(rot_k + v[k] * dt) with dt = (double)dt_us * 1.0e-6, every
+ * product and sum rounded to nearest in fp64 (no fused multiply-add), and rot_k the fp64 value the parent entry rounds to float.
+ *   * velocity_imu == NULL, or all three components exactly +-0: the term is skipped (not added as +0.0), and every output is
+ *     bit-identical to the parent entry's.
+ *   * a NaN or infinite component: FLS_ERR_INVALID_ARG before anything, counts included, is written.
+ *   * no IMU samples (imu == NULL or n_imu == 0): no de-skew at all, velocity_imu is ignored.
+ * Everything else is the parent's: the range gate, the points outside the IMU buffer dropped, the empty result when ref_time_us is
+ * outside the buffer, and the projector's cell depth and column, which stay those of the raw point. */
+int fls_preprocess_motion(int device, const float* raw_xyzit, size_t n, const fls_imu_buffer* imu, float min_distance, float max_distance,
+                          int32_t jump_span, float planar_leaf, float* ordered, size_t* n_ordered, float* planar, size_t* n_planar,
+                          const double velocity_imu[3]);
+int fls_preprocess_device_motion(int device, const float* d_xyzi, const float* d_time, size_t n, const fls_imu_buffer* imu, float min_distance,
+                                 float max_distance, int32_t jump_span, float planar_leaf, float* ordered, float* d_ordered, size_t* n_ordered,
+                                 float* planar, float* d_planar, size_t* n_planar, const double velocity_imu[3]);
+int fls_project_imu_motion(int device, const void* raw, const int32_t* ring, const float* time, size_t n, size_t stride_bytes, const fls_imu_buffer* imu,
+                           int32_t n_rows, int32_t n_cols, float horizontal_resolution, float min_distance, float max_distance, float* ordered,
+                           float* depth, int32_t* col, int32_t* row_start, int32_t* row_end, size_t* n_ordered, const double velocity_imu[3]);
+int fls_preprocess_loam_motion(const fls_loam_frontend_cfg* cfg, const void* raw, const int32_t* ring, const float* time, size_t n, size_t stride_bytes,
+                               const fls_imu_buffer* imu, float* corner, float* planar, float* d_corner, float* d_planar, size_t* n_corner,
+                               size_t* n_planar, fls_match_stats* stats, const double velocity_imu[3]);
+int fls_preprocess_loam_device_motion(const fls_loam_frontend_cfg* cfg, const float* d_xyzi, const int32_t* d_ring, const float* d_time, size_t n,
+                                      const fls_imu_buffer* imu, float* corner, float* planar, float* d_corner, float* d_planar, size_t* n_corner,
+                                      size_t* n_planar, fls_match_stats* stats, const double velocity_imu[3]);
 
 /* ---- Keyframe maps on the device: System::SaveMap, System::VisualizeGlobalMap, LoopClosure::GetSubMap ---- */
 
